@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py — headline benchmark of the librosa FFT time-frequency hot path on B200.
+"""bench.py — headline benchmark of the librosa FFT time-frequency hot path on H100.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload cfg2|cfg3|cfg4|cfg5|stats|speech400]
+                    [--dump-outputs DIR]
 
 Metric (BASELINE.json): mel-spectrogram frames/sec, n_fft=2048, hop=512, n_mels=128, float32, on
 BASELINE.json configs[1] — batch = 1024 clips x 10 s mono @ 22050 Hz per GPU.  One "step" is one pass of
@@ -9,7 +10,8 @@ the fused stft -> |.|^2 -> mel kernel over that batch.  Weak scaling: every rank
 no collective on the data path; `value` = frames of all ranks / max-over-ranks device time.
 
 One JSON line on stdout (rank 0).  Extra keys beyond the base contract:
-  roofline      dominant kernel vs the measured HBM peak (MEASURED_PEAKS.json), algorithmic bytes
+  roofline      dominant kernel vs the HBM peak (MEASURED_PEAKS.json if present, else the H100 SXM data sheet),
+                algorithmic bytes
   cpu_baseline  the oracle port (oracle/ref_np.py == the reference's algorithm, bit-exact here) timed on
                 this box's host cores on a bounded sample: the three ways SURVEY 8d lists (batched call /
                 one-process loop / forked workers), best reported, all listed under `variants`
@@ -19,6 +21,8 @@ One JSON line on stdout (rank 0).  Extra keys beyond the base contract:
   secondary     device-resident ms / frames/s / roofline of BASELINE.json configs 3, 4, 5 (per-GPU shards) and of the
                 n_fft = 400 speech front end (`speech400`, mixed-radix kernel; not a BASELINE.json config)
   clocks        NVML samples taken during the timed region
+
+--dump-outputs DIR writes the last timed step's result (a seeded sample of clips, < 64 MB) to compare builds.
 """
 from __future__ import annotations
 
@@ -93,17 +97,7 @@ def measured_peak():
         with open(path) as fh:
             return float(json.load(fh)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
-
-
-def profiled_traffic(workload):
-    """DRAM bytes per launch of the dominant kernel from the committed ncu --set full capture, if any."""
-    path = os.path.join(ROOT, "profiles", "dram_traffic.json")
-    try:
-        with open(path) as fh:
-            return json.load(fh).get(workload)
-    except Exception:
-        return None
+        return 3350.0, "data sheet (H100 SXM HBM3 3.35 TB/s; not measured)"
 
 
 class ClockSampler:
@@ -347,19 +341,23 @@ def run_reference(args, w, rank, world):
 def make_steps(lb, w, dev, host):
     kw, op, sr = w["kw"], w["op"], w["sr"]
 
-    def step_resident():
+    def step_resident(keep=False):
+        """One device-resident step; keep=True returns the result (a DeviceArray) instead of releasing it."""
         if op == "mel":
-            lb.feature.melspectrogram(y=dev, sr=sr, **kw).free()
+            out = lb.feature.melspectrogram(y=dev, sr=sr, **kw)
         elif op == "stft":
-            lb.stft(dev, **kw).free()
+            out = lb.stft(dev, **kw)
         elif op == "mfcc":
-            lb.feature.mfcc(y=dev, sr=sr, **kw).free()
+            out = lb.feature.mfcc(y=dev, sr=sr, **kw)
         elif op == "centroid":
-            lb.feature.spectral_centroid(y=dev, sr=sr, **kw).free()
+            out = lb.feature.spectral_centroid(y=dev, sr=sr, **kw)
         else:
             D = lb.stft(dev, **kw)
-            lb.istft(D, hop_length=kw["hop_length"], length=w["n"]).free()
+            out = lb.istft(D, hop_length=kw["hop_length"], length=w["n"])
             D.free()
+        if keep:
+            return out
+        out.free()
 
     def step_e2e(src=None):
         y = host if src is None else src
@@ -416,8 +414,9 @@ def run_ours(args, w, rank, world, local_rank):
 
     peak, peak_src = measured_peak()
 
-    def resident(wl, steps, warmup, sample_clocks):
-        """Device-resident timing of one workload: (ms per step max over ranks, launches, clocks, frames per GPU)."""
+    def resident(wl, steps, warmup, sample_clocks, keep_last=False):
+        """Device-resident timing of one workload: (ms per step max over ranks, launches, clocks, frames per GPU);
+        keep_last: also return the result of the last timed step (`last`)."""
         T = n_frames(wl["n"], wl["kw"]["n_fft"], wl["kw"]["hop_length"])
         host = lb.pinned_empty((wl["clips"], wl["n"]), np.float32)
         host[...] = make_batch(wl, rank)
@@ -429,9 +428,10 @@ def run_ours(args, w, rank, world, local_rank):
         sampler = ClockSampler(local_rank) if (rank == 0 and sample_clocks) else None
         launches0 = ctx.launch_count
         e0, e1 = ctx.event(), ctx.event()
+        last = None
         e0.record()
-        for _ in range(steps):
-            step_resident()
+        for i in range(steps):
+            last = step_resident(keep=keep_last and i == steps - 1)
         e1.record()
         ms = e0.elapsed_ms(e1)
         barrier()
@@ -439,20 +439,23 @@ def run_ours(args, w, rank, world, local_rank):
         clocks = sampler.stop() if sampler else None
         ms_per_step = max_over_ranks(ms) / steps
         return dict(ms_per_step=ms_per_step, launches=launches, clocks=clocks, frames=wl["clips"] * T, host=host,
-                    dev=dev, step_e2e=step_e2e)
+                    dev=dev, step_e2e=step_e2e, last=last)
 
     def roofline_of(wl, ms_per_step, name):
         alg_bytes = algorithmic_bytes_per_step(wl)
         achieved = alg_bytes / (ms_per_step * 1e-3) / 1e9
         return {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                "traffic": profiled_traffic(name), "peak_source": peak_src, "algorithmic_bytes_per_launch": alg_bytes,
+                "peak_source": peak_src, "algorithmic_bytes_per_launch": alg_bytes,
                 "kernel": "mr_kernel<2> (mixed radix 5,5,8)" if name == "speech400" else KERNEL_NAMES[wl["op"]],
                 "note": "kernel time == step time (CUDA events on the launching stream); bytes = inputs read once + outputs written once"}
 
-    # ---- device-resident: warm-up, then K steps between events (inputs 0.9 GB >> 126 MB L2: no flush needed)
-    r = resident(w, args.steps, args.warmup, True)
+    # ---- device-resident: warm-up, then K steps between events (inputs 0.9 GB >> 50 MB L2: no flush needed)
+    r = resident(w, args.steps, args.warmup, True, keep_last=bool(args.dump_outputs))
     ms_per_step, launches, clocks, frames_per_step = r["ms_per_step"], r["launches"], r["clocks"], r["frames"]
     host, dev, step_e2e = r["host"], r["dev"], r["step_e2e"]
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, args.workload, w, r["last"], rank)
+        r["last"].free()
     value = world * frames_per_step / (ms_per_step * 1e-3)
 
     # ---- end to end through the public call with host buffers (H2D + D2H inside the timed region)
@@ -584,7 +587,7 @@ def run_ours(args, w, rank, world, local_rank):
         "config": {"workload": w["desc"], "name": args.workload, "per_gpu_clips": w["clips"],
                    "frames_per_step_per_gpu": frames_per_step, "parallelism": f"clips sharded x{world}, no collective",
                    "host_cpus_bound_to_gpu": len(numa_cpus) if numa_cpus else None,
-                   "l2": "inputs (%.0f MB per step) exceed the 126 MB L2; no flush" % (w["clips"] * w["n"] * 4 / 1e6)},
+                   "l2": "inputs (%.0f MB per step) exceed the 50 MB L2; no flush" % (w["clips"] * w["n"] * 4 / 1e6)},
         "clocks": clocks, "gpu_launches": launches,
         "e2e": {"value": e2e_value, "unit": "frames/s", "h2d_bytes_per_step": h2d_bytes,
                 "d2h_bytes_per_step": d2h, "ms_per_step": e2e_s * 1e3,
@@ -599,6 +602,29 @@ def run_ours(args, w, rank, world, local_rank):
     if dist is not None:
         dist.barrier()
         dist.destroy_process_group()
+
+
+DUMP_LIMIT_BYTES = 64 * 10**6
+
+
+def dump_outputs(out_dir, name, w, out, rank):
+    """out_dir/<workload>.npy: the clips at seeded indices (out_dir/<workload>_clips.npy) that fit in
+    DUMP_LIMIT_BYTES, as float32; complex spectra get a trailing (re, im) axis."""
+    from librosa_b200 import _native as nat
+
+    clips = out.shape[0]
+    per_clip = out.nbytes // clips                 # every result is clip-major: one contiguous block per clip
+    k = max(1, min(clips, DUMP_LIMIT_BYTES // per_clip - 1))   # - 1: room for the index file
+    idx = np.sort(np.random.default_rng(0).choice(clips, size=k, replace=False))
+    rows = [np.ascontiguousarray(nat.DeviceArray(out.ctx, out.ptr + int(c) * per_clip, out.shape[1:], out.dtype,
+                                                 layout=out.layout, owner=False).get()) for c in idx]
+    data = np.stack(rows)
+    if np.iscomplexobj(data):
+        data = np.stack([data.real, data.imag], axis=-1)
+    os.makedirs(out_dir, exist_ok=True)
+    suffix = "" if rank == 0 else f"_rank{rank}"
+    np.save(os.path.join(out_dir, f"{name}{suffix}.npy"), data.astype(np.float32, copy=False))
+    np.save(os.path.join(out_dir, f"{name}{suffix}_clips.npy"), idx.astype(np.float64))
 
 
 _REAL_STDOUT = None
@@ -629,7 +655,11 @@ def main():
     ap.add_argument("--no-cpu", action="store_true", help="skip the cpu_baseline leg")
     ap.add_argument("--no-secondary", action="store_true", help="skip the cfg3 / cfg4 / cfg5 / speech400 secondary numbers")
     ap.add_argument("--no-join", action="store_true", help="skip the NCCL scatter -> mel -> gather leg (N > 1)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's result (a fixed, seeded sample of clips) as DIR/<workload>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))

@@ -1,4 +1,4 @@
-/* b2l.h — C ABI of libb2l.so, the B200 (sm_100a) replacement for librosa's FFT time-frequency path.
+/* b2l.h — C ABI of libb2l.so, the H100 (sm_90a) replacement for librosa's FFT time-frequency path.
  *
  * librosa has no FFI: its boundary for this path is the public Python API.  The Python package
  * `librosa_b200` mirrors those signatures and makes one call into this library per public function;
@@ -11,7 +11,7 @@
  *   - plain pointers and sizes only; device pointers are marked d_, host pointers h_;
  *   - all work is enqueued on the context's stream; b2l_ctx_sync() waits for it;
  *   - a context is bound to one CUDA device and is not thread-safe; use one context per thread / GPU;
- *   - there is no CPU fallback: without a usable sm_100 device b2l_ctx_create fails.
+ *   - there is no CPU fallback: without a usable sm_90 device b2l_ctx_create fails.
  */
 #ifndef B2L_H_
 #define B2L_H_

@@ -1,4 +1,4 @@
-"""librosa_b200 — B200 (sm_100a) implementation of librosa's FFT time-frequency hot path.
+"""librosa_b200 — H100 (sm_90a) implementation of librosa's FFT time-frequency hot path.
 
 Drop-in for this path only: ``import librosa_b200 as librosa`` gives ``stft``, ``istft``,
 ``power_to_db``, ``feature.melspectrogram``, ``feature.mfcc``, ``filters.mel / get_window /

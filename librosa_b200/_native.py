@@ -1,7 +1,7 @@
 """ctypes binding of ``libb2l.so`` (C ABI declared in ``include/b2l.h``).
 
 No PyTorch, no CuPy: device memory, streams and launches all live behind the C ABI.  There is no
-CPU fallback — if the shared library is missing or no sm_100 GPU is present, every entry point raises.
+CPU fallback — if the shared library is missing or no sm_90 GPU is present, every entry point raises.
 """
 from __future__ import annotations
 
@@ -32,7 +32,7 @@ class NativeLibraryError(RuntimeError):
 
 
 class UnsupportedOnGPU(NotImplementedError):
-    """Valid for librosa but not built for the sm_100a path yet (never a silent CPU fallback)."""
+    """Valid for librosa but not built for the sm_90a path yet (never a silent CPU fallback)."""
 
 
 class PlanDesc(C.Structure):
@@ -275,8 +275,8 @@ class Context:
         self._sizes = {}
         self._pooled_bytes = 0
         # cached (released but not returned to the driver) device memory: blocks are exact-size, so variable-length
-        # workloads reuse little — keep the cache well below the 180 GB of the device
-        self.pool_limit_bytes = int(os.environ.get("B2L_POOL_LIMIT_MB", "32768")) << 20
+        # workloads reuse little — keep the cache well below the 80 GB of the device
+        self.pool_limit_bytes = int(os.environ.get("B2L_POOL_LIMIT_MB", "16384")) << 20
         self._finalizer = weakref.finalize(self, Context._destroy, self._h, self._plans, self._wss, self._sizes)
 
     @staticmethod

@@ -59,7 +59,7 @@ def check_real_dtype(dtype, what: str, native_ok: bool = False) -> np.dtype:
             return dtype
         if float64_policy() == "error":
             raise nat.UnsupportedOnGPU(
-                f"{what}: dtype {dtype} is not supported by the float32 sm_100a kernels and B2L_FLOAT64=error "
+                f"{what}: dtype {dtype} is not supported by the float32 sm_90a kernels and B2L_FLOAT64=error "
                 "(there is no CPU fallback)")
         _note_float64(what)
         return dtype
@@ -206,7 +206,7 @@ def require_supported_n_fft(n_fft: int, inverse: bool = False):
         if MIN_N_FFT <= n_fft <= MAX_N_FFT:
             return
         raise nat.UnsupportedOnGPU(
-            f"n_fft={n_fft}: the sm_100a kernels are built for powers of two from {MIN_N_FFT} to {MAX_N_FFT} "
+            f"n_fft={n_fft}: the sm_90a kernels are built for powers of two from {MIN_N_FFT} to {MAX_N_FFT} "
             "(no CPU fallback)")
     if not (3 <= n_fft <= MAX_CZT_N_FFT) and not mr_covers(n_fft):
         raise nat.UnsupportedOnGPU(f"n_fft={n_fft}: non-power-of-two sizes are supported from 3 to {MAX_CZT_N_FFT}, and "

@@ -1,5 +1,5 @@
 """``stft`` / ``istft`` / ``_spectrogram`` / ``power_to_db`` with librosa's signatures, executed by
-libb2l.so on a B200 (reference: librosa/core/spectrum.py:58-391, 395-626, 2920-3015, 1735-1883).
+libb2l.so on an H100 (reference: librosa/core/spectrum.py:58-391, 395-626, 2920-3015, 1735-1883).
 
 Inputs may be NumPy arrays (results come back as NumPy arrays with librosa's shapes and dtypes) or
 ``DeviceArray`` objects (results stay on the device, so ``stft -> istft`` or ``melspectrogram`` chains

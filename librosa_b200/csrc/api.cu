@@ -216,8 +216,8 @@ extern "C" int b2l_ctx_create(int device, b2l_ctx** out) {
   if (device < 0 || device >= n) return fail(B2L_ERR_INVALID, "device %d out of range (have %d)", device, n);
   cudaDeviceProp prop;
   CUDA_TRY(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10)
-    return fail(B2L_ERR_UNSUPPORTED, "device %d is sm_%d%d; libb2l is built for sm_100a only (no fallback path)",
+  if (prop.major != 9 || prop.minor != 0)
+    return fail(B2L_ERR_UNSUPPORTED, "device %d is sm_%d%d; libb2l is built for sm_90a only (no fallback path)",
                 device, prop.major, prop.minor);
   DeviceGuard g(device);
   b2l_ctx* c = new b2l_ctx();
@@ -580,7 +580,7 @@ extern "C" int b2l_plan_create(b2l_ctx* c, const b2l_plan_desc* d, b2l_plan** ou
                   "has no prime factor above 5 (no CPU fallback)", d->n_fft);
   } else if (l2n - 1 < kMinLog2M || l2n - 1 > kMaxLog2M) {
     return fail(B2L_ERR_UNSUPPORTED,
-                "n_fft=%d: the sm_100a kernels are built for powers of two from %d to %d (no CPU fallback)",
+                "n_fft=%d: the sm_90a kernels are built for powers of two from %d to %d (no CPU fallback)",
                 d->n_fft, 2 << kMinLog2M, 2 << kMaxLog2M);
   }
   if (!d->h_window) return fail(B2L_ERR_INVALID, "window is NULL");
@@ -896,14 +896,8 @@ static int get_row_table(b2l_ctx* c, const b2l_plan* p, int H, int hw, const b2l
 
 // Kernel variants tried in order (first that fits shared memory wins): 116 = 16 warps as two independent
 // 8-warp halves, 16 / 8 = plain CTAs.  B2L_FWD_VARIANT forces one (A/B measurements).
-#ifndef B2L_MEL2_DEFAULT
-#define B2L_MEL2_DEFAULT false
-#endif
 #ifndef B2L_DCT_FPL_DEFAULT
 #define B2L_DCT_FPL_DEFAULT 4
-#endif
-#ifndef B2L_TMEM_DEFAULT
-#define B2L_TMEM_DEFAULT true
 #endif
 static int fwd_variants(const HostFftCfg& cfg, int out[6]) {
   int n = 0;
@@ -912,14 +906,7 @@ static int fwd_variants(const HostFftCfg& cfg, int out[6]) {
     out[n++] = atoi(force);
     return n;
   }
-  // + 1000: window / twiddle tables in Tensor Memory (B2L_TMEM=0 keeps them in shared memory)
-  const char* tm_env = getenv("B2L_TMEM");
-  const bool tm = tm_env && *tm_env ? atoi(tm_env) != 0 : B2L_TMEM_DEFAULT;
-  if (cfg.log2m >= 9 && cfg.log2m <= 11) {
-    if (tm) out[n++] = 1116;
-    out[n++] = 116;
-  }
-  if (tm && cfg.log2m == 12) out[n++] = 1016;
+  if (cfg.log2m >= 9 && cfg.log2m <= 11) out[n++] = 116;
   int nws[2];
   const int k = cfg.nw_options(nws);
   for (int i = 0; i < k; ++i) out[n++] = nws[i];
@@ -950,77 +937,13 @@ static int run_forward(b2l_ctx* c, const b2l_plan* p, int mode, int log_mode, co
   const int n_opt = fwd_variants(cfg, variants);
   FwdArgs a;
   memset(&a, 0, sizeof(a));
-  // melspectrogram, n_fft = 2048, hop = n_fft / 4, no dB epilogue: autonomous frame groups (mel2_kernel.cuh);
-  // B2L_MEL2=0 keeps fwd_kernel
-  {
-    const char* e2 = getenv("B2L_MEL2");
-    const bool forced = getenv("B2L_FWD_VARIANT") && *getenv("B2L_FWD_VARIANT");
-    if (mode == MODE_MEL && !log_mode && p->log2m == 10 && 4 * p->hop == N && !forced &&
-        (e2 && *e2 ? atoi(e2) != 0 : B2L_MEL2_DEFAULT)) {
-      const b2l_plan::RowTable* t = nullptr;
-      int rc = get_row_table(c, p, mel_rows_per_warp(8), 8, &t);
-      if (rc) return rc;
-      const int PRS = ((M + 4 + 31) / 32) * 32 + 8;
-      size_t off = 0;
-      a.off_bar = (int)off; off = align_up(off + 64, 128);
-      a.off_win = (int)off; off = align_up(off + 2 * 8 * sizeof(long long), 128);       // per-row output offsets
-      a.off_melw = (int)off; off = align_up(off + (size_t)t->w_count * 4, 16);
-      a.off_melband = (int)off; off = align_up(off + (size_t)t->n_rows * sizeof(MelRow), 16);
-      a.off_melorder = (int)off; off = align_up(off + (size_t)std::max(1, t->list_len) * 8 * 2, 128);
-      a.off_in = (int)off; off = align_up(off + (size_t)2 * 8 * PRS * 4, 128);           // power tiles of the two halves
-      a.off_xbuf = (int)off; off += (size_t)16 * cfg.xbuf_f2() * 8;
-      if (off <= c->smem_optin) {
-        a.y = d_y;
-        a.clip_stride = y_stride;
-        a.n = (int)n;
-        a.n_clips = (int)n_clips;
-        a.n_fft = N;
-        a.hop = p->hop;
-        a.pad = p->center ? N / 2 : 0;
-        a.pad_mode = p->pad_mode;
-        a.n_frames = (int)T;
-        a.tma_ok = (((uintptr_t)d_y & 7) == 0) && (y_stride % 2 == 0) && (a.pad % 2 == 0);   // 8-byte sample loads
-        a.window = p->d_win_fwd;
-        a.tw = p->d_tw;
-        a.twn = p->d_twn;
-        a.out_r = out_r;
-        a.power_mode = p->power_mode;
-        a.power = p->power;
-        a.n_mels = p->n_mels;
-        a.mel_w_count = t->w_count;
-        a.mel_w = t->d_w;
-        a.mel_rows = t->d_rows;
-        a.n_mel_rows = t->n_rows;
-        a.mel_order = t->d_order;
-        a.mel_list_len = t->list_len;
-        a.status = c->d_status;
-        const long long total_frames = (long long)n_clips * T;
-        long long grid = c->sm_count;
-        if (grid * 16 > total_frames) grid = (total_frames + 15) / 16;
-        const long long fpg = (total_frames + grid * 16 - 1) / (grid * 16);
-        if (fpg <= 0x7fffffffLL) {
-          a.tiles_per_clip = (int)fpg;                     // steps: frames per frame group
-          const unsigned long long kkey = (7ULL << 60);
-          if (c->launch_cache.find(kkey) == c->launch_cache.end()) {
-            CUDA_TRY(op(OP_SET_SMEM, 3016, mode, &a, 0, c->smem_optin, c->stream, nullptr));
-            c->launch_cache[kkey] = 1;
-          }
-          CUDA_TRY(op(OP_LAUNCH, 3016, mode, &a, (int)grid, off, c->stream, nullptr));
-          c->launches++;
-          return B2L_OK;
-        }
-      }
-      memset(&a, 0, sizeof(a));
-    }
-  }
   int variant = 0, ft = 0, halves = 1;
   size_t smem = 0;
   const b2l_plan::RowTable* rt = nullptr;
   for (int i = 0; i < n_opt && !variant; ++i) {
     const int v = variants[i];
-    const bool tmem = v >= 1000;
-    const int nh = (v % 1000) == 116 ? 2 : 1;
-    const int nw = nh > 1 ? 16 : v % 1000;
+    const int nh = v == 116 ? 2 : 1;
+    const int nw = nh > 1 ? 16 : v;
     if (nw * 32 % (cfg.tpf * nh) != 0) continue;
     const int f = nw * 32 / nh / cfg.tpf;
     if (f < 1 || f > 32) continue;
@@ -1032,9 +955,9 @@ static int run_forward(b2l_ctx* c, const b2l_plan* p, int mode, int log_mode, co
       if (rc) return rc;
     }
     size_t off = 0;
-    a.off_win = (int)off; if (!tmem) off = align_up(off + (size_t)N * 4, 16);       // TMEM variants keep these
-    a.off_tw = (int)off; if (!tmem) off = align_up(off + (size_t)cfg.tw_count() * 8, 16);   // tables off shared memory
-    a.off_bar = (int)off; off = align_up(off + 64, 16);   // "tile landed" mbarrier per half, TMEM base address, "staging consumed" mbarriers
+    a.off_win = (int)off; off = align_up(off + (size_t)N * 4, 16);
+    a.off_tw = (int)off; off = align_up(off + (size_t)cfg.tw_count() * 8, 16);
+    a.off_bar = (int)off; off = align_up(off + 64, 16);   // "tile landed" mbarrier per half, "staging consumed" mbarriers
     if (t) {
       a.off_melw = (int)off; off = align_up(off + (size_t)t->w_count * 4, 16);
       a.off_melband = (int)off; off = align_up(off + (size_t)t->n_rows * sizeof(MelRow), 16);
@@ -1667,52 +1590,6 @@ extern "C" int b2l_istft(b2l_ctx* c, const b2l_plan* p, const void* d_D, int64_t
   }
   InvArgs a;
   memset(&a, 0, sizeof(a));
-  // hop = n_fft / 4 or / 2, one or more whole warps per frame: autonomous frame groups with the overlap-add
-  // state in Tensor Memory (inv2_kernel.cuh); B2L_INV2=0 keeps the gather kernel
-  {
-    const char* e2 = getenv("B2L_INV2");
-    const bool want2 = !(e2 && *e2 && atoi(e2) == 0) && !(getenv("B2L_INV_VARIANT") && *getenv("B2L_INV_VARIANT"));
-    const int R = p->hop > 0 && N % p->hop == 0 ? N / p->hop : 0;
-    if (want2 && cfg.log2m >= 10 && cfg.log2m <= 12 && (R == 4 || R == 2)) {
-      const int NG = 16 * 32 / cfg.tpf;
-      size_t off = 0;
-      a.off_acc = (int)off; off = align_up(off + 16, 128);            // TMEM base address
-      a.off_xbuf = (int)off; off += (size_t)NG * cfg.xbuf_f2() * 8;
-      if (off <= c->smem_optin) {
-        a.D = (const float2*)d_D;
-        a.d_clip_stride = (long long)n_frames_stored * (M + 1);
-        a.n_clips = (int)n_clips;
-        a.n_frames = (int)n_frames_used;
-        a.n_fft = N;
-        a.hop = p->hop;
-        a.start = p->center ? N / 2 : 0;
-        a.out_len = (int)out_len;
-        a.y_clip_stride = y_stride;
-        a.y = d_y;
-        a.window = p->d_win_inv;
-        a.inv_wss = d_inv_wss;
-        a.tw = p->d_tw;
-        a.twn = p->d_twn;
-        a.vec4 = (y_stride % 2 == 0) && (((uintptr_t)d_y & 7) == 0) && (((uintptr_t)d_inv_wss & 7) == 0);   // 8-byte stores
-        const long long total_frames = (long long)n_clips * n_frames_used;
-        const long long groups = (long long)c->sm_count * NG;
-        long long fps = (total_frames + groups - 1) / groups;
-        if (fps < 8) fps = 8;                                          // replayed frames stay a bounded fraction
-        a.frames_per_slot = (int)fps;
-        {
-          const char* ea = getenv("B2L_INV2_AHEAD");           // spectrum rows prefetched to L2 ahead of the transform
-          a.acc_floats = ea && *ea ? std::max(1, std::min(4, atoi(ea))) : 1;
-        }
-        const long long runs = (total_frames + fps - 1) / fps;
-        const long long grid = (runs + NG - 1) / NG;
-        const int v2 = 2000 + R;
-        CUDA_TRY(op(OP_SET_SMEM, v2, &a, 0, off, c->stream, nullptr));
-        CUDA_TRY(op(OP_LAUNCH, v2, &a, (int)grid, off, c->stream, nullptr));
-        c->launches++;
-        return B2L_OK;
-      }
-    }
-  }
   int variant = 0, G = 0, halves = 1;
   size_t smem = 0;
   const int clen = N > p->hop ? N - p->hop : 0;

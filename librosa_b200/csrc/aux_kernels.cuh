@@ -2,7 +2,7 @@
 // power_to_db for S= inputs, and a batched transpose used as a layout adapter.
 #pragma once
 #include "common.cuh"
-#include "fft_engine.cuh"   // packed FP32 helpers (fma2, bc2)
+#include "fft_engine.cuh"   // float2 helpers (fma2, bc2)
 
 namespace b2l {
 
@@ -130,8 +130,8 @@ __global__ void dct_clamp_kernel(const float* __restrict__ L, const float* __res
 // 16-byte load of four DCT coefficients costs four wavefronts, so a mel row costs 8 + FPL wavefronts per warp
 // for 8 * FPL FMAs (0.625 per FMA at FPL = 2).  Here a tile is 128 frames (two 64-frame blocks of the tiled
 // scratch, contiguous in memory), lane l owns frames 4l .. 4l+3 — one 16-byte load per mel row — and the 32
-// accumulators of a lane are 16 register pairs fed by packed FMAs (coefficient broadcast, frame pair): 12
-// wavefronts and 16 FFMA2 per mel row and warp, 0.375 wavefronts per FMA.  One tile buffer per block; two blocks
+// accumulators of a lane are 16 register pairs fed by FMAs (coefficient broadcast, frame pair): 12
+// wavefronts and 32 FFMA per mel row and warp, 0.375 wavefronts per FMA.  One tile buffer per block; two blocks
 // per SM alternate between streaming and multiplying (cp.async), which is what the double buffer did before.
 // KS = 2: two warp sets split the mel rows of a tile and add their partial sums through the (then idle) tile
 // buffer — twice the warps per SM (20 for 40 coefficients, five per scheduler) for one more barrier per tile.

@@ -1,4 +1,4 @@
-// common.cuh — shared declarations for the b2l kernels (sm_100a only).
+// common.cuh — shared declarations for the b2l kernels (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

@@ -4,7 +4,7 @@
 //
 // This is the correctness path for float64 callers, not the throughput path: one CTA per frame, the transform in
 // shared memory (in-place radix-2 for powers of two, a direct O(n_fft^2) DFT with an exact twiddle table for any
-// other length), FP64 arithmetic throughout.  The float32 kernels (fwd_kernel / inv_kernel / inv2_kernel) remain
+// other length), FP64 arithmetic throughout.  The float32 kernels (fwd_kernel / inv_kernel) remain
 // the product's hot path; these kernels make `stft(float64)` mean float64 instead of a relabelled float32 result.
 #pragma once
 #include <cuda_runtime.h>

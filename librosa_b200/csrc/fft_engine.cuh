@@ -1,4 +1,4 @@
-// fft_engine.cuh — register-resident Stockham complex FFT for sm_100a.
+// fft_engine.cuh — register-resident Stockham complex FFT for sm_90a.
 //
 // One "frame group" of TPF threads transforms M = 2^LOG2M complex points; every thread keeps
 // PPT = M / TPF points (32 for all production sizes) in registers.  Each pass is a radix-R DFT done
@@ -76,42 +76,24 @@ struct TwC {   // W_N^J = exp(-2*pi*i*J/N)
 };
 
 // ------------------------------------------------------------------ complex helpers
-// Packed FP32 (sm_100: FADD2 / FMUL2 / FFMA2 work on an aligned register pair, take a scalar or an immediate
-// broadcast to both halves, and swap / negate halves with operand modifiers).  A complex value (re, im) is one
-// such pair, so every butterfly below costs half the issue slots of its scalar form at the same FP32 lane rate
-// (tools/micro/ffma2_rate.cu: 0.49 warp-instructions per clock and sub-partition, 125 lanes per clock and SM,
-// against 0.90-0.96 and 116-123 for FFMA / FADD / FMUL).  The operation order inside every component is the
-// scalar one, so the results are bit-identical.  B2L_PACKED=0 builds the scalar forms (A/B only).
-#ifndef B2L_PACKED
-#define B2L_PACKED 1
-#endif
+// Component-wise FP32 operations on a complex value (re, im).  Every butterfly below is written with them, so the
+// operation order inside each component is fixed by the source (FFMA / FADD / FMUL per component on sm_90).
 __device__ __forceinline__ float2 bc2(float a) { return make_float2(a, a); }
 __device__ __forceinline__ float2 neg2(float2 a) { return make_float2(-a.x, -a.y); }
 __device__ __forceinline__ float2 muli2(float2 a) { return make_float2(-a.y, a.x); }    //  i * a
 __device__ __forceinline__ float2 mulni2(float2 a) { return make_float2(a.y, -a.x); }   // -i * a
-#if B2L_PACKED
-__device__ __forceinline__ float2 add2(float2 a, float2 b) { return __fadd2_rn(a, b); }
-__device__ __forceinline__ float2 sub2(float2 a, float2 b) { return __fadd2_rn(a, neg2(b)); }
-__device__ __forceinline__ float2 mul2(float2 a, float2 b) { return __fmul2_rn(a, b); }
-__device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) { return __ffma2_rn(a, b, c); }
-#else
 __device__ __forceinline__ float2 add2(float2 a, float2 b) { return make_float2(a.x + b.x, a.y + b.y); }
 __device__ __forceinline__ float2 sub2(float2 a, float2 b) { return make_float2(a.x - b.x, a.y - b.y); }
 __device__ __forceinline__ float2 mul2(float2 a, float2 b) { return make_float2(a.x * b.x, a.y * b.y); }
 __device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) {
   return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y));
 }
-#endif
 
-// a * b = b.x * a + b.y * (i a).  Operand order matters to ptxas: the swapped / half-negated pair must be the FIRST
-// operand of the FFMA2 and the broadcast scalar the second (FFMA2 Rd, -Ra.LO_HI.NP, Rb.F32, Rc); the other way
-// round it builds the pair with a MOV and an FADD.
+// a * b = b.x * a + b.y * (i a)
 __device__ __forceinline__ float2 cmul(float2 a, float2 b) {
   return fma2(muli2(a), bc2(b.y), mul2(a, bc2(b.x)));
 }
-// Shared-memory store of a complex value.  ptxas copies the result pair of a packed instruction (two MOVs, half
-// of them IMAD.MOVs on the FMA pipe) in front of an ordinary 64-bit store; it does not for a v2.f32 store written
-// in PTX (nor for 32-bit or 128-bit stores).  saddr: 32-bit shared-window address.
+// Shared-memory store of a complex value as one v2.f32 store written in PTX.  saddr: 32-bit shared-window address.
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
 __device__ __forceinline__ void sts_c64(uint32_t saddr, float2 v) {
   // no "memory" clobber: the statement stays ordered against the barriers (volatile asm, and they do clobber), and
@@ -119,7 +101,7 @@ __device__ __forceinline__ void sts_c64(uint32_t saddr, float2 v) {
   asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(saddr), "f"(v.x), "f"(v.y));
 }
 // Predicated global store of a complex value: one @p STG.64, never a branch (a branch per bin pair serialises the
-// un-mix loop: ptxas stops interleaving the pairs), and no pair copy after a packed instruction.
+// un-mix loop: ptxas stops interleaving the pairs).
 __device__ __forceinline__ void stg_c64_if(float2* p, float2 v, bool ok) {
   asm volatile(
       "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %3, 0;\n\t@p st.global.v2.f32 [%0], {%1, %2};\n\t}" ::"l"(p), "f"(v.x), "f"(v.y),
@@ -264,19 +246,10 @@ __host__ __device__ constexpr int pass0_slot_of_pair(int c) {
   return -1;
 }
 
-// ------------------------------------------------------------------ constant tables: shared memory or TMEM
+// ------------------------------------------------------------------ constant tables in shared memory
 // The window and the inter-pass twiddles are per-thread constants (thread t of a frame group always touches
-// the same elements), read once per frame: 2 x 8 KB per frame for n_fft = 2048, a fifth of the kernel's
-// shared-memory wavefronts.  Two sources with the same interface:
-//   SmemTab  tables staged in shared memory (any size)
-//   TmemTab  tables parked in Tensor Memory, one 32-bit column per value and thread (PPT == 32 only):
-//            lane = thread of the warp, read back 16 columns at a time with tcgen05.ld — a datapath that
-//            does not go through the shared-memory pipe.  Column map (NCOLS = 64 * NPASS):
-//              [0, 64)                   window pair of pass-0 slot s at columns 2s, 2s+1
-//              [64*s, 64*s + 64), s>=1   twiddle of flattened operand f = b*R_s + r of pass s at 2f, 2f+1
-//                                        (r == 0 entries are (1, 0) and never fetched)
-//              [64*NPASS, +32)           un-mix twiddle W_N^(t + TPF*c) of bin pair c at 2c, 2c+1
-// Protocol (both): begin_window() ... window<SLOT>(t) for SLOT = 0 .. PPT-1 in increasing order;
+// the same elements), read once per frame from tables staged in shared memory.
+// Protocol: begin_window() ... window<SLOT>(t) for SLOT = 0 .. PPT-1 in increasing order;
 // begin_pass<S>() ... step<S, F>() for every F = 0 .. PPT-1 in increasing order, twiddle<S, F>(i) after the
 // step of the same F when r > 0.
 template <class Cfg>
@@ -303,60 +276,6 @@ struct SmemTab {
   __device__ __forceinline__ float2 unmix(float2 wt) {
     if constexpr (C == 0) return wt;
     else return cmul(wt, make_float2(TwC<C, 2 * Cfg::PPT>::re, TwC<C, 2 * Cfg::PPT>::im));
-  }
-};
-
-template <class Cfg>
-struct TmemTab {
-  static constexpr int UNMIX_COL = 64 * Cfg::NPASS;
-  static constexpr int NCOLS = UNMIX_COL + Cfg::PPT;
-  uint32_t taddr;          // TMEM address of column 0 in this warp's lane quarter
-  uint32_t q[16];          // chunk in flight (16 columns = 8 slots / 8 twiddles)
-  float c[16];             // chunk being consumed
-  template <int COL>
-  __device__ __forceinline__ void issue() {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(q[0]), "=r"(q[1]), "=r"(q[2]), "=r"(q[3]), "=r"(q[4]), "=r"(q[5]), "=r"(q[6]), "=r"(q[7]), "=r"(q[8]),
-          "=r"(q[9]), "=r"(q[10]), "=r"(q[11]), "=r"(q[12]), "=r"(q[13]), "=r"(q[14]), "=r"(q[15])
-        : "r"(taddr + COL));
-  }
-  // wait for the chunk in flight (the registers are in-out operands so that no use can move above the wait)
-  __device__ __forceinline__ void arrive() {
-    asm volatile("tcgen05.wait::ld.sync.aligned;"
-                 : "+r"(q[0]), "+r"(q[1]), "+r"(q[2]), "+r"(q[3]), "+r"(q[4]), "+r"(q[5]), "+r"(q[6]), "+r"(q[7]),
-                   "+r"(q[8]), "+r"(q[9]), "+r"(q[10]), "+r"(q[11]), "+r"(q[12]), "+r"(q[13]), "+r"(q[14]), "+r"(q[15])
-                 :
-                 : "memory");
-#pragma unroll
-    for (int i = 0; i < 16; ++i) c[i] = __uint_as_float(q[i]);
-  }
-  template <int BASE, int F, int COUNT = Cfg::PPT>
-  __device__ __forceinline__ void advance() {   // called for every F in order: chunk hand-over every 8 entries
-    if constexpr (F % 8 == 0) {
-      arrive();
-      if constexpr (F + 8 < COUNT) issue<BASE + 2 * (F + 8)>();
-    }
-  }
-  __device__ __forceinline__ void begin_window() { issue<0>(); }
-  template <int SLOT>
-  __device__ __forceinline__ float2 window(int) {
-    advance<0, SLOT>();
-    return make_float2(c[2 * (SLOT % 8)], c[2 * (SLOT % 8) + 1]);
-  }
-  template <int S>
-  __device__ __forceinline__ void begin_pass() { issue<64 * S>(); }
-  template <int S, int F>
-  __device__ __forceinline__ void step() { advance<64 * S, F>(); }
-  template <int S, int F>
-  __device__ __forceinline__ float2 twiddle(int) {
-    return make_float2(c[2 * (F % 8)], c[2 * (F % 8) + 1]);
-  }
-  __device__ __forceinline__ void begin_unmix() { issue<UNMIX_COL>(); }
-  template <int C>
-  __device__ __forceinline__ float2 unmix(float2) {   // bin pairs in increasing order, each exactly once
-    advance<UNMIX_COL, C, Cfg::PPT / 2>();
-    return make_float2(c[2 * (C % 8)], c[2 * (C % 8) + 1]);
   }
 };
 
@@ -440,7 +359,7 @@ __device__ __forceinline__ void fft_forward_tab(float2 (&v)[Cfg::PPT], int t, in
           });
         });
       }
-      tab.template begin_pass<s + 1>();   // TMEM: the first twiddle chunk travels while the group synchronises
+      tab.template begin_pass<s + 1>();
       group_sync<TPF>(barrier_id);
     }
   });

@@ -1,6 +1,5 @@
 // fwd_inst.cu — instantiates fwd_kernel for one transform size (compile with -DB2L_LOG2M=k).
 #include "fwd_kernel.cuh"
-#include "mel2_kernel.cuh"
 #include "internal.h"
 
 #ifndef B2L_LOG2M
@@ -18,13 +17,13 @@ cudaError_t run_op(K kern, int op, int nt, const FwdArgs* a, int grid, size_t sm
   return cudaGetLastError();
 }
 
-template <int L, int TPF, int NW, int DUAL, bool TM = false>
+template <int L, int TPF, int NW, int DUAL>
 cudaError_t by_mode(int op, int mode, const FwdArgs* a, int grid, size_t smem, cudaStream_t st, int* result) {
   switch (mode) {
-    case MODE_STFT: return run_op(fwd_kernel<L, TPF, NW, MODE_STFT, DUAL, TM>, op, NW * 32, a, grid, smem, st, result);
-    case MODE_MEL: return run_op(fwd_kernel<L, TPF, NW, MODE_MEL, DUAL, TM>, op, NW * 32, a, grid, smem, st, result);
-    case MODE_SPEC: return run_op(fwd_kernel<L, TPF, NW, MODE_SPEC, DUAL, TM>, op, NW * 32, a, grid, smem, st, result);
-    case MODE_STATS: return run_op(fwd_kernel<L, TPF, NW, MODE_STATS, DUAL, TM>, op, NW * 32, a, grid, smem, st, result);
+    case MODE_STFT: return run_op(fwd_kernel<L, TPF, NW, MODE_STFT, DUAL>, op, NW * 32, a, grid, smem, st, result);
+    case MODE_MEL: return run_op(fwd_kernel<L, TPF, NW, MODE_MEL, DUAL>, op, NW * 32, a, grid, smem, st, result);
+    case MODE_SPEC: return run_op(fwd_kernel<L, TPF, NW, MODE_SPEC, DUAL>, op, NW * 32, a, grid, smem, st, result);
+    case MODE_STATS: return run_op(fwd_kernel<L, TPF, NW, MODE_STATS, DUAL>, op, NW * 32, a, grid, smem, st, result);
   }
   return cudaErrorInvalidValue;
 }
@@ -34,30 +33,21 @@ cudaError_t by_mode(int op, int mode, const FwdArgs* a, int grid, size_t smem, c
 #define B2L_CAT2(a, b) a##b
 #define B2L_CAT(a, b) B2L_CAT2(a, b)
 
-// `nw` selects the variant: 16 or 8 warps; 116 = 16 warps as two independent 8-warp halves (NSPLIT = 2);
-// + 1000 = the same with the window / twiddle tables in Tensor Memory (TM).
+// `nw` selects the variant: 16 or 8 warps; 116 = 16 warps as two independent 8-warp halves (NSPLIT = 2).
 template <int L>
 cudaError_t fwd_dispatch(int op, int nw, int mode, const FwdArgs* a, int grid, size_t smem, cudaStream_t st,
                          int* result) {
   constexpr int M = 1 << L;
   constexpr int TPF = M >= 32 ? M / 32 : 1;
-  if constexpr (L == 10) {
-    if (nw == 3016) return run_op(mel2_kernel<L>, op, 512, a, grid, smem, st, result);   // autonomous frame groups
-  }
   if constexpr (L >= 10) {
     if (nw == 16) return by_mode<L, TPF, 16, 1>(op, mode, a, grid, smem, st, result);
     if (nw == 8) return by_mode<L, TPF, 8, 1>(op, mode, a, grid, smem, st, result);
     if (nw == 116) return by_mode<L, TPF, 16, 2>(op, mode, a, grid, smem, st, result);
-    if (nw == 1016) return by_mode<L, TPF, 16, 1, true>(op, mode, a, grid, smem, st, result);
-    if constexpr (L <= 11) {
-      if (nw == 1116) return by_mode<L, TPF, 16, 2, true>(op, mode, a, grid, smem, st, result);
-    }
   } else {
     constexpr int NW = TPF > 16 ? 16 : TPF;
     if (nw == NW) return by_mode<L, TPF, NW, 1>(op, mode, a, grid, smem, st, result);
     if constexpr (L == 9) {
       if (nw == 116) return by_mode<L, TPF, 16, 2>(op, mode, a, grid, smem, st, result);
-      if (nw == 1116) return by_mode<L, TPF, 16, 2, true>(op, mode, a, grid, smem, st, result);
     }
   }
   return cudaErrorInvalidValue;

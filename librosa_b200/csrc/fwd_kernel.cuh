@@ -70,28 +70,6 @@ __device__ __forceinline__ void tma_load_1d(void* dst_smem, const void* src_gmem
       : "memory");
 }
 
-// ------------------------------------------------------------------ Tensor Memory as a per-thread constant store
-// (tcgen05.alloc / st / ld; SASS UTCALLOC, STTM, LDTM).  One warp allocates, the address comes back through
-// shared memory; a warp reaches only the 32 lanes of its own quarter (warp index mod 4).
-template <int NCOLS>
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result) {
-  constexpr int cols = NCOLS <= 32 ? 32 : NCOLS <= 64 ? 64 : NCOLS <= 128 ? 128 : NCOLS <= 256 ? 256 : 512;
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)), "r"(cols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <int NCOLS>
-__device__ __forceinline__ void tmem_free(uint32_t taddr) {
-  constexpr int cols = NCOLS <= 32 ? 32 : NCOLS <= 64 ? 64 : NCOLS <= 128 ? 128 : NCOLS <= 256 ? 256 : 512;
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(cols) : "memory");
-}
-__device__ __forceinline__ void tmem_store1(uint32_t taddr, float v) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x1.b32 [%0], {%1};" ::"r"(taddr), "r"(__float_as_uint(v)) : "memory");
-}
-__device__ __forceinline__ void tmem_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_fence_before_sync() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tmem_fence_after_sync() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
 // ------------------------------------------------------------------ padded sample fetch
 // Virtual sample j of a clip of n samples under np.pad semantics (librosa/core/spectrum.py:252-328,
 // equivalence to np.pad(y, n_fft//2, mode) per SURVEY Appendix A.2).
@@ -169,9 +147,7 @@ __device__ __forceinline__ int partner_slot(int t) {
 // tables are shared.  The halves drift apart, so the shared-memory-bound phases of one (operand fetch,
 // exchange, mel gather) overlap the FP32-bound butterflies of the other instead of all warps of the SM
 // hitting the same pipe at once.
-// TM: the window and the inter-pass twiddles live in Tensor Memory (TmemTab, fft_engine.cuh) instead of shared
-// memory — a fifth of the shared-memory wavefronts of a frame move to the tcgen05.ld datapath.
-template <int LOG2M, int TPF, int NW, int MODE, int NSPLIT, bool TM>
+template <int LOG2M, int TPF, int NW, int MODE, int NSPLIT>
 __global__ void __launch_bounds__(NW * 32, 1) fwd_kernel(const FwdArgs a) {
   using Cfg = FftCfg<LOG2M, TPF>;
   constexpr int M = Cfg::M, N = 2 * M, PPT = Cfg::PPT;
@@ -184,8 +160,7 @@ __global__ void __launch_bounds__(NW * 32, 1) fwd_kernel(const FwdArgs a) {
   static_assert(NW % NSPLIT == 0, "the warps are split evenly");
   static_assert(TPF <= 32 || NH + NT / TPF <= 15, "named barriers: 1..NH for the halves, then one per frame group");
   static_assert(FT >= 1 && FT <= 32, "tile must hold 1..32 frames");
-  static_assert(!TM || (PPT == 32 && NW >= 4 && (TPF <= 32 || (4 * 32) % TPF == 0)), "TMEM tables: 32 points per thread, all four lane quarters in use");
-  using Tab = typename std::conditional<TM, TmemTab<Cfg>, SmemTab<Cfg>>::type;
+  using Tab = SmemTab<Cfg>;
   using ML = MelLayout<M, FT>;
   constexpr int H = ML::H;                     // mel rows handled concurrently by one warp (common.cuh)
   constexpr int NPAIR = PPT / 2;               // bin pairs (k, M-k) per thread
@@ -221,43 +196,10 @@ __global__ void __launch_bounds__(NW * 32, 1) fwd_kernel(const FwdArgs a) {
 
   // ---- one-time table staging (whole CTA)
   Tab tab;
-  if constexpr (TM) {
-    // Warps 0..3 each fill the lane quarter they can reach: lane i of quarter q serves thread
-    // t = (i + 32 q) mod TPF of a frame group (every warp w of the CTA sits in quarter w mod 4).
-    uint32_t* s_taddr = reinterpret_cast<uint32_t*>(smem + a.off_bar + 8 * NH);
-    if (tid < 32) tmem_alloc<Tab::NCOLS>(s_taddr);
-    tmem_fence_before_sync();
-    __syncthreads();
-    tmem_fence_after_sync();
-    const uint32_t tbase = *s_taddr + ((uint32_t)(((tid >> 5) & 3) * 32) << 16);
-    if (tid < 128) {
-      const int tt = tid % TPF;
-      for (int col = 0; col < 64; ++col)          // window pair of pass-0 slot col/2
-        tmem_store1(tbase + col, a.window[2 * (tt + pass0_offset<Cfg>(col >> 1)) + (col & 1)]);
-      for (int sp = 1; sp < Cfg::NPASS; ++sp) {
-        const int R = Cfg::radix(sp), p = Cfg::sublen(sp);
-        for (int f = 0; f < PPT; ++f) {
-          const int b = f / R, r = f % R, k = (tt + TPF * b) & (p - 1);
-          const float2 w = r == 0 ? make_float2(1.0f, 0.0f) : a.tw[Cfg::tw_offset(sp) + (r - 1) * p + k];
-          tmem_store1(tbase + 64 * sp + 2 * f, w.x);
-          tmem_store1(tbase + 64 * sp + 2 * f + 1, w.y);
-        }
-      }
-      for (int cp = 0; cp < NPAIR; ++cp) {        // un-mix twiddles W_N^(t + TPF*c)
-        const float2 w = a.twn[tt + TPF * cp];
-        tmem_store1(tbase + Tab::UNMIX_COL + 2 * cp, w.x);
-        tmem_store1(tbase + Tab::UNMIX_COL + 2 * cp + 1, w.y);
-      }
-      tmem_wait_st();
-    }
-    tmem_fence_before_sync();
-    tab.taddr = tbase;
-  } else {
-    for (int i = tid; i < N; i += NT) s_win[i] = a.window[i];
-    for (int i = tid; i < Cfg::TW_COUNT; i += NT) s_tw[i] = a.tw[i];
-    tab.win = s_win;
-    tab.tw = s_tw;
-  }
+  for (int i = tid; i < N; i += NT) s_win[i] = a.window[i];
+  for (int i = tid; i < Cfg::TW_COUNT; i += NT) s_tw[i] = a.tw[i];
+  tab.win = s_win;
+  tab.tw = s_tw;
   if constexpr (MODE == MODE_MEL) {
     for (int i = tid; i < a.mel_w_count; i += NT) s_melw[i] = a.mel_w[i];
     for (int i = tid; i < a.n_mel_rows; i += NT) s_row[i] = a.mel_rows[i];
@@ -273,11 +215,10 @@ __global__ void __launch_bounds__(NW * 32, 1) fwd_kernel(const FwdArgs a) {
     fence_mbar_init();
   }
   __syncthreads();
-  if constexpr (TM) tmem_fence_after_sync();
 
   const int span = a.in_floats;
   const bool hop_even = (a.hop & 1) == 0;
-  // un-mix twiddle of bin k = t + TPF*c: one register x compile-time constant (SmemTab) or a TMEM column pair
+  // un-mix twiddle of bin k = t + TPF*c: one register x compile-time constant
   const float2 wt = __ldg(a.twn + t);
   auto unmix_tw = [&](auto C) -> float2 { return tab.template unmix<decltype(C)::value>(wt); };
 
@@ -342,7 +283,6 @@ __global__ void __launch_bounds__(NW * 32, 1) fwd_kernel(const FwdArgs a) {
   TileInfo nxt;
   // ---------------- stage a tile's sample span and turn it into windowed pass-0 operands (first stage fused in)
   auto stage_and_fetch = [&](const TileInfo& ti) {
-    if constexpr (TM) tab.begin_window();   // first window chunk travels while the tile lands
     if (ti.kind == TILE_GATHER) {
       const float* yc = a.y + (long long)ti.clip * a.clip_stride;
       const long long s0 = (long long)ti.tix * FT * a.hop - a.pad;
@@ -682,14 +622,6 @@ __global__ void __launch_bounds__(NW * 32, 1) fwd_kernel(const FwdArgs a) {
       }
     }
     if constexpr (!PIPE) cur = nxt;   // (pipelined form: already advanced in front of the mel phase)
-  }
-  if constexpr (TM) {
-    tmem_fence_before_sync();
-    __syncthreads();
-    if (tid < 32) {
-      tmem_fence_after_sync();
-      tmem_free<Tab::NCOLS>(tab.taddr);   // warp 0 sits in quarter 0: its address is the allocation base
-    }
   }
 }
 

@@ -1,6 +1,5 @@
 // inv_inst.cu — instantiates inv_kernel for one transform size (compile with -DB2L_LOG2M=k).
 #include "inv_kernel.cuh"
-#include "inv2_kernel.cuh"
 #include "internal.h"
 
 #ifndef B2L_LOG2M
@@ -21,16 +20,11 @@ cudaError_t run_op(K kern, int op, int nt, const InvArgs* a, int grid, size_t sm
 #define B2L_CAT2(a, b) a##b
 #define B2L_CAT(a, b) B2L_CAT2(a, b)
 
-// `nw`: 16 or 8 warps; 116 = 16 warps as two independent 8-warp halves (DUAL);
-// 2004 / 2002 = inv2_kernel (autonomous frame groups, overlap-add state in Tensor Memory) for hop = n_fft / 4, / 2.
+// `nw`: 16 or 8 warps; 116 = 16 warps as two independent 8-warp halves (DUAL).
 template <int L>
 cudaError_t inv_dispatch(int op, int nw, const InvArgs* a, int grid, size_t smem, cudaStream_t st, int* result) {
   constexpr int M = 1 << L;
   constexpr int TPF = M >= 32 ? M / 32 : 1;
-  if constexpr (L >= 10 && L <= 12) {
-    if (nw == 2004) return run_op(inv2_kernel<L, TPF, 16, 4>, op, 16 * 32, a, grid, smem, st, result);
-    if (nw == 2002) return run_op(inv2_kernel<L, TPF, 16, 2>, op, 16 * 32, a, grid, smem, st, result);
-  }
   if constexpr (L >= 10) {
     if (nw == 16) return run_op(inv_kernel<L, TPF, 16, false>, op, 16 * 32, a, grid, smem, st, result);
     if (nw == 8) return run_op(inv_kernel<L, TPF, 8, false>, op, 8 * 32, a, grid, smem, st, result);

@@ -12,7 +12,7 @@ for p in (ROOT, os.path.join(ROOT, "tests"), os.path.join(ROOT, "tools")):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (run with -m gpu)")
 
 
 def _gpu_ok():

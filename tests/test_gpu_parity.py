@@ -1,4 +1,4 @@
-"""GPU (-m gpu): the CUDA path, called through the public drop-in API (ctypes -> C ABI -> sm_100a
+"""GPU (-m gpu): the CUDA path, called through the public drop-in API (ctypes -> C ABI -> sm_90a
 kernels), against the oracle on identical inputs and against the fixtures produced by the unmodified
 reference.  Nothing here reads /root/reference.
 

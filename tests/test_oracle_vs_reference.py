@@ -1,58 +1,52 @@
-"""CPU, build container only: the oracle against the live, unmodified reference imported from
-/root/reference (tools/ref_shim.py).  Skipped where the reference tree is absent (e.g. the GPU box);
-tests/test_oracle_golden.py covers those boxes through the committed fixtures."""
+"""CPU: the oracle and the product's host-side constants against the unmodified reference's outputs, stored
+by tools/make_golden.py (tests/reference_pins.py).  Every comparison is exact."""
+import os
 import warnings
 
 import numpy as np
 import pytest
 
-import ref_shim
+import reference_pins as RP
 
-pytestmark = pytest.mark.skipif(not ref_shim.available(), reason="/root/reference not present")
+PINS_PATH = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_pins_v1.npz")
 
 
 @pytest.fixture(scope="module")
 def ref():
-    return ref_shim.load_reference()
+    with np.load(PINS_PATH) as z:
+        return {k: z[k] for k in z.files}
 
 
-@pytest.mark.parametrize("n,n_fft,hop,center,pad_mode", [
-    (22050, 2048, 512, True, "constant"), (5000, 1024, 256, True, "reflect"), (4000, 512, None, False, "constant"),
-    (1000, 2048, 512, True, "constant"), (3000, 501, 128, True, "edge"), (7000, 1025, 300, True, "symmetric"),
-    (6000, 256, 64, True, "linear_ramp"), (900, 64, 7, True, "reflect"),
-])
+@pytest.mark.parametrize("n,n_fft,hop,center,pad_mode", RP.STFT_GRID)
 def test_stft_istft_bit_exact(ref, oracle, n, n_fft, hop, center, pad_mode):
-    y = (0.1 * np.random.default_rng(n).standard_normal(n)).astype(np.float32)
-    kw = dict(n_fft=n_fft, hop_length=hop, center=center, pad_mode=pad_mode)
+    y = RP.stft_input(n)
+    key = RP.stft_key(n, n_fft, hop, center, pad_mode)
     with warnings.catch_warnings():
         warnings.simplefilter("ignore")
-        D, Do = ref.stft(y, **kw), oracle.stft(y, **kw)
-        np.testing.assert_array_equal(D, Do)
+        D = oracle.stft(y, n_fft=n_fft, hop_length=hop, center=center, pad_mode=pad_mode)
+        RP.assert_pinned(ref, key, D)
         for length in (None, n):
-            a = ref.istft(D, hop_length=hop, n_fft=n_fft, center=center, length=length)
             b = oracle.istft(D, hop_length=hop, n_fft=n_fft, center=center, length=length)
-            np.testing.assert_array_equal(a, b)
+            RP.assert_pinned(ref, f"{key}/istft_{length}", b)
 
 
 def test_features_bit_exact(ref, oracle):
-    y = (0.1 * np.random.default_rng(5).standard_normal((2, 3, 8000))).astype(np.float32)
-    np.testing.assert_array_equal(ref.feature.melspectrogram(y=y, sr=16000, n_fft=1024, hop_length=256),
-                                  oracle.melspectrogram(y=y, sr=16000, n_fft=1024, hop_length=256))
-    np.testing.assert_array_equal(ref.feature.mfcc(y=y, sr=16000, n_mfcc=40, n_fft=1024, hop_length=256),
-                                  oracle.mfcc(y=y, sr=16000, n_mfcc=40, n_fft=1024, hop_length=256))
-    np.testing.assert_array_equal(ref.feature.mfcc(y=y, sr=16000, n_mfcc=13, lifter=22, dct_type=3),
-                                  oracle.mfcc(y=y, sr=16000, n_mfcc=13, lifter=22, dct_type=3))
+    y = RP.features_input()
+    RP.assert_pinned(ref, "features/mel", oracle.melspectrogram(y=y, sr=16000, n_fft=1024, hop_length=256))
+    RP.assert_pinned(ref, "features/mfcc40", oracle.mfcc(y=y, sr=16000, n_mfcc=40, n_fft=1024, hop_length=256))
+    RP.assert_pinned(ref, "features/mfcc13_lifter_dct3", oracle.mfcc(y=y, sr=16000, n_mfcc=13, lifter=22, dct_type=3))
 
 
-def test_frame_statistics_bit_exact(ref, oracle, golden):
-    from feature_cases import FEATURE_CASES, call, outputs
+def test_frame_statistics_bit_exact(oracle, golden):
+    # tests/golden/features_v1.npz holds the reference's outputs of the same cases on the same inputs
+    from feature_cases import FEATURE_CASES, call, fixture_names, outputs
 
     for case in FEATURE_CASES:
         with warnings.catch_warnings():
             warnings.simplefilter("ignore")
-            A, B = outputs(call(ref, case, golden)), outputs(call(oracle, case, golden))
-        assert len(A) == len(B)
-        for a, b in zip(A, B):
+            B = outputs(call(oracle, case, golden))
+        for key, b in zip(fixture_names(case, len(B)), B):
+            a = golden[key]
             assert a.dtype == b.dtype and a.shape == b.shape, case["name"]
             np.testing.assert_array_equal(a, b, err_msg=case["name"])
 
@@ -60,18 +54,16 @@ def test_frame_statistics_bit_exact(ref, oracle, golden):
 def test_product_chroma_filter_matches_reference(ref):
     import librosa_b200 as lb
 
-    for kw in [dict(sr=22050, n_fft=2048), dict(sr=16000, n_fft=1024, tuning=0.27), dict(sr=22050, n_fft=400, n_chroma=24, octwidth=None),
-               dict(sr=44100, n_fft=4096, norm=None, base_c=False, ctroct=4.0, octwidth=1.5), dict(sr=22050, n_fft=1025, tuning=-0.3)]:
-        np.testing.assert_array_equal(lb.filters.chroma(**kw), ref.filters.chroma(**kw))
-    f = np.array([27.5, 55.0, 440.0, 1234.5])
-    np.testing.assert_array_equal(lb.hz_to_octs(f, tuning=0.2, bins_per_octave=24), ref.hz_to_octs(f, tuning=0.2, bins_per_octave=24))
+    for i, kw in enumerate(RP.CHROMA_KW):
+        RP.assert_pinned(ref, f"chroma/{i}", lb.filters.chroma(**kw))
+    RP.assert_pinned(ref, "hz_to_octs", lb.hz_to_octs(RP.OCTS_F, tuning=0.2, bins_per_octave=24))
 
 
 def test_griffinlim_bit_exact(ref, oracle):
-    y = (0.1 * np.random.default_rng(2).standard_normal(6000)).astype(np.float32)
-    S = np.abs(ref.stft(y, n_fft=512, hop_length=128))
-    for kw in [dict(n_iter=4, rng=0), dict(n_iter=3, init=None, momentum=0.5), dict(n_iter=2, rng=7, length=6000)]:
-        np.testing.assert_array_equal(ref.griffinlim(S, hop_length=128, **kw), oracle.griffinlim(S, hop_length=128, **kw))
+    S = np.abs(oracle.stft(RP.griffinlim_input(), n_fft=512, hop_length=128))
+    RP.assert_pinned(ref, "griffinlim/S", S)
+    for i, kw in enumerate(RP.GL_KW):
+        RP.assert_pinned(ref, f"griffinlim/{i}", oracle.griffinlim(S, hop_length=128, **kw))
 
 
 def test_product_host_constants_match_reference(ref):
@@ -79,60 +71,45 @@ def test_product_host_constants_match_reference(ref):
     reference — these feed the GPU plans, so they are pinned as tightly as the oracle."""
     import librosa_b200 as lb
 
-    for kw in [dict(sr=22050, n_fft=2048), dict(sr=44100, n_fft=4096), dict(sr=16000, n_fft=1024, n_mels=40, htk=True),
-               dict(sr=22050, n_fft=2048, norm=1), dict(sr=22050, n_fft=2048, norm=None, fmin=300, fmax=8000),
-               dict(sr=22050, n_fft=2048, norm=np.inf), dict(sr=8000, n_fft=512, n_mels=20, dtype=np.float64)]:
-        np.testing.assert_array_equal(ref.filters.mel(**kw), lb.filters.mel(**kw))
-    np.testing.assert_array_equal(ref.filters.window_sumsquare(window="hann", n_frames=50),
-                                  lb.filters.window_sumsquare(window="hann", n_frames=50))
-    for w in ["hann", "hamming", ("kaiser", 4.0), np.ones(64)]:
-        np.testing.assert_array_equal(ref.filters.get_window(w, 64), lb.filters.get_window(w, 64))
-    f = np.array([0.0, 60.0, 999.0, 1000.0, 5000.0])
+    for i, kw in enumerate(RP.MEL_KW):
+        RP.assert_pinned(ref, f"mel/{i}", lb.filters.mel(**kw))
+    RP.assert_pinned(ref, "window_sumsquare_hann_50", lb.filters.window_sumsquare(window="hann", n_frames=50))
+    for i, w in enumerate(RP.WINDOWS):
+        RP.assert_pinned(ref, f"get_window/{i}", lb.filters.get_window(w, 64))
     for htk in (False, True):
-        np.testing.assert_array_equal(ref.hz_to_mel(f, htk=htk), lb.hz_to_mel(f, htk=htk))
-        np.testing.assert_array_equal(ref.mel_to_hz(f / 50, htk=htk), lb.mel_to_hz(f / 50, htk=htk))
-    assert ref.hz_to_mel(60.0) == lb.hz_to_mel(60.0) and ref.mel_to_hz(20.0) == lb.mel_to_hz(20.0)
-    x = np.arange(40.0).reshape(2, 20)
+        RP.assert_pinned(ref, f"hz_to_mel/{htk}", lb.hz_to_mel(RP.HZ, htk=htk))
+        RP.assert_pinned(ref, f"mel_to_hz/{htk}", lb.mel_to_hz(RP.HZ / 50, htk=htk))
+    assert ref["hz_to_mel_60"] == lb.hz_to_mel(60.0) and ref["mel_to_hz_20"] == lb.mel_to_hz(20.0)
+    x = RP.frame_input()
     for axis in (-1, 0, 1):
         if x.shape[axis] >= 5:
-            np.testing.assert_array_equal(ref.util.frame(x, frame_length=5, hop_length=2, axis=axis),
-                                          lb.util.frame(x, frame_length=5, hop_length=2, axis=axis))
-    np.testing.assert_array_equal(ref.util.pad_center(np.ones(5), size=12), lb.util.pad_center(np.ones(5), size=12))
-    np.testing.assert_array_equal(ref.util.fix_length(np.ones(5), size=3), lb.util.fix_length(np.ones(5), size=3))
-    assert ref.util.tiny(np.float32(1)) == lb.util.tiny(np.float32(1))
+            RP.assert_pinned(ref, f"frame/{axis}", lb.util.frame(x, frame_length=5, hop_length=2, axis=axis))
+    RP.assert_pinned(ref, "pad_center", lb.util.pad_center(np.ones(5), size=12))
+    RP.assert_pinned(ref, "fix_length", lb.util.fix_length(np.ones(5), size=3))
+    assert ref["tiny_float32"] == lb.util.tiny(np.float32(1))
 
 
 def test_power_to_db_axes_and_float64_bit_exact(ref, oracle):
     """power_to_db with explicit reduction axes, and the float64 behaviour of the whole path (the reference
     computes float64 audio in float64: complex128 STFT, float64 mel / MFCC)."""
-    rng = np.random.default_rng(9)
-    P = np.abs(rng.standard_normal((2, 3, 40, 30))) ** 2
-    for kw in (dict(), dict(axes=(-1,)), dict(axes=(-2,)), dict(axes=None, ref=np.max), dict(axes=(0, -1), top_db=30.0),
-               dict(axes=(-1,), ref=np.max)):
-        np.testing.assert_array_equal(ref.power_to_db(P, **kw), oracle.power_to_db(P, **kw))
-    y = 0.1 * rng.standard_normal((2, 9000))
-    for fn_ref, fn_or, kw in ((ref.stft, oracle.stft, dict(n_fft=1024, hop_length=256)),
-                              (ref.stft, oracle.stft, dict(n_fft=1000, hop_length=250, pad_mode="reflect"))):
-        a, b = fn_ref(y, **kw), fn_or(y, **kw)
-        assert a.dtype == b.dtype == np.complex128
-        np.testing.assert_array_equal(a, b)
-        np.testing.assert_array_equal(ref.istft(a, hop_length=kw["hop_length"], n_fft=kw["n_fft"]),
-                                      oracle.istft(a, hop_length=kw["hop_length"], n_fft=kw["n_fft"]))
-    m_ref, m_or = ref.feature.melspectrogram(y=y, sr=16000, n_fft=1024), oracle.melspectrogram(y=y, sr=16000, n_fft=1024)
-    assert m_ref.dtype == m_or.dtype == np.float64
-    np.testing.assert_array_equal(m_ref, m_or)
-    np.testing.assert_array_equal(ref.feature.mfcc(y=y, sr=16000, n_fft=1024), oracle.mfcc(y=y, sr=16000, n_fft=1024))
+    P, y = RP.db_inputs()
+    for i, kw in enumerate(RP.DB_KW):
+        RP.assert_pinned(ref, f"power_to_db/{i}", oracle.power_to_db(P, **kw))
+    for i, kw in enumerate(RP.F64_STFT_KW):
+        b = oracle.stft(y, **kw)
+        assert b.dtype == np.complex128
+        RP.assert_pinned(ref, f"f64/stft/{i}", b)
+        RP.assert_pinned(ref, f"f64/istft/{i}", oracle.istft(b, hop_length=kw["hop_length"], n_fft=kw["n_fft"]))
+    m_or = oracle.melspectrogram(y=y, sr=16000, n_fft=1024)
+    assert m_or.dtype == np.float64
+    RP.assert_pinned(ref, "f64/mel", m_or)
+    RP.assert_pinned(ref, "f64/mfcc", oracle.mfcc(y=y, sr=16000, n_fft=1024))
 
 
 def test_feature_inverse_bit_exact(ref, oracle):
     """mel_to_stft (NNLS through SciPy's L-BFGS-B) and mfcc_to_mel restated in the oracle."""
-    rng = np.random.default_rng(21)
-    for dtype in (np.float32, np.float64):
-        basis = ref.filters.mel(sr=22050, n_fft=1024, n_mels=64, dtype=dtype)
-        S = np.abs(rng.standard_normal((513, 6))).astype(dtype) ** 2
-        M = basis.dot(S)
-        np.testing.assert_array_equal(ref.feature.inverse.mel_to_stft(M, n_fft=1024, power=2.0),
-                                      oracle.mel_to_stft(M, n_fft=1024, power=2.0))
-    mf = rng.standard_normal((2, 13, 20)).astype(np.float32) * 10
-    for kw in (dict(), dict(lifter=3, dct_type=3), dict(n_mels=64, norm=None), dict(ref=2.5, lifter=22)):
-        np.testing.assert_array_equal(ref.feature.inverse.mfcc_to_mel(mf, **kw), oracle.mfcc_to_mel(mf, **kw))
+    _, _, mf = RP.inverse_inputs()
+    for name in ("float32", "float64"):
+        RP.assert_pinned(ref, f"inverse/mel_to_stft_{name}", oracle.mel_to_stft(ref[f"inverse/M_{name}"], n_fft=1024, power=2.0))
+    for i, kw in enumerate(RP.MFCC_TO_MEL_KW):
+        RP.assert_pinned(ref, f"inverse/mfcc_to_mel/{i}", oracle.mfcc_to_mel(mf, **kw))

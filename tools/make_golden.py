@@ -1,9 +1,10 @@
-"""Generate tests/golden/hotpath_v1.npz (tests/cases.py) and tests/golden/features_v1.npz
-(tests/feature_cases.py) by running the cases through the UNMODIFIED reference.
+"""Generate tests/golden/hotpath_v1.npz (tests/cases.py), tests/golden/features_v1.npz
+(tests/feature_cases.py) and tests/golden/reference_pins_v1.npz (tests/reference_pins.py) by running the
+cases through the UNMODIFIED reference.
 
-Build-container only (needs /root/reference; see tools/ref_shim.py).  The fixtures travel to the GPU box,
-where /root/reference does not exist.  Also stores a handful of constant tables (mel bases, window
-sum-square, mel-scale known answers) produced by the reference.
+Needs a checkout of the reference (see tools/ref_shim.py); the tests only read the stored fixtures.  Also
+stores a handful of constant tables (mel bases, window sum-square, mel-scale known answers) produced by the
+reference.
 
     python tools/make_golden.py
 """
@@ -87,6 +88,16 @@ def main():
             print(f"{key:40s} {arr.shape} {arr.dtype}")
     path = os.path.join(ROOT, "tests", "golden", "features_v1.npz")
     np.savez_compressed(path, **feats)
+    print("wrote", path, os.path.getsize(path), "bytes")
+    write_reference_pins(ref)
+
+
+def write_reference_pins(ref):
+    """tests/golden/reference_pins_v1.npz: what tests/test_oracle_vs_reference.py compares against."""
+    import reference_pins
+
+    path = os.path.join(ROOT, "tests", "golden", "reference_pins_v1.npz")
+    np.savez_compressed(path, **reference_pins.pack(reference_pins.reference_outputs(ref)))
     print("wrote", path, os.path.getsize(path), "bytes")
 
 

@@ -1,5 +1,5 @@
 // Standalone check of contrast_kernel's tail extraction against a host sort (development aid).
-//   nvcc -std=c++17 -O3 -gencode arch=compute_100a,code=sm_100a -I librosa_b200/csrc -o /tmp/contrast_test tools/micro/contrast_test.cu
+//   nvcc -std=c++17 -O3 -gencode arch=compute_90a,code=sm_90a -I librosa_b200/csrc -o /tmp/contrast_test tools/micro/contrast_test.cu
 #include <cstdio>
 #include <cstdlib>
 #include <vector>

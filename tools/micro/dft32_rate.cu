@@ -1,7 +1,6 @@
 // Register-only radix-32 DFT throughput: the butterfly network of fft_engine.cuh with no memory traffic, at the
 // occupancy of the production kernels (512 threads and 128 registers per thread, one CTA per SM).
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -DB2L_PACKED=1 -o dft32_packed dft32_rate.cu
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -DB2L_PACKED=0 -o dft32_scalar dft32_rate.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o dft32_rate dft32_rate.cu
 #include "../../librosa_b200/csrc/fft_engine.cuh"
 #include <cstdio>
 using namespace b2l;
@@ -42,7 +41,7 @@ void run(const char* name, float2* out, int sms) {
 int main() {
   cudaDeviceProp p; cudaGetDeviceProperties(&p, 0);
   float2* out; cudaMalloc(&out, size_t(p.multiProcessorCount) * 512 * sizeof(float2));
-  printf("%s  B2L_PACKED=%d\n", p.name, B2L_PACKED);
+  printf("%s\n", p.name);
   run<0>("radix-32 DFT", out, p.multiProcessorCount);
   run<1>("31 twiddle products + radix-32 DFT", out, p.multiProcessorCount);
   printf("%s\n", cudaGetErrorString(cudaDeviceSynchronize()));

@@ -1,8 +1,7 @@
 """Import the *unmodified* reference librosa from /root/reference in this container.
 
 Build-container-only helper (the GPU box has no /root/reference). It is used by
-``tools/make_golden.py`` to generate the committed fixtures under ``tests/golden/`` and by
-``tests/test_oracle_vs_reference.py`` (skipped when the reference tree is absent) to pin the
+``tools/make_golden.py`` to generate the committed fixtures under ``tests/golden/`` that pin the
 ``oracle/`` restatement against the real thing.
 
 librosa imports four modules at import time that are missing from the image and never called on
