@@ -14,7 +14,8 @@ from typing import Optional, Tuple
 import numpy as np
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-# B2L_LIB_PATH selects another build flavour of the same C ABI (A/B measurements); there is still no fallback.
+# B2L_LIB_PATH loads another build of the same C ABI (another flavour or revision, to compare outputs and timings);
+# there is still no fallback.
 LIB_PATH = os.environ.get("B2L_LIB_PATH") or os.path.join(_HERE, "csrc", "libb2l.so")
 
 B2L_OK = 0

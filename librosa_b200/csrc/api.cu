@@ -144,7 +144,7 @@ struct b2l_plan {
   float* d_mel_wT = nullptr;     // n_mels <= 16: dense transposed weights [bin][16] (dense_project_kernel)
   std::vector<MelBand> h_band;
   std::vector<float> h_mel_w;
-  struct RowTable { MelRow* d_rows = nullptr; float* d_w = nullptr; unsigned short* d_order = nullptr; int n_rows = 0, w_count = 0, list_len = 0; };
+  struct RowTable { MelRow* d_rows = nullptr; float* d_w = nullptr; int n_rows = 0, w_count = 0; };
   mutable std::map<int, RowTable> row_tables;
   int power_mode = 2;
   float power = 2.0f;
@@ -542,7 +542,6 @@ extern "C" int b2l_plan_destroy(b2l_plan* p) {
   for (auto& kv : p->row_tables) {
     cudaFree(kv.second.d_rows);
     cudaFree(kv.second.d_w);
-    cudaFree(kv.second.d_order);
   }
   cudaFree(p->d_dct);
   delete p;
@@ -744,7 +743,7 @@ extern "C" int b2l_plan_create(b2l_ctx* c, const b2l_plan_desc* d, b2l_plan** ou
     }
   }
   if (d->n_mfcc > 0) {
-    // transposed and zero padded to 8-coefficient groups: dctT[m][8*KG] (dct_clamp_kernel)
+    // transposed and zero padded to 8-coefficient groups: dctT[m][8*KG] (dct_clamp4_kernel)
     const int KP = (d->n_mfcc + 7) / 8 * 8;
     std::vector<float> dct((size_t)d->n_mels * KP, 0.0f);
     for (int k = 0; k < d->n_mfcc; ++k)
@@ -806,11 +805,9 @@ static int ensure_clip_max(b2l_ctx* c, size_t n_clips) {
   return B2L_OK;
 }
 
-// MelRow table for warps that process H mel rows at a time (see MelRow / MelLayout in common.cuh), plus the
-// work-item lists of the `hw` warps of a half: items sorted by length and dealt longest-first to the least
-// loaded warp (the bands of the highest mel rows are ten times longer than those of the lowest).
-static int get_row_table(b2l_ctx* c, const b2l_plan* p, int H, int hw, const b2l_plan::RowTable** out) {
-  const int key = H * 64 + hw;
+// MelRow table for warps that process H mel rows at a time (see MelRow / MelLayout in common.cuh).
+static int get_row_table(b2l_ctx* c, const b2l_plan* p, int H, const b2l_plan::RowTable** out) {
+  const int key = H;
   auto it = p->row_tables.find(key);
   if (it != p->row_tables.end()) {
     *out = &it->second;
@@ -821,7 +818,6 @@ static int get_row_table(b2l_ctx* c, const b2l_plan* p, int H, int hw, const b2l
   const int n_items = n_rows / H;
   std::vector<MelRow> rows(n_rows);
   std::vector<float> w;
-  std::vector<int> item_quads(n_items, 0);
   for (int item = 0; item < n_items; ++item) {
     std::vector<int> start(H), lenp(H);
     int quads = 0;
@@ -840,7 +836,6 @@ static int get_row_table(b2l_ctx* c, const b2l_plan* p, int H, int hw, const b2l
       }
       quads = std::max(quads, (lenp[j] + 3) / 4);
     }
-    item_quads[item] = quads;
     for (int j = 0; j < H; ++j) {
       const int m = item * H + j;
       MelRow r;
@@ -856,56 +851,20 @@ static int get_row_table(b2l_ctx* c, const b2l_plan* p, int H, int hw, const b2l
       rows[m] = r;
     }
   }
-  // longest-processing-time-first: cost of an item = its trip count + a fixed part (row fetch, stores)
-  std::vector<int> idx(n_items);
-  for (int i = 0; i < n_items; ++i) idx[i] = i;
-  // B2L_MEL_LPT=1: longest-first deal to the least loaded warp.  Measured neutral to slightly negative on cfg 2
-  // (1.148 vs 1.139 ms): the natural order, dealt round-robin, keeps neighbouring rows (whose bands overlap
-  // in shared memory) on warps that run at the same time.  Default: round-robin.
-  const char* lpt_env = getenv("B2L_MEL_LPT");
-  const bool round_robin = !(lpt_env && *lpt_env && atoi(lpt_env) != 0);
-  if (!round_robin)
-    std::stable_sort(idx.begin(), idx.end(), [&](int x, int y) { return item_quads[x] > item_quads[y]; });
-  std::vector<std::vector<int>> lists(hw);
-  std::vector<int> load(hw, 0);
-  int rr = 0;
-  for (int i : idx) {
-    int best = 0;
-    for (int wv = 1; wv < hw; ++wv)
-      if (load[wv] < load[best]) best = wv;
-    if (round_robin) best = (rr++) % hw;
-    lists[best].push_back(i);
-    load[best] += item_quads[i] + 3;
-  }
-  size_t list_len = 0;
-  for (auto& l : lists) list_len = std::max(list_len, l.size());
-  std::vector<unsigned short> order(list_len * hw, (unsigned short)0xffff);
-  for (int wv = 0; wv < hw; ++wv)
-    for (size_t k = 0; k < lists[wv].size(); ++k) order[k * hw + wv] = (unsigned short)lists[wv][k];
-  if (order.empty()) order.push_back(0xffff);
   b2l_plan::RowTable t;
   t.n_rows = n_rows;
   t.w_count = (int)w.size();
-  t.list_len = (int)list_len;
   int rc;
-  if ((rc = upload(c, rows, &t.d_rows)) || (rc = upload(c, w, &t.d_w)) || (rc = upload(c, order, &t.d_order))) return rc;
+  if ((rc = upload(c, rows, &t.d_rows)) || (rc = upload(c, w, &t.d_w))) return rc;
   auto ins = p->row_tables.emplace(key, t);
   *out = &ins.first->second;
   return B2L_OK;
 }
 
-// Kernel variants tried in order (first that fits shared memory wins): 116 = 16 warps as two independent
-// 8-warp halves, 16 / 8 = plain CTAs.  B2L_FWD_VARIANT forces one (A/B measurements).
-#ifndef B2L_DCT_FPL_DEFAULT
-#define B2L_DCT_FPL_DEFAULT 4
-#endif
-static int fwd_variants(const HostFftCfg& cfg, int out[6]) {
+// CTA variants of the forward and inverse kernels, tried in order (first that fits shared memory wins):
+// 116 = 16 warps as two independent 8-warp halves, 16 / 8 = plain CTAs.
+static int cta_variants(const HostFftCfg& cfg, int out[3]) {
   int n = 0;
-  const char* force = getenv("B2L_FWD_VARIANT");
-  if (force && *force) {
-    out[n++] = atoi(force);
-    return n;
-  }
   if (cfg.log2m >= 9 && cfg.log2m <= 11) out[n++] = 116;
   int nws[2];
   const int k = cfg.nw_options(nws);
@@ -933,8 +892,8 @@ static int run_forward(b2l_ctx* c, const b2l_plan* p, int mode, int log_mode, co
   HostFftCfg cfg(p->log2m);
   const int N = p->n_fft, M = N / 2;
   fwd_op_fn op = fwd_table(p->log2m);
-  int variants[6];
-  const int n_opt = fwd_variants(cfg, variants);
+  int variants[3];
+  const int n_opt = cta_variants(cfg, variants);
   FwdArgs a;
   memset(&a, 0, sizeof(a));
   int variant = 0, ft = 0, halves = 1;
@@ -951,17 +910,16 @@ static int run_forward(b2l_ctx* c, const b2l_plan* p, int mode, int log_mode, co
     if (span > 0x3fffffff) continue;
     const b2l_plan::RowTable* t = nullptr;
     if (mode == MODE_MEL) {
-      int rc = get_row_table(c, p, mel_rows_per_warp(f), nw / nh, &t);
+      int rc = get_row_table(c, p, mel_rows_per_warp(f), &t);
       if (rc) return rc;
     }
     size_t off = 0;
     a.off_win = (int)off; off = align_up(off + (size_t)N * 4, 16);
     a.off_tw = (int)off; off = align_up(off + (size_t)cfg.tw_count() * 8, 16);
-    a.off_bar = (int)off; off = align_up(off + 64, 16);   // "tile landed" mbarrier per half, "staging consumed" mbarriers
+    a.off_bar = (int)off; off = align_up(off + 8 * nh, 16);   // "tile landed" mbarrier per half
     if (t) {
       a.off_melw = (int)off; off = align_up(off + (size_t)t->w_count * 4, 16);
       a.off_melband = (int)off; off = align_up(off + (size_t)t->n_rows * sizeof(MelRow), 16);
-      a.off_melorder = (int)off; off = align_up(off + (size_t)std::max(1, t->list_len) * (nw / nh) * 2, 16);
     }
     if (mode == MODE_STATS) {   // bin frequencies take the place of the mel weights
       a.off_melw = (int)off; off = align_up(off + (size_t)(M + 1) * 4, 16);
@@ -1024,8 +982,6 @@ static int run_forward(b2l_ctx* c, const b2l_plan* p, int mode, int log_mode, co
     a.mel_w = rt->d_w;
     a.mel_rows = rt->d_rows;
     a.n_mel_rows = rt->n_rows;
-    a.mel_order = rt->d_order;
-    a.mel_list_len = rt->list_len;
   }
   a.log_mode = log_mode ? 1 : 0;
   a.out_tiled = log_mode == 2 ? 1 : 0;   // b2l_mfcc: log-mel goes to the tiled scratch
@@ -1140,13 +1096,8 @@ static int run_czt(b2l_ctx* c, const b2l_plan* p, int mode, const float* d_y, in
 
 // ------------------------------------------------------------------ mixed-radix launch (even n_fft, 5-smooth half)
 // mode 0: complex STFT, 1: |X|^power, 2: mel (log_mode 1: dB values + per-clip maximum for mfcc)
-// frames per warp of mr_kernel: 2 (16 lanes each) for short frames, else 1; B2L_MR_LANES = 16 / 32 forces one (A/B)
-static int mr_frames_per_warp(int M) {
-  int lanes = M <= 512 ? 16 : 32;
-  const char* e = getenv("B2L_MR_LANES");
-  if (e && *e && (atoi(e) == 16 || atoi(e) == 32)) lanes = atoi(e);
-  return 32 / lanes;
-}
+// frames per warp of mr_kernel: 2 (16 lanes each) for short frames, else 1
+static int mr_frames_per_warp(int M) { return M <= 512 ? 2 : 1; }
 static bool mr_enabled(const b2l_plan* p) {
   if (p->log2p == 0) return true;   // no chirp-z tables for this size
   const char* e = getenv("B2L_MR");
@@ -1329,10 +1280,8 @@ extern "C" int b2l_frame_feature(b2l_ctx* c, int32_t what, const float* d_y, int
   DeviceGuard g(c->device);
   // frame_length a multiple of hop_length: block form, every sample read once (feat_kernels.cuh)
   {
-    const char* env = getenv("B2L_TD_BLOCK");
     const long long tiles = (T + TD_FRAMES - 1) / TD_FRAMES;
-    if (!(env && *env && atoi(env) == 0) && frame_length % hop_length == 0 && frame_length / hop_length <= 64 &&
-        n_clips <= 65535 && tiles <= 0x7fffffffLL) {
+    if (frame_length % hop_length == 0 && frame_length / hop_length <= 64 && n_clips <= 65535 && tiles <= 0x7fffffffLL) {
       const int R = frame_length / hop_length;
       const size_t smem = (size_t)(TD_FRAMES + R - 1) * 8;
       frame_td_block_kernel<<<dim3((unsigned)tiles, (unsigned)n_clips), 256, smem, c->stream>>>(
@@ -1368,7 +1317,8 @@ static int launch_dct(b2l_ctx* c, const b2l_plan* p, const float* d_L, int64_t n
                       float* d_out, int tiled = 0) {
   const int KG = (p->n_mfcc + 7) / 8;
   if (KG > 16) return fail(B2L_ERR_UNSUPPORTED, "n_mfcc=%d > 128 is not supported", p->n_mfcc);
-  size_t smem = ((size_t)p->n_mels * 8 * KG + 2 * (size_t)p->n_mels * DCT_TILE) * 4;
+  // DCT rows plus one tile buffer of two 64-frame blocks (dct_clamp4_kernel)
+  const size_t smem = ((size_t)p->n_mels * 8 * KG + 2 * (size_t)p->n_mels * 64) * 4;
   if (smem > c->smem_optin) {
     // too many input rows for the shared-memory tile (e.g. mfcc(S=...) of a 1025-bin spectrogram): generic kernel
     if (tiled) return fail(B2L_ERR_UNSUPPORTED, "n_mels=%d is too large for the fused mfcc path", p->n_mels);
@@ -1380,45 +1330,20 @@ static int launch_dct(b2l_ctx* c, const b2l_plan* p, const float* d_L, int64_t n
     c->launches++;
     return B2L_OK;
   }
-  // frames per lane: 2 halves the shared-memory traffic per FMA (B2L_DCT_FPL=1 selects the two-warp-set form)
-  const char* env = getenv("B2L_DCT_FPL");
-  const int fpl = env && *env ? atoi(env) : B2L_DCT_FPL_DEFAULT;
-  if (fpl == 4) {
-    // four frames per lane, 128-frame tiles, one tile buffer per block (dct_clamp4_kernel)
-    const size_t smem4 = ((size_t)p->n_mels * 8 * KG + 2 * (size_t)p->n_mels * 64) * 4;
-    // two warp sets over the mel rows (B2L_DCT_KS=1: one) when the partial sums fit in the tile buffer
-    const char* ks_env = getenv("B2L_DCT_KS");
-    const int ks = (ks_env && *ks_env ? atoi(ks_env) : 2) == 2 && KG <= 10 && p->n_mels >= 8 * KG ? 2 : 1;   // 640 threads at most; 32*KG*32 partial sums <= 2*n_mels*64 tile words
-    auto dct_clamp4 = ks == 2 ? dct_clamp4_kernel<2> : dct_clamp4_kernel<1>;
-    const int threads4 = KG * 32 * ks;
-    CUDA_TRY(cudaFuncSetAttribute(dct_clamp4, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem4));
-    const int tiles4 = (int)((T + DCT4_TILE - 1) / DCT4_TILE);
-    const long long total4 = (long long)tiles4 * n_clips;
-    int occ4 = 0;
-    CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ4, dct_clamp4, threads4, smem4));
-    if (occ4 < 1) return fail(B2L_ERR_CUDA, "DCT kernel does not fit on an SM");
-    long long grid4 = (long long)c->sm_count * occ4;
-    if (grid4 > total4) grid4 = total4;
-    dct_clamp4<<<(int)grid4, threads4, smem4, c->stream>>>(d_L, p->d_dct, clamp ? c->d_clip_max : nullptr,
-                                                                  clamp ? p->top_db : -1.0f, p->n_mels, p->n_mfcc, (int)T,
-                                                                  tiles4, total4, tiled, d_out);
-    CUDA_TRY(cudaGetLastError());
-    c->launches++;
-    return B2L_OK;
-  }
-  auto kern = fpl == 2 ? dct_clamp_kernel<2> : dct_clamp_kernel<1>;
-  const int threads = fpl == 2 ? KG * 32 : KG * 64;
+  // two warp sets over the mel rows when the partial sums fit in the tile buffer
+  const int ks = KG <= 10 && p->n_mels >= 8 * KG ? 2 : 1;   // 640 threads at most; 32*KG*32 partial sums <= 2*n_mels*64 tile words
+  auto kern = ks == 2 ? dct_clamp4_kernel<2> : dct_clamp4_kernel<1>;
+  const int threads = KG * 32 * ks;
   CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  const int tiles = (int)((T + DCT_TILE - 1) / DCT_TILE);
+  const int tiles = (int)((T + DCT4_TILE - 1) / DCT4_TILE);
   const long long total = (long long)tiles * n_clips;
   int occ = 0;
   CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, threads, smem));
   if (occ < 1) return fail(B2L_ERR_CUDA, "DCT kernel does not fit on an SM");
   long long grid = (long long)c->sm_count * occ;
   if (grid > total) grid = total;
-  kern<<<(int)grid, threads, smem, c->stream>>>(d_L, p->d_dct, clamp ? c->d_clip_max : nullptr,
-                                                clamp ? p->top_db : -1.0f, p->n_mels, p->n_mfcc, (int)T, tiles, total,
-                                                tiled, d_out);
+  kern<<<(int)grid, threads, smem, c->stream>>>(d_L, p->d_dct, clamp ? c->d_clip_max : nullptr, clamp ? p->top_db : -1.0f,
+                                                p->n_mels, p->n_mfcc, (int)T, tiles, total, tiled, d_out);
   CUDA_TRY(cudaGetLastError());
   c->launches++;
   return B2L_OK;
@@ -1439,7 +1364,7 @@ extern "C" int b2l_mfcc(b2l_ctx* c, const b2l_plan* p, const float* d_y, int64_t
   if (rc) return rc;
   CUDA_TRY(cudaMemsetAsync(c->d_clip_max, 0, (size_t)n_clips * sizeof(unsigned int), c->stream));
   float* scratch = d_logmel;
-  // the log-mel scratch is tiled: [clip][ceil(T/64)][n_mels][64] (see dct_clamp_kernel)
+  // the log-mel scratch is tiled: [clip][ceil(T/64)][n_mels][64] (see dct_clamp4_kernel)
   if (!scratch) CUDA_TRY(cudaMalloc((void**)&scratch, (size_t)n_clips * p->n_mels * ((T + 63) / 64 * 64) * sizeof(float)));
   // mixed-radix frames (mr_kernel): the dB rows go to the scratch in the plain [clip][mel][frame] layout
   const int tiled = p->czt ? 0 : 1;
@@ -1576,18 +1501,7 @@ extern "C" int b2l_istft(b2l_ctx* c, const b2l_plan* p, const void* d_D, int64_t
   const int N = p->n_fft, M = N / 2;
   inv_op_fn op = inv_table(p->log2m);
   int variants[3];
-  int n_opt = 0;
-  {
-    const char* force = getenv("B2L_INV_VARIANT");
-    if (force && *force) {
-      variants[n_opt++] = atoi(force);
-    } else {
-      if (cfg.log2m >= 9 && cfg.log2m <= 11) variants[n_opt++] = 116;
-      int nws[2];
-      const int k = cfg.nw_options(nws);
-      for (int i = 0; i < k; ++i) variants[n_opt++] = nws[i];
-    }
-  }
+  const int n_opt = cta_variants(cfg, variants);
   InvArgs a;
   memset(&a, 0, sizeof(a));
   int variant = 0, G = 0, halves = 1;
@@ -1661,11 +1575,9 @@ extern "C" int b2l_mel_project(b2l_ctx* c, const b2l_plan* p, const float* d_S, 
   DeviceGuard g(c->device);
   const int F = p->n_fft / 2 + 1;
   {
-    // a few rows whose bands cover most of the spectrum (chroma): dense_project_kernel (B2L_DENSE_PROJECT=0: off)
-    const char* e = getenv("B2L_DENSE_PROJECT");
+    // a few rows whose bands cover most of the spectrum (chroma): dense_project_kernel
     const size_t dsmem = ((((size_t)F * 33 + 3) & ~(size_t)3) + (size_t)F * 16 + 8 * 16 * 32) * 4;
-    if (p->d_mel_wT && (long long)p->mel_w_count * 4 >= (long long)p->n_mels * F && dsmem <= c->smem_optin &&
-        !(e && *e && atoi(e) == 0)) {
+    if (p->d_mel_wT && (long long)p->mel_w_count * 4 >= (long long)p->n_mels * F && dsmem <= c->smem_optin) {
       const int r4 = (p->n_mels + 3) / 4;
       auto kern = r4 == 1 ? dense_project_kernel<1> : r4 == 2 ? dense_project_kernel<2> : r4 == 3 ? dense_project_kernel<3> : dense_project_kernel<4>;
       CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dsmem));

@@ -92,16 +92,14 @@ struct FwdArgs {
   const float* mel_w;        // padded weights of the MelRow table built for this tile geometry
   const MelRow* mel_rows;    // n_mel_rows = n_mels rounded up to a multiple of H
   int n_mel_rows;
-  const unsigned short* mel_order;   // [mel_list_len][warps per half]: k-th work item of each warp (0xffff: none)
-  int mel_list_len;
   int log_mode;              // 1: write 10*log10(max(amin, S)) - db_sub and track the per-clip max
-  int out_tiled;             // MODE_MEL: out_r is the mfcc scratch [clip][tile of 64 frames][mel][64] (dct_clamp_kernel)
+  int out_tiled;             // MODE_MEL: out_r is the mfcc scratch [clip][tile of 64 frames][mel][64] (dct_clamp4_kernel)
   float amin, db_sub;
   unsigned int* clip_max;    // order-preserving uint keys of the per-clip max (log_mode)
   int* status;               // bit 0 is set when a non-finite sample reached a frame (util.valid_audio)
   StatsParams stats;         // MODE_STATS (the frequency table travels in mel_w / mel_w_count)
   // dynamic shared-memory layout (byte offsets)
-  int off_win, off_tw, off_in, off_xbuf, off_melw, off_melband, off_melorder, off_bar;
+  int off_win, off_tw, off_in, off_xbuf, off_melw, off_melband, off_bar;
   int in_stride, xbuf_stride; // per-half strides (bytes) of the staging / exchange areas (DUAL)
   int in_floats;             // staged span length (floats)
 };

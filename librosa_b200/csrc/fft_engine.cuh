@@ -237,8 +237,6 @@ __host__ __device__ constexpr int pass0_offset(int slot) {
   constexpr int R = Cfg::radix(0), LOGR = Cfg::log_radix(0), T = Cfg::M / R;
   return Cfg::TPF * (slot / R) + bitrevc(slot % R, LOGR) * T;   // bitrevc is an involution
 }
-template <class Cfg, int SLOT>
-__host__ __device__ constexpr int pass0_offset_c() { return pass0_offset<Cfg>(SLOT); }
 template <class Cfg>
 __host__ __device__ constexpr int pass0_slot_of_pair(int c) {
   for (int s = 0; s < Cfg::PPT; ++s)
@@ -246,49 +244,18 @@ __host__ __device__ constexpr int pass0_slot_of_pair(int c) {
   return -1;
 }
 
-// ------------------------------------------------------------------ constant tables in shared memory
-// The window and the inter-pass twiddles are per-thread constants (thread t of a frame group always touches
-// the same elements), read once per frame from tables staged in shared memory.
-// Protocol: begin_window() ... window<SLOT>(t) for SLOT = 0 .. PPT-1 in increasing order;
-// begin_pass<S>() ... step<S, F>() for every F = 0 .. PPT-1 in increasing order, twiddle<S, F>(i) after the
-// step of the same F when r > 0.
-template <class Cfg>
-struct SmemTab {
-  const float* win;        // [n_fft]
-  const float2* tw;        // FftCfg::tw_offset layout
-  __device__ __forceinline__ void begin_window() {}
-  template <int SLOT>
-  __device__ __forceinline__ float2 window(int t) {
-    return *reinterpret_cast<const float2*>(win + 2 * (t + pass0_offset_c<Cfg, SLOT>()));
-  }
-  template <int S>
-  __device__ __forceinline__ void begin_pass() {}
-  template <int S, int F>
-  __device__ __forceinline__ void step() {}
-  template <int S, int F>
-  __device__ __forceinline__ float2 twiddle(int i) {
-    constexpr int R = Cfg::radix(S), p = Cfg::sublen(S), r = F % R;
-    return tw[Cfg::tw_offset(S) + (r - 1) * p + (i & (p - 1))];
-  }
-  // un-mix twiddle of bin k = t + TPF*c:  W_N^k = W_N^t * W_(2*PPT)^c  (register x compile-time constant)
-  __device__ __forceinline__ void begin_unmix() {}
-  template <int C>
-  __device__ __forceinline__ float2 unmix(float2 wt) {
-    if constexpr (C == 0) return wt;
-    else return cmul(wt, make_float2(TwC<C, 2 * Cfg::PPT>::re, TwC<C, 2 * Cfg::PPT>::im));
-  }
-};
-
 // v[] must hold the pass-0 operands (see load_pass0) and receives the spectrum:
 //   v[b*RL + q] = Z[t + TPF*b + q*pL]   (RL, pL = radix / sub-length of the last pass, b = 0 .. PPT/RL-1).
+// tw: the inter-pass twiddles in shared memory (FftCfg::tw_offset layout: per-thread constants, since thread t of a
+// frame group always touches the same elements).
 // FUSED0: the first butterfly stage of pass 0 was already done by load_pass0_windowed.
 // pre_store() runs once, right before the first write to xbuf (multi-pass schedules only): callers that share
 // the exchange area with something else (the power rows of the previous tile) synchronise there instead of
 // before the transform, so that the register-only part of pass 0 overlaps the wait.
 struct NoHook { __device__ __forceinline__ void operator()() const {} };
-template <class Cfg, bool FUSED0 = false, class Tab, class Pre = NoHook>
-__device__ __forceinline__ void fft_forward_tab(float2 (&v)[Cfg::PPT], int t, int barrier_id,
-                                                float2* __restrict__ xbuf, Tab& tab, Pre&& pre_store = Pre()) {
+template <class Cfg, bool FUSED0 = false, class Pre = NoHook>
+__device__ __forceinline__ void fft_forward(float2 (&v)[Cfg::PPT], int t, int barrier_id, float2* __restrict__ xbuf,
+                                            const float2* __restrict__ tw, Pre&& pre_store = Pre()) {
   constexpr int M = Cfg::M, TPF = Cfg::TPF, PPT = Cfg::PPT;
   static_for<0, Cfg::NPASS>([&](auto S) {
     constexpr int s = decltype(S)::value;
@@ -311,7 +278,6 @@ __device__ __forceinline__ void fft_forward_tab(float2 (&v)[Cfg::PPT], int t, in
         constexpr int r = decltype(Rr)::value;
         constexpr int slot = b * R + bitrevc(r, LOGR);
         if constexpr (s > 0) {
-          tab.template step<s, b * R + r>();
           float2 x;
           if constexpr (AFFINE_LD) {
             constexpr int D = TPF * b + r * T;
@@ -319,7 +285,7 @@ __device__ __forceinline__ void fft_forward_tab(float2 (&v)[Cfg::PPT], int t, in
           } else {
             x = xbuf[xphys(i + r * T)];
           }
-          if constexpr (r > 0) x = cmul(x, tab.template twiddle<s, b * R + r>(i));
+          if constexpr (r > 0) x = cmul(x, tw[Cfg::tw_offset(s) + (r - 1) * p + (i & (p - 1))]);
           v[slot] = x;
         }
       });
@@ -359,17 +325,9 @@ __device__ __forceinline__ void fft_forward_tab(float2 (&v)[Cfg::PPT], int t, in
           });
         });
       }
-      tab.template begin_pass<s + 1>();
       group_sync<TPF>(barrier_id);
     }
   });
-}
-// Table in shared memory, given as a bare pointer (inverse / chirp-z kernels).
-template <class Cfg>
-__device__ __forceinline__ void fft_forward(float2 (&v)[Cfg::PPT], int t, int barrier_id,
-                                            float2* __restrict__ xbuf, const float2* __restrict__ tw) {
-  SmemTab<Cfg> tab{nullptr, tw};
-  fft_forward_tab<Cfg, false>(v, t, barrier_id, xbuf, tab);
 }
 
 // Offset (index minus t) of the spectrum element held in v[slot] after fft_forward, and the inverse map

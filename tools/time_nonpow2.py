@@ -29,4 +29,4 @@ for mr in ("1", "0"):
         e0.record()
         for _ in range(10): fn().free()
         e1.record(); ctx.synchronize()
-        print(json.dumps({"what": name, "B2L_MR": mr, "lanes": os.environ.get("B2L_MR_LANES", ""), "ms": round(e0.elapsed_ms(e1) / 10, 3), "frames": 1024 * 1001}), flush=True)
+        print(json.dumps({"what": name, "B2L_MR": mr, "ms": round(e0.elapsed_ms(e1) / 10, 3), "frames": 1024 * 1001}), flush=True)
