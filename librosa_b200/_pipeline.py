@@ -175,7 +175,7 @@ def is_pow2(n: int) -> bool:
 def mr_covers(n_fft: int) -> bool:
     """True when the mixed-radix kernel (csrc/mr_kernel.cuh) takes the forward transform: even n_fft that is not a
     power of two and whose half has no prime factor above 5 (400, 320, 480, 800, 960, 1200, ...).  Mirror of
-    ``mr_factor`` in csrc/api.cu; ``B2L_MR=0`` sends these sizes back to the chirp-z kernels."""
+    ``mr_factor`` in csrc/plan.cu; ``B2L_MR=0`` sends these sizes back to the chirp-z kernels."""
     n_fft = int(n_fft)
     if is_pow2(n_fft) or n_fft < 12 or n_fft > MAX_MR_N_FFT or (n_fft & 1):
         return False

@@ -1,865 +1,47 @@
-// api.cu — C ABI of libb2l.so (see include/b2l.h): contexts, memory, plans and the launch logic for
-// the forward (stft / spectrogram / melspectrogram / mfcc) and inverse (istft) kernels.
+// api.cu — C ABI of libb2l.so (see include/b2l.h): every entry point that launches a kernel — the forward
+// (stft / spectrogram / melspectrogram / mfcc / spectral statistics) and inverse (istft) transforms and the
+// feature kernels.  The only unit that includes aux_kernels.cuh, mr_kernel.cuh and feat_kernels.cuh: they define
+// non-template kernels, whose host stubs a second including unit would define again.
 #include <cuda_runtime.h>
-#include <dlfcn.h>
 #include <math.h>
-#include <stdarg.h>
-#include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
 
 #include <algorithm>
-#include <atomic>
-#include <map>
-#include <string>
-#include <thread>
-#include <vector>
 
-#include "../../include/b2l.h"
 #include "aux_kernels.cuh"
-#include "common.cuh"
 #include "czt_kernel.cuh"
-#include "mr_kernel.cuh"
 #include "feat_kernels.cuh"
 #include "internal.h"
-#include <complex>
+#include "mr_kernel.cuh"
 
 using namespace b2l;
 
-// ------------------------------------------------------------------ errors
-static thread_local std::string g_last_error;
-
-static int fail(int code, const char* fmt, ...) {
-  char buf[1024];
-  va_list ap;
-  va_start(ap, fmt);
-  vsnprintf(buf, sizeof(buf), fmt, ap);
-  va_end(ap);
-  g_last_error = buf;
-  return code;
-}
-
-#define CUDA_TRY(expr)                                                                        \
-  do {                                                                                        \
-    cudaError_t _e = (expr);                                                                  \
-    if (_e != cudaSuccess) {                                                                  \
-      cudaGetLastError();                                                                     \
-      return fail(_e == cudaErrorMemoryAllocation ? B2L_ERR_OOM : B2L_ERR_CUDA, "%s: %s (%s:%d)", #expr, \
-                  cudaGetErrorString(_e), __FILE__, __LINE__);                                \
-    }                                                                                         \
-  } while (0)
-
-// ------------------------------------------------------------------ NCCL (loaded on demand)
-// Only the handful of entry points needed for the batch split / join; resolved from libnccl.so.2 with
-// dlopen so that single-GPU use has no NCCL dependency.
-typedef struct ncclComm* ncclComm_t;
-typedef struct { char internal[128]; } ncclUniqueId;
-typedef int ncclResult_t;
-enum { ncclChar = 0 };
-struct NcclApi {
-  void* handle = nullptr;
-  ncclResult_t (*GetUniqueId)(ncclUniqueId*) = nullptr;
-  ncclResult_t (*CommInitRank)(ncclComm_t*, int, ncclUniqueId, int) = nullptr;
-  ncclResult_t (*CommDestroy)(ncclComm_t) = nullptr;
-  ncclResult_t (*Broadcast)(const void*, void*, size_t, int, int, ncclComm_t, cudaStream_t) = nullptr;
-  ncclResult_t (*Send)(const void*, size_t, int, int, ncclComm_t, cudaStream_t) = nullptr;
-  ncclResult_t (*Recv)(void*, size_t, int, int, ncclComm_t, cudaStream_t) = nullptr;
-  ncclResult_t (*GroupStart)() = nullptr;
-  ncclResult_t (*GroupEnd)() = nullptr;
-  ncclResult_t (*AllReduce)(const void*, void*, size_t, int, int, ncclComm_t, cudaStream_t) = nullptr;
-  const char* (*GetErrorString)(ncclResult_t) = nullptr;
-};
-static NcclApi g_nccl;
-
-static int nccl_load() {
-  if (g_nccl.handle) return B2L_OK;
-  const char* names[] = {"libnccl.so.2", "libnccl.so"};
-  void* h = nullptr;
-  for (const char* n : names) {
-    h = dlopen(n, RTLD_NOW | RTLD_GLOBAL);
-    if (h) break;
-  }
-  if (!h) return fail(B2L_ERR_NCCL, "cannot dlopen libnccl.so.2: %s", dlerror());
-#define SYM(field, name)                                                       \
-  *(void**)(&g_nccl.field) = dlsym(h, name);                                   \
-  if (!g_nccl.field) return fail(B2L_ERR_NCCL, "libnccl is missing %s", name);
-  SYM(GetUniqueId, "ncclGetUniqueId")
-  SYM(CommInitRank, "ncclCommInitRank")
-  SYM(CommDestroy, "ncclCommDestroy")
-  SYM(Broadcast, "ncclBroadcast")
-  SYM(Send, "ncclSend")
-  SYM(Recv, "ncclRecv")
-  SYM(GroupStart, "ncclGroupStart")
-  SYM(GroupEnd, "ncclGroupEnd")
-  SYM(AllReduce, "ncclAllReduce")
-  SYM(GetErrorString, "ncclGetErrorString")
-#undef SYM
-  g_nccl.handle = h;
-  return B2L_OK;
-}
-#define NCCL_TRY(expr)                                                                            \
-  do {                                                                                            \
-    ncclResult_t _r = (expr);                                                                     \
-    if (_r != 0) return fail(B2L_ERR_NCCL, "%s: %s", #expr, g_nccl.GetErrorString ? g_nccl.GetErrorString(_r) : "?"); \
-  } while (0)
-
-// ------------------------------------------------------------------ objects
-struct b2l_ctx {
-  int device = 0;
-  int sm_count = 0;
-  size_t smem_optin = 0;
-  cudaStream_t stream = nullptr;
-  uint64_t launches = 0;
-  ncclComm_t comm = nullptr;
-  int rank = 0, world = 1;
-  unsigned int* d_clip_max = nullptr;   // scratch for per-clip maxima
-  int* d_status = nullptr;              // bit 0: a non-finite input sample was seen since the last reset
-  float* d_scratch = nullptr;           // grow-only scratch (chirp-z istft frames)
-  size_t scratch_bytes = 0;
-  std::map<unsigned long long, int> launch_cache;   // (kernel variant, smem) -> blocks/SM, attribute already set
-  size_t clip_max_cap = 0;
-  // pinned staging ring for uploads from pageable host memory (staged_h2d)
-  std::vector<void*> stage_bufs;
-  std::vector<cudaEvent_t> stage_evs;
-};
-
-struct b2l_event {
-  cudaEvent_t ev;
-  int device;
-};
-
-struct b2l_plan {
-  b2l_ctx* ctx = nullptr;
-  int n_fft = 0, hop = 0, center = 0, pad_mode = 0, log2m = 0;
-  float* d_win_fwd = nullptr;   // window * 1/2
-  float* d_win_inv = nullptr;   // window * 1/n_fft
-  float2* d_tw = nullptr;
-  float2* d_twn = nullptr;
-  int tw_count = 0;
-  // mel: band-sparse rows (bins [lo, lo+len) of each mel row); d_mel_w / d_band feed mel_project, the
-  // fused kernel uses a MelRow table built per tile geometry (H rows per warp step), cached here
-  int n_mels = 0, mel_w_count = 0;
-  float* d_mel_w = nullptr;
-  MelBand* d_band = nullptr;
-  float* d_mel_wT = nullptr;     // n_mels <= 16: dense transposed weights [bin][16] (dense_project_kernel)
-  std::vector<MelBand> h_band;
-  std::vector<float> h_mel_w;
-  struct RowTable { MelRow* d_rows = nullptr; float* d_w = nullptr; int n_rows = 0, w_count = 0; };
-  mutable std::map<int, RowTable> row_tables;
-  int power_mode = 2;
-  float power = 2.0f;
-  // chirp-z path for n_fft that is not a power of two (czt_kernel.cuh): transform size P = 2^log2p
-  int czt = 0, log2p = 0;
-  float2* d_czt_wb = nullptr;   // [n_fft] window * b
-  float2* d_czt_bk = nullptr;   // [1 + n_fft/2] b
-  float2* d_czt_hf = nullptr;   // [P] FFT_P(h)/P followed by the engine's inter-pass twiddles
-  float2* d_czt_bfull = nullptr;   // [n_fft] b (inverse)
-  float2* d_czt_wbi = nullptr;     // [n_fft] conj(b) * window / n_fft (inverse)
-  // mixed-radix forward path for even n_fft whose half is 5-smooth (mr_kernel.cuh); the inverse stays chirp-z
-  int mr = 0, mr_n_pass = 0, mr_tw_count = 0;
-  int mr_radix[kMrMaxPass] = {0}, mr_tw_off[kMrMaxPass] = {0};
-  float* d_mr_win = nullptr;       // [n_fft] window * 1/2
-  float* d_mr_win_inv = nullptr;   // [n_fft] window / n_fft (inverse)
-  float2* d_mr_tw = nullptr;       // pass twiddles
-  float2* d_mr_twn = nullptr;      // [n_fft/4 + 1] exp(-2 pi i k / n_fft)
-  // mfcc
-  int n_mfcc = 0;
-  float* d_dct = nullptr;
-  float amin = 1e-10f, ref_value = 1.0f, top_db = 80.0f;
-};
-
-struct DeviceGuard {
-  int prev = -1;
-  explicit DeviceGuard(int dev) {
-    cudaGetDevice(&prev);
-    if (prev != dev) cudaSetDevice(dev);
-    else prev = -1;
-  }
-  ~DeviceGuard() {
-    if (prev >= 0) cudaSetDevice(prev);
-  }
-};
-
-static size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
-
-// ------------------------------------------------------------------ glue for the other translation units
-cudaStream_t b2l_internal_stream(b2l_ctx* c) { return c->stream; }
-int b2l_internal_device(b2l_ctx* c) { return c->device; }
-int* b2l_internal_status(b2l_ctx* c) { return c->d_status; }
-size_t b2l_internal_smem_optin(b2l_ctx* c) { return c->smem_optin; }
-int b2l_internal_sm_count(b2l_ctx* c) { return c->sm_count; }
-void b2l_internal_count_launches(b2l_ctx* c, int n) { c->launches += n; }
-int b2l_internal_fail(int code, const char* fmt, ...) {
-  char buf[1024];
-  va_list ap;
-  va_start(ap, fmt);
-  vsnprintf(buf, sizeof(buf), fmt, ap);
-  va_end(ap);
-  g_last_error = buf;
-  return code;
-}
-
-// ------------------------------------------------------------------ library / device
-extern "C" int b2l_version(void) { return B2L_VERSION; }
-extern "C" const char* b2l_last_error(void) { return g_last_error.c_str(); }
-
-extern "C" int b2l_device_count(int* count) {
-  if (!count) return fail(B2L_ERR_INVALID, "count is NULL");
-  CUDA_TRY(cudaGetDeviceCount(count));
-  return B2L_OK;
-}
-
-extern "C" int b2l_ctx_create(int device, b2l_ctx** out) {
-  if (!out) return fail(B2L_ERR_INVALID, "ctx out pointer is NULL");
-  int n = 0;
-  CUDA_TRY(cudaGetDeviceCount(&n));
-  if (device < 0 || device >= n) return fail(B2L_ERR_INVALID, "device %d out of range (have %d)", device, n);
-  cudaDeviceProp prop;
-  CUDA_TRY(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 9 || prop.minor != 0)
-    return fail(B2L_ERR_UNSUPPORTED, "device %d is sm_%d%d; libb2l is built for sm_90a only (no fallback path)",
-                device, prop.major, prop.minor);
-  DeviceGuard g(device);
-  b2l_ctx* c = new b2l_ctx();
-  c->device = device;
-  c->sm_count = prop.multiProcessorCount;
-  c->smem_optin = prop.sharedMemPerBlockOptin;
-  cudaError_t e = cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking);
-  if (e == cudaSuccess) e = cudaMalloc((void**)&c->d_status, 256);
-  if (e == cudaSuccess) e = cudaMemset(c->d_status, 0, 256);
-  if (e != cudaSuccess) {
-    if (c->stream) cudaStreamDestroy(c->stream);
-    delete c;
-    return fail(B2L_ERR_CUDA, "context setup: %s", cudaGetErrorString(e));
-  }
-  *out = c;
-  return B2L_OK;
-}
-
-extern "C" int b2l_ctx_destroy(b2l_ctx* c) {
-  if (!c) return B2L_OK;
-  DeviceGuard g(c->device);
-  if (c->comm && g_nccl.CommDestroy) g_nccl.CommDestroy(c->comm);
-  if (c->d_clip_max) cudaFree(c->d_clip_max);
-  if (c->d_status) cudaFree(c->d_status);
-  if (c->d_scratch) cudaFree(c->d_scratch);
-  if (c->stream) cudaStreamSynchronize(c->stream);
-  for (void* b : c->stage_bufs) cudaFreeHost(b);
-  for (cudaEvent_t e : c->stage_evs) cudaEventDestroy(e);
-  if (c->stream) cudaStreamDestroy(c->stream);
-  delete c;
-  return B2L_OK;
-}
-
-extern "C" int b2l_ctx_sync(b2l_ctx* c) {
-  if (!c) return fail(B2L_ERR_INVALID, "ctx is NULL");
-  DeviceGuard g(c->device);
-  CUDA_TRY(cudaStreamSynchronize(c->stream));
-  return B2L_OK;
-}
-extern "C" int b2l_ctx_device(const b2l_ctx* c, int* device) {
-  if (!c || !device) return fail(B2L_ERR_INVALID, "NULL argument");
-  *device = c->device;
-  return B2L_OK;
-}
-extern "C" int b2l_ctx_sm_count(const b2l_ctx* c, int* sms) {
-  if (!c || !sms) return fail(B2L_ERR_INVALID, "NULL argument");
-  *sms = c->sm_count;
-  return B2L_OK;
-}
-extern "C" int b2l_ctx_launch_count(const b2l_ctx* c, uint64_t* launches) {
-  if (!c || !launches) return fail(B2L_ERR_INVALID, "NULL argument");
-  *launches = c->launches;
-  return B2L_OK;
-}
-
-// ------------------------------------------------------------------ device-side input validation
-extern "C" int b2l_status_reset(b2l_ctx* c) {
-  if (!c) return fail(B2L_ERR_INVALID, "ctx is NULL");
-  DeviceGuard g(c->device);
-  CUDA_TRY(cudaMemsetAsync(c->d_status, 0, sizeof(int), c->stream));
-  return B2L_OK;
-}
-extern "C" int b2l_status_read(b2l_ctx* c, int* status) {
-  if (!c || !status) return fail(B2L_ERR_INVALID, "NULL argument");
-  DeviceGuard g(c->device);
-  CUDA_TRY(cudaMemcpyAsync(status, c->d_status, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-  CUDA_TRY(cudaStreamSynchronize(c->stream));
-  return B2L_OK;
-}
-extern "C" int b2l_scan_finite(b2l_ctx* c, const float* d_y, int64_t n_clips, int64_t n, int64_t y_stride,
-                               int64_t begin) {
-  if (!c || !d_y) return fail(B2L_ERR_INVALID, "NULL argument");
-  if (n_clips <= 0 || begin >= n) return B2L_OK;
-  if (n > 0x7fffffffLL) return fail(B2L_ERR_UNSUPPORTED, "scan_finite: clips longer than 2^31-1 samples");
-  DeviceGuard g(c->device);
-  long long bx = ((n - begin) + 1023) / 1024;
-  if (bx > 64) bx = 64;
-  dim3 grid((unsigned)bx, (unsigned)(n_clips > 65535 ? 65535 : n_clips));
-  finite_scan_kernel<<<grid, 256, 0, c->stream>>>(d_y, y_stride, (int)n, (int)(begin < 0 ? 0 : begin), n_clips,
-                                                  c->d_status);
-  CUDA_TRY(cudaGetLastError());
-  c->launches++;
-  return B2L_OK;
-}
-
-// ------------------------------------------------------------------ memory
-extern "C" int b2l_alloc(b2l_ctx* c, size_t bytes, void** d_ptr) {
-  if (!c || !d_ptr) return fail(B2L_ERR_INVALID, "NULL argument");
-  DeviceGuard g(c->device);
-  *d_ptr = nullptr;
-  if (bytes == 0) bytes = 16;
-  CUDA_TRY(cudaMalloc(d_ptr, bytes));
-  return B2L_OK;
-}
-extern "C" int b2l_free(b2l_ctx* c, void* d_ptr) {
-  if (!c) return fail(B2L_ERR_INVALID, "ctx is NULL");
-  if (!d_ptr) return B2L_OK;
-  DeviceGuard g(c->device);
-  CUDA_TRY(cudaStreamSynchronize(c->stream));
-  CUDA_TRY(cudaFree(d_ptr));
-  return B2L_OK;
-}
-extern "C" int b2l_memset(b2l_ctx* c, void* d_ptr, int value, size_t bytes) {
-  if (!c) return fail(B2L_ERR_INVALID, "ctx is NULL");
-  DeviceGuard g(c->device);
-  CUDA_TRY(cudaMemsetAsync(d_ptr, value, bytes, c->stream));
-  return B2L_OK;
-}
-// Upload from PAGEABLE host memory (what a drop-in caller's ndarray is): cudaMemcpyAsync would stage it through
-// the driver's single bounce buffer on the calling thread (10-20 GB/s).  Instead `nthreads` host threads copy
-// 4 MB pieces into a ring of pinned buffers (two per thread) and enqueue the DMA of each piece on the context's
-// stream as soon as it is staged, so the host-side copies run in parallel and overlap the PCIe transfer.
-// Piece order on the stream is arbitrary (the pieces are disjoint); work enqueued after the call returns is
-// ordered behind all of them.
-static const size_t kStagePiece = 4u << 20;
-static int staged_h2d(b2l_ctx* c, char* d_dst, const char* h_src, size_t bytes, int nthreads) {
-  const size_t want = 2 * (size_t)nthreads;
-  while (c->stage_bufs.size() < want) {
-    void* b = nullptr;
-    CUDA_TRY(cudaHostAlloc(&b, kStagePiece, cudaHostAllocPortable));
-    c->stage_bufs.push_back(b);
-    cudaEvent_t e;
-    CUDA_TRY(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-    c->stage_evs.push_back(e);
-  }
-  std::atomic<size_t> next(0);
-  std::atomic<int> err(0);
-  auto worker = [&](int w) {
-    cudaSetDevice(c->device);
-    for (int k = 0;; ++k) {
-      const size_t off = next.fetch_add(1) * kStagePiece;
-      if (off >= bytes || err.load()) break;
-      const size_t len = std::min(kStagePiece, bytes - off);
-      const int b = 2 * w + (k & 1);
-      cudaError_t e = cudaEventSynchronize(c->stage_evs[b]);   // the DMA that last used this buffer is done
-      if (e == cudaSuccess) {
-        memcpy(c->stage_bufs[b], h_src + off, len);
-        e = cudaMemcpyAsync(d_dst + off, c->stage_bufs[b], len, cudaMemcpyHostToDevice, c->stream);
-      }
-      if (e == cudaSuccess) e = cudaEventRecord(c->stage_evs[b], c->stream);
-      if (e != cudaSuccess) err.store((int)e);
-    }
-  };
-  std::vector<std::thread> pool;
-  for (int w = 1; w < nthreads; ++w) pool.emplace_back(worker, w);
-  worker(0);
-  for (auto& t : pool) t.join();
-  if (err.load()) {
-    cudaGetLastError();
-    return fail(B2L_ERR_CUDA, "staged upload: %s", cudaGetErrorString((cudaError_t)err.load()));
-  }
-  return B2L_OK;
-}
-
-extern "C" int b2l_h2d(b2l_ctx* c, void* d_dst, const void* h_src, size_t bytes) {
-  if (!c) return fail(B2L_ERR_INVALID, "ctx is NULL");
-  DeviceGuard g(c->device);
-  if (bytes >= (16u << 20)) {
-    static int threads = -1;   // B2L_H2D_THREADS: staging threads for pageable sources (0 = plain cudaMemcpyAsync)
-    if (threads < 0) {
-      const char* e = getenv("B2L_H2D_THREADS");
-      threads = e && *e ? atoi(e) : 6;
-      if (threads > 32) threads = 32;
-    }
-    cudaPointerAttributes attr;
-    if (threads > 0 && cudaPointerGetAttributes(&attr, h_src) == cudaSuccess && attr.type == cudaMemoryTypeUnregistered)
-      return staged_h2d(c, (char*)d_dst, (const char*)h_src, bytes, threads);
-    cudaGetLastError();
-  }
-  CUDA_TRY(cudaMemcpyAsync(d_dst, h_src, bytes, cudaMemcpyHostToDevice, c->stream));
-  return B2L_OK;
-}
-extern "C" int b2l_d2h(b2l_ctx* c, void* h_dst, const void* d_src, size_t bytes) {
-  if (!c) return fail(B2L_ERR_INVALID, "ctx is NULL");
-  DeviceGuard g(c->device);
-  CUDA_TRY(cudaMemcpyAsync(h_dst, d_src, bytes, cudaMemcpyDeviceToHost, c->stream));
-  return B2L_OK;
-}
-extern "C" int b2l_d2d(b2l_ctx* c, void* d_dst, const void* d_src, size_t bytes) {
-  if (!c) return fail(B2L_ERR_INVALID, "ctx is NULL");
-  DeviceGuard g(c->device);
-  CUDA_TRY(cudaMemcpyAsync(d_dst, d_src, bytes, cudaMemcpyDeviceToDevice, c->stream));
-  return B2L_OK;
-}
-extern "C" int b2l_copy2d(b2l_ctx* c, void* d_dst, size_t dst_pitch, const void* d_src, size_t src_pitch,
-                          size_t width_bytes, size_t rows) {
-  if (!c || !d_dst || !d_src) return fail(B2L_ERR_INVALID, "NULL argument");
-  if (width_bytes == 0 || rows == 0) return B2L_OK;
-  if (dst_pitch < width_bytes || src_pitch < width_bytes) return fail(B2L_ERR_INVALID, "pitch smaller than the row width");
-  DeviceGuard g(c->device);
-  CUDA_TRY(cudaMemcpy2DAsync(d_dst, dst_pitch, d_src, src_pitch, width_bytes, rows, cudaMemcpyDeviceToDevice, c->stream));
-  return B2L_OK;
-}
-extern "C" int b2l_host_alloc(size_t bytes, void** h_ptr) {
-  if (!h_ptr) return fail(B2L_ERR_INVALID, "NULL argument");
-  if (bytes == 0) bytes = 16;
-  CUDA_TRY(cudaHostAlloc(h_ptr, bytes, cudaHostAllocPortable));
-  return B2L_OK;
-}
-extern "C" int b2l_host_free(void* h_ptr) {
-  if (!h_ptr) return B2L_OK;
-  CUDA_TRY(cudaFreeHost(h_ptr));
-  return B2L_OK;
-}
-extern "C" int b2l_mem_info(b2l_ctx* c, size_t* free_bytes, size_t* total_bytes) {
-  if (!c || !free_bytes || !total_bytes) return fail(B2L_ERR_INVALID, "NULL argument");
-  DeviceGuard g(c->device);
-  CUDA_TRY(cudaMemGetInfo(free_bytes, total_bytes));
-  return B2L_OK;
-}
-
-// ------------------------------------------------------------------ events
-extern "C" int b2l_event_create(b2l_ctx* c, b2l_event** ev) {
-  if (!c || !ev) return fail(B2L_ERR_INVALID, "NULL argument");
-  DeviceGuard g(c->device);
-  b2l_event* e = new b2l_event();
-  e->device = c->device;
-  cudaError_t r = cudaEventCreate(&e->ev);
-  if (r != cudaSuccess) {
-    delete e;
-    return fail(B2L_ERR_CUDA, "cudaEventCreate: %s", cudaGetErrorString(r));
-  }
-  *ev = e;
-  return B2L_OK;
-}
-extern "C" int b2l_event_record(b2l_ctx* c, b2l_event* ev) {
-  if (!c || !ev) return fail(B2L_ERR_INVALID, "NULL argument");
-  DeviceGuard g(c->device);
-  CUDA_TRY(cudaEventRecord(ev->ev, c->stream));
-  return B2L_OK;
-}
-extern "C" int b2l_event_elapsed_ms(b2l_event* start, b2l_event* stop, float* ms) {
-  if (!start || !stop || !ms) return fail(B2L_ERR_INVALID, "NULL argument");
-  DeviceGuard g(stop->device);
-  CUDA_TRY(cudaEventSynchronize(stop->ev));
-  CUDA_TRY(cudaEventElapsedTime(ms, start->ev, stop->ev));
-  return B2L_OK;
-}
-extern "C" int b2l_event_destroy(b2l_event* ev) {
-  if (!ev) return B2L_OK;
-  DeviceGuard g(ev->device);
-  cudaEventDestroy(ev->ev);
-  delete ev;
-  return B2L_OK;
-}
-
-// ------------------------------------------------------------------ plans
-static int ilog2_exact(int x) {
-  int l = 0;
-  while ((1 << l) < x) ++l;
-  return (1 << l) == x ? l : -1;
-}
-
-template <class T>
-static int upload(b2l_ctx* c, const std::vector<T>& h, T** d) {
-  *d = nullptr;
-  size_t bytes = h.size() * sizeof(T);
-  CUDA_TRY(cudaMalloc((void**)d, bytes ? bytes : 16));
-  if (bytes) CUDA_TRY(cudaMemcpy(*d, h.data(), bytes, cudaMemcpyHostToDevice));
-  return B2L_OK;
-}
-
-// inter-pass twiddles of the register FFT for a complex size 2^log2m (FftCfg::tw_offset layout)
-static std::vector<float2> engine_twiddles(const HostFftCfg& cfg) {
-  const double two_pi = 6.283185307179586476925286766559;
-  std::vector<float2> tw((size_t)cfg.tw_count());
-  for (int s = 1; s < cfg.npass; ++s) {
-    const int R = cfg.radix(s), pl = cfg.sublen(s), off = cfg.tw_offset(s);
-    for (int r = 1; r < R; ++r)
-      for (int k = 0; k < pl; ++k) {
-        // exp(-2*pi*i * r*k / (p*R)); reduce the integer phase first to keep the argument small
-        long long num = ((long long)r * k) % ((long long)pl * R);
-        double ang = -two_pi * (double)num / (double)((long long)pl * R);
-        tw[(size_t)off + (size_t)(r - 1) * pl + k] = make_float2((float)cos(ang), (float)sin(ang));
-      }
-  }
-  return tw;
-}
-
-// in-place radix-2 FFT in double precision (host, plan construction only)
-static void host_fft(std::vector<std::complex<double>>& x) {
-  const size_t n = x.size();
-  for (size_t i = 1, j = 0; i < n; ++i) {
-    size_t bit = n >> 1;
-    for (; j & bit; bit >>= 1) j ^= bit;
-    j ^= bit;
-    if (i < j) std::swap(x[i], x[j]);
-  }
-  const double pi = 3.14159265358979323846264338327950288;
-  for (size_t len = 2; len <= n; len <<= 1) {
-    for (size_t i = 0; i < n; i += len)
-      for (size_t k = 0; k < len / 2; ++k) {
-        const double ang = -2.0 * pi * (double)k / (double)len;
-        const std::complex<double> w(cos(ang), sin(ang));
-        const std::complex<double> u = x[i + k], v = x[i + k + len / 2] * w;
-        x[i + k] = u + v;
-        x[i + k + len / 2] = u - v;
-      }
-  }
-}
-
-extern "C" int b2l_plan_destroy(b2l_plan* p) {
-  if (!p) return B2L_OK;
-  DeviceGuard g(p->ctx->device);
-  cudaStreamSynchronize(p->ctx->stream);
-  cudaFree(p->d_win_fwd);
-  cudaFree(p->d_win_inv);
-  cudaFree(p->d_tw);
-  cudaFree(p->d_twn);
-  cudaFree(p->d_mel_w);
-  cudaFree(p->d_mel_wT);
-  cudaFree(p->d_czt_wb);
-  cudaFree(p->d_czt_bk);
-  cudaFree(p->d_czt_hf);
-  cudaFree(p->d_czt_bfull);
-  cudaFree(p->d_czt_wbi);
-  cudaFree(p->d_mr_win);
-  cudaFree(p->d_mr_win_inv);
-  cudaFree(p->d_mr_tw);
-  cudaFree(p->d_mr_twn);
-  cudaFree(p->d_band);
-  for (auto& kv : p->row_tables) {
-    cudaFree(kv.second.d_rows);
-    cudaFree(kv.second.d_w);
-  }
-  cudaFree(p->d_dct);
-  delete p;
-  return B2L_OK;
-}
-
-// Radix schedule of the mixed-radix kernel for n_fft = 2 M: M = 5^c 3^b 2^a as c fives, b threes, then eights and a
-// four / two.  False when n_fft is odd, M has another prime factor, or the schedule / buffers would not fit.
-static bool mr_factor(int n_fft, std::vector<int>& radices) {
-  radices.clear();
-  if (n_fft < 12 || (n_fft & 1) || n_fft > 4096) return false;
-  int m = n_fft / 2;
-  while (m % 5 == 0) { radices.push_back(5); m /= 5; }
-  while (m % 3 == 0) { radices.push_back(3); m /= 3; }
-  while (m % 8 == 0) { radices.push_back(8); m /= 8; }
-  if (m % 4 == 0) { radices.push_back(4); m /= 4; }
-  if (m % 2 == 0) { radices.push_back(2); m /= 2; }
-  return m == 1 && (int)radices.size() <= kMrMaxPass && !radices.empty();
-}
-
-extern "C" int b2l_plan_create(b2l_ctx* c, const b2l_plan_desc* d, b2l_plan** out) {
-  if (!c || !d || !out) return fail(B2L_ERR_INVALID, "NULL argument");
-  if (d->n_fft < 1) return fail(B2L_ERR_INVALID, "n_fft=%d must be positive", d->n_fft);
-  if (d->hop_length < 1) return fail(B2L_ERR_INVALID, "hop_length=%d must be a positive integer", d->hop_length);
-  int l2n = ilog2_exact(d->n_fft);
-  int czt_log2p = 0;
-  if (l2n < 0) {
-    // not a power of two: Bluestein with P = next power of two >= 2*n_fft - 1 (czt_kernel.cuh)
-    while ((1 << czt_log2p) < 2 * d->n_fft - 1) ++czt_log2p;
-    if (czt_log2p < 5) czt_log2p = 5;
-    std::vector<int> probe;
-    if (d->n_fft < 3 || (czt_log2p > 12 && !mr_factor(d->n_fft, probe)))
-      return fail(B2L_ERR_UNSUPPORTED,
-                  "n_fft=%d: non-power-of-two sizes are supported from 3 to 2047, and even sizes up to 4096 whose half "
-                  "has no prime factor above 5 (no CPU fallback)", d->n_fft);
-  } else if (l2n - 1 < kMinLog2M || l2n - 1 > kMaxLog2M) {
-    return fail(B2L_ERR_UNSUPPORTED,
-                "n_fft=%d: the sm_90a kernels are built for powers of two from %d to %d (no CPU fallback)",
-                d->n_fft, 2 << kMinLog2M, 2 << kMaxLog2M);
-  }
-  if (!d->h_window) return fail(B2L_ERR_INVALID, "window is NULL");
-  if (d->pad_mode < 0 || d->pad_mode > B2L_PAD_EMPTY) return fail(B2L_ERR_INVALID, "bad pad_mode %d", d->pad_mode);
-  if (d->n_mels < 0 || d->n_mfcc < 0) return fail(B2L_ERR_INVALID, "negative n_mels / n_mfcc");
-  if (d->n_mels > 0 && !d->h_mel_basis) return fail(B2L_ERR_INVALID, "mel basis is NULL");
-  if (d->n_mfcc > 0 && (!d->h_dct_basis || d->n_mels == 0))
-    return fail(B2L_ERR_INVALID, "mfcc stage needs a mel stage and a DCT basis");
-  if (d->n_mfcc > 0 && !(d->amin > 0.0f)) return fail(B2L_ERR_INVALID, "amin must be strictly positive");
-
-  DeviceGuard g(c->device);
-  b2l_plan* p = new b2l_plan();
-  p->ctx = c;
-  p->n_fft = d->n_fft;
-  p->hop = d->hop_length;
-  p->center = d->center ? 1 : 0;
-  p->pad_mode = d->pad_mode;
-  p->log2m = l2n - 1;
-  p->power = d->power;
-  p->power_mode = d->power == 2.0f ? 2 : (d->power == 1.0f ? 1 : 0);
-  p->amin = d->amin;
-  p->ref_value = d->ref_value;
-  p->top_db = d->top_db;
-  const int N = d->n_fft, M = N / 2;
-  int rc = B2L_OK;
-  if (l2n < 0) {
-    // ---- chirp-z tables (double precision on the host)
-    p->czt = 1;
-    p->log2p = czt_log2p;
-    p->log2m = -1;
-    const int L = N, P = 1 << czt_log2p;
-    const double pi = 3.14159265358979323846264338327950288;
-    if (czt_log2p > 12) p->log2p = 0;   // beyond the chirp-z range: the mixed-radix kernels alone serve this size
-    if (czt_log2p <= 12) {
-    std::vector<std::complex<double>> b(L);
-    for (int n = 0; n < L; ++n) {
-      const long long q = ((long long)n * n) % (2LL * L);          // n^2 mod 2L keeps the phase exact
-      const double ang = -pi * (double)q / (double)L;
-      b[n] = std::complex<double>(cos(ang), sin(ang));
-    }
-    std::vector<float2> wb(L), bk(L / 2 + 1);
-    for (int n = 0; n < L; ++n) {
-      const std::complex<double> z = d->h_window[n] * b[n];
-      wb[n] = make_float2((float)z.real(), (float)z.imag());
-    }
-    for (int k = 0; k <= L / 2; ++k) bk[k] = make_float2((float)b[k].real(), (float)b[k].imag());
-    std::vector<std::complex<double>> h(P, std::complex<double>(0.0, 0.0));
-    h[0] = std::conj(b[0]);
-    for (int m = 1; m < L; ++m) h[m] = h[P - m] = std::conj(b[m]);
-    host_fft(h);
-    HostFftCfg ccfg(czt_log2p);
-    std::vector<float2> hf((size_t)P);
-    for (int i = 0; i < P; ++i) hf[i] = make_float2((float)(h[i].real() / P), (float)(h[i].imag() / P));
-    std::vector<float2> tw = engine_twiddles(ccfg);
-    hf.insert(hf.end(), tw.begin(), tw.end());
-    std::vector<float2> bfull(L), wbi(L);
-    for (int n = 0; n < L; ++n) {
-      bfull[n] = make_float2((float)b[n].real(), (float)b[n].imag());
-      const std::complex<double> z = std::conj(b[n]) * (d->h_window[n] / (double)L);
-      wbi[n] = make_float2((float)z.real(), (float)z.imag());
-    }
-    if ((rc = upload(c, wb, &p->d_czt_wb)) || (rc = upload(c, bk, &p->d_czt_bk)) || (rc = upload(c, hf, &p->d_czt_hf)) ||
-        (rc = upload(c, bfull, &p->d_czt_bfull)) || (rc = upload(c, wbi, &p->d_czt_wbi)))
-      goto bad;
-    }
-    // ---- mixed-radix tables when n_fft = 2 M with M = 2^a 3^b 5^c (odd radices first, see mr_kernel.cuh)
-    {
-      std::vector<int> radices;
-      if (mr_factor(N, radices)) {
-        p->mr = 1;
-        p->mr_n_pass = (int)radices.size();
-        std::vector<float2> tw;
-        int sub = 1;
-        for (int s = 0; s < p->mr_n_pass; ++s) {
-          const int R = radices[s];
-          p->mr_radix[s] = R;
-          p->mr_tw_off[s] = (int)tw.size();
-          if (sub > 1)
-            for (int r = 1; r < R; ++r)
-              for (int k = 0; k < sub; ++k) {
-                const long long num = ((long long)r * k) % ((long long)sub * R);
-                const double ang = -2.0 * pi * (double)num / (double)((long long)sub * R);
-                tw.push_back(make_float2((float)cos(ang), (float)sin(ang)));
-              }
-          sub *= R;
-        }
-        if (tw.empty()) tw.push_back(make_float2(1.0f, 0.0f));
-        p->mr_tw_count = (int)tw.size();
-        std::vector<float> wf(N), wi(N);
-        for (int i = 0; i < N; ++i) {
-          wf[i] = (float)(d->h_window[i] * 0.5);
-          wi[i] = (float)(d->h_window[i] / (double)N);
-        }
-        std::vector<float2> twn((size_t)M / 2 + 1);
-        for (int k = 0; k <= M / 2; ++k) {
-          const double ang = -2.0 * pi * (double)k / (double)N;
-          twn[k] = make_float2((float)cos(ang), (float)sin(ang));
-        }
-        if ((rc = upload(c, wf, &p->d_mr_win)) || (rc = upload(c, wi, &p->d_mr_win_inv)) || (rc = upload(c, tw, &p->d_mr_tw)) ||
-            (rc = upload(c, twn, &p->d_mr_twn)))
-          goto bad;
-      }
-    }
-  } else {
-    HostFftCfg cfg(p->log2m);
-    {
-      std::vector<float> wf(N), wi(N);
-      for (int i = 0; i < N; ++i) {
-        wf[i] = (float)(d->h_window[i] * 0.5);
-        wi[i] = (float)(d->h_window[i] / (double)N);
-      }
-      if ((rc = upload(c, wf, &p->d_win_fwd)) || (rc = upload(c, wi, &p->d_win_inv))) goto bad;
-    }
-    {
-      const double two_pi = 6.283185307179586476925286766559;
-      std::vector<float2> tw = engine_twiddles(cfg);
-      p->tw_count = cfg.tw_count();
-      std::vector<float2> twn((size_t)M / 2 + 1);
-      for (int k = 0; k <= M / 2; ++k) {
-        double ang = -two_pi * (double)k / (double)N;
-        twn[k] = make_float2((float)cos(ang), (float)sin(ang));
-      }
-      if ((rc = upload(c, tw, &p->d_tw)) || (rc = upload(c, twn, &p->d_twn))) goto bad;
-    }
-  }
-  if (d->n_mels > 0) {
-    const int F = M + 1;
-    std::vector<MelBand> bands(d->n_mels);
-    std::vector<float> w;
-    for (int m = 0; m < d->n_mels; ++m) {
-      const float* row = d->h_mel_basis + (size_t)m * F;
-      int lo = -1, hi = -1;
-      for (int k = 0; k < F; ++k)
-        if (row[k] != 0.0f) {
-          if (lo < 0) lo = k;
-          hi = k;
-        }
-      MelBand b;
-      b.off = (int)w.size();
-      b.pad = 0;
-      if (lo < 0) {
-        b.lo = 0;
-        b.len = 0;
-      } else {
-        b.lo = lo;
-        b.len = hi - lo + 1;
-        w.insert(w.end(), row + lo, row + hi + 1);
-      }
-      bands[m] = b;
-    }
-    p->n_mels = d->n_mels;
-    p->mel_w_count = (int)w.size();
-    p->h_band = bands;
-    p->h_mel_w = w;
-    if ((rc = upload(c, w, &p->d_mel_w)) || (rc = upload(c, bands, &p->d_band))) goto bad;
-    if (d->n_mels <= 16) {
-      std::vector<float> wT((size_t)F * 16, 0.0f);
-      for (int m = 0; m < d->n_mels; ++m)
-        for (int k = 0; k < F; ++k) wT[(size_t)k * 16 + m] = d->h_mel_basis[(size_t)m * F + k];
-      if ((rc = upload(c, wT, &p->d_mel_wT))) goto bad;
-    }
-  }
-  if (d->n_mfcc > 0) {
-    // transposed and zero padded to 8-coefficient groups: dctT[m][8*KG] (dct_clamp4_kernel)
-    const int KP = (d->n_mfcc + 7) / 8 * 8;
-    std::vector<float> dct((size_t)d->n_mels * KP, 0.0f);
-    for (int k = 0; k < d->n_mfcc; ++k)
-      for (int m = 0; m < d->n_mels; ++m) dct[(size_t)m * KP + k] = d->h_dct_basis[(size_t)k * d->n_mels + m];
-    p->n_mfcc = d->n_mfcc;
-    if ((rc = upload(c, dct, &p->d_dct))) goto bad;
-  }
-  *out = p;
-  return B2L_OK;
-bad:
-  b2l_plan_destroy(p);
-  return rc;
-}
-
-static long long plan_frames(const b2l_plan* p, long long n) {
-  long long padded = n + (p->center ? 2LL * (p->n_fft / 2) : 0);
-  if (padded < p->n_fft) return 0;
-  return 1 + (padded - p->n_fft) / p->hop;
-}
-
-extern "C" int b2l_plan_n_frames(const b2l_plan* p, int64_t n, int64_t* n_frames) {
-  if (!p || !n_frames) return fail(B2L_ERR_INVALID, "NULL argument");
-  *n_frames = plan_frames(p, n);
-  return B2L_OK;
-}
-
-// ------------------------------------------------------------------ forward launches
-typedef cudaError_t (*fwd_op_fn)(int, int, int, const FwdArgs*, int, size_t, cudaStream_t, int*);
-typedef cudaError_t (*inv_op_fn)(int, int, const InvArgs*, int, size_t, cudaStream_t, int*);
-static fwd_op_fn fwd_table(int log2m) {
-  switch (log2m) {
-    case 2: return fwd_op_2; case 3: return fwd_op_3; case 4: return fwd_op_4; case 5: return fwd_op_5;
-    case 6: return fwd_op_6; case 7: return fwd_op_7; case 8: return fwd_op_8; case 9: return fwd_op_9;
-    case 10: return fwd_op_10; case 11: return fwd_op_11; case 12: return fwd_op_12;
-  }
+// ------------------------------------------------------------------ per-size kernels (fwd_inst.cu, inv_inst.cu, czt_inst.cu)
+#define B2L_CASE(L) case L: return fwd_kernel_##L(variant, mode);
+static FwdKernel fwd_kernel_for(int log2m, int variant, int mode) {
+  switch (log2m) { B2L_FFT_SIZES(B2L_CASE) }
   return nullptr;
 }
-static inv_op_fn inv_table(int log2m) {
-  switch (log2m) {
-    case 2: return inv_op_2; case 3: return inv_op_3; case 4: return inv_op_4; case 5: return inv_op_5;
-    case 6: return inv_op_6; case 7: return inv_op_7; case 8: return inv_op_8; case 9: return inv_op_9;
-    case 10: return inv_op_10; case 11: return inv_op_11; case 12: return inv_op_12;
-  }
+#undef B2L_CASE
+#define B2L_CASE(L) case L: return inv_kernel_##L(variant);
+static InvKernel inv_kernel_for(int log2m, int variant) {
+  switch (log2m) { B2L_FFT_SIZES(B2L_CASE) }
   return nullptr;
 }
-
-static int ensure_clip_max(b2l_ctx* c, size_t n_clips) {
-  if (c->clip_max_cap < n_clips) {
-    if (c->d_clip_max) {
-      CUDA_TRY(cudaStreamSynchronize(c->stream));
-      CUDA_TRY(cudaFree(c->d_clip_max));
-      c->d_clip_max = nullptr;
-      c->clip_max_cap = 0;
-    }
-    size_t cap = n_clips < 1024 ? 1024 : n_clips;
-    CUDA_TRY(cudaMalloc((void**)&c->d_clip_max, cap * sizeof(unsigned int)));
-    c->clip_max_cap = cap;
-  }
-  return B2L_OK;
+#undef B2L_CASE
+#define B2L_CASE(L) case L: return czt_kernel_##L();
+static CztKernel czt_kernel_for(int log2p) {
+  switch (log2p) { B2L_CZT_SIZES(B2L_CASE) }
+  return nullptr;
 }
-
-// MelRow table for warps that process H mel rows at a time (see MelRow / MelLayout in common.cuh).
-static int get_row_table(b2l_ctx* c, const b2l_plan* p, int H, const b2l_plan::RowTable** out) {
-  const int key = H;
-  auto it = p->row_tables.find(key);
-  if (it != p->row_tables.end()) {
-    *out = &it->second;
-    return B2L_OK;
-  }
-  const int rsm = H < 4 ? 4 : H, G = rsm / 4;   // row starts: lo_j == 4*(j mod G) (mod rsm)
-  const int n_rows = (p->n_mels + H - 1) / H * H;
-  const int n_items = n_rows / H;
-  std::vector<MelRow> rows(n_rows);
-  std::vector<float> w;
-  for (int item = 0; item < n_items; ++item) {
-    std::vector<int> start(H), lenp(H);
-    int quads = 0;
-    for (int j = 0; j < H; ++j) {
-      const int m = item * H + j;
-      if (m < p->n_mels && p->h_band[m].len > 0) {
-        const MelBand& b = p->h_band[m];
-        const int want = 4 * (j % G);
-        int st = b.lo - ((((b.lo - want) % rsm) + rsm) % rsm);   // largest bin <= lo congruent to `want` mod rsm
-        if (st < 0) st = b.lo - (b.lo % 4);                       // lowest rows: keep the 16-byte alignment only
-        start[j] = st;
-        lenp[j] = b.lo + b.len - st;
-      } else {
-        start[j] = 4 * (j % G);
-        lenp[j] = 0;
-      }
-      quads = std::max(quads, (lenp[j] + 3) / 4);
-    }
-    for (int j = 0; j < H; ++j) {
-      const int m = item * H + j;
-      MelRow r;
-      r.lo = (unsigned short)start[j];
-      r.quads = (unsigned short)quads;
-      r.off = (unsigned int)w.size();
-      size_t base = w.size();
-      w.resize(base + (size_t)4 * quads, 0.0f);
-      if (lenp[j] > 0) {
-        const MelBand& b = p->h_band[m];
-        for (int i = 0; i < b.len; ++i) w[base + (b.lo - start[j]) + i] = p->h_mel_w[b.off + i];
-      }
-      rows[m] = r;
-    }
-  }
-  b2l_plan::RowTable t;
-  t.n_rows = n_rows;
-  t.w_count = (int)w.size();
-  int rc;
-  if ((rc = upload(c, rows, &t.d_rows)) || (rc = upload(c, w, &t.d_w))) return rc;
-  auto ins = p->row_tables.emplace(key, t);
-  *out = &ins.first->second;
-  return B2L_OK;
+#undef B2L_CASE
+#define B2L_CASE(L) case L: return czt_inv_kernel_##L();
+static CztInvKernel czt_inv_kernel_for(int log2p) {
+  switch (log2p) { B2L_CZT_SIZES(B2L_CASE) }
+  return nullptr;
 }
+#undef B2L_CASE
 
 // CTA variants of the forward and inverse kernels, tried in order (first that fits shared memory wins):
 // 116 = 16 warps as two independent 8-warp halves, 16 / 8 = plain CTAs.
@@ -871,27 +53,59 @@ static int cta_variants(const HostFftCfg& cfg, int out[3]) {
   for (int i = 0; i < k; ++i) out[n++] = nws[i];
   return n;
 }
+static int variant_threads(int variant) { return variant == 116 ? 512 : variant * 32; }
+
+// ------------------------------------------------------------------ which kernels serve a plan
+enum Path { PATH_POW2, PATH_MR, PATH_CZT, PATH_NONE };
+enum Entry {
+  ENTRY_SPECTRUM,   // stft, spectrogram, istft
+  ENTRY_MEL,        // melspectrogram, mfcc
+  ENTRY_STATS,      // spectral_stats
+};
+// B2L_MR=0 sends the spectrum entry points of the mixed-radix sizes back to the chirp-z kernels where those exist
+// (n_fft <= 2047).  Read on every call: a plan outlives changes of the environment.
+static bool mr_enabled(const b2l_plan* p) {
+  if (p->log2p == 0) return true;   // no chirp-z tables for this size
+  const char* e = getenv("B2L_MR");
+  return !(e && *e) || atoi(e) != 0;
+}
+static Path route(const b2l_plan* p, Entry entry) {
+  if (!p->czt) return PATH_POW2;
+  switch (entry) {
+    case ENTRY_SPECTRUM: return p->mr && mr_enabled(p) ? PATH_MR : PATH_CZT;
+    case ENTRY_MEL: return p->mr ? PATH_MR : PATH_NONE;   // B2L_MR does not apply here
+    default: return PATH_NONE;
+  }
+}
+
+// ------------------------------------------------------------------ forward launches
+// The checks the forward paths share, in order: plan ownership, clip geometry, signal length, then the device
+// pointers of a non-empty batch.  *T: frames per clip, 0 for an empty batch (nothing to launch).
+static int frame_count(b2l_ctx* c, const b2l_plan* p, int64_t n_clips, int64_t n, int64_t y_stride, const float* d_y,
+                       const void* d_out, long long* T) {
+  if (p->ctx != c) return fail(B2L_ERR_INVALID, "plan belongs to another context");
+  if (n_clips < 0 || n < 0 || y_stride < n) return fail(B2L_ERR_INVALID, "bad clip geometry");
+  if (n > 0x7fffffffLL) return fail(B2L_ERR_UNSUPPORTED, "clips longer than 2^31-1 samples are not supported");
+  *T = plan_frames(p, n);
+  if (*T <= 0)
+    return fail(B2L_ERR_INVALID, "n_fft=%d is too large for input signal of length=%lld", p->n_fft, (long long)n);
+  if (n_clips == 0) *T = 0;
+  else if (!d_y || !d_out) return fail(B2L_ERR_INVALID, "NULL device pointer");
+  return B2L_OK;
+}
 
 struct StatsCall { StatsParams sp; const float* d_freq; };
 
 static int run_forward(b2l_ctx* c, const b2l_plan* p, int mode, int log_mode, const float* d_y, int64_t n_clips,
                        int64_t n, int64_t y_stride, float2* out_c, float* out_r, const StatsCall* stats = nullptr) {
-  if (!c || !p) return fail(B2L_ERR_INVALID, "NULL ctx / plan");
-  if (p->ctx != c) return fail(B2L_ERR_INVALID, "plan belongs to another context");
-  if (n_clips < 0 || n < 0 || y_stride < n) return fail(B2L_ERR_INVALID, "bad clip geometry");
-  if (n > 0x7fffffffLL) return fail(B2L_ERR_UNSUPPORTED, "clips longer than 2^31-1 samples are not supported");
-  const long long T = plan_frames(p, n);
-  if (T <= 0)
-    return fail(B2L_ERR_INVALID, "n_fft=%d is too large for input signal of length=%lld", p->n_fft, (long long)n);
-  if (n_clips == 0) return B2L_OK;
-  if (!d_y || (mode == MODE_STFT ? (void*)out_c : (void*)out_r) == nullptr)
-    return fail(B2L_ERR_INVALID, "NULL device pointer");
+  long long T = 0;
+  int rc = frame_count(c, p, n_clips, n, y_stride, d_y, mode == MODE_STFT ? (void*)out_c : (void*)out_r, &T);
+  if (rc || T == 0) return rc;
   if (mode == MODE_MEL && p->n_mels == 0) return fail(B2L_ERR_INVALID, "plan has no mel stage");
   DeviceGuard g(c->device);
 
   HostFftCfg cfg(p->log2m);
   const int N = p->n_fft, M = N / 2;
-  fwd_op_fn op = fwd_table(p->log2m);
   int variants[3];
   const int n_opt = cta_variants(cfg, variants);
   FwdArgs a;
@@ -910,7 +124,7 @@ static int run_forward(b2l_ctx* c, const b2l_plan* p, int mode, int log_mode, co
     if (span > 0x3fffffff) continue;
     const b2l_plan::RowTable* t = nullptr;
     if (mode == MODE_MEL) {
-      int rc = get_row_table(c, p, mel_rows_per_warp(f), &t);
+      rc = get_row_table(p, mel_rows_per_warp(f), &t);
       if (rc) return rc;
     }
     size_t off = 0;
@@ -990,60 +204,32 @@ static int run_forward(b2l_ctx* c, const b2l_plan* p, int mode, int log_mode, co
   a.clip_max = c->d_clip_max;
   a.status = c->d_status;
 
-  // cudaFuncSetAttribute + the occupancy query cost tens of microseconds: raise the kernel's dynamic
-  // shared-memory limit to the device maximum once per kernel, cache blocks/SM per (kernel, smem)
-  const unsigned long long kkey = ((unsigned long long)p->log2m << 56) | ((unsigned long long)variant << 44) |
-                                  ((unsigned long long)mode << 40);
-  if (c->launch_cache.find(kkey) == c->launch_cache.end()) {
-    CUDA_TRY(op(OP_SET_SMEM, variant, mode, &a, 0, c->smem_optin, c->stream, nullptr));
-    c->launch_cache[kkey] = 1;
-  }
+  const FwdKernel fn = fwd_kernel_for(p->log2m, variant, mode);
+  if (!fn) return fail(B2L_ERR_CUDA, "no forward kernel variant %d for n_fft=%d", variant, N);
+  const int threads = variant_threads(variant);
   int occ = 0;
-  auto hit = c->launch_cache.find(kkey | (unsigned long long)smem);
-  if (hit != c->launch_cache.end()) {
-    occ = hit->second;
-  } else {
-    CUDA_TRY(op(OP_OCCUPANCY, variant, mode, &a, 0, smem, c->stream, &occ));
-    c->launch_cache[kkey | (unsigned long long)smem] = occ;
-  }
+  if ((rc = blocks_per_sm(c, fn, threads, smem, &occ))) return rc;
   if (occ < 1) return fail(B2L_ERR_CUDA, "forward kernel does not fit on an SM (smem %zu)", smem);
   long long grid = (long long)c->sm_count * occ;
   const long long ctas_needed = (a.total_tiles + halves - 1) / halves;
   if (grid > ctas_needed) grid = ctas_needed;
-  CUDA_TRY(op(OP_LAUNCH, variant, mode, &a, (int)grid, smem, c->stream, nullptr));
-  c->launches++;
-  return B2L_OK;
+  return launch(c, fn, (unsigned)grid, threads, smem, a);
 }
 
 // ------------------------------------------------------------------ chirp-z launch (n_fft not a power of two)
-typedef cudaError_t (*czt_op_fn)(int, const CztArgs*, int, size_t, cudaStream_t, int*);
-static czt_op_fn czt_table(int log2p) {
-  switch (log2p) {
-    case 5: return czt_op_5; case 6: return czt_op_6; case 7: return czt_op_7; case 8: return czt_op_8;
-    case 9: return czt_op_9; case 10: return czt_op_10; case 11: return czt_op_11; case 12: return czt_op_12;
-  }
-  return nullptr;
-}
-
-typedef cudaError_t (*czt_inv_op_fn)(int, const CztInvArgs*, int, size_t, cudaStream_t, int*);
-static czt_inv_op_fn czt_inv_table(int log2p) {
-  switch (log2p) {
-    case 5: return czt_inv_op_5; case 6: return czt_inv_op_6; case 7: return czt_inv_op_7; case 8: return czt_inv_op_8;
-    case 9: return czt_inv_op_9; case 10: return czt_inv_op_10; case 11: return czt_inv_op_11; case 12: return czt_inv_op_12;
-  }
-  return nullptr;
+// Shared memory of czt_kernel / czt_inv_kernel with G frame groups: engine twiddles, exchange buffers, FFT_P(h)/P,
+// the window * chirp table (even length) and, forward only, the chirp of the n_fft/2 + 1 output bins.
+static size_t czt_smem(const b2l_plan* p, const HostFftCfg& cfg, int G, bool forward) {
+  const size_t bins = forward ? (size_t)(1 + p->n_fft / 2) : 0;
+  return (size_t)((cfg.tw_count() + 15) & ~15) * 8 + (size_t)G * cfg.xbuf_f2() * 8 +
+         ((size_t)(1 << p->log2p) + (size_t)((p->n_fft + 1) & ~1) + bins) * 8;
 }
 
 static int run_czt(b2l_ctx* c, const b2l_plan* p, int mode, const float* d_y, int64_t n_clips, int64_t n,
                    int64_t y_stride, float2* out_c, float* out_r) {
-  if (p->ctx != c) return fail(B2L_ERR_INVALID, "plan belongs to another context");
-  if (n_clips < 0 || n < 0 || y_stride < n) return fail(B2L_ERR_INVALID, "bad clip geometry");
-  if (n > 0x7fffffffLL) return fail(B2L_ERR_UNSUPPORTED, "clips longer than 2^31-1 samples are not supported");
-  const long long T = plan_frames(p, n);
-  if (T <= 0)
-    return fail(B2L_ERR_INVALID, "n_fft=%d is too large for input signal of length=%lld", p->n_fft, (long long)n);
-  if (n_clips == 0) return B2L_OK;
-  if (!d_y || (mode == 0 ? (void*)out_c : (void*)out_r) == nullptr) return fail(B2L_ERR_INVALID, "NULL device pointer");
+  long long T = 0;
+  int rc = frame_count(c, p, n_clips, n, y_stride, d_y, mode == 0 ? (void*)out_c : (void*)out_r, &T);
+  if (rc || T == 0) return rc;
   DeviceGuard g(c->device);
   HostFftCfg cfg(p->log2p);
   const int nw = cfg.czt_nw();
@@ -1069,50 +255,43 @@ static int run_czt(b2l_ctx* c, const b2l_plan* p, int mode, const float* d_y, in
   a.power_mode = p->power_mode;
   a.power = p->power;
   a.status = c->d_status;
-  const size_t smem = (size_t)((cfg.tw_count() + 15) & ~15) * 8 + (size_t)G * cfg.xbuf_f2() * 8 +
-                      ((size_t)(1 << p->log2p) + (size_t)((p->n_fft + 1) & ~1) + (size_t)a.n_bins) * 8;   // + the three tables
-  czt_op_fn op = czt_table(p->log2p);
-  const unsigned long long kkey = (1ULL << 63) | ((unsigned long long)p->log2p << 40);
+  const size_t smem = czt_smem(p, cfg, G, true);
+  const CztKernel fn = czt_kernel_for(p->log2p);
+  // the table part of the shared memory depends on n_fft, not only on P: size the grid for the largest case (the
+  // kernels run one block per SM anyway)
   int occ = 0;
-  auto hit = c->launch_cache.find(kkey);
-  if (hit != c->launch_cache.end()) {
-    occ = hit->second;
-  } else {
-    // the table part of the shared memory depends on n_fft, not only on P: allow the device maximum once and
-    // size the grid for the largest case (the kernels run one block per SM anyway)
-    CUDA_TRY(op(OP_SET_SMEM, &a, 0, c->smem_optin, c->stream, nullptr));
-    CUDA_TRY(op(OP_OCCUPANCY, &a, 0, c->smem_optin / 2 + 1, c->stream, &occ));
-    c->launch_cache[kkey] = occ;
-  }
+  if ((rc = blocks_per_sm(c, fn, nw * 32, c->smem_optin / 2 + 1, &occ))) return rc;
   if (smem > c->smem_optin) return fail(B2L_ERR_UNSUPPORTED, "n_fft=%d needs more shared memory than one SM has", p->n_fft);
   if (occ < 1) return fail(B2L_ERR_CUDA, "chirp-z kernel does not fit on an SM (smem %zu)", smem);
   const long long steps = ((long long)n_clips * ((T + 1) / 2) + G - 1) / G;   // frames go in pairs inside a clip
   long long grid = (long long)c->sm_count * occ;
   if (grid > steps) grid = steps;
-  CUDA_TRY(op(OP_LAUNCH, &a, (int)grid, smem, c->stream, nullptr));
-  c->launches++;
-  return B2L_OK;
+  return launch(c, fn, (unsigned)grid, nw * 32, smem, a);
 }
 
 // ------------------------------------------------------------------ mixed-radix launch (even n_fft, 5-smooth half)
-// mode 0: complex STFT, 1: |X|^power, 2: mel (log_mode 1: dB values + per-clip maximum for mfcc)
-// frames per warp of mr_kernel: 2 (16 lanes each) for short frames, else 1
-static int mr_frames_per_warp(int M) { return M <= 512 ? 2 : 1; }
-static bool mr_enabled(const b2l_plan* p) {
-  if (p->log2p == 0) return true;   // no chirp-z tables for this size
-  const char* e = getenv("B2L_MR");
-  return !(e && *e) || atoi(e) != 0;
+// Warps per block (*nw) and shared memory (*smem) of mr_kernel / mr_inv_kernel: the tables (with n_mels mel rows of
+// mel_w_count weights) plus two M-point buffers per frame, fpw frames per warp.  Two resident blocks per SM when
+// they fit: at most half of the SM's shared memory each.
+static int mr_block(const b2l_ctx* c, const b2l_plan* p, int n_mels, int mel_w_count, int fpw, int* nw, size_t* smem) {
+  const size_t tables = mr_table_bytes(p->n_fft, p->mr_tw_count, n_mels, mel_w_count);
+  const size_t per_warp = (size_t)2 * (p->n_fft / 2) * sizeof(float2) * (size_t)fpw;
+  const size_t budget = (c->smem_optin + 1024) / 2 - 1024;
+  int w = 16;
+  while (w > 1 && tables + w * per_warp > budget) --w;
+  if (tables + w * per_warp > c->smem_optin)
+    return fail(B2L_ERR_UNSUPPORTED, "n_fft=%d needs more shared memory than one SM has", p->n_fft);
+  *nw = w;
+  *smem = tables + w * per_warp;
+  return B2L_OK;
 }
+
+// mode 0: complex STFT, 1: |X|^power, 2: mel (log_mode 1: dB values + per-clip maximum for mfcc)
 static int run_mr(b2l_ctx* c, const b2l_plan* p, int mode, int log_mode, const float* d_y, int64_t n_clips, int64_t n,
                   int64_t y_stride, float2* out_c, float* out_r) {
-  if (p->ctx != c) return fail(B2L_ERR_INVALID, "plan belongs to another context");
-  if (n_clips < 0 || n < 0 || y_stride < n) return fail(B2L_ERR_INVALID, "bad clip geometry");
-  if (n > 0x7fffffffLL) return fail(B2L_ERR_UNSUPPORTED, "clips longer than 2^31-1 samples are not supported");
-  const long long T = plan_frames(p, n);
-  if (T <= 0)
-    return fail(B2L_ERR_INVALID, "n_fft=%d is too large for input signal of length=%lld", p->n_fft, (long long)n);
-  if (n_clips == 0) return B2L_OK;
-  if (!d_y || (mode == 0 ? (void*)out_c : (void*)out_r) == nullptr) return fail(B2L_ERR_INVALID, "NULL device pointer");
+  long long T = 0;
+  int rc = frame_count(c, p, n_clips, n, y_stride, d_y, mode == 0 ? (void*)out_c : (void*)out_r, &T);
+  if (rc || T == 0) return rc;
   if (mode == 2 && p->n_mels == 0) return fail(B2L_ERR_INVALID, "plan has no mel stage");
   if (n_clips > 0x7fffffffLL || T > 0x7fffffffLL) return fail(B2L_ERR_UNSUPPORTED, "batch too large");
   DeviceGuard g(c->device);
@@ -1154,51 +333,57 @@ static int run_mr(b2l_ctx* c, const b2l_plan* p, int mode, int log_mode, const f
     a.db_sub = 10.0f * log10f(fmaxf(p->amin, fabsf(p->ref_value)));
     a.clip_max = c->d_clip_max;
   }
-  const size_t tables = mr_table_bytes(a.L, a.tw_count, a.n_mels, a.mel_w_count);
-  const size_t per_warp = (size_t)2 * a.M * sizeof(float2) * (size_t)mr_frames_per_warp(a.M);
-  // two resident blocks per SM when they fit: at most half of the SM's shared memory each
-  const size_t budget = (c->smem_optin + 1024) / 2 - 1024;
-  int nw = 16;
-  while (nw > 1 && tables + nw * per_warp > budget) --nw;
-  if (tables + nw * per_warp > c->smem_optin)
-    return fail(B2L_ERR_UNSUPPORTED, "n_fft=%d needs more shared memory than one SM has", p->n_fft);
-  const size_t smem = tables + nw * per_warp;
-  // lanes per frame: short frames ride two to a warp (their butterfly rounds fill 16 lanes better than 32)
-  const int fpw = mr_frames_per_warp(a.M);
-  const int lanes = 32 / fpw;
-  auto kern = lanes == 16 ? (mode == 0 ? mr_kernel<0, 16> : (mode == 1 ? mr_kernel<1, 16> : mr_kernel<2, 16>))
-                          : (mode == 0 ? mr_kernel<0, 32> : (mode == 1 ? mr_kernel<1, 32> : mr_kernel<2, 32>));
-  const unsigned long long kkey = (1ULL << 62) | (unsigned long long)(mode + 8 * fpw);
-  if (c->launch_cache.find(kkey) == c->launch_cache.end()) {
-    CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c->smem_optin));
-    c->launch_cache[kkey] = 1;
-  }
+  // frames per warp: short frames ride two to a warp (their butterfly rounds fill 16 lanes better than 32)
+  const int fpw = a.M <= 512 ? 2 : 1;
+  int nw = 0;
+  size_t smem = 0;
+  if ((rc = mr_block(c, p, a.n_mels, a.mel_w_count, fpw, &nw, &smem))) return rc;
+  auto kern = fpw == 2 ? (mode == 0 ? mr_kernel<0, 16> : (mode == 1 ? mr_kernel<1, 16> : mr_kernel<2, 16>))
+                       : (mode == 0 ? mr_kernel<0, 32> : (mode == 1 ? mr_kernel<1, 32> : mr_kernel<2, 32>));
   int occ = 0;
-  CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, nw * 32, smem));
+  if ((rc = blocks_per_sm(c, kern, nw * 32, smem, &occ))) return rc;
   if (occ < 1) return fail(B2L_ERR_CUDA, "mixed-radix kernel does not fit on an SM (smem %zu)", smem);
   const long long total = (long long)n_clips * T;
   long long grid = (long long)c->sm_count * occ;
   const long long need = (total + (long long)nw * fpw - 1) / ((long long)nw * fpw);
   if (grid > need) grid = need;
-  kern<<<(int)grid, nw * 32, smem, c->stream>>>(a);
-  CUDA_TRY(cudaGetLastError());
-  c->launches++;
-  return B2L_OK;
+  return launch(c, kern, (unsigned)grid, nw * 32, smem, a);
 }
 
 extern "C" int b2l_stft(b2l_ctx* c, const b2l_plan* p, const float* d_y, int64_t n_clips, int64_t n, int64_t y_stride,
                         void* d_D) {
-  if (c && p && p->czt)
-    return p->mr && mr_enabled(p) ? run_mr(c, p, 0, 0, d_y, n_clips, n, y_stride, (float2*)d_D, nullptr)
-                                 : run_czt(c, p, 0, d_y, n_clips, n, y_stride, (float2*)d_D, nullptr);
-  return run_forward(c, p, MODE_STFT, 0, d_y, n_clips, n, y_stride, (float2*)d_D, nullptr);
+  if (!c || !p) return fail(B2L_ERR_INVALID, "NULL ctx / plan");
+  switch (route(p, ENTRY_SPECTRUM)) {
+    case PATH_MR: return run_mr(c, p, 0, 0, d_y, n_clips, n, y_stride, (float2*)d_D, nullptr);
+    case PATH_CZT: return run_czt(c, p, 0, d_y, n_clips, n, y_stride, (float2*)d_D, nullptr);
+    default: return run_forward(c, p, MODE_STFT, 0, d_y, n_clips, n, y_stride, (float2*)d_D, nullptr);
+  }
 }
 extern "C" int b2l_spectrogram(b2l_ctx* c, const b2l_plan* p, const float* d_y, int64_t n_clips, int64_t n,
                                int64_t y_stride, float* d_S) {
-  if (c && p && p->czt)
-    return p->mr && mr_enabled(p) ? run_mr(c, p, 1, 0, d_y, n_clips, n, y_stride, nullptr, d_S)
-                                 : run_czt(c, p, 1, d_y, n_clips, n, y_stride, nullptr, d_S);
-  return run_forward(c, p, MODE_SPEC, 0, d_y, n_clips, n, y_stride, nullptr, d_S);
+  if (!c || !p) return fail(B2L_ERR_INVALID, "NULL ctx / plan");
+  switch (route(p, ENTRY_SPECTRUM)) {
+    case PATH_MR: return run_mr(c, p, 1, 0, d_y, n_clips, n, y_stride, nullptr, d_S);
+    case PATH_CZT: return run_czt(c, p, 1, d_y, n_clips, n, y_stride, nullptr, d_S);
+    default: return run_forward(c, p, MODE_SPEC, 0, d_y, n_clips, n, y_stride, nullptr, d_S);
+  }
+}
+
+// ------------------------------------------------------------------ device-side input validation
+extern "C" int b2l_scan_finite(b2l_ctx* c, const float* d_y, int64_t n_clips, int64_t n, int64_t y_stride,
+                               int64_t begin) {
+  if (!c || !d_y) return fail(B2L_ERR_INVALID, "NULL argument");
+  if (n_clips <= 0 || begin >= n) return B2L_OK;
+  if (n > 0x7fffffffLL) return fail(B2L_ERR_UNSUPPORTED, "scan_finite: clips longer than 2^31-1 samples");
+  DeviceGuard g(c->device);
+  long long bx = ((n - begin) + 1023) / 1024;
+  if (bx > 64) bx = 64;
+  dim3 grid((unsigned)bx, (unsigned)(n_clips > 65535 ? 65535 : n_clips));
+  finite_scan_kernel<<<grid, 256, 0, c->stream>>>(d_y, y_stride, (int)n, (int)(begin < 0 ? 0 : begin), n_clips,
+                                                  c->d_status);
+  CUDA_TRY(cudaGetLastError());
+  c->launches++;
+  return B2L_OK;
 }
 // ------------------------------------------------------------------ frame-wise spectral statistics / framings
 static int check_stats_desc(const b2l_stats_desc* d, StatsParams* sp) {
@@ -1233,22 +418,20 @@ extern "C" int b2l_spectral_stats_from_spec(b2l_ctx* c, const b2l_stats_desc* d,
   while (nw > 1 && (size_t)(nw + 1) * Fp * 4 > c->smem_optin) nw >>= 1;
   const size_t smem = (size_t)(nw + 1) * Fp * 4;
   if (smem > c->smem_optin) return fail(B2L_ERR_UNSUPPORTED, "n_bins=%d rows do not fit in shared memory", n_bins);
-  CUDA_TRY(cudaFuncSetAttribute(stats_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c->smem_optin));
+  rc = blocks_per_sm(c, stats_kernel, nw * 32, smem, nullptr);
+  if (rc) return rc;
   const long long rows = (long long)n_clips * n_frames;
   long long grid = (rows + nw - 1) / nw;
   const long long cap = (long long)c->sm_count * 8;
   if (grid > cap) grid = cap;
-  stats_kernel<<<(int)grid, nw * 32, smem, c->stream>>>(d_S, rows, (int)n_frames, n_bins, d_freq, sc.sp, d_out,
-                                                        c->d_status);
-  CUDA_TRY(cudaGetLastError());
-  c->launches++;
-  return B2L_OK;
+  return launch(c, stats_kernel, (unsigned)grid, nw * 32, smem, d_S, rows, (int)n_frames, n_bins, d_freq, sc.sp, d_out,
+                c->d_status);
 }
 
 extern "C" int b2l_spectral_stats(b2l_ctx* c, const b2l_plan* p, const b2l_stats_desc* d, const float* d_y,
                                   int64_t n_clips, int64_t n, int64_t y_stride, const float* d_freq, float* d_out) {
   if (!c || !p) return fail(B2L_ERR_INVALID, "NULL ctx / plan");
-  if (p->czt)
+  if (route(p, ENTRY_STATS) == PATH_NONE)
     return fail(B2L_ERR_UNSUPPORTED,
                 "n_fft=%d: compose b2l_spectrogram + b2l_spectral_stats_from_spec for non-power-of-two sizes", p->n_fft);
   StatsCall sc;
@@ -1306,11 +489,14 @@ extern "C" int b2l_frame_feature(b2l_ctx* c, int32_t what, const float* d_y, int
 
 extern "C" int b2l_melspectrogram(b2l_ctx* c, const b2l_plan* p, const float* d_y, int64_t n_clips, int64_t n,
                                   int64_t y_stride, float* d_mel) {
-  if (c && p && p->czt && p->mr) return run_mr(c, p, 2, 0, d_y, n_clips, n, y_stride, nullptr, d_mel);
-  if (p && p->czt)
-    return fail(B2L_ERR_UNSUPPORTED, "n_fft=%d: compose b2l_spectrogram + b2l_mel_project for non-power-of-two sizes",
-                p->n_fft);
-  return run_forward(c, p, MODE_MEL, 0, d_y, n_clips, n, y_stride, nullptr, d_mel);
+  if (!c || !p) return fail(B2L_ERR_INVALID, "NULL ctx / plan");
+  switch (route(p, ENTRY_MEL)) {
+    case PATH_MR: return run_mr(c, p, 2, 0, d_y, n_clips, n, y_stride, nullptr, d_mel);
+    case PATH_NONE:
+      return fail(B2L_ERR_UNSUPPORTED, "n_fft=%d: compose b2l_spectrogram + b2l_mel_project for non-power-of-two sizes",
+                  p->n_fft);
+    default: return run_forward(c, p, MODE_MEL, 0, d_y, n_clips, n, y_stride, nullptr, d_mel);
+  }
 }
 
 static int launch_dct(b2l_ctx* c, const b2l_plan* p, const float* d_L, int64_t n_clips, int64_t T, int clamp,
@@ -1334,26 +520,24 @@ static int launch_dct(b2l_ctx* c, const b2l_plan* p, const float* d_L, int64_t n
   const int ks = KG <= 10 && p->n_mels >= 8 * KG ? 2 : 1;   // 640 threads at most; 32*KG*32 partial sums <= 2*n_mels*64 tile words
   auto kern = ks == 2 ? dct_clamp4_kernel<2> : dct_clamp4_kernel<1>;
   const int threads = KG * 32 * ks;
-  CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const int tiles = (int)((T + DCT4_TILE - 1) / DCT4_TILE);
   const long long total = (long long)tiles * n_clips;
   int occ = 0;
-  CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, threads, smem));
+  const int rc = blocks_per_sm(c, kern, threads, smem, &occ);
+  if (rc) return rc;
   if (occ < 1) return fail(B2L_ERR_CUDA, "DCT kernel does not fit on an SM");
   long long grid = (long long)c->sm_count * occ;
   if (grid > total) grid = total;
-  kern<<<(int)grid, threads, smem, c->stream>>>(d_L, p->d_dct, clamp ? c->d_clip_max : nullptr, clamp ? p->top_db : -1.0f,
-                                                p->n_mels, p->n_mfcc, (int)T, tiles, total, tiled, d_out);
-  CUDA_TRY(cudaGetLastError());
-  c->launches++;
-  return B2L_OK;
+  return launch(c, kern, (unsigned)grid, threads, smem, d_L, p->d_dct, clamp ? c->d_clip_max : nullptr,
+                clamp ? p->top_db : -1.0f, p->n_mels, p->n_mfcc, (int)T, tiles, total, tiled, d_out);
 }
 
 extern "C" int b2l_mfcc(b2l_ctx* c, const b2l_plan* p, const float* d_y, int64_t n_clips, int64_t n, int64_t y_stride,
                         float* d_mfcc, float* d_logmel) {
   if (!c || !p) return fail(B2L_ERR_INVALID, "NULL ctx / plan");
   if (p->n_mfcc == 0) return fail(B2L_ERR_INVALID, "plan has no mfcc stage");
-  if (p->czt && !p->mr)
+  const Path path = route(p, ENTRY_MEL);
+  if (path == PATH_NONE)
     return fail(B2L_ERR_UNSUPPORTED, "n_fft=%d: compose spectrogram, mel_project, power_to_db and dct_project for "
                 "non-power-of-two sizes", p->n_fft);
   if (n_clips <= 0) return n_clips == 0 ? B2L_OK : fail(B2L_ERR_INVALID, "negative n_clips");
@@ -1367,9 +551,9 @@ extern "C" int b2l_mfcc(b2l_ctx* c, const b2l_plan* p, const float* d_y, int64_t
   // the log-mel scratch is tiled: [clip][ceil(T/64)][n_mels][64] (see dct_clamp4_kernel)
   if (!scratch) CUDA_TRY(cudaMalloc((void**)&scratch, (size_t)n_clips * p->n_mels * ((T + 63) / 64 * 64) * sizeof(float)));
   // mixed-radix frames (mr_kernel): the dB rows go to the scratch in the plain [clip][mel][frame] layout
-  const int tiled = p->czt ? 0 : 1;
-  rc = p->czt ? run_mr(c, p, 2, 1, d_y, n_clips, n, y_stride, nullptr, scratch)
-              : run_forward(c, p, MODE_MEL, 2, d_y, n_clips, n, y_stride, nullptr, scratch);
+  const int tiled = path == PATH_POW2 ? 1 : 0;
+  rc = path == PATH_MR ? run_mr(c, p, 2, 1, d_y, n_clips, n, y_stride, nullptr, scratch)
+                       : run_forward(c, p, MODE_MEL, 2, d_y, n_clips, n, y_stride, nullptr, scratch);
   if (rc == B2L_OK) rc = launch_dct(c, p, scratch, n_clips, T, 1, d_mfcc, tiled);
   if (!d_logmel) {
     cudaStreamSynchronize(c->stream);
@@ -1378,128 +562,29 @@ extern "C" int b2l_mfcc(b2l_ctx* c, const b2l_plan* p, const float* d_y, int64_t
   return rc;
 }
 
-// ------------------------------------------------------------------ inverse launch
-extern "C" int b2l_istft(b2l_ctx* c, const b2l_plan* p, const void* d_D, int64_t n_clips, int64_t n_frames_stored,
-                         int64_t n_frames_used, const float* d_inv_wss, int64_t out_len, float* d_y,
-                         int64_t y_stride) {
-  if (!c || !p) return fail(B2L_ERR_INVALID, "NULL ctx / plan");
-  if (p->ctx != c) return fail(B2L_ERR_INVALID, "plan belongs to another context");
-  if (n_clips < 0 || n_frames_used < 1 || n_frames_used > n_frames_stored || out_len < 0 || y_stride < out_len)
-    return fail(B2L_ERR_INVALID, "bad istft geometry");
-  if (n_clips == 0 || out_len == 0) return B2L_OK;
-  if (!d_D || !d_inv_wss || !d_y) return fail(B2L_ERR_INVALID, "NULL device pointer");
-  if (p->czt) {
-    // chirp-z inverse frames into scratch, then a gather overlap-add (czt_kernel.cuh)
-    if (out_len > 0x7fffffffLL || n_clips > 65535) return fail(B2L_ERR_UNSUPPORTED, "istft batch too large");
-    DeviceGuard g(c->device);
-    const int L = p->n_fft;
-    const size_t need = (size_t)n_clips * (size_t)n_frames_used * L * sizeof(float);
-    if (c->scratch_bytes < need) {
-      CUDA_TRY(cudaStreamSynchronize(c->stream));
-      if (c->d_scratch) CUDA_TRY(cudaFree(c->d_scratch));
-      c->d_scratch = nullptr;
-      c->scratch_bytes = 0;
-      CUDA_TRY(cudaMalloc((void**)&c->d_scratch, need));
-      c->scratch_bytes = need;
-    }
-    if (p->mr && mr_enabled(p)) {
-      // mixed-radix inverse frames (mr_inv_kernel) into the scratch array, then the same overlap-add
-      MrInvArgs ma;
-      memset(&ma, 0, sizeof(ma));
-      ma.D = (const float2*)d_D;
-      ma.d_clip_stride = (long long)n_frames_stored * (L / 2 + 1);
-      ma.n_clips = (int)n_clips;
-      ma.n_frames = (int)n_frames_used;
-      ma.L = L;
-      ma.M = L / 2;
-      ma.n_bins = L / 2 + 1;
-      ma.n_pass = p->mr_n_pass;
-      for (int s = 0; s < p->mr_n_pass; ++s) {
-        ma.radix[s] = p->mr_radix[s];
-        ma.tw_off[s] = p->mr_tw_off[s];
-      }
-      ma.tw_count = p->mr_tw_count;
-      ma.win = p->d_mr_win_inv;
-      ma.tw = p->d_mr_tw;
-      ma.twn = p->d_mr_twn;
-      ma.ytmp = c->d_scratch;
-      const size_t tables = mr_table_bytes(L, ma.tw_count, 0, 0);
-      const size_t per_warp = (size_t)2 * ma.M * sizeof(float2);
-      const size_t budget = (c->smem_optin + 1024) / 2 - 1024;
-      int nw = 16;
-      while (nw > 1 && tables + nw * per_warp > budget) --nw;
-      if (tables + nw * per_warp > c->smem_optin)
-        return fail(B2L_ERR_UNSUPPORTED, "n_fft=%d needs more shared memory than one SM has", L);
-      const size_t smem = tables + nw * per_warp;
-      const unsigned long long kkey = (1ULL << 62) | 7ULL;
-      if (c->launch_cache.find(kkey) == c->launch_cache.end()) {
-        CUDA_TRY(cudaFuncSetAttribute(mr_inv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c->smem_optin));
-        c->launch_cache[kkey] = 1;
-      }
-      int occ = 0;
-      CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, mr_inv_kernel, nw * 32, smem));
-      if (occ < 1) return fail(B2L_ERR_CUDA, "mixed-radix inverse kernel does not fit on an SM (smem %zu)", smem);
-      const long long total = (long long)n_clips * n_frames_used;
-      long long grid = (long long)c->sm_count * occ;
-      const long long need_blocks = (total + nw - 1) / nw;
-      if (grid > need_blocks) grid = need_blocks;
-      mr_inv_kernel<<<(int)grid, nw * 32, smem, c->stream>>>(ma);
-      CUDA_TRY(cudaGetLastError());
-      c->launches++;
-    } else {
-    HostFftCfg cfg(p->log2p);
-    const int nw = cfg.czt_nw();
-    const int G = nw * 32 / cfg.tpf;
-    CztInvArgs a;
-    memset(&a, 0, sizeof(a));
-    a.D = (const float2*)d_D;
-    a.d_clip_stride = (long long)n_frames_stored * (L / 2 + 1);
-    a.n_clips = (int)n_clips;
-    a.n_frames = (int)n_frames_used;
-    a.L = L;
-    a.n_bins = L / 2 + 1;
-    a.bfull = p->d_czt_bfull;
-    a.wbi = p->d_czt_wbi;
-    a.hf = p->d_czt_hf;
-    a.ytmp = c->d_scratch;
-    const size_t smem = (size_t)((cfg.tw_count() + 15) & ~15) * 8 + (size_t)G * cfg.xbuf_f2() * 8 +
-                        ((size_t)(1 << p->log2p) + (size_t)((L + 1) & ~1)) * 8;   // + FFT_P(h)/P and window * chirp
-    if (smem > c->smem_optin) return fail(B2L_ERR_UNSUPPORTED, "n_fft=%d needs more shared memory than one SM has", L);
-    czt_inv_op_fn op = czt_inv_table(p->log2p);
-    const unsigned long long kkey = (3ULL << 62) | ((unsigned long long)p->log2p << 40);
-    int occ = 0;
-    auto hit = c->launch_cache.find(kkey);
-    if (hit != c->launch_cache.end()) {
-      occ = hit->second;
-    } else {
-      CUDA_TRY(op(OP_SET_SMEM, &a, 0, c->smem_optin, c->stream, nullptr));
-      CUDA_TRY(op(OP_OCCUPANCY, &a, 0, c->smem_optin / 2 + 1, c->stream, &occ));
-      c->launch_cache[kkey] = occ;
-    }
-    if (occ < 1) return fail(B2L_ERR_CUDA, "chirp-z inverse kernel does not fit on an SM");
-    const long long steps = ((long long)n_clips * ((n_frames_used + 1) / 2) + G - 1) / G;   // frames go in pairs inside a clip
-    long long grid = (long long)c->sm_count * occ;
-    if (grid > steps) grid = steps;
-    CUDA_TRY(op(OP_LAUNCH, &a, (int)grid, smem, c->stream, nullptr));
-    c->launches++;
-    }
-    long long bx = (out_len + 255) / 256;
-    const long long cap = (8LL * c->sm_count + n_clips - 1) / n_clips;
-    if (bx > cap) bx = cap;
-    if (bx < 1) bx = 1;
-    dim3 og((unsigned)bx, (unsigned)n_clips);
-    ola_kernel<<<og, 256, 0, c->stream>>>(c->d_scratch, (int)n_frames_used, L, p->hop, p->center ? L / 2 : 0, (int)out_len,
-                                          y_stride, d_inv_wss, d_y);
-    CUDA_TRY(cudaGetLastError());
-    c->launches++;
-    return B2L_OK;
+// ------------------------------------------------------------------ inverse launches
+// Grows the context's scratch array to at least `bytes` (the contents are not kept).
+static int ensure_scratch(b2l_ctx* c, size_t bytes) {
+  if (c->scratch_bytes >= bytes) return B2L_OK;
+  if (c->d_scratch) {
+    CUDA_TRY(cudaStreamSynchronize(c->stream));
+    CUDA_TRY(cudaFree(c->d_scratch));
+    c->d_scratch = nullptr;
+    c->scratch_bytes = 0;
   }
+  CUDA_TRY(cudaMalloc((void**)&c->d_scratch, bytes));
+  c->scratch_bytes = bytes;
+  return B2L_OK;
+}
+
+// n_fft a power of two: inv_kernel (irFFT, window and overlap-add in one pass)
+static int run_inverse(b2l_ctx* c, const b2l_plan* p, const void* d_D, int64_t n_clips, int64_t n_frames_stored,
+                       int64_t n_frames_used, const float* d_inv_wss, int64_t out_len, float* d_y, int64_t y_stride) {
   if (out_len > 0x7fffffffLL || n_frames_stored > 0x7fffffffLL)
     return fail(B2L_ERR_UNSUPPORTED, "istft output longer than 2^31-1 samples is not supported");
   DeviceGuard g(c->device);
   HostFftCfg cfg(p->log2m);
   const int N = p->n_fft, M = N / 2;
-  inv_op_fn op = inv_table(p->log2m);
   int variants[3];
   const int n_opt = cta_variants(cfg, variants);
   InvArgs a;
@@ -1560,8 +645,109 @@ extern "C" int b2l_istft(b2l_ctx* c, const b2l_plan* p, const void* d_D, int64_t
   a.frames_per_slot = (int)fps;
   const long long items = (total_frames + fps - 1) / fps;
   const long long grid = (items + halves - 1) / halves;
-  CUDA_TRY(op(OP_SET_SMEM, variant, &a, 0, smem, c->stream, nullptr));
-  CUDA_TRY(op(OP_LAUNCH, variant, &a, (int)grid, smem, c->stream, nullptr));
+  const InvKernel fn = inv_kernel_for(p->log2m, variant);
+  if (!fn) return fail(B2L_ERR_CUDA, "no inverse kernel variant %d for n_fft=%d", variant, N);
+  const int threads = variant_threads(variant);
+  int rc = blocks_per_sm(c, fn, threads, smem, nullptr);
+  return rc ? rc : launch(c, fn, (unsigned)grid, threads, smem, a);
+}
+
+// mixed-radix inverse frames (mr_inv_kernel) into the scratch array
+static int run_mr_inverse(b2l_ctx* c, const b2l_plan* p, const void* d_D, int64_t n_clips, int64_t n_frames_stored,
+                          int64_t n_frames_used) {
+  const int L = p->n_fft;
+  MrInvArgs a;
+  memset(&a, 0, sizeof(a));
+  a.D = (const float2*)d_D;
+  a.d_clip_stride = (long long)n_frames_stored * (L / 2 + 1);
+  a.n_clips = (int)n_clips;
+  a.n_frames = (int)n_frames_used;
+  a.L = L;
+  a.M = L / 2;
+  a.n_bins = L / 2 + 1;
+  a.n_pass = p->mr_n_pass;
+  for (int s = 0; s < p->mr_n_pass; ++s) {
+    a.radix[s] = p->mr_radix[s];
+    a.tw_off[s] = p->mr_tw_off[s];
+  }
+  a.tw_count = p->mr_tw_count;
+  a.win = p->d_mr_win_inv;
+  a.tw = p->d_mr_tw;
+  a.twn = p->d_mr_twn;
+  a.ytmp = c->d_scratch;
+  int nw = 0, occ = 0;
+  size_t smem = 0;
+  int rc = mr_block(c, p, 0, 0, 1, &nw, &smem);
+  if (rc || (rc = blocks_per_sm(c, mr_inv_kernel, nw * 32, smem, &occ))) return rc;
+  if (occ < 1) return fail(B2L_ERR_CUDA, "mixed-radix inverse kernel does not fit on an SM (smem %zu)", smem);
+  const long long total = (long long)n_clips * n_frames_used;
+  long long grid = (long long)c->sm_count * occ;
+  const long long need_blocks = (total + nw - 1) / nw;
+  if (grid > need_blocks) grid = need_blocks;
+  return launch(c, mr_inv_kernel, (unsigned)grid, nw * 32, smem, a);
+}
+
+// chirp-z inverse frames (czt_inv_kernel) into the scratch array
+static int run_czt_inverse(b2l_ctx* c, const b2l_plan* p, const void* d_D, int64_t n_clips, int64_t n_frames_stored,
+                           int64_t n_frames_used) {
+  const int L = p->n_fft;
+  HostFftCfg cfg(p->log2p);
+  const int nw = cfg.czt_nw();
+  const int G = nw * 32 / cfg.tpf;
+  CztInvArgs a;
+  memset(&a, 0, sizeof(a));
+  a.D = (const float2*)d_D;
+  a.d_clip_stride = (long long)n_frames_stored * (L / 2 + 1);
+  a.n_clips = (int)n_clips;
+  a.n_frames = (int)n_frames_used;
+  a.L = L;
+  a.n_bins = L / 2 + 1;
+  a.bfull = p->d_czt_bfull;
+  a.wbi = p->d_czt_wbi;
+  a.hf = p->d_czt_hf;
+  a.ytmp = c->d_scratch;
+  const size_t smem = czt_smem(p, cfg, G, false);
+  if (smem > c->smem_optin) return fail(B2L_ERR_UNSUPPORTED, "n_fft=%d needs more shared memory than one SM has", L);
+  const CztInvKernel fn = czt_inv_kernel_for(p->log2p);
+  int occ = 0;
+  int rc = blocks_per_sm(c, fn, nw * 32, c->smem_optin / 2 + 1, &occ);   // sized like the forward (run_czt)
+  if (rc) return rc;
+  if (occ < 1) return fail(B2L_ERR_CUDA, "chirp-z inverse kernel does not fit on an SM");
+  const long long steps = ((long long)n_clips * ((n_frames_used + 1) / 2) + G - 1) / G;   // frames go in pairs inside a clip
+  long long grid = (long long)c->sm_count * occ;
+  if (grid > steps) grid = steps;
+  return launch(c, fn, (unsigned)grid, nw * 32, smem, a);
+}
+
+extern "C" int b2l_istft(b2l_ctx* c, const b2l_plan* p, const void* d_D, int64_t n_clips, int64_t n_frames_stored,
+                         int64_t n_frames_used, const float* d_inv_wss, int64_t out_len, float* d_y,
+                         int64_t y_stride) {
+  if (!c || !p) return fail(B2L_ERR_INVALID, "NULL ctx / plan");
+  if (p->ctx != c) return fail(B2L_ERR_INVALID, "plan belongs to another context");
+  if (n_clips < 0 || n_frames_used < 1 || n_frames_used > n_frames_stored || out_len < 0 || y_stride < out_len)
+    return fail(B2L_ERR_INVALID, "bad istft geometry");
+  if (n_clips == 0 || out_len == 0) return B2L_OK;
+  if (!d_D || !d_inv_wss || !d_y) return fail(B2L_ERR_INVALID, "NULL device pointer");
+  const Path path = route(p, ENTRY_SPECTRUM);
+  if (path == PATH_POW2)
+    return run_inverse(c, p, d_D, n_clips, n_frames_stored, n_frames_used, d_inv_wss, out_len, d_y, y_stride);
+  // mixed-radix or chirp-z frames into the scratch array, then a gather overlap-add
+  if (out_len > 0x7fffffffLL || n_clips > 65535) return fail(B2L_ERR_UNSUPPORTED, "istft batch too large");
+  DeviceGuard g(c->device);
+  const int L = p->n_fft;
+  int rc = ensure_scratch(c, (size_t)n_clips * (size_t)n_frames_used * L * sizeof(float));
+  if (rc == B2L_OK)
+    rc = path == PATH_MR ? run_mr_inverse(c, p, d_D, n_clips, n_frames_stored, n_frames_used)
+                         : run_czt_inverse(c, p, d_D, n_clips, n_frames_stored, n_frames_used);
+  if (rc) return rc;
+  long long bx = (out_len + 255) / 256;
+  const long long cap = (8LL * c->sm_count + n_clips - 1) / n_clips;
+  if (bx > cap) bx = cap;
+  if (bx < 1) bx = 1;
+  dim3 og((unsigned)bx, (unsigned)n_clips);
+  ola_kernel<<<og, 256, 0, c->stream>>>(c->d_scratch, (int)n_frames_used, L, p->hop, p->center ? L / 2 : 0, (int)out_len,
+                                        y_stride, d_inv_wss, d_y);
+  CUDA_TRY(cudaGetLastError());
   c->launches++;
   return B2L_OK;
 }
@@ -1580,28 +766,25 @@ extern "C" int b2l_mel_project(b2l_ctx* c, const b2l_plan* p, const float* d_S, 
     if (p->d_mel_wT && (long long)p->mel_w_count * 4 >= (long long)p->n_mels * F && dsmem <= c->smem_optin) {
       const int r4 = (p->n_mels + 3) / 4;
       auto kern = r4 == 1 ? dense_project_kernel<1> : r4 == 2 ? dense_project_kernel<2> : r4 == 3 ? dense_project_kernel<3> : dense_project_kernel<4>;
-      CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dsmem));
+      const int rc = blocks_per_sm(c, kern, 256, dsmem, nullptr);
+      if (rc) return rc;
       const int tiles_d = (int)((n_frames + 31) / 32);
       const long long total = (long long)tiles_d * n_clips;
       long long grid_d = c->sm_count;
       if (grid_d > total) grid_d = total;
-      kern<<<(int)grid_d, 256, dsmem, c->stream>>>(d_S, p->d_mel_wT, p->n_mels, F, (int)n_frames, tiles_d, total, d_mel);
-      CUDA_TRY(cudaGetLastError());
-      c->launches++;
-      return B2L_OK;
+      return launch(c, kern, (unsigned)grid_d, 256, dsmem, d_S, p->d_mel_wT, p->n_mels, F, (int)n_frames, tiles_d, total,
+                    d_mel);
     }
   }
   size_t smem = (size_t)F * 33 * 4;
   if (smem > c->smem_optin) return fail(B2L_ERR_UNSUPPORTED, "n_fft too large for mel_project");
-  CUDA_TRY(cudaFuncSetAttribute(mel_project_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  const int rc = blocks_per_sm(c, mel_project_kernel, 256, smem, nullptr);
+  if (rc) return rc;
   const int tiles = (int)((n_frames + 31) / 32);
   const long long grid = (long long)tiles * n_clips;
   if (grid > 0x7fffffffLL) return fail(B2L_ERR_UNSUPPORTED, "too many tiles");
-  mel_project_kernel<<<(int)grid, 256, smem, c->stream>>>(d_S, p->d_mel_w, p->d_band, p->n_mels, F, (int)n_frames,
-                                                          tiles, d_mel);
-  CUDA_TRY(cudaGetLastError());
-  c->launches++;
-  return B2L_OK;
+  return launch(c, mel_project_kernel, (unsigned)grid, 256, smem, d_S, p->d_mel_w, p->d_band, p->n_mels, F, (int)n_frames,
+                tiles, d_mel);
 }
 
 // ------------------------------------------------------------------ polyphase resampling
@@ -1753,15 +936,14 @@ extern "C" int b2l_spectral_contrast(b2l_ctx* c, const b2l_contrast_desc* d, con
   while (nw > 1 && per_warp * nw > c->smem_optin) nw >>= 1;
   const size_t smem = per_warp * nw;
   if (smem > c->smem_optin) return fail(B2L_ERR_UNSUPPORTED, "n_bins=%d rows do not fit in shared memory", n_bins);
-  CUDA_TRY(cudaFuncSetAttribute(contrast_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c->smem_optin));
+  const int rc = blocks_per_sm(c, contrast_kernel, nw * 32, smem, nullptr);
+  if (rc) return rc;
   const long long rows = (long long)n_clips * n_frames;
   long long grid = (rows + nw - 1) / nw;
   const long long lim = (long long)c->sm_count * 8;
   if (grid > lim) grid = lim;
-  contrast_kernel<<<(int)grid, nw * 32, smem, c->stream>>>(d_S, rows, (int)n_frames, n_bins, cap, a, d_peak, d_valley);
-  CUDA_TRY(cudaGetLastError());
-  c->launches++;
-  return B2L_OK;
+  return launch(c, contrast_kernel, (unsigned)grid, nw * 32, smem, d_S, rows, (int)n_frames, n_bins, cap, a, d_peak,
+                d_valley);
 }
 
 extern "C" int b2l_sub(b2l_ctx* c, const float* d_x, const float* d_y, int64_t n, float* d_out) {
@@ -1787,17 +969,8 @@ extern "C" int b2l_pip_pass(b2l_ctx* c, const b2l_pip_desc* d, const float* d_S,
   for (int i = 0; i < n_hist; ++i) h_hist[i] = 0;
   if (n_rows <= 0 || d->k_hi <= d->k_lo) return B2L_OK;
   DeviceGuard g(c->device);
-  const size_t need = 2048 * sizeof(unsigned long long) + 2049 * sizeof(double);
-  if (c->scratch_bytes < need) {
-    if (c->d_scratch) {
-      CUDA_TRY(cudaStreamSynchronize(c->stream));
-      CUDA_TRY(cudaFree(c->d_scratch));
-      c->d_scratch = nullptr;
-      c->scratch_bytes = 0;
-    }
-    CUDA_TRY(cudaMalloc((void**)&c->d_scratch, need));
-    c->scratch_bytes = need;
-  }
+  int rc = ensure_scratch(c, 2048 * sizeof(unsigned long long) + 2049 * sizeof(double));
+  if (rc) return rc;
   unsigned long long* d_hist = reinterpret_cast<unsigned long long*>(c->d_scratch);
   double* d_edges = reinterpret_cast<double*>(d_hist + 2048);
   CUDA_TRY(cudaMemsetAsync(d_hist, 0, 2048 * sizeof(unsigned long long), c->stream));
@@ -1819,13 +992,12 @@ extern "C" int b2l_pip_pass(b2l_ctx* c, const b2l_pip_desc* d, const float* d_S,
   while (nw > 1 && per_warp * nw + 8192 + 1024 > c->smem_optin) nw >>= 1;
   const size_t smem = per_warp * nw;
   if (smem + 8192 + 1024 > c->smem_optin) return fail(B2L_ERR_UNSUPPORTED, "n_bins=%d rows do not fit in shared memory", n_bins);
-  CUDA_TRY(cudaFuncSetAttribute(pip_pass_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(c->smem_optin - 8192 - 1024)));
+  // 8 KB of static shared memory (the block's histogram) and 1 KB reserved by the system
+  if ((rc = blocks_per_sm(c, pip_pass_kernel, nw * 32, smem, nullptr, c->smem_optin - 8192 - 1024))) return rc;
   long long grid = (n_rows + nw - 1) / nw;
   const long long lim = (long long)c->sm_count * 4;
   if (grid > lim) grid = lim;
-  pip_pass_kernel<<<(int)grid, nw * 32, smem, c->stream>>>(d_S, n_rows, n_bins, a, d_edges, d_hist);
-  CUDA_TRY(cudaGetLastError());
-  c->launches++;
+  if ((rc = launch(c, pip_pass_kernel, (unsigned)grid, nw * 32, smem, d_S, n_rows, n_bins, a, d_edges, d_hist))) return rc;
   CUDA_TRY(cudaMemcpyAsync(h_hist, d_hist, (size_t)n_hist * sizeof(unsigned long long), cudaMemcpyDeviceToHost, c->stream));
   CUDA_TRY(cudaStreamSynchronize(c->stream));
   return B2L_OK;
@@ -1997,76 +1169,5 @@ extern "C" int b2l_transpose(b2l_ctx* c, const void* d_in, int64_t n_clips, int6
     CUDA_TRY(cudaGetLastError());
     c->launches++;
   }
-  return B2L_OK;
-}
-
-// ------------------------------------------------------------------ multi-GPU split / join
-extern "C" int b2l_comm_unique_id(void* id128) {
-  if (!id128) return fail(B2L_ERR_INVALID, "NULL argument");
-  int rc = nccl_load();
-  if (rc) return rc;
-  ncclUniqueId id;
-  NCCL_TRY(g_nccl.GetUniqueId(&id));
-  memcpy(id128, &id, sizeof(id));
-  return B2L_OK;
-}
-extern "C" int b2l_comm_init(b2l_ctx* c, const void* id128, int rank, int world) {
-  if (!c || !id128) return fail(B2L_ERR_INVALID, "NULL argument");
-  if (world < 1 || rank < 0 || rank >= world) return fail(B2L_ERR_INVALID, "bad rank %d / world %d", rank, world);
-  int rc = nccl_load();
-  if (rc) return rc;
-  DeviceGuard g(c->device);
-  ncclUniqueId id;
-  memcpy(&id, id128, sizeof(id));
-  NCCL_TRY(g_nccl.CommInitRank(&c->comm, world, id, rank));
-  c->rank = rank;
-  c->world = world;
-  return B2L_OK;
-}
-extern "C" int b2l_comm_destroy(b2l_ctx* c) {
-  if (!c || !c->comm) return B2L_OK;
-  DeviceGuard g(c->device);
-  cudaStreamSynchronize(c->stream);
-  NCCL_TRY(g_nccl.CommDestroy(c->comm));
-  c->comm = nullptr;
-  c->world = 1;
-  c->rank = 0;
-  return B2L_OK;
-}
-extern "C" int b2l_comm_broadcast(b2l_ctx* c, void* d_buf, size_t bytes, int root) {
-  if (!c || !c->comm) return fail(B2L_ERR_INVALID, "communicator not initialised");
-  DeviceGuard g(c->device);
-  NCCL_TRY(g_nccl.Broadcast(d_buf, d_buf, bytes, ncclChar, root, c->comm, c->stream));
-  return B2L_OK;
-}
-extern "C" int b2l_comm_scatter(b2l_ctx* c, const void* d_full, void* d_shard, size_t shard_bytes, int root) {
-  if (!c || !c->comm) return fail(B2L_ERR_INVALID, "communicator not initialised");
-  DeviceGuard g(c->device);
-  NCCL_TRY(g_nccl.GroupStart());
-  if (c->rank == root)
-    for (int r = 0; r < c->world; ++r)
-      NCCL_TRY(g_nccl.Send((const char*)d_full + (size_t)r * shard_bytes, shard_bytes, ncclChar, r, c->comm, c->stream));
-  NCCL_TRY(g_nccl.Recv(d_shard, shard_bytes, ncclChar, root, c->comm, c->stream));
-  NCCL_TRY(g_nccl.GroupEnd());
-  return B2L_OK;
-}
-extern "C" int b2l_comm_gather(b2l_ctx* c, const void* d_shard, void* d_full, size_t shard_bytes, int root) {
-  if (!c || !c->comm) return fail(B2L_ERR_INVALID, "communicator not initialised");
-  DeviceGuard g(c->device);
-  NCCL_TRY(g_nccl.GroupStart());
-  if (c->rank == root)
-    for (int r = 0; r < c->world; ++r)
-      NCCL_TRY(g_nccl.Recv((char*)d_full + (size_t)r * shard_bytes, shard_bytes, ncclChar, r, c->comm, c->stream));
-  NCCL_TRY(g_nccl.Send(d_shard, shard_bytes, ncclChar, root, c->comm, c->stream));
-  NCCL_TRY(g_nccl.GroupEnd());
-  return B2L_OK;
-}
-extern "C" int b2l_comm_barrier(b2l_ctx* c) {
-  if (!c || !c->comm) return fail(B2L_ERR_INVALID, "communicator not initialised");
-  DeviceGuard g(c->device);
-  int rc = ensure_clip_max(c, 1);
-  if (rc) return rc;
-  NCCL_TRY(g_nccl.AllReduce(c->d_clip_max, c->d_clip_max, 1, ncclChar, 0 /* ncclSum */, c->comm, c->stream));
-  CUDA_TRY(cudaStreamSynchronize(c->stream));
   return B2L_OK;
 }

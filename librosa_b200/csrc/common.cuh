@@ -21,6 +21,8 @@ enum FwdMode : int {
   MODE_STATS = 3,  // per-frame statistics of |X| (centroid, bandwidth, rolloff, flatness, rms) [clip][stat][frame]
 };
 
+constexpr int kMrMaxPass = 12;   // radix passes of the mixed-radix kernels (mr_kernel.cuh)
+
 struct MelBand { int lo, len, off, pad; };   // bins [lo, lo+len), weights at mel_w[off ..] (mel_project kernel)
 // Fused-kernel form of one mel row: `quads` groups of 4 consecutive bins starting at bin `lo` (a multiple of
 // 4), weights at mel_w[off ..] (zero padded to 4*quads, off % 4 == 0).  Rows are grouped H at a time (a work

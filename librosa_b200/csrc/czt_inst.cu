@@ -11,30 +11,12 @@ namespace b2l {
 #define B2L_CAT2(a, b) a##b
 #define B2L_CAT(a, b) B2L_CAT2(a, b)
 
-cudaError_t B2L_CAT(czt_op_, B2L_LOG2M)(int op, const CztArgs* a, int grid, size_t smem, cudaStream_t st, int* result) {
-  constexpr int L = B2L_LOG2M;
-  constexpr int P = 1 << L;
-  constexpr int TPF = P >= 32 ? P / 32 : 1;
-  constexpr int NW = L >= 10 ? 16 : (TPF > 16 ? 16 : TPF);
-  auto kern = czt_kernel<L, TPF, NW>;
-  if (op == OP_SET_SMEM) return cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (op == OP_OCCUPANCY) return cudaOccupancyMaxActiveBlocksPerMultiprocessor(result, kern, NW * 32, smem);
-  kern<<<grid, NW * 32, smem, st>>>(*a);
-  return cudaGetLastError();
-}
+constexpr int L = B2L_LOG2M;
+constexpr int P = 1 << L;
+constexpr int TPF = P >= 32 ? P / 32 : 1;
+constexpr int NW = L >= 10 ? 16 : (TPF > 16 ? 16 : TPF);   // HostFftCfg::czt_nw
 
-
-cudaError_t B2L_CAT(czt_inv_op_, B2L_LOG2M)(int op, const CztInvArgs* a, int grid, size_t smem, cudaStream_t st,
-                                             int* result) {
-  constexpr int L = B2L_LOG2M;
-  constexpr int P = 1 << L;
-  constexpr int TPF = P >= 32 ? P / 32 : 1;
-  constexpr int NW = L >= 10 ? 16 : (TPF > 16 ? 16 : TPF);
-  auto kern = czt_inv_kernel<L, TPF, NW>;
-  if (op == OP_SET_SMEM) return cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (op == OP_OCCUPANCY) return cudaOccupancyMaxActiveBlocksPerMultiprocessor(result, kern, NW * 32, smem);
-  kern<<<grid, NW * 32, smem, st>>>(*a);
-  return cudaGetLastError();
-}
+CztKernel B2L_CAT(czt_kernel_, B2L_LOG2M)() { return czt_kernel<L, TPF, NW>; }
+CztInvKernel B2L_CAT(czt_inv_kernel_, B2L_LOG2M)() { return czt_inv_kernel<L, TPF, NW>; }
 
 }  // namespace b2l

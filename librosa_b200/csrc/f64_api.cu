@@ -7,59 +7,12 @@
 
 #include <vector>
 
-#include "../../include/b2l.h"
 #include "f64_kernels.cuh"
 #include "internal.h"
 
 using namespace b2l;
 
-#define F64_TRY(expr)                                                                                      \
-  do {                                                                                                     \
-    cudaError_t _e = (expr);                                                                               \
-    if (_e != cudaSuccess) {                                                                               \
-      cudaGetLastError();                                                                                  \
-      return b2l_internal_fail(_e == cudaErrorMemoryAllocation ? B2L_ERR_OOM : B2L_ERR_CUDA, "%s: %s (%s:%d)", #expr, \
-                               cudaGetErrorString(_e), __FILE__, __LINE__);                                \
-    }                                                                                                      \
-  } while (0)
-
 namespace {
-
-struct DevGuard {
-  int prev = -1;
-  explicit DevGuard(int dev) {
-    cudaGetDevice(&prev);
-    if (prev != dev) cudaSetDevice(dev);
-    else prev = -1;
-  }
-  ~DevGuard() {
-    if (prev >= 0) cudaSetDevice(prev);
-  }
-};
-
-// stream-ordered temporary: freed behind the work that uses it, no host synchronisation
-struct Temp {
-  void* p = nullptr;
-  cudaStream_t st;
-  explicit Temp(cudaStream_t s) : st(s) {}
-  cudaError_t alloc(size_t bytes) { return cudaMallocAsync(&p, bytes ? bytes : 16, st); }
-  ~Temp() {
-    if (p) cudaFreeAsync(p, st);
-  }
-};
-
-template <class T>
-cudaError_t upload(Temp& t, const T* h, size_t count) {
-  cudaError_t e = t.alloc(count * sizeof(T));
-  if (e != cudaSuccess) return e;
-  return cudaMemcpyAsync(t.p, h, count * sizeof(T), cudaMemcpyHostToDevice, t.st);   // pageable source: returns after the copy is staged
-}
-
-int ilog2_exact(int x) {
-  int l = 0;
-  while ((1 << l) < x) ++l;
-  return (1 << l) == x ? l : -1;
-}
 
 // exp(-2*pi*i*j/n), j < count, octant-reduced in long double
 std::vector<double2> twiddles(int n, int count) {
@@ -79,24 +32,24 @@ const int kMaxDft64 = 1 << 16;   // any other n_fft: direct O(n_fft^2) DFT
 
 extern "C" int b2l_stft_f64(b2l_ctx* c, const double* d_y, int64_t n_clips, int64_t n, int64_t y_stride, int32_t n_fft,
                             int32_t hop, int32_t center, int32_t pad_mode, const double* h_window, void* d_out) {
-  if (!c || !h_window) return b2l_internal_fail(B2L_ERR_INVALID, "NULL argument");
-  if (n_fft < 2 || hop < 1 || n_clips < 0 || n < 0 || y_stride < n) return b2l_internal_fail(B2L_ERR_INVALID, "bad geometry");
-  if (n > 0x7fffffffLL) return b2l_internal_fail(B2L_ERR_UNSUPPORTED, "clips longer than 2^31-1 samples are not supported");
+  if (!c || !h_window) return fail(B2L_ERR_INVALID, "NULL argument");
+  if (n_fft < 2 || hop < 1 || n_clips < 0 || n < 0 || y_stride < n) return fail(B2L_ERR_INVALID, "bad geometry");
+  if (n > 0x7fffffffLL) return fail(B2L_ERR_UNSUPPORTED, "clips longer than 2^31-1 samples are not supported");
   const long long padded = n + (center ? 2LL * (n_fft / 2) : 0);
-  if (padded < n_fft) return b2l_internal_fail(B2L_ERR_INVALID, "n_fft=%d is too large for input signal of length=%lld", n_fft, (long long)n);
+  if (padded < n_fft) return fail(B2L_ERR_INVALID, "n_fft=%d is too large for input signal of length=%lld", n_fft, (long long)n);
   const long long T = 1 + (padded - n_fft) / hop;
   if (n_clips == 0) return B2L_OK;
-  if (!d_y || !d_out) return b2l_internal_fail(B2L_ERR_INVALID, "NULL device pointer");
-  if (n_clips * T > 0x7fffffffLL) return b2l_internal_fail(B2L_ERR_UNSUPPORTED, "float64 stft: more than 2^31-1 frames in one call");
-  DevGuard g(b2l_internal_device(c));
-  cudaStream_t st = b2l_internal_stream(c);
+  if (!d_y || !d_out) return fail(B2L_ERR_INVALID, "NULL device pointer");
+  if (n_clips * T > 0x7fffffffLL) return fail(B2L_ERR_UNSUPPORTED, "float64 stft: more than 2^31-1 frames in one call");
+  DeviceGuard g(c->device);
+  cudaStream_t st = c->stream;
   const int l2 = ilog2_exact(n_fft);
   const bool fft = l2 >= 2 && n_fft <= kMaxFft64;
-  if (!fft && n_fft > kMaxDft64) return b2l_internal_fail(B2L_ERR_UNSUPPORTED, "float64 stft: n_fft=%d (direct DFT path is limited to %d)", n_fft, kMaxDft64);
+  if (!fft && n_fft > kMaxDft64) return fail(B2L_ERR_UNSUPPORTED, "float64 stft: n_fft=%d (direct DFT path is limited to %d)", n_fft, kMaxDft64);
   std::vector<double2> tw = twiddles(n_fft, fft ? n_fft / 2 + 1 : n_fft);
   Temp d_tw(st), d_win(st), d_z(st);
-  F64_TRY(upload(d_tw, tw.data(), tw.size()));
-  F64_TRY(upload(d_win, h_window, (size_t)n_fft));
+  CUDA_TRY(upload(d_tw, tw.data(), tw.size()));
+  CUDA_TRY(upload(d_win, h_window, (size_t)n_fft));
   F64FwdArgs a;
   memset(&a, 0, sizeof(a));
   a.y = d_y;
@@ -112,42 +65,39 @@ extern "C" int b2l_stft_f64(b2l_ctx* c, const double* d_y, int64_t n_clips, int6
   a.window = (const double*)d_win.p;
   a.tw = (const double2*)d_tw.p;
   a.out = (double2*)d_out;
-  a.status = b2l_internal_status(c);
+  a.status = c->d_status;
   size_t smem = fft ? (size_t)(n_fft / 2) * sizeof(double2) : (size_t)n_fft * sizeof(double);
   if (smem > 128 * 1024) {   // work area in global memory (L2 resident), one slice per frame
-    F64_TRY(d_z.alloc((size_t)n_clips * (size_t)T * smem));
+    CUDA_TRY(d_z.alloc((size_t)n_clips * (size_t)T * smem));
     a.zscratch = (double2*)d_z.p;
     smem = 0;
   }
-  F64_TRY(cudaFuncSetAttribute(stft64_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(smem ? smem : 16)));
-  stft64_kernel<<<(unsigned)(n_clips * T), 256, smem, st>>>(a);
-  F64_TRY(cudaGetLastError());
-  b2l_internal_count_launches(c, 1);
-  return B2L_OK;
+  int rc = blocks_per_sm(c, stft64_kernel, 256, smem, nullptr);
+  return rc ? rc : launch(c, stft64_kernel, (unsigned)(n_clips * T), 256, smem, a);
 }
 
 extern "C" int b2l_istft_f64(b2l_ctx* c, const void* d_D, int64_t n_clips, int64_t n_frames_stored, int64_t n_frames_used,
                              int32_t n_fft, int32_t hop, int32_t center, const double* h_window, const double* h_inv_wss,
                              int64_t out_len, double* d_y, int64_t y_stride) {
-  if (!c || !h_window || !h_inv_wss) return b2l_internal_fail(B2L_ERR_INVALID, "NULL argument");
+  if (!c || !h_window || !h_inv_wss) return fail(B2L_ERR_INVALID, "NULL argument");
   if (n_fft < 2 || hop < 1 || n_clips < 0 || n_frames_used < 1 || n_frames_used > n_frames_stored || out_len < 0 || y_stride < out_len)
-    return b2l_internal_fail(B2L_ERR_INVALID, "bad istft geometry");
+    return fail(B2L_ERR_INVALID, "bad istft geometry");
   if (n_clips == 0 || out_len == 0) return B2L_OK;
-  if (!d_D || !d_y) return b2l_internal_fail(B2L_ERR_INVALID, "NULL device pointer");
+  if (!d_D || !d_y) return fail(B2L_ERR_INVALID, "NULL device pointer");
   if (n_clips * n_frames_used > 0x7fffffffLL || out_len > 0x7fffffffLL || n_clips > 65535)
-    return b2l_internal_fail(B2L_ERR_UNSUPPORTED, "float64 istft: batch too large for one call");
-  DevGuard g(b2l_internal_device(c));
-  cudaStream_t st = b2l_internal_stream(c);
+    return fail(B2L_ERR_UNSUPPORTED, "float64 istft: batch too large for one call");
+  DeviceGuard g(c->device);
+  cudaStream_t st = c->stream;
   const int l2 = ilog2_exact(n_fft);
   const bool fft = l2 >= 2 && n_fft <= kMaxFft64;
-  if (!fft && n_fft > kMaxDft64) return b2l_internal_fail(B2L_ERR_UNSUPPORTED, "float64 istft: n_fft=%d (direct DFT path is limited to %d)", n_fft, kMaxDft64);
+  if (!fft && n_fft > kMaxDft64) return fail(B2L_ERR_UNSUPPORTED, "float64 istft: n_fft=%d (direct DFT path is limited to %d)", n_fft, kMaxDft64);
   const int F = n_fft / 2 + 1;
   std::vector<double2> tw = twiddles(n_fft, fft ? n_fft / 2 + 1 : n_fft);
   Temp d_tw(st), d_win(st), d_wss(st), d_frames(st), d_z(st);
-  F64_TRY(upload(d_tw, tw.data(), tw.size()));
-  F64_TRY(upload(d_win, h_window, (size_t)n_fft));
-  F64_TRY(upload(d_wss, h_inv_wss, (size_t)out_len));
-  F64_TRY(d_frames.alloc((size_t)n_clips * (size_t)n_frames_used * (size_t)n_fft * sizeof(double)));
+  CUDA_TRY(upload(d_tw, tw.data(), tw.size()));
+  CUDA_TRY(upload(d_win, h_window, (size_t)n_fft));
+  CUDA_TRY(upload(d_wss, h_inv_wss, (size_t)out_len));
+  CUDA_TRY(d_frames.alloc((size_t)n_clips * (size_t)n_frames_used * (size_t)n_fft * sizeof(double)));
   F64InvArgs a;
   memset(&a, 0, sizeof(a));
   a.D = (const double2*)d_D;
@@ -167,42 +117,41 @@ extern "C" int b2l_istft_f64(b2l_ctx* c, const void* d_D, int64_t n_clips, int64
   a.y_stride = y_stride;
   size_t smem = fft ? (size_t)(n_fft / 2) * sizeof(double2) : (size_t)F * sizeof(double2);
   if (smem > 128 * 1024) {
-    F64_TRY(d_z.alloc((size_t)n_clips * (size_t)n_frames_used * smem));
+    CUDA_TRY(d_z.alloc((size_t)n_clips * (size_t)n_frames_used * smem));
     a.zscratch = (double2*)d_z.p;
     smem = 0;
   }
-  F64_TRY(cudaFuncSetAttribute(istft64_frames_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(smem ? smem : 16)));
-  istft64_frames_kernel<<<(unsigned)(n_clips * n_frames_used), 256, smem, st>>>(a);
-  F64_TRY(cudaGetLastError());
+  int rc = blocks_per_sm(c, istft64_frames_kernel, 256, smem, nullptr);
+  if (rc || (rc = launch(c, istft64_frames_kernel, (unsigned)(n_clips * n_frames_used), 256, smem, a))) return rc;
   long long bx = (out_len + 255) / 256;
-  const long long cap = (8LL * b2l_internal_sm_count(c) + n_clips - 1) / n_clips;
+  const long long cap = (8LL * c->sm_count + n_clips - 1) / n_clips;
   if (bx > cap) bx = cap;
   if (bx < 1) bx = 1;
   ola64_kernel<<<dim3((unsigned)bx, (unsigned)n_clips), 256, 0, st>>>(a);
-  F64_TRY(cudaGetLastError());
-  b2l_internal_count_launches(c, 2);
+  CUDA_TRY(cudaGetLastError());
+  c->launches++;
   return B2L_OK;
 }
 
 extern "C" int b2l_f64_abs_pow(b2l_ctx* c, const void* d_D, int64_t n, double power, double* d_S) {
-  if (!c || !d_D || !d_S) return b2l_internal_fail(B2L_ERR_INVALID, "NULL argument");
+  if (!c || !d_D || !d_S) return fail(B2L_ERR_INVALID, "NULL argument");
   if (n <= 0) return B2L_OK;
-  DevGuard g(b2l_internal_device(c));
+  DeviceGuard g(c->device);
   long long grid = (n + 255) / 256;
-  const long long cap = 16LL * b2l_internal_sm_count(c);
+  const long long cap = 16LL * c->sm_count;
   if (grid > cap) grid = cap;
-  abs_pow64_kernel<<<(unsigned)grid, 256, 0, b2l_internal_stream(c)>>>((const double2*)d_D, n, power, d_S);
-  F64_TRY(cudaGetLastError());
-  b2l_internal_count_launches(c, 1);
+  abs_pow64_kernel<<<(unsigned)grid, 256, 0, c->stream>>>((const double2*)d_D, n, power, d_S);
+  CUDA_TRY(cudaGetLastError());
+  c->launches++;
   return B2L_OK;
 }
 
 extern "C" int b2l_f64_mel(b2l_ctx* c, const double* d_S, int64_t n_clips, int64_t n_frames, int32_t n_bins,
                            const float* h_mel, int32_t n_mels, double* d_out) {
-  if (!c || !d_S || !h_mel || !d_out) return b2l_internal_fail(B2L_ERR_INVALID, "NULL argument");
+  if (!c || !d_S || !h_mel || !d_out) return fail(B2L_ERR_INVALID, "NULL argument");
   if (n_clips <= 0 || n_frames <= 0 || n_mels <= 0) return B2L_OK;
-  DevGuard g(b2l_internal_device(c));
-  cudaStream_t st = b2l_internal_stream(c);
+  DeviceGuard g(c->device);
+  cudaStream_t st = c->stream;
   std::vector<MelBand> bands((size_t)n_mels);
   std::vector<float> w;
   for (int m = 0; m < n_mels; ++m) {
@@ -225,61 +174,59 @@ extern "C" int b2l_f64_mel(b2l_ctx* c, const double* d_S, int64_t n_clips, int64
   }
   if (w.empty()) w.push_back(0.0f);
   Temp d_w(st), d_b(st);
-  F64_TRY(upload(d_w, w.data(), w.size()));
-  F64_TRY(upload(d_b, bands.data(), bands.size()));
+  CUDA_TRY(upload(d_w, w.data(), w.size()));
+  CUDA_TRY(upload(d_b, bands.data(), bands.size()));
   const long long rows = n_clips * n_frames;
   const long long blocks = (rows * 32 + 255) / 256;
-  if (blocks > 0x7fffffffLL) return b2l_internal_fail(B2L_ERR_UNSUPPORTED, "float64 mel: too many frames in one call");
+  if (blocks > 0x7fffffffLL) return fail(B2L_ERR_UNSUPPORTED, "float64 mel: too many frames in one call");
   mel64_kernel<<<(unsigned)blocks, 256, 0, st>>>(d_S, (const float*)d_w.p, (const MelBand*)d_b.p, n_mels, n_bins, (int)n_frames, rows, d_out);
-  F64_TRY(cudaGetLastError());
-  b2l_internal_count_launches(c, 1);
+  CUDA_TRY(cudaGetLastError());
+  c->launches++;
   return B2L_OK;
 }
 
 extern "C" int b2l_f64_db(b2l_ctx* c, const double* d_in, int64_t n_clips, int64_t per_clip, double amin, double ref_value,
                           double top_db, double* d_out) {
-  if (!c || !d_in || !d_out) return b2l_internal_fail(B2L_ERR_INVALID, "NULL argument");
-  if (!(amin > 0.0)) return b2l_internal_fail(B2L_ERR_INVALID, "amin must be strictly positive");
+  if (!c || !d_in || !d_out) return fail(B2L_ERR_INVALID, "NULL argument");
+  if (!(amin > 0.0)) return fail(B2L_ERR_INVALID, "amin must be strictly positive");
   if (n_clips <= 0 || per_clip <= 0) return B2L_OK;
-  if (n_clips > 65535) return b2l_internal_fail(B2L_ERR_UNSUPPORTED, "float64 power_to_db: more than 65535 leading indices");
-  DevGuard g(b2l_internal_device(c));
-  cudaStream_t st = b2l_internal_stream(c);
+  if (n_clips > 65535) return fail(B2L_ERR_UNSUPPORTED, "float64 power_to_db: more than 65535 leading indices");
+  DeviceGuard g(c->device);
+  cudaStream_t st = c->stream;
   Temp d_max(st);
-  F64_TRY(d_max.alloc((size_t)n_clips * sizeof(unsigned long long)));
-  F64_TRY(cudaMemsetAsync(d_max.p, 0, (size_t)n_clips * sizeof(unsigned long long), st));
+  CUDA_TRY(d_max.alloc((size_t)n_clips * sizeof(unsigned long long)));
+  CUDA_TRY(cudaMemsetAsync(d_max.p, 0, (size_t)n_clips * sizeof(unsigned long long), st));
   long long bx = (per_clip + 255) / 256;
-  const long long cap = (8LL * b2l_internal_sm_count(c) + n_clips - 1) / n_clips;
+  const long long cap = (8LL * c->sm_count + n_clips - 1) / n_clips;
   if (bx > cap) bx = cap;
   if (bx < 1) bx = 1;
   const double db_sub = 10.0 * log10(fmax(amin, fabs(ref_value)));
   db64_kernel<<<dim3((unsigned)bx, (unsigned)n_clips), 256, 0, st>>>(d_in, per_clip, amin, db_sub, d_out, (unsigned long long*)d_max.p);
-  F64_TRY(cudaGetLastError());
-  int launches = 1;
+  CUDA_TRY(cudaGetLastError());
+  c->launches++;
   if (top_db >= 0.0) {
     db64_clamp_kernel<<<dim3((unsigned)bx, (unsigned)n_clips), 256, 0, st>>>(d_out, per_clip, top_db, (const unsigned long long*)d_max.p);
-    F64_TRY(cudaGetLastError());
-    ++launches;
+    CUDA_TRY(cudaGetLastError());
+    c->launches++;
   }
-  b2l_internal_count_launches(c, launches);
   return B2L_OK;
 }
 
 extern "C" int b2l_f64_dct(b2l_ctx* c, const double* d_L, int64_t n_clips, int32_t n_mels, int64_t n_frames,
                            const double* h_dct, int32_t n_mfcc, double* d_out) {
-  if (!c || !d_L || !h_dct || !d_out) return b2l_internal_fail(B2L_ERR_INVALID, "NULL argument");
+  if (!c || !d_L || !h_dct || !d_out) return fail(B2L_ERR_INVALID, "NULL argument");
   if (n_clips <= 0 || n_frames <= 0 || n_mfcc <= 0) return B2L_OK;
-  if (n_clips > 65535) return b2l_internal_fail(B2L_ERR_UNSUPPORTED, "float64 dct: more than 65535 leading indices");
-  DevGuard g(b2l_internal_device(c));
-  cudaStream_t st = b2l_internal_stream(c);
+  if (n_clips > 65535) return fail(B2L_ERR_UNSUPPORTED, "float64 dct: more than 65535 leading indices");
+  DeviceGuard g(c->device);
+  cudaStream_t st = c->stream;
   const size_t smem = (size_t)n_mfcc * n_mels * sizeof(double);
-  if (smem > b2l_internal_smem_optin(c)) return b2l_internal_fail(B2L_ERR_UNSUPPORTED, "float64 dct: matrix does not fit in shared memory");
+  if (smem > c->smem_optin) return fail(B2L_ERR_UNSUPPORTED, "float64 dct: matrix does not fit in shared memory");
   Temp d_dct(st);
-  F64_TRY(upload(d_dct, h_dct, (size_t)n_mfcc * n_mels));
-  F64_TRY(cudaFuncSetAttribute(dct64_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  CUDA_TRY(upload(d_dct, h_dct, (size_t)n_mfcc * n_mels));
+  int rc = blocks_per_sm(c, dct64_kernel, 128, smem, nullptr);
+  if (rc) return rc;
   long long bx = (n_frames + 127) / 128;
   if (bx < 1) bx = 1;
-  dct64_kernel<<<dim3((unsigned)bx, (unsigned)n_clips), 128, smem, st>>>(d_L, (const double*)d_dct.p, n_mels, n_mfcc, (int)n_frames, d_out);
-  F64_TRY(cudaGetLastError());
-  b2l_internal_count_launches(c, 1);
-  return B2L_OK;
+  return launch(c, dct64_kernel, dim3((unsigned)bx, (unsigned)n_clips), 128, smem, d_L, (const double*)d_dct.p, n_mels,
+                n_mfcc, (int)n_frames, d_out);
 }

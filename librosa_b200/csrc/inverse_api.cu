@@ -15,21 +15,10 @@
 
 #include <vector>
 
-#include "../../include/b2l.h"
 #include "common.cuh"
 #include "internal.h"
 
 using namespace b2l;
-
-#define INV_TRY(expr)                                                                                        \
-  do {                                                                                                       \
-    cudaError_t _e = (expr);                                                                                 \
-    if (_e != cudaSuccess) {                                                                                 \
-      cudaGetLastError();                                                                                    \
-      return b2l_internal_fail(_e == cudaErrorMemoryAllocation ? B2L_ERR_OOM : B2L_ERR_CUDA, "%s: %s (%s:%d)", #expr, \
-                               cudaGetErrorString(_e), __FILE__, __LINE__);                                  \
-    }                                                                                                        \
-  } while (0)
 
 namespace {
 
@@ -103,36 +92,17 @@ __global__ void nnls_fista_kernel(const float* __restrict__ Mel, long long n_col
   }
 }
 
-struct Temp {
-  void* p = nullptr;
-  cudaStream_t st;
-  explicit Temp(cudaStream_t s) : st(s) {}
-  cudaError_t alloc(size_t bytes) { return cudaMallocAsync(&p, bytes ? bytes : 16, st); }
-  ~Temp() {
-    if (p) cudaFreeAsync(p, st);
-  }
-};
-template <class T>
-cudaError_t upload(Temp& t, const T* h, size_t count) {
-  cudaError_t e = t.alloc(count * sizeof(T));
-  if (e != cudaSuccess) return e;
-  return cudaMemcpyAsync(t.p, h, count * sizeof(T), cudaMemcpyHostToDevice, t.st);
-}
-
 }  // namespace
 
 extern "C" int b2l_nnls_mel(b2l_ctx* c, const float* d_mel, int64_t n_clips, int64_t n_frames, int32_t n_mels,
                             int32_t n_bins, const float* h_basis, const float* h_pinv, float step, int32_t n_iter,
                             float inv_power, float* d_out) {
-  if (!c || !d_mel || !h_basis || !h_pinv || !d_out) return b2l_internal_fail(B2L_ERR_INVALID, "NULL argument");
+  if (!c || !d_mel || !h_basis || !h_pinv || !d_out) return fail(B2L_ERR_INVALID, "NULL argument");
   if (n_clips <= 0 || n_frames <= 0) return B2L_OK;
   if (n_mels < 1 || n_mels > 65535 || n_bins < 1 || n_iter < 0 || !(step > 0.0f))
-    return b2l_internal_fail(B2L_ERR_INVALID, "bad nnls geometry");
-  int prev = -1;
-  cudaGetDevice(&prev);
-  const int dev = b2l_internal_device(c);
-  if (prev != dev) cudaSetDevice(dev);
-  cudaStream_t st = b2l_internal_stream(c);
+    return fail(B2L_ERR_INVALID, "bad nnls geometry");
+  DeviceGuard g(c->device);
+  cudaStream_t st = c->stream;
   // band form of the rows and the transposed (bin -> rows) form
   std::vector<MelBand> bands((size_t)n_mels);
   std::vector<float> w;
@@ -161,10 +131,8 @@ extern "C" int b2l_nnls_mel(b2l_ctx* c, const float* d_mel, int64_t n_clips, int
     }
     bands[(size_t)m] = b;
   }
-  if (too_dense) {
-    if (prev != dev) cudaSetDevice(prev);
-    return b2l_internal_fail(B2L_ERR_UNSUPPORTED, "nnls: a frequency bin feeds more than two filters (not a triangular mel basis)");
-  }
+  if (too_dense)
+    return fail(B2L_ERR_UNSUPPORTED, "nnls: a frequency bin feeds more than two filters (not a triangular mel basis)");
   if (w.empty()) w.push_back(0.0f);
   // FISTA momentum coefficients (the same for every column)
   std::vector<float> beta((size_t)(n_iter > 0 ? n_iter : 1));
@@ -174,37 +142,22 @@ extern "C" int b2l_nnls_mel(b2l_ctx* c, const float* d_mel, int64_t n_clips, int
     beta[(size_t)i] = (float)((tk - 1.0) / tn);
     tk = tn;
   }
-  int rc = B2L_OK;
-  {
-    Temp d_band(st), d_w(st), d_bins(st), d_pinv(st), d_beta(st);
-    cudaError_t e = upload(d_band, bands.data(), bands.size());
-    if (e == cudaSuccess) e = upload(d_w, w.data(), w.size());
-    if (e == cudaSuccess) e = upload(d_bins, bins.data(), bins.size());
-    if (e == cudaSuccess) e = upload(d_pinv, h_pinv, (size_t)n_bins * n_mels);
-    if (e == cudaSuccess) e = upload(d_beta, beta.data(), beta.size());
-    const size_t smem = (size_t)n_mels * sizeof(MelBand) + ((w.size() + 3) & ~(size_t)3) * 4 + (size_t)n_bins * sizeof(BinRows) +
-                        (size_t)NNLS_WARPS * (2 * (size_t)n_bins + 2 * (size_t)n_mels) * 4;
-    if (e == cudaSuccess && smem > b2l_internal_smem_optin(c)) {
-      rc = b2l_internal_fail(B2L_ERR_UNSUPPORTED, "nnls: n_fft too large for the shared-memory iterate");
-    } else if (e == cudaSuccess) {
-      e = cudaFuncSetAttribute(nnls_fista_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-      if (e == cudaSuccess) {
-        const long long cols = n_clips * n_frames;
-        long long grid = (cols + NNLS_WARPS - 1) / NNLS_WARPS;
-        const long long cap = 2LL * b2l_internal_sm_count(c);
-        if (grid > cap) grid = cap;
-        nnls_fista_kernel<<<(unsigned)grid, NNLS_WARPS * 32, smem, st>>>(
-            d_mel, cols, (int)n_frames, n_mels, n_bins, (const MelBand*)d_band.p, (const float*)d_w.p, (int)w.size(),
-            (const BinRows*)d_bins.p, (const float*)d_pinv.p, (const float*)d_beta.p, n_iter, step, inv_power, d_out);
-        e = cudaGetLastError();
-        if (e == cudaSuccess) b2l_internal_count_launches(c, 1);
-      }
-    }
-    if (e != cudaSuccess) {
-      cudaGetLastError();
-      rc = b2l_internal_fail(e == cudaErrorMemoryAllocation ? B2L_ERR_OOM : B2L_ERR_CUDA, "nnls: %s", cudaGetErrorString(e));
-    }
-  }
-  if (prev != dev) cudaSetDevice(prev);
-  return rc;
+  Temp d_band(st), d_w(st), d_bins(st), d_pinv(st), d_beta(st);
+  CUDA_TRY(upload(d_band, bands.data(), bands.size()));
+  CUDA_TRY(upload(d_w, w.data(), w.size()));
+  CUDA_TRY(upload(d_bins, bins.data(), bins.size()));
+  CUDA_TRY(upload(d_pinv, h_pinv, (size_t)n_bins * n_mels));
+  CUDA_TRY(upload(d_beta, beta.data(), beta.size()));
+  const size_t smem = (size_t)n_mels * sizeof(MelBand) + ((w.size() + 3) & ~(size_t)3) * 4 + (size_t)n_bins * sizeof(BinRows) +
+                      (size_t)NNLS_WARPS * (2 * (size_t)n_bins + 2 * (size_t)n_mels) * 4;
+  if (smem > c->smem_optin) return fail(B2L_ERR_UNSUPPORTED, "nnls: n_fft too large for the shared-memory iterate");
+  int rc = blocks_per_sm(c, nnls_fista_kernel, NNLS_WARPS * 32, smem, nullptr);
+  if (rc) return rc;
+  const long long cols = n_clips * n_frames;
+  long long grid = (cols + NNLS_WARPS - 1) / NNLS_WARPS;
+  const long long cap = 2LL * c->sm_count;
+  if (grid > cap) grid = cap;
+  return launch(c, nnls_fista_kernel, (unsigned)grid, NNLS_WARPS * 32, smem, d_mel, cols, (int)n_frames, n_mels, n_bins,
+                (const MelBand*)d_band.p, (const float*)d_w.p, (int)w.size(), (const BinRows*)d_bins.p,
+                (const float*)d_pinv.p, (const float*)d_beta.p, n_iter, step, inv_power, d_out);
 }

@@ -22,8 +22,6 @@
 
 namespace b2l {
 
-constexpr int kMrMaxPass = 12;
-
 struct MrArgs {
   const float* y;
   long long clip_stride;

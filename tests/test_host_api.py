@@ -311,7 +311,7 @@ def test_resample_argument_handling_without_a_gpu():
 
 
 def test_frame_length_routing_table():
-    """Which kernels a frame length goes to (host mirror of csrc/api.cu: b2l_plan_create / mr_factor): powers of two
+    """Which kernels a frame length goes to (host mirror of csrc/plan.cu: b2l_plan_create / mr_factor): powers of two
     8 .. 8192 -> fwd_kernel, the 96 even sizes 12 .. 4096 with a 5-smooth half -> the mixed-radix kernels (unless
     B2L_MR=0), any other size up to 2047 -> chirp-z; the rest is refused by the float32 path."""
     from librosa_b200 import _pipeline as pl
