@@ -129,7 +129,7 @@ static int run_forward(b2l_ctx* c, const b2l_plan* p, int mode, int log_mode, co
     }
     size_t off = 0;
     a.off_win = (int)off; off = align_up(off + (size_t)N * 4, 16);
-    a.off_tw = (int)off; off = align_up(off + (size_t)cfg.tw_count() * 8, 16);
+    a.off_tw = (int)off; off = align_up(off + (size_t)cfg.tw_count(true) * 8, 16);
     a.off_bar = (int)off; off = align_up(off + 8 * nh, 16);   // "tile landed" mbarrier per half
     if (t) {
       a.off_melw = (int)off; off = align_up(off + (size_t)t->w_count * 4, 16);
@@ -176,7 +176,7 @@ static int run_forward(b2l_ctx* c, const b2l_plan* p, int mode, int log_mode, co
   a.total_tiles = (long long)a.tiles_per_clip * n_clips;
   a.tma_ok = (((uintptr_t)d_y & 15) == 0) && (y_stride % 4 == 0) && (a.in_floats % 4 == 0);
   a.window = p->d_win_fwd;
-  a.tw = p->d_tw;
+  a.tw = p->d_tw_fwd;
   a.twn = p->d_twn;
   a.out_c = out_c;
   a.out_r = out_r;

@@ -82,7 +82,7 @@ struct FwdArgs {
   int tma_ok;                // host-checked alignment of base pointer / stride / span
   // constants (device)
   const float* window;       // [n_fft] float32, already scaled by 1/2 for the packed real FFT
-  const float2* tw;          // inter-pass twiddles, FftCfg::tw_offset layout
+  const float2* tw;          // inter-pass twiddles, split table (FftCfg::tw_offset(s, true) layout)
   const float2* twn;         // exp(-2*pi*i*k/n_fft), k = 0 .. n_fft/4
   // outputs
   float2* out_c;             // MODE_STFT

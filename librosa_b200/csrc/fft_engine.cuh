@@ -147,6 +147,19 @@ __device__ __forceinline__ void dft_reg(float2 (&v)[N]) {
 }
 
 // ------------------------------------------------------------------ schedule
+// Split twiddle table of a radix-32 pass: r = kTwSplitLo*a + b.  Row j holds W^(e k) with e = tw_row_exponent(j):
+// the kTwSplitLo - 1 "low" factors (e = b), then the 32/kTwSplitLo - 1 "high" ones (e = kTwSplitLo*a).
+constexpr int kTwSplitLo = 8;
+constexpr int kTwSplitRows = (kTwSplitLo - 1) + (32 / kTwSplitLo - 1);
+__host__ __device__ constexpr int tw_row_exponent(int row, bool split_pass) {
+  return !split_pass || row < kTwSplitLo - 1 ? row + 1 : kTwSplitLo * (row - kTwSplitLo + 2);
+}
+// Passes of 2^log2m points that take the split table: radix-32 passes after the first, up to n_fft 4096 (the n_fft
+// 8192 STFT kernel spills 16 instead of 8 bytes with it).
+__host__ __device__ constexpr bool tw_split_pass(int log2m, int s, int radix) {
+  return s > 0 && radix == 32 && log2m <= 11;
+}
+
 template <int LOG2M_, int TPF_>
 struct FftCfg {
   static constexpr int LOG2M = LOG2M_;
@@ -163,13 +176,19 @@ struct FftCfg {
   }
   __host__ __device__ static constexpr int radix(int s) { return 1 << log_radix(s); }
   __host__ __device__ static constexpr int sublen(int s) { return 1 << (s * LOGP); }   // p before pass s
-  // twiddle table: pass s >= 1 stores (R_s - 1) rows of p_s entries: tw[s][(r-1)*p + k]
-  __host__ __device__ static constexpr int tw_offset(int s) {
+  // twiddle table: pass s >= 1 stores tw_rows(s) rows of p_s entries, row j at tw[tw_offset(s) + j*p + k].
+  // Full table: row r-1 = W_(pR)^(r k).  Split table: a pass of tw_split_pass stores the factors of r = 8a + b,
+  // rows W^(b k) for b = 1..7 and then W^(8a k) for a = 1..3 (see tw_row_exponent); other passes as the full table.
+  __host__ __device__ static constexpr int tw_rows(int s, bool split) {
+    return split && tw_split_pass(LOG2M_, s, radix(s)) ? kTwSplitRows : radix(s) - 1;
+  }
+  __host__ __device__ static constexpr int tw_offset(int s, bool split = false) {
     int off = 0;
-    for (int q = 1; q < s; ++q) off += (radix(q) - 1) * sublen(q);
+    for (int q = 1; q < s; ++q) off += tw_rows(q, split) * sublen(q);
     return off;
   }
   static constexpr int TW_COUNT = tw_offset(NPASS);
+  static constexpr int TW_COUNT_SPLIT = tw_offset(NPASS, true);
   // exchange buffer: M complex values, one pad slot per 32
   static constexpr int XBUF_F2 = M + M / 32;
 };
@@ -249,11 +268,13 @@ __host__ __device__ constexpr int pass0_slot_of_pair(int c) {
 // tw: the inter-pass twiddles in shared memory (FftCfg::tw_offset layout: per-thread constants, since thread t of a
 // frame group always touches the same elements).
 // FUSED0: the first butterfly stage of pass 0 was already done by load_pass0_windowed.
+// SPLIT_TW: tw is the split table (FftCfg::tw_offset(s, true)): a pass of tw_split_pass loads 10 factors per thread
+// instead of 31 twiddles and forms W^((8a + b) k) = W^(8a k) * W^(b k) right before use (one more float32 rounding).
 // pre_store() runs once, right before the first write to xbuf (multi-pass schedules only): callers that share
 // the exchange area with something else (the power rows of the previous tile) synchronise there instead of
 // before the transform, so that the register-only part of pass 0 overlaps the wait.
 struct NoHook { __device__ __forceinline__ void operator()() const {} };
-template <class Cfg, bool FUSED0 = false, class Pre = NoHook>
+template <class Cfg, bool FUSED0 = false, bool SPLIT_TW = false, class Pre = NoHook>
 __device__ __forceinline__ void fft_forward(float2 (&v)[Cfg::PPT], int t, int barrier_id, float2* __restrict__ xbuf,
                                             const float2* __restrict__ tw, Pre&& pre_store = Pre()) {
   constexpr int M = Cfg::M, TPF = Cfg::TPF, PPT = Cfg::PPT;
@@ -264,6 +285,8 @@ __device__ __forceinline__ void fft_forward(float2 (&v)[Cfg::PPT], int t, int ba
     constexpr int p = Cfg::sublen(s);
     constexpr int T = M / R;
     constexpr int NB = PPT / R;
+    constexpr bool SPLIT = SPLIT_TW && tw_split_pass(Cfg::LOG2M, s, R);
+    const float2* tws = tw + Cfg::tw_offset(s, SPLIT_TW);
     // ---- load (+ inter-pass twiddle)
     // Padded addresses: xphys(A + D) == xphys(A) + D + D/32 whenever the low five bits of A and D do not carry.
     // For groups of whole warps every offset below is a multiple of 32, so one run-time base per pass and
@@ -274,6 +297,14 @@ __device__ __forceinline__ void fft_forward(float2 (&v)[Cfg::PPT], int t, int ba
     static_for<0, NB>([&](auto B) {
       constexpr int b = decltype(B)::value;
       const int i = t + TPF * b;
+      const float2* twk = tws + (i & (p - 1));
+      float2 wlo[kTwSplitLo];   // SPLIT: wlo[b] = W^(b k), b >= 1
+      if constexpr (SPLIT) {
+        static_for<1, kTwSplitLo>([&](auto L) {
+          constexpr int lo = decltype(L)::value;
+          wlo[lo] = twk[(lo - 1) * p];
+        });
+      }
       static_for<0, R>([&](auto Rr) {
         constexpr int r = decltype(Rr)::value;
         constexpr int slot = b * R + bitrevc(r, LOGR);
@@ -285,7 +316,18 @@ __device__ __forceinline__ void fft_forward(float2 (&v)[Cfg::PPT], int t, int ba
           } else {
             x = xbuf[xphys(i + r * T)];
           }
-          if constexpr (r > 0) x = cmul(x, tw[Cfg::tw_offset(s) + (r - 1) * p + (i & (p - 1))]);
+          if constexpr (r > 0) {
+            constexpr int lo = r % kTwSplitLo, hi = r / kTwSplitLo;
+            if constexpr (!SPLIT) {
+              x = cmul(x, twk[(r - 1) * p]);
+            } else if constexpr (hi == 0) {
+              x = cmul(x, wlo[lo]);
+            } else if constexpr (lo == 0) {
+              x = cmul(x, twk[(kTwSplitLo - 2 + hi) * p]);                     // W^(8a k), a = hi
+            } else {
+              x = cmul(x, cmul(twk[(kTwSplitLo - 2 + hi) * p], wlo[lo]));
+            }
+          }
           v[slot] = x;
         }
       });

@@ -178,7 +178,7 @@ __global__ void __launch_bounds__(NW * 32, 1) fwd_kernel(const FwdArgs a) {
 
   // ---- one-time table staging (whole CTA)
   for (int i = tid; i < N; i += NT) s_win[i] = a.window[i];
-  for (int i = tid; i < Cfg::TW_COUNT; i += NT) s_tw[i] = a.tw[i];
+  for (int i = tid; i < Cfg::TW_COUNT_SPLIT; i += NT) s_tw[i] = a.tw[i];   // split layout (fft_forward SPLIT_TW)
   if constexpr (MODE == MODE_MEL) {
     for (int i = tid; i < a.mel_w_count; i += NT) s_melw[i] = a.mel_w[i];
     for (int i = tid; i < a.n_mel_rows; i += NT) s_row[i] = a.mel_rows[i];
@@ -297,30 +297,42 @@ __global__ void __launch_bounds__(NW * 32, 1) fwd_kernel(const FwdArgs a) {
     };
 
     // ---------------- M-point complex FFT
-    fft_forward<Cfg, true>(v, t, gbar, xbuf, s_tw, rows_consumed);
+    fft_forward<Cfg, true, true>(v, t, gbar, xbuf, s_tw, rows_consumed);
     if constexpr (Cfg::NPASS == 1) rows_consumed();
     // Bin pair (k, M-k), k = t + TPF*c < M/2: Z[k] is already in one of this thread's registers; only the
-    // upper half of the spectrum (indices >= M/2) has to reach its partner thread, through shared memory.
+    // upper half of the spectrum (indices >= M/2) has to reach its partner thread.
+    // One-warp groups in the row modes (n_fft 2048): v[q] = Z[t + 32q], so the partner Z[M-k] of k = t + 32c is
+    // register 31-c of lane 32-t (lane 0: its own register (32-c) mod 32, since Z[M] == Z[0]) and comes by warp
+    // shuffle, which keeps 16 stores and 16 loads per thread off the shared-memory pipe.  Everything else goes
+    // through shared memory.
+    constexpr bool SHFL_UNMIX = TPF == 32 && (MODE == MODE_MEL || MODE == MODE_STATS);
+    static_assert(!SHFL_UNMIX || (PPT == 32 && spectrum_offset<Cfg>(1) == 32), "v[q] = Z[t + 32q]");
     // un-mix addresses as one pointer per thread plus constants: measured -1.4 % (mel), -1.9 % (statistics) for
     // one-warp groups in the row modes and -0.5 % for the two-warp groups of n_fft 4096, but +6 % for the plain
     // STFT of n_fft 2048 (register allocation), which therefore keeps the index form
     constexpr bool AFFINE_UNMIX = (TPF % 32 == 0) && (TPF > 32 || MODE == MODE_MEL || MODE == MODE_STATS);
-    if constexpr (Cfg::NPASS > 1) group_sync<TPF>(gbar);
-    static_for<0, PPT>([&](auto S) {
-      constexpr int slot = decltype(S)::value;
-      constexpr int D = spectrum_offset<Cfg>(slot);
-      if constexpr (D >= M / 2) {
-        if constexpr (AFFINE_UNMIX && D % 32 == 0) sts_c64(smem_u32(xb_t) + 8u * (D + D / 32), v[slot]);   // xphys(t + D), D a multiple of 32
-        else sts_c64(smem_u32(xbuf) + 8u * xphys(t + D), v[slot]);
-      }
-    });
-    group_sync<TPF>(gbar);
+    if constexpr (!SHFL_UNMIX) {
+      if constexpr (Cfg::NPASS > 1) group_sync<TPF>(gbar);
+      static_for<0, PPT>([&](auto S) {
+        constexpr int slot = decltype(S)::value;
+        constexpr int D = spectrum_offset<Cfg>(slot);
+        if constexpr (D >= M / 2) {
+          if constexpr (AFFINE_UNMIX && D % 32 == 0) sts_c64(smem_u32(xb_t) + 8u * (D + D / 32), v[slot]);   // xphys(t + D), D a multiple of 32
+          else sts_c64(smem_u32(xbuf) + 8u * xphys(t + D), v[slot]);
+        }
+      });
+      group_sync<TPF>(gbar);
+    }
     auto pair_operands = [&](auto C, float2& A, float2& B) {
       constexpr int c = decltype(C)::value;
       constexpr int sa = slot_of_pair<Cfg>(c);
       static_assert(sa >= 0, "pair operand must be register resident");
       A = v[sa];
-      if constexpr (AFFINE_UNMIX) {
+      if constexpr (SHFL_UNMIX) {
+        const float2 send = t == 0 ? v[(32 - c) & 31] : v[31 - c];
+        B.x = __shfl_sync(0xffffffffu, send.x, (32 - t) & 31);
+        B.y = __shfl_sync(0xffffffffu, send.y, (32 - t) & 31);
+      } else if constexpr (AFFINE_UNMIX) {
         // padded slot of Z[M - k], k = t + TPF*c:  K_c - xphys(t) (+ 1 in lane 0 of a warp), K_c a constant —
         // see partner_slot; folded into one pointer per thread
         constexpr int K = 33 * (M / 32 - 1 - (TPF / 32) * c) + 32;
@@ -332,6 +344,10 @@ __global__ void __launch_bounds__(NW * 32, 1) fwd_kernel(const FwdArgs a) {
           if (t == 0) B = A;   // k = 0 pairs with itself (Z[M] == Z[0])
         }
       }
+    };
+    auto middle_bin = [&]() -> float2 {   // Z[M/2], read by t == 0 only
+      if constexpr (SHFL_UNMIX) return v[PPT / 2];
+      else return xbuf[xphys(M / 2)];
     };
 
     const int frame = t0 + grp;
@@ -353,7 +369,7 @@ __global__ void __launch_bounds__(NW * 32, 1) fwd_kernel(const FwdArgs a) {
       });
       if (t == 0) {
         float2 xa, xb;
-        float2 zc = xbuf[xphys(M / 2)];
+        float2 zc = middle_bin();
         r2c_pair(zc, zc, make_float2(0.0f, -1.0f), xa, xb);   // W_N^(M/2) = -i
         stg_c64_if(orow + M / 2, xa, frame_ok);
       }
@@ -371,7 +387,7 @@ __global__ void __launch_bounds__(NW * 32, 1) fwd_kernel(const FwdArgs a) {
       pw[PPT] = 0.0f;
       if (t == 0) {
         float2 xa, xb;
-        float2 zc = xbuf[xphys(M / 2)];
+        float2 zc = middle_bin();
         r2c_pair(zc, zc, make_float2(0.0f, -1.0f), xa, xb);
         pw[PPT] = sqmag(xa);
       }
@@ -403,7 +419,7 @@ __global__ void __launch_bounds__(NW * 32, 1) fwd_kernel(const FwdArgs a) {
         // MelLayout): only the group itself has to be done with its Z before the row is written.  Bins
         // M+1 .. M+3 of every row are kept at zero so that 4-bin groups may run past the Nyquist bin.
         constexpr int RS = ML::RS;
-        group_sync<TPF>(gbar);   // every thread of the group has fetched its pair operands
+        group_sync<TPF>(gbar);   // every thread of the group is done reading the exchange region (last pass, pairs)
         float* prow = reinterpret_cast<float*>(xbuf);
         static_for<0, NPAIR>([&](auto C) {
           constexpr int c = decltype(C)::value;

@@ -11,6 +11,7 @@
 
 #include "../../include/b2l.h"
 #include "common.cuh"
+#include "fft_engine.cuh"
 
 namespace b2l {
 
@@ -51,12 +52,14 @@ struct HostFftCfg {
   int log_radix(int s) const { int left = log2m - s * logp; return left >= logp ? logp : left; }
   int radix(int s) const { return 1 << log_radix(s); }
   int sublen(int s) const { return 1 << (s * logp); }
-  int tw_offset(int s) const {
+  bool split_pass(int s, bool split) const { return split && tw_split_pass(log2m, s, radix(s)); }
+  int tw_rows(int s, bool split) const { return split_pass(s, split) ? kTwSplitRows : radix(s) - 1; }
+  int tw_offset(int s, bool split = false) const {
     int off = 0;
-    for (int q = 1; q < s; ++q) off += (radix(q) - 1) * sublen(q);
+    for (int q = 1; q < s; ++q) off += tw_rows(q, split) * sublen(q);
     return off;
   }
-  int tw_count() const { return tw_offset(npass); }
+  int tw_count(bool split = false) const { return tw_offset(npass, split); }
   int xbuf_f2() const { return M + M / 32; }
   // warps per CTA of czt_kernel for P = 2^log2p (mirror of czt_inst.cu)
   int czt_nw() const { return log2m >= 10 ? 16 : (tpf > 16 ? 16 : tpf); }
@@ -112,7 +115,8 @@ struct b2l_plan {
   mutable std::vector<void*> allocs;
   float* d_win_fwd = nullptr;   // window * 1/2
   float* d_win_inv = nullptr;   // window * 1/n_fft
-  float2* d_tw = nullptr;
+  float2* d_tw = nullptr;       // inter-pass twiddles, full table (inv_kernel)
+  float2* d_tw_fwd = nullptr;   // inter-pass twiddles, split table (fwd_kernel)
   float2* d_twn = nullptr;
   int tw_count = 0;
   // mel: band-sparse rows (bins [lo, lo+len) of each mel row); d_mel_w / d_band feed mel_project, the

@@ -23,21 +23,22 @@ static int upload(const b2l_plan* p, const std::vector<T>& h, T** d) {
   return B2L_OK;
 }
 
-static const double kPi = 3.14159265358979323846264338327950288;
-
-// inter-pass twiddles of the register FFT for a complex size 2^log2m (FftCfg::tw_offset layout)
-static std::vector<float2> engine_twiddles(const HostFftCfg& cfg) {
+// inter-pass twiddles of the register FFT for a complex size 2^log2m (FftCfg::tw_offset layout): the full table, or
+// the split one of fwd_kernel (radix-32 passes as the factors of tw_row_exponent)
+static std::vector<float2> engine_twiddles(const HostFftCfg& cfg, bool split = false) {
   const double two_pi = 6.283185307179586476925286766559;
-  std::vector<float2> tw((size_t)cfg.tw_count());
+  std::vector<float2> tw((size_t)cfg.tw_count(split));
   for (int s = 1; s < cfg.npass; ++s) {
-    const int R = cfg.radix(s), pl = cfg.sublen(s), off = cfg.tw_offset(s);
-    for (int r = 1; r < R; ++r)
+    const int R = cfg.radix(s), pl = cfg.sublen(s), off = cfg.tw_offset(s, split);
+    for (int j = 0; j < cfg.tw_rows(s, split); ++j) {
+      const int e = tw_row_exponent(j, cfg.split_pass(s, split));
       for (int k = 0; k < pl; ++k) {
-        // exp(-2*pi*i * r*k / (p*R)); reduce the integer phase first to keep the argument small
-        long long num = ((long long)r * k) % ((long long)pl * R);
+        // exp(-2*pi*i * e*k / (p*R)); reduce the integer phase first to keep the argument small
+        long long num = ((long long)e * k) % ((long long)pl * R);
         double ang = -two_pi * (double)num / (double)((long long)pl * R);
-        tw[(size_t)off + (size_t)(r - 1) * pl + k] = make_float2((float)cos(ang), (float)sin(ang));
+        tw[(size_t)off + (size_t)j * pl + k] = make_float2((float)cos(ang), (float)sin(ang));
       }
+    }
   }
   return tw;
 }
@@ -100,7 +101,8 @@ static int build_pow2(b2l_plan* p, const double* window) {
   p->tw_count = cfg.tw_count();
   int rc;
   if ((rc = upload(p, wf, &p->d_win_fwd)) || (rc = upload(p, wi, &p->d_win_inv)) ||
-      (rc = upload(p, engine_twiddles(cfg), &p->d_tw)) || (rc = upload(p, unmix_twiddles(N), &p->d_twn)))
+      (rc = upload(p, engine_twiddles(cfg), &p->d_tw)) || (rc = upload(p, engine_twiddles(cfg, true), &p->d_tw_fwd)) ||
+      (rc = upload(p, unmix_twiddles(N), &p->d_twn)))
     return rc;
   return B2L_OK;
 }
