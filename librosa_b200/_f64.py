@@ -13,6 +13,7 @@ from typing import Optional
 import numpy as np
 
 from . import _native as nat
+from . import _pipeline as pl
 from . import filters
 from .util.exceptions import ParameterError
 from .util.utils import fix_length, tiny
@@ -36,25 +37,20 @@ def require_supported(n_fft: int):
                                    f"{MAX_FFT}, other sizes up to {MAX_DFT}; no CPU fallback)")
 
 
-def _clips(shape_lead):
-    return int(np.prod(shape_lead, dtype=np.int64)) if shape_lead else 1
-
-
-def to_device(ctx, y: np.ndarray) -> nat.DeviceArray:
-    return ctx.to_device(np.ascontiguousarray(y, dtype=np.float64))
-
-
-def stft(ctx, yd: nat.DeviceArray, *, n_fft, hop_length, center, mode, win: np.ndarray) -> nat.DeviceArray:
-    """complex128 STFT of a float64 device batch ``(..., n)`` -> DeviceArray ``(..., F, T)`` in the native
-    ``[frame][bin]`` memory layout."""
-    lead, n = tuple(yd.shape[:-1]), yd.shape[-1]
-    F = 1 + n_fft // 2
-    T = 1 + (n + (2 * (n_fft // 2) if center else 0) - n_fft) // hop_length
-    D = nat.DeviceArray.empty(ctx, lead + (F, T), np.complex128, layout="ft")
+def stft(y, *, n_fft, hop_length, center, mode, win: np.ndarray):
+    """complex128 STFT of a float64 signal batch ``(..., n)``, host or device -> (its StagedInput, DeviceArray
+    ``(..., F, T)`` in the native ``[frame][bin]`` memory layout).  ``staged.result`` gives the caller's value."""
+    require_supported(n_fft)
+    staged = pl.StagedInput(y, np.float64)
+    ctx, n = staged.ctx, staged.n
+    D = nat.DeviceArray.empty(ctx, staged.lead + (1 + n_fft // 2, pl.frame_count(n, n_fft, hop_length, center)),
+                              np.complex128, layout="ft")
     w = np.ascontiguousarray(win, dtype=np.float64)
-    nat.check(nat.lib().b2l_stft_f64(ctx.handle, _vp(yd.ptr), _clips(lead), n, n, int(n_fft), int(hop_length),
-                                     1 if center else 0, nat.PAD_MODES[mode], w.ctypes.data_as(_dp), _vp(D.ptr)))
-    return D
+    nat.check(nat.lib().b2l_stft_f64(ctx.handle, _vp(staged.dev.ptr), staged.n_clips, n, n, int(n_fft),
+                                     int(hop_length), 1 if center else 0, nat.PAD_MODES[mode], w.ctypes.data_as(_dp),
+                                     _vp(D.ptr)))
+    staged.release()
+    return staged, D
 
 
 def inv_wss(window, n_frames, win_length, n_fft, hop_length, start, out_len) -> np.ndarray:
@@ -74,9 +70,9 @@ def istft(ctx, Dd: nat.DeviceArray, *, n_frames_used, n_fft, hop_length, center,
     y = nat.DeviceArray.empty(ctx, lead + (out_len,), np.float64)
     w = np.ascontiguousarray(win, dtype=np.float64)
     iv = np.ascontiguousarray(inv, dtype=np.float64)
-    nat.check(nat.lib().b2l_istft_f64(ctx.handle, _vp(Dd.ptr), _clips(lead), T_stored, int(n_frames_used), int(n_fft),
-                                      int(hop_length), 1 if center else 0, w.ctypes.data_as(_dp), iv.ctypes.data_as(_dp),
-                                      int(out_len), _vp(y.ptr), int(out_len)))
+    nat.check(nat.lib().b2l_istft_f64(ctx.handle, _vp(Dd.ptr), pl.clip_count(lead), T_stored, int(n_frames_used),
+                                      int(n_fft), int(hop_length), 1 if center else 0, w.ctypes.data_as(_dp),
+                                      iv.ctypes.data_as(_dp), int(out_len), _vp(y.ptr), int(out_len)))
     return y
 
 
@@ -95,8 +91,8 @@ def mel(ctx, Sd: nat.DeviceArray, basis: np.ndarray) -> nat.DeviceArray:
     if b.shape[1] != F:
         raise ParameterError(f"mel basis has {b.shape[1]} bins, the spectrogram {F}")
     out = nat.DeviceArray.empty(ctx, lead + (b.shape[0], T), np.float64)
-    nat.check(nat.lib().b2l_f64_mel(ctx.handle, _vp(Sd.ptr), _clips(lead), T, F, b.ctypes.data_as(C.POINTER(C.c_float)),
-                                    b.shape[0], _vp(out.ptr)))
+    nat.check(nat.lib().b2l_f64_mel(ctx.handle, _vp(Sd.ptr), pl.clip_count(lead), T, F,
+                                    b.ctypes.data_as(C.POINTER(C.c_float)), b.shape[0], _vp(out.ptr)))
     return out
 
 
@@ -105,7 +101,7 @@ def power_to_db(ctx, Sd: nat.DeviceArray, *, ref_value: float, amin: float, top_
     lead = tuple(Sd.shape[:-2])
     per = Sd.shape[-2] * Sd.shape[-1]
     out = nat.DeviceArray.empty(ctx, Sd.shape, np.float64, layout=Sd.layout)
-    nat.check(nat.lib().b2l_f64_db(ctx.handle, _vp(Sd.ptr), _clips(lead), per, float(amin), float(ref_value),
+    nat.check(nat.lib().b2l_f64_db(ctx.handle, _vp(Sd.ptr), pl.clip_count(lead), per, float(amin), float(ref_value),
                                    -1.0 if top_db is None else float(top_db), _vp(out.ptr)))
     return out
 
@@ -114,18 +110,6 @@ def dct(ctx, Ld: nat.DeviceArray, basis64: np.ndarray) -> nat.DeviceArray:
     lead, n_mels, T = tuple(Ld.shape[:-2]), Ld.shape[-2], Ld.shape[-1]
     b = np.ascontiguousarray(basis64, dtype=np.float64)
     out = nat.DeviceArray.empty(ctx, lead + (b.shape[0], T), np.float64)
-    nat.check(nat.lib().b2l_f64_dct(ctx.handle, _vp(Ld.ptr), _clips(lead), n_mels, T, b.ctypes.data_as(_dp), b.shape[0],
-                                    _vp(out.ptr)))
+    nat.check(nat.lib().b2l_f64_dct(ctx.handle, _vp(Ld.ptr), pl.clip_count(lead), n_mels, T, b.ctypes.data_as(_dp),
+                                    b.shape[0], _vp(out.ptr)))
     return out
-
-
-def fetch(ctx, dev: nat.DeviceArray, validate: bool = False) -> np.ndarray:
-    """Device result -> NumPy (logical shape; "ft" arrays come back as a swapped view of [frame][bin] memory)."""
-    arr = dev.get()
-    dev.free()
-    if validate:
-        flag = C.c_int(0)
-        nat.check(nat.lib().b2l_status_read(ctx.handle, C.byref(flag)))
-        if flag.value & 1:
-            raise ParameterError("Audio buffer is not finite everywhere")
-    return arr

@@ -271,17 +271,17 @@ class Context:
         check(lib().b2l_ctx_create(int(device), C.byref(self._h)))
         self.device = int(device)
         self._plans = LRUCache()
-        self._wss = LRUCache()
+        self._constants = LRUCache()
         self._pool = {}
         self._sizes = {}
         self._pooled_bytes = 0
         # cached (released but not returned to the driver) device memory: blocks are exact-size, so variable-length
         # workloads reuse little — keep the cache well below the 80 GB of the device
         self.pool_limit_bytes = int(os.environ.get("B2L_POOL_LIMIT_MB", "16384")) << 20
-        self._finalizer = weakref.finalize(self, Context._destroy, self._h, self._plans, self._wss, self._sizes)
+        self._finalizer = weakref.finalize(self, Context._destroy, self._h, self._plans, self._constants, self._sizes)
 
     @staticmethod
-    def _destroy(h, plans, wss, sizes):
+    def _destroy(h, plans, constants, sizes):
         try:
             L = lib()
             for p in plans.values():
@@ -290,7 +290,7 @@ class Context:
             for ptr in list(sizes):
                 L.b2l_free(h, _vp(ptr))
             sizes.clear()
-            wss.clear()
+            constants.clear()
             L.b2l_ctx_destroy(h)
         except Exception:  # pragma: no cover - interpreter shutdown
             pass
@@ -370,6 +370,22 @@ class Context:
         check(lib().b2l_h2d(self._h, _vp(out.ptr), arr.ctypes.data_as(_vp), arr.nbytes))
         self.synchronize()
         return out
+
+    def constant(self, key, build) -> int:
+        """Device pointer of a small float32 table (bin frequencies, reciprocal window-sum-square, ...) cached per
+        context under ``key``; ``build()`` makes its values on a miss.  At most 32 tables: the least recently used
+        goes first, so a table fetched earlier in the same call (the youngest entry) stays."""
+        ptr = self._constants.fetch(key)
+        if ptr is None:
+            arr = np.ascontiguousarray(build(), dtype=np.float32)
+            while len(self._constants) >= 32:
+                _, old = self._constants.evict_oldest()
+                self.free(old)
+            ptr = self.alloc(max(arr.nbytes, 16))
+            check(lib().b2l_h2d(self._h, _vp(ptr), arr.ctypes.data_as(_vp), arr.nbytes))
+            self.synchronize()
+            self._constants[key] = ptr
+        return ptr
 
     # ---- events
     def event(self) -> "Event":

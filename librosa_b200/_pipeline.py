@@ -7,7 +7,7 @@ import hashlib
 import os
 import warnings
 from functools import lru_cache
-from typing import Tuple
+from typing import NamedTuple, Tuple
 
 import numpy as np
 
@@ -39,18 +39,19 @@ def native_float64(dtype) -> bool:
 _warned_float64 = False
 
 
-def _note_float64(what: str):
+def _note_float64(what: str, stacklevel: int = 4):
     global _warned_float64
     if float64_policy() in ("downcast", "native") and not _warned_float64:
         _warned_float64 = True
         warnings.warn(f"{what}: float64 data is computed in float32 by this function on the GPU (results agree with "
                       "librosa to about 1e-6 relative, not to float64 precision; stft / istft / melspectrogram / mfcc "
                       "/ power_to_db have FP64 kernels); set B2L_FLOAT64=error to refuse instead, or B2L_FLOAT64=quiet "
-                      "to silence this warning", stacklevel=4)
+                      "to silence this warning", stacklevel=stacklevel)
 
 
-def check_real_dtype(dtype, what: str, native_ok: bool = False) -> np.dtype:
-    """``native_ok``: the caller has an FP64 path for float64 data (no downcast, no warning)."""
+def check_real_dtype(dtype, what: str, native_ok: bool = False, stacklevel: int = 4) -> np.dtype:
+    """``native_ok``: the caller has an FP64 path for float64 data (no downcast, no warning); ``stacklevel``: of
+    the downcast warning, counted from ``_note_float64``."""
     dtype = np.dtype(dtype)
     if dtype == np.float32:
         return dtype
@@ -61,7 +62,7 @@ def check_real_dtype(dtype, what: str, native_ok: bool = False) -> np.dtype:
             raise nat.UnsupportedOnGPU(
                 f"{what}: dtype {dtype} is not supported by the float32 sm_90a kernels and B2L_FLOAT64=error "
                 "(there is no CPU fallback)")
-        _note_float64(what)
+        _note_float64(what, stacklevel)
         return dtype
     raise ParameterError(f"{what}: data must be floating-point, got {dtype}")
 
@@ -133,14 +134,14 @@ def check_stft_geometry(n: int, n_fft: int, center: bool, pad_mode):
         if pad_mode not in nat.PAD_MODES:
             raise ValueError(f"mode '{pad_mode}' is not supported")   # what np.pad raises
         if n_fft > n:
-            warnings.warn(f"n_fft={n_fft} is too large for input signal of length={n}", stacklevel=4)
+            warnings.warn(f"n_fft={n_fft} is too large for input signal of length={n}", stacklevel=5)
     elif n_fft > n:
         raise ParameterError(
             f"n_fft={n_fft} is too large for uncentered analysis of input signal of length={n}")
     return pad_mode if (center and isinstance(pad_mode, str)) else "constant"
 
 
-def precheck_signal(y, native_ok: bool = False):
+def precheck_signal(y, native_ok: bool = False, stacklevel: int = 4):
     """Host-side validation of an input signal, done before any GPU resource is touched so that
     argument errors surface exactly as in the reference (util.valid_audio, core/spectrum.py:240).
     Returns ``(length, requested dtype)``.  ``native_ok``: the caller has an FP64 path."""
@@ -153,14 +154,14 @@ def precheck_signal(y, native_ok: bool = False):
             raise ParameterError("Audio data must be at least one-dimensional")
         return y.shape[-1], np.dtype(np.float32)
     # util.valid_audio's type / dtype / ndim checks on the host; its O(n) np.isfinite(y).all() pass runs on
-    # the GPU instead (status word set by the kernels, see StagedInput.scan_uncovered and finish()).
+    # the GPU instead (status word set by the kernels, see StagedInput).
     if not isinstance(y, np.ndarray):
         raise ParameterError("Audio data must be of type numpy.ndarray")
     if not np.issubdtype(y.dtype, np.floating):
         raise ParameterError("Audio data must be floating-point")
     if y.ndim == 0:
         raise ParameterError(f"Audio data must be at least one-dimensional, given y.shape={y.shape}")
-    return y.shape[-1], check_real_dtype(y.dtype, "input signal", native_ok)
+    return y.shape[-1], check_real_dtype(y.dtype, "input signal", native_ok, stacklevel)
 
 
 MIN_N_FFT, MAX_N_FFT = 8, 8192   # powers of two: kMinLog2M / kMaxLog2M in csrc/internal.h
@@ -238,62 +239,166 @@ def context_for(x):
     return x.ctx if isinstance(x, nat.DeviceArray) else nat.default_context()
 
 
-class StagedInput:
-    """A batch of clips resident on the device as ``[n_clips][n]`` float32 (call precheck_signal first)."""
-
-    def __init__(self, ctx, y):
-        self.ctx = ctx
-        if isinstance(y, nat.DeviceArray):
-            if y.ctx is not ctx:
-                raise ParameterError("DeviceArray belongs to a different context")
-            self.dev = y
-            self.on_device = True
-            self.req_dtype = np.dtype(np.float32)
-        else:
-            self.req_dtype = np.dtype(y.dtype)
-            nat.check(nat.lib().b2l_status_reset(ctx.handle))
-            host = np.ascontiguousarray(y, dtype=np.float32)
-            self.dev = nat.DeviceArray.empty(ctx, host.shape, np.float32)
-            if host.nbytes:
-                nat.check(nat.lib().b2l_h2d(ctx.handle, C.c_void_p(self.dev.ptr), host.ctypes.data_as(C.c_void_p),
-                                            host.nbytes))
-            self._host = host   # keep alive until the stream has consumed it
-            self.on_device = False
-        self.lead = self.dev.shape[:-1]
-        self.n = self.dev.shape[-1]
-        self.n_clips = int(np.prod(self.lead, dtype=np.int64)) if self.lead else 1
+def clip_count(lead) -> int:
+    """Number of clips in a batch with leading dimensions ``lead`` (one for a single clip)."""
+    return int(np.prod(lead, dtype=np.int64)) if lead else 1
 
 
-    def scan_uncovered(self, n_fft: int, hop: int, center: bool, n_frames: int):
-        """Host inputs only: samples that no frame reads (the tail after the last frame, or everything
-        when hop > n_fft leaves gaps) still have to be finite for util.valid_audio — scan just those."""
-        if self.on_device or self.n_clips == 0:
-            return
-        pad = n_fft // 2 if center else 0
-        begin = 0 if hop > n_fft else max(0, (n_frames - 1) * hop + n_fft - pad)
-        if begin < self.n:
-            nat.check(nat.lib().b2l_scan_finite(self.ctx.handle, C.c_void_p(self.dev.ptr), self.n_clips, self.n,
-                                                self.n, begin))
+def frame_count(n: int, n_fft: int, hop: int, center: bool) -> int:
+    """STFT frames of an ``n``-sample signal (Appendix A.1; librosa pads ``n_fft // 2`` on each side when centred)."""
+    return 1 + (n + (2 * (n_fft // 2) if center else 0) - n_fft) // hop
 
 
-def finish(ctx, dev_out: nat.DeviceArray, to_host: bool, host_dtype=None, validate: bool = False):
-    """Return the device array itself (device-resident pipelines) or copy it to a NumPy array; with
-    ``validate`` also fetch the device-side valid_audio verdict and raise like the reference."""
-    if not to_host:
-        return dev_out
-    arr = dev_out.get()
-    dev_out.free()
-    if validate:
-        flag = C.c_int(0)
-        nat.check(nat.lib().b2l_status_read(ctx.handle, C.byref(flag)))
-        if flag.value & 1:
-            raise ParameterError("Audio buffer is not finite everywhere")
-    if host_dtype is not None and arr.dtype != host_dtype:
-        arr = arr.astype(host_dtype)
+class Front(NamedTuple):
+    n: int
+    dtype: np.dtype
+    hop: int
+    window: np.ndarray
+    wkey: str
+    mode: str
+    n_frames: int
+
+
+def forward_front(y, n_fft, hop_length, win_length, window, center, pad_mode, native_ok=True) -> Front:
+    """Argument checks of a forward op (stft, _spectrogram, melspectrogram, mfcc, the spectral statistics) in the
+    reference's order — hop, util.valid_audio, window, padding — before any GPU resource is touched."""
+    hop, win_length = frame_params(n_fft, hop_length, win_length)
+    n, dtype = precheck_signal(y, native_ok, stacklevel=5)
+    win, wkey = resolve_window(window, win_length, n_fft)
+    mode = check_stft_geometry(n, n_fft, center, pad_mode)
+    return Front(n, dtype, hop, win, wkey, mode, frame_count(n, n_fft, hop, center))
+
+
+# --------------------------------------------------------------------------------------------- status word
+def status_word(ctx) -> int:
+    """The context's status word once its stream has drained: bit 0 — a kernel saw a non-finite input sample
+    (the device half of util.valid_audio), bit 1 — a negative spectrogram entry."""
+    flag = C.c_int(0)
+    nat.check(nat.lib().b2l_status_read(ctx.handle, C.byref(flag)))
+    return flag.value
+
+
+_NOT_FINITE = "Audio buffer is not finite everywhere"
+
+
+def finish(dev: nat.DeviceArray, dtype=None, validate: bool = False) -> np.ndarray:
+    """Copy a device result to a NumPy array of its logical shape (a swapped view for "ft"), free it and cast it
+    to ``dtype``; ``validate``: raise like util.valid_audio when a kernel flagged a non-finite sample."""
+    arr = dev.get()
+    dev.free()
+    if validate and status_word(dev.ctx) & 1:
+        raise ParameterError(_NOT_FINITE)
+    if dtype is not None and arr.dtype != dtype:
+        arr = arr.astype(dtype)
     return arr
 
 
-# --------------------------------------------------------------------------------------------- host batches
+def _uncovered_begin(n_fft: int, hop: int, center: bool, n_frames: int) -> int:
+    """First sample that no frame reads; 0 when hop > n_fft leaves gaps between the frames."""
+    return 0 if hop > n_fft else max(0, (n_frames - 1) * hop + n_fft - (n_fft // 2 if center else 0))
+
+
+class StagedInput:
+    """A signal batch resident on the device as ``[n_clips][n]`` (call precheck_signal first).
+
+    For a host signal this object also runs util.valid_audio's finite check on the device: the upload resets the
+    context's status word, the kernels flag the samples they read, ``scan_uncovered`` / ``scan_all`` cover the
+    rest, and ``result`` reads the verdict with the result.  Device signals are returned as they are computed."""
+
+    def __init__(self, y, dtype=np.float32):
+        self.ctx = context_for(y)
+        self.on_device = isinstance(y, nat.DeviceArray)
+        if self.on_device:
+            self.dev = y
+        else:
+            nat.check(nat.lib().b2l_status_reset(self.ctx.handle))
+            host = np.ascontiguousarray(y, dtype=dtype)
+            self.dev = nat.DeviceArray.empty(self.ctx, host.shape, dtype)
+            if host.nbytes:
+                nat.check(nat.lib().b2l_h2d(self.ctx.handle, C.c_void_p(self.dev.ptr),
+                                            host.ctypes.data_as(C.c_void_p), host.nbytes))
+            self._host = host   # keep alive until the stream has consumed it
+        self.lead = self.dev.shape[:-1]
+        self.n = self.dev.shape[-1]
+        self.n_clips = clip_count(self.lead)
+
+    def _scan(self, begin: int):
+        if not self.on_device and self.n_clips and begin < self.n:
+            nat.check(nat.lib().b2l_scan_finite(self.ctx.handle, C.c_void_p(self.dev.ptr), self.n_clips, self.n,
+                                                self.n, begin))
+
+    def scan_uncovered(self, n_fft: int, hop_length, win_length, center: bool, n_frames: int):
+        """Scan the samples that no STFT frame reads (the tail after the last frame, or everything when the hop
+        leaves gaps); ``hop_length`` / ``win_length`` as passed to stft (None: the defaults)."""
+        hop, _ = frame_params(n_fft, hop_length, win_length)
+        self._scan(_uncovered_begin(n_fft, hop, center, n_frames))
+
+    def scan_all(self):
+        """Scan every sample (for consumers that do not flag what they read)."""
+        self._scan(0)
+
+    def release(self):
+        """Free the upload of a host signal right after the work on it is enqueued (a device signal stays)."""
+        if not self.on_device:
+            self.dev.free()
+
+    def check_finite(self):
+        if not self.on_device and status_word(self.ctx) & 1:
+            raise ParameterError(_NOT_FINITE)
+
+    def result(self, dev: nat.DeviceArray, dtype=None):
+        """The caller's return value: ``dev`` itself for a device signal, else a NumPy array of ``dtype``,
+        validated with the status verdict."""
+        return dev if self.on_device else finish(dev, dtype, validate=True)
+
+
+# --------------------------------------------------------------------------------------------- spectrogram inputs
+def spectrogram_input(S):
+    """A real spectrogram-like argument ``(..., rows, frames)``, host or device -> (DeviceArray, requested dtype,
+    input was on the device).  Host arrays are uploaded C-ordered; device arrays keep their layout."""
+    if isinstance(S, nat.DeviceArray):
+        if S.dtype != np.float32:
+            raise ParameterError("device spectrogram must be float32")
+        return S, np.dtype(np.float32), True
+    S = np.asarray(S)
+    if np.iscomplexobj(S):
+        raise ParameterError("spectrogram input must be real")
+    req = check_real_dtype(S.dtype if np.issubdtype(S.dtype, np.floating) else np.float32, "S")
+    return nat.default_context().to_device(np.ascontiguousarray(S, dtype=np.float32)), req, False
+
+
+def to_native(S, dtype=None, host_transpose: bool = False, ctx=None):
+    """A spectrogram-like array ``(..., bins, frames)``, host or device, real or complex, in any layout ->
+    (DeviceArray in the kernels' native [frame][bin] "ft" layout, whether the caller owns it).
+
+    A device array already in "ft" comes back as it is; any other goes through the transpose kernel, host arrays
+    after a C-ordered upload as ``dtype``.  ``host_transpose``: reorder a host array with NumPy instead (no copy
+    when its memory already is [frame][bin]) — for complex128, which the transpose kernel does not take.  Host
+    arrays go to ``ctx`` (default: the default context)."""
+    if not isinstance(S, nat.DeviceArray):
+        ctx = ctx or nat.default_context()
+        if not host_transpose:
+            raw = ctx.to_device(np.ascontiguousarray(S, dtype=dtype))
+            out, _ = to_native(raw)
+            raw.free()
+            return out, True
+        view = np.swapaxes(S, -1, -2)
+        mem = np.ascontiguousarray(view, dtype=dtype)
+        out = nat.DeviceArray.empty(ctx, S.shape, dtype, layout="ft")
+        if mem.nbytes:
+            nat.check(nat.lib().b2l_h2d(ctx.handle, C.c_void_p(out.ptr), mem.ctypes.data_as(C.c_void_p), mem.nbytes))
+            if mem is not view:   # a staging copy made here must outlive the upload
+                ctx.synchronize()
+        return out, True
+    if S.layout == "ft":
+        return S, False
+    out = nat.DeviceArray.empty(S.ctx, S.shape, S.dtype, layout="ft")
+    nat.check(nat.lib().b2l_transpose(S.ctx.handle, C.c_void_p(S.ptr), clip_count(S.shape[:-2]), S.shape[-2],
+                                      S.shape[-1], S.dtype.itemsize, C.c_void_p(out.ptr)))
+    return out, True
+
+
+# --------------------------------------------------------------------------------------------- forward ops
 _secondary = {}
 
 
@@ -317,31 +422,40 @@ def host_chunks(n_clips: int, nbytes: int) -> int:
     return int(min(16, n_clips // 4))   # 16 chunks: the un-overlapped head / tail is 1/16 of the transfer
 
 
-def run_host_forward(y: np.ndarray, *, n_fft: int, hop_length: int, center: bool, n_frames: int,
-                     out_mem_tail, out_dtype, make_plan, launch, scratch_per_clip: int = 0):
-    """Run one forward op over a host batch ``y`` (..., n), float32-convertible, already validated.
+def run_forward(y, *, plan_key, plan_kw, n_frames: int, out_tail, dtype, launch, layout: str = "c",
+                scratch_per_clip: int = 0):
+    """Run one forward op over a signal batch ``y`` (..., n) that forward_front has accepted.
 
-    ``make_plan(ctx)`` returns the Plan; ``launch(ctx, plan, d_in, n_clips, n, d_out, d_scratch)`` enqueues
-    the kernels; ``out_mem_tail`` is the per-clip memory shape of the result.  Large batches are cut into
-    chunks that alternate between two streams: chunk i+1 uploads while chunk i computes and downloads.
-    Returns the result as an array of memory shape ``lead + out_mem_tail`` (pinned when large).
-    """
+    ``nat.make_plan(ctx, plan_key, **plan_kw)`` gives the Plan; ``launch(ctx, plan, d_in, n_clips, n, d_out,
+    d_scratch)`` enqueues the kernels; ``out_tail`` is the logical per-clip shape of the result in ``layout``.
+    A DeviceArray ``y`` gets one launch on ``y.ctx`` and a DeviceArray result.  A host batch is validated like
+    util.valid_audio and comes back as a NumPy array (pinned when large; "ft": a swapped view of [frame][bin]
+    memory); large batches are cut into chunks that alternate between two streams, so that chunk i+1 uploads
+    while chunk i computes and downloads."""
+    n_fft, hop, center = plan_kw["n_fft"], plan_kw["hop_length"], plan_kw["center"]
+    primary = context_for(y)
+    lead, n = tuple(y.shape[:-1]), y.shape[-1]
+    n_clips = clip_count(lead)
+    plan = nat.make_plan(primary, plan_key, **plan_kw)
+    assert plan.n_frames(n) == n_frames
+    dtype = np.dtype(dtype)
+    out_tail = tuple(out_tail)
+    if isinstance(y, nat.DeviceArray):
+        out = nat.DeviceArray.empty(primary, lead + out_tail, dtype, layout=layout)
+        d_scr = primary.alloc(n_clips * scratch_per_clip * 4) if scratch_per_clip else 0
+        launch(primary, plan, y.ptr, n_clips, n, out.ptr, d_scr)
+        primary.free(d_scr)   # stream-ordered pool: the block can be handed out again without a sync
+        return out
     L = nat.lib()
-    host = np.ascontiguousarray(y, dtype=np.float32)
-    lead = host.shape[:-1]
-    n = host.shape[-1]
-    n_clips = int(np.prod(lead, dtype=np.int64)) if lead else 1
-    flat = host.reshape(n_clips, n)
-    per_clip_out = int(np.prod(out_mem_tail, dtype=np.int64))
-    out_dtype = np.dtype(out_dtype)
-    total_out = n_clips * per_clip_out * out_dtype.itemsize
-    out = nat.pinned_empty((n_clips,) + tuple(out_mem_tail), out_dtype) if total_out >= (1 << 20) else \
-        np.empty((n_clips,) + tuple(out_mem_tail), out_dtype)
-    primary = nat.default_context()
-    k = host_chunks(n_clips, host.nbytes)
+    flat = np.ascontiguousarray(y, dtype=np.float32).reshape(n_clips, n)
+    mem_tail = out_tail[::-1] if layout == "ft" else out_tail
+    per_clip_out = int(np.prod(mem_tail, dtype=np.int64))
+    total_out = n_clips * per_clip_out * dtype.itemsize
+    out = nat.pinned_empty((n_clips,) + mem_tail, dtype) if total_out >= (1 << 20) else \
+        np.empty((n_clips,) + mem_tail, dtype)
+    k = host_chunks(n_clips, flat.nbytes)
     ctxs = [primary] if k == 1 else [primary, _second_context(primary)]
-    pad = n_fft // 2 if center else 0
-    tail_begin = 0 if hop_length > n_fft else max(0, (n_frames - 1) * hop_length + n_fft - pad)
+    tail_begin = _uncovered_begin(n_fft, hop, center, n_frames)
     bounds = [(i * n_clips) // k for i in range(k + 1)]
     held = []
     used = []
@@ -354,10 +468,10 @@ def run_host_forward(y: np.ndarray, *, n_fft: int, hop_length: int, center: bool
             if ctx not in used:
                 nat.check(L.b2l_status_reset(ctx.handle))
                 used.append(ctx)
-            plan = make_plan(ctx)
+            plan = nat.make_plan(ctx, plan_key, **plan_kw)
             m = hi - lo
             d_in = ctx.alloc(m * n * 4)
-            d_out = ctx.alloc(max(m * per_clip_out * out_dtype.itemsize, 16))
+            d_out = ctx.alloc(max(m * per_clip_out * dtype.itemsize, 16))
             d_scr = ctx.alloc(m * scratch_per_clip * 4) if scratch_per_clip else 0
             held.append((ctx, d_in, d_out, d_scr))
             src = flat[lo:hi]
@@ -368,17 +482,13 @@ def run_host_forward(y: np.ndarray, *, n_fft: int, hop_length: int, center: bool
             dst = out[lo:hi]
             if dst.nbytes:
                 nat.check(L.b2l_d2h(ctx.handle, dst.ctypes.data_as(C.c_void_p), C.c_void_p(d_out), dst.nbytes))
-        bad = False
-        for ctx in used:
-            flag = C.c_int(0)
-            nat.check(L.b2l_status_read(ctx.handle, C.byref(flag)))   # synchronises that stream
-            bad |= bool(flag.value & 1)
+        flags = [status_word(ctx) for ctx in used]   # reads every stream's word: each read synchronises it
     finally:
         for ctx, d_in, d_out, d_scr in held:
             ctx.free(d_in)
             ctx.free(d_out)
-            if d_scr:
-                ctx.free(d_scr)
-    if bad:
-        raise ParameterError("Audio buffer is not finite everywhere")
-    return out.reshape(tuple(lead) + tuple(out_mem_tail))
+            ctx.free(d_scr)
+    if any(f & 1 for f in flags):
+        raise ParameterError(_NOT_FINITE)
+    res = out.reshape(lead + mem_tail)
+    return np.swapaxes(res, -1, -2) if layout == "ft" else res

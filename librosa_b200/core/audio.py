@@ -118,18 +118,14 @@ def resample(y, *, orig_sr: float, target_sr: float, res_type: str = "soxr_hq", 
     h, n_pre_remove = _poly_filter(up, down)
     n_out = (n * up + down - 1) // down                       # resample_poly's own output length
     n_total = n_samples if fix else n_out
-    on_device = isinstance(y, nat.DeviceArray)
-    ctx = y.ctx if on_device else nat.default_context()
-    staged = pl.StagedInput(ctx, y)
-    L = nat.lib()
-    if not on_device and staged.n_clips and n:
-        nat.check(L.b2l_scan_finite(ctx.handle, C.c_void_p(staged.dev.ptr), staged.n_clips, n, n, 0))
+    staged = pl.StagedInput(y)
+    staged.scan_all()
+    ctx = staged.ctx
     d_h = ctx.to_device(h)
     out = nat.DeviceArray.empty(ctx, tuple(staged.lead) + (n_total,), np.float32)
-    nat.check(L.b2l_resample_poly(ctx.handle, C.c_void_p(staged.dev.ptr), staged.n_clips, n, n, C.c_void_p(d_h.ptr),
-                                  len(h), up, down, n_pre_remove, min(n_out, n_total), n_total,
-                                  float(1.0 / np.sqrt(ratio)) if scale else 1.0, C.c_void_p(out.ptr)))
+    nat.check(nat.lib().b2l_resample_poly(ctx.handle, C.c_void_p(staged.dev.ptr), staged.n_clips, n, n,
+                                          C.c_void_p(d_h.ptr), len(h), up, down, n_pre_remove, min(n_out, n_total),
+                                          n_total, float(1.0 / np.sqrt(ratio)) if scale else 1.0, C.c_void_p(out.ptr)))
     d_h.free()
-    if not on_device:
-        staged.dev.free()
-    return out if on_device else pl.finish(ctx, out, True, req, validate=True)
+    staged.release()
+    return staged.result(out, req)

@@ -29,15 +29,8 @@ def _key_to_float(key: int) -> np.float32:
 def _tuning_from_device_spec(ctx, Sd, sr, n_fft, *, resolution, bins_per_octave, fmin, fmax, threshold, ref):
     """Sd: float32 DeviceArray (..., bins, frames), any layout.  Returns the tuning estimate (float)."""
     F, T = Sd.shape[-2], Sd.shape[-1]
-    lead = Sd.shape[:-2]
-    n_clips = int(np.prod(lead, dtype=np.int64)) if lead else 1
     L = nat.lib()
-    if Sd.layout == "ft":
-        src = Sd
-    else:
-        src = nat.DeviceArray.empty(ctx, Sd.shape, np.float32, layout="ft")
-        if n_clips and F and T:
-            nat.check(L.b2l_transpose(ctx.handle, _vp(Sd.ptr), n_clips, F, T, 4, _vp(src.ptr)))
+    src, own = pl.to_native(Sd)
     freqs = fft_frequencies(sr=sr, n_fft=n_fft)
     fmin = np.maximum(fmin, 0)
     fmax = np.minimum(fmax, float(sr) / 2)
@@ -49,7 +42,7 @@ def _tuning_from_device_spec(ctx, Sd, sr, n_fft, *, resolution, bins_per_octave,
         if callable(ref):
             raise nat.UnsupportedOnGPU("piptrack(ref=callable) other than np.max is not supported on the GPU")
         desc.ref_abs = float(np.abs(ref))
-    rows = n_clips * T
+    rows = pl.clip_count(Sd.shape[:-2]) * T
     hist = (C.c_uint64 * 2048)()
 
     def run(mode, prefix=0, mag_threshold=0.0, edges=None, n_res=0):
@@ -89,7 +82,7 @@ def _tuning_from_device_spec(ctx, Sd, sr, n_fft, *, resolution, bins_per_octave,
         counts = run(3, mag_threshold=med, edges=np.ascontiguousarray(edges, dtype=np.float64), n_res=len(edges) - 1)
         return edges[int(np.argmax(counts))]
     finally:
-        if src is not Sd:
+        if own:
             src.free()
 
 
@@ -99,7 +92,6 @@ def estimate_tuning(*, y=None, sr: float = 22050, S=None, n_fft: Optional[int] =
     ``librosa.estimate_tuning`` (``kwargs`` go to ``piptrack``: hop_length, fmin, fmax, threshold, win_length,
     window, center, pad_mode, ref — ``ref`` a number or ``np.max``)."""
     from .spectrum import _spectrogram
-    from ..feature.spectral import _spec_to_device
 
     allowed = {"hop_length", "fmin", "fmax", "threshold", "win_length", "window", "center", "pad_mode", "ref"}
     extra = set(kwargs) - allowed
@@ -107,42 +99,31 @@ def estimate_tuning(*, y=None, sr: float = 22050, S=None, n_fft: Optional[int] =
         raise TypeError(f"piptrack() got an unexpected keyword argument '{sorted(extra)[0]}'")
     pip = dict(fmin=kwargs.get("fmin", 150.0), fmax=kwargs.get("fmax", 4000.0), threshold=kwargs.get("threshold", 0.1),
                ref=kwargs.get("ref", None))
-    own = False
+    staged = None
     if S is None:
         if y is None:
             raise ParameterError("Input signal must be provided to compute a spectrogram")
         pl.precheck_signal(y)
-        validate = not isinstance(y, nat.DeviceArray)
-        if validate:
-            ctx = nat.default_context()
-            staged = pl.StagedInput(ctx, y)
-            yd = staged.dev
-        else:
-            ctx, yd = y.ctx, y
-        Sd, n_fft = _spectrogram(y=yd, n_fft=n_fft, hop_length=kwargs.get("hop_length"), power=1,
+        staged = pl.StagedInput(y)
+        Sd, n_fft = _spectrogram(y=staged.dev, n_fft=n_fft, hop_length=kwargs.get("hop_length"), power=1,
                                  win_length=kwargs.get("win_length"), window=kwargs.get("window", "hann"),
                                  center=kwargs.get("center", True), pad_mode=kwargs.get("pad_mode", "constant"))
         own = True
-        if validate:
-            hop_eff, _ = pl.frame_params(n_fft, kwargs.get("hop_length"), kwargs.get("win_length"))
-            staged.scan_uncovered(n_fft, hop_eff, kwargs.get("center", True), Sd.shape[-1])
+        staged.scan_uncovered(n_fft, kwargs.get("hop_length"), kwargs.get("win_length"), kwargs.get("center", True),
+                              Sd.shape[-1])
     else:
-        validate = False
         if not isinstance(S, nat.DeviceArray) and np.iscomplexobj(S):
             S = np.abs(S)
-        ctx = S.ctx if isinstance(S, nat.DeviceArray) else nat.default_context()
-        Sd, _, on_device = _spec_to_device(ctx, S)
+        Sd, _, on_device = pl.spectrogram_input(S)
         own = not on_device
         if n_fft is None or n_fft // 2 + 1 != Sd.shape[-2]:
             n_fft = 2 * (Sd.shape[-2] - 1)
     try:
-        est = _tuning_from_device_spec(ctx, Sd, sr, n_fft, resolution=resolution, bins_per_octave=bins_per_octave, **pip)
+        est = _tuning_from_device_spec(Sd.ctx, Sd, sr, n_fft, resolution=resolution, bins_per_octave=bins_per_octave,
+                                       **pip)
     finally:
         if own:
             Sd.free()
-    if validate:
-        flag = C.c_int(0)
-        nat.check(nat.lib().b2l_status_read(ctx.handle, C.byref(flag)))
-        if flag.value & 1:
-            raise ParameterError("Audio buffer is not finite everywhere")
+    if staged is not None:
+        staged.check_finite()
     return est

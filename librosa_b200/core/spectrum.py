@@ -30,62 +30,34 @@ def stft(y, *, n_fft: int = 2048, hop_length: Optional[int] = None, win_length: 
     Returns ``(..., 1 + n_fft/2, n_frames)`` complex64.  For a NumPy input the result is a view whose
     memory is ``[..., frame, bin]`` — for a 1-D signal that is the Fortran order librosa returns.
     """
-    hop_length, win_length = pl.frame_params(n_fft, hop_length, win_length)
-    # host-side validation in the reference's order (valid_audio, window, padding), before any GPU work
-    n, req_dtype = pl.precheck_signal(y, native_ok=True)
-    win, wkey = pl.resolve_window(window, win_length, n_fft)
-    mode = pl.check_stft_geometry(n, n_fft, center, pad_mode)
+    fr = pl.forward_front(y, n_fft, hop_length, win_length, window, center, pad_mode)
     if dtype is None:
-        dtype = dtype_r2c(req_dtype)
+        dtype = dtype_r2c(fr.dtype)
     dtype = np.dtype(dtype)
-    if pl.wide_route(y, req_dtype, n_fft):
-        y64 = y if req_dtype == np.float64 else np.asarray(y, dtype=np.float64)
-        return _stft_f64(y64, n, n_fft, hop_length, center, mode, win, dtype, out)
+    if pl.wide_route(y, fr.dtype, n_fft):
+        return _stft_f64(y, fr, n_fft, center, dtype, out)
     if dtype != np.complex64 and not (dtype.kind == "c" and pl.wide_complex_ok("stft dtype")):
         raise nat.UnsupportedOnGPU(f"stft dtype={dtype}: only complex64 is computed on the GPU "
                                    "(B2L_FLOAT64=error forbids returning float32 results in a wider dtype)")
-    F = 1 + n_fft // 2
-    T = 1 + (n + (2 * (n_fft // 2) if center else 0) - n_fft) // hop_length   # Appendix A.1 frame count
-    shape = tuple(y.shape[:-1]) + (F, T)
+    shape = tuple(y.shape[:-1]) + (1 + n_fft // 2, fr.n_frames)
     if out is not None:
-        if isinstance(out, nat.DeviceArray):
-            raise ParameterError("out= must be a NumPy array")
-        if not (tuple(out.shape[:-1]) == tuple(shape[:-1]) and out.shape[-1] >= shape[-1]):
-            raise ParameterError(f"Shape mismatch for provided output array out.shape={out.shape} and "
-                                 f"target shape={list(shape)}")
-        if not np.iscomplexobj(out):
-            raise ParameterError(f"output with dtype={out.dtype} is not of complex type")
+        _check_out(out, shape)
     pl.require_supported_n_fft(n_fft)
-    key = ("stft", n_fft, hop_length, bool(center), mode, wkey)
 
-    def make_plan(ctx):
-        return nat.make_plan(ctx, key, n_fft=n_fft, hop_length=hop_length, center=center, pad_mode=mode, window=win)
+    def launch(ctx, plan, d_in, m, n_, d_out, d_scr):
+        nat.check(nat.lib().b2l_stft(ctx.handle, plan.handle, _vp(d_in), m, n_, n_, _vp(d_out)))
 
-    if isinstance(y, nat.DeviceArray):
-        ctx = y.ctx
-        staged = pl.StagedInput(ctx, y)
-        plan = make_plan(ctx)
-        assert plan.n_frames(staged.n) == T
-        D = nat.DeviceArray.empty(ctx, shape, np.complex64, layout="ft")
-        nat.check(nat.lib().b2l_stft(ctx.handle, plan.handle, _vp(staged.dev.ptr), staged.n_clips, staged.n,
-                                     staged.n, _vp(D.ptr)))
+    res = pl.run_forward(y, plan_key=("stft", n_fft, fr.hop, bool(center), fr.mode, fr.wkey),
+                         plan_kw=dict(n_fft=n_fft, hop_length=fr.hop, center=center, pad_mode=fr.mode,
+                                      window=fr.window),
+                         n_frames=fr.n_frames, out_tail=shape[-2:], dtype=np.complex64, layout="ft", launch=launch)
+    if isinstance(res, nat.DeviceArray):
         if out is None:
-            return D
-        res = pl.finish(ctx, D, True, dtype)
-    else:
-        def launch(ctx, plan, d_in, m, n_, d_out, d_scr):
-            nat.check(nat.lib().b2l_stft(ctx.handle, plan.handle, _vp(d_in), m, n_, n_, _vp(d_out)))
-
-        mem = pl.run_host_forward(y, n_fft=n_fft, hop_length=hop_length, center=center, n_frames=T,
-                                  out_mem_tail=(T, F), out_dtype=np.complex64, make_plan=make_plan, launch=launch)
-        res = np.swapaxes(mem, -1, -2)
-        if res.dtype != dtype:
-            res = res.astype(dtype)
-    if out is None:
-        return res
-    target = out if out.shape[-1] == shape[-1] else out[..., : shape[-1]]
-    target[...] = res
-    return target
+            return res
+        res = pl.finish(res, dtype)
+    elif res.dtype != dtype:
+        res = res.astype(dtype)
+    return res if out is None else _write_out(out, res)
 
 
 def _check_out(out, shape):
@@ -98,56 +70,53 @@ def _check_out(out, shape):
         raise ParameterError(f"output with dtype={out.dtype} is not of complex type")
 
 
-def _stft_f64(y, n, n_fft, hop_length, center, mode, win, dtype, out):
-    """float64 signal -> complex128 STFT in FP64 on the device (what the reference computes: dtype_r2c,
-    core/spectrum.py:341; window product and rfft in double, :388)."""
-    if dtype.kind != "c":
-        raise ParameterError(f"stft dtype={dtype} is not complex")
-    F = 1 + n_fft // 2
-    T = 1 + (n + (2 * (n_fft // 2) if center else 0) - n_fft) // hop_length
-    shape = tuple(y.shape[:-1]) + (F, T)
-    if out is not None:
-        _check_out(out, shape)
-    f64.require_supported(n_fft)
-    on_device = isinstance(y, nat.DeviceArray)
-    ctx = y.ctx if on_device else nat.default_context()
-    if not on_device:
-        nat.check(nat.lib().b2l_status_reset(ctx.handle))
-    yd = y if on_device else f64.to_device(ctx, y)
-    D = f64.stft(ctx, yd, n_fft=n_fft, hop_length=hop_length, center=center, mode=mode, win=win)
-    if not on_device:
-        yd.free()
-    if on_device and out is None:
-        return D
-    res = f64.fetch(ctx, D, validate=not on_device)
-    if res.dtype != dtype:
-        res = res.astype(dtype)
-    if out is None:
-        return res
-    target = out if out.shape[-1] == shape[-1] else out[..., : shape[-1]]
+def _write_out(out, res):
+    """stft(out=...): the result goes into the first frames of ``out`` (librosa allows a longer buffer)."""
+    target = out if out.shape[-1] == res.shape[-1] else out[..., : res.shape[-1]]
     target[...] = res
     return target
 
 
+def _stft_f64(y, fr, n_fft, center, dtype, out):
+    """float64 signal -> complex128 STFT in FP64 on the device (what the reference computes: dtype_r2c,
+    core/spectrum.py:341; window product and rfft in double, :388)."""
+    if dtype.kind != "c":
+        raise ParameterError(f"stft dtype={dtype} is not complex")
+    if out is not None:
+        _check_out(out, tuple(y.shape[:-1]) + (1 + n_fft // 2, fr.n_frames))
+    staged, D = f64.stft(y, n_fft=n_fft, hop_length=fr.hop, center=center, mode=fr.mode, win=fr.window)
+    if staged.on_device and out is None:
+        return D
+    res = pl.finish(D, dtype, validate=not staged.on_device)
+    return res if out is None else _write_out(out, res)
+
+
 def _inv_wss(ctx, window, n_frames, win_length, n_fft, hop_length, start, out_len, wkey):
     """Reciprocal window-sum-square, trimmed as istft does (core/spectrum.py:606-624), cached on device."""
-    key = ("wss", wkey, n_frames, n_fft, hop_length, start, out_len)
-    ptr = ctx._wss.fetch(key)
-    if ptr is None:
+    def build():
         wss = filters.window_sumsquare(window=window, n_frames=n_frames, win_length=win_length, n_fft=n_fft,
                                        hop_length=hop_length, dtype=np.float32)
         wss = fix_length(wss[start:], size=out_len)
         inv = np.ones(out_len, dtype=np.float32)
         nz = wss > tiny(wss)
         inv[nz] = (np.float32(1.0) / wss[nz]).astype(np.float32)
-        while len(ctx._wss) >= 32:                 # least recently used first
-            _, old = ctx._wss.evict_oldest()
-            ctx.free(old)
-        ptr = ctx.alloc(max(inv.nbytes, 16))
-        nat.check(nat.lib().b2l_h2d(ctx.handle, _vp(ptr), inv.ctypes.data_as(_vp), inv.nbytes))
-        ctx.synchronize()
-        ctx._wss[key] = ptr
-    return ptr
+        return inv
+
+    return ctx.constant(("wss", wkey, n_frames, n_fft, hop_length, start, out_len), build)
+
+
+def _istft_out_len(n_fft, hop_length, n_frames, center, length) -> int:
+    if length:
+        return int(length)
+    return n_fft + hop_length * (n_frames - 1) - (2 * (n_fft // 2) if center else 0)
+
+
+def _check_istft_out(out, shape):
+    if out is not None:
+        if isinstance(out, nat.DeviceArray):
+            raise ParameterError("out= must be a NumPy array")
+        if tuple(out.shape) != shape:
+            raise ParameterError(f"Shape mismatch for provided output array out.shape={out.shape} != {list(shape)}")
 
 
 def _istft_f64(stft_matrix, on_device, n_frames, T_stored, F, n_fft, hop_length, win_length, window, win, center,
@@ -158,45 +127,22 @@ def _istft_f64(stft_matrix, on_device, n_frames, T_stored, F, n_fft, hop_length,
     dtype = np.dtype(dtype)
     if not np.issubdtype(dtype, np.floating):
         raise ParameterError(f"istft dtype={dtype} must be a floating-point type")
-    full_len = n_fft + hop_length * (n_frames - 1)
-    if length:
-        out_len = int(length)
-    elif center:
-        out_len = full_len - 2 * (n_fft // 2)
-    else:
-        out_len = full_len
-    lead = tuple(stft_matrix.shape[:-2])
-    shape = lead + (out_len,)
-    if out is not None:
-        if isinstance(out, nat.DeviceArray):
-            raise ParameterError("out= must be a NumPy array")
-        if tuple(out.shape) != shape:
-            raise ParameterError(f"Shape mismatch for provided output array out.shape={out.shape} != {list(shape)}")
+    out_len = _istft_out_len(n_fft, hop_length, n_frames, center, length)
+    _check_istft_out(out, tuple(stft_matrix.shape[:-2]) + (out_len,))
     f64.require_supported(n_fft)
-    ctx = stft_matrix.ctx if on_device else nat.default_context()
-    if on_device:
-        if stft_matrix.layout != "ft":
-            raise ParameterError("device complex128 stft_matrix must be in the native [frame][bin] layout")
-        Dd, own = stft_matrix, False
-    else:
-        mem = np.ascontiguousarray(np.swapaxes(stft_matrix, -1, -2))      # [..., frame, bin]
-        Dd = nat.DeviceArray(ctx, ctx.alloc(max(mem.nbytes, 16)), stft_matrix.shape, np.complex128, layout="ft")
-        if mem.nbytes:
-            nat.check(nat.lib().b2l_h2d(ctx.handle, _vp(Dd.ptr), mem.ctypes.data_as(_vp), mem.nbytes))
-            ctx.synchronize()
-        own = True
+    if on_device and stft_matrix.layout != "ft":
+        raise ParameterError("device complex128 stft_matrix must be in the native [frame][bin] layout")
+    Dd, own = pl.to_native(stft_matrix, np.complex128, host_transpose=True)
+    ctx = Dd.ctx
     start = n_fft // 2 if center else 0
     inv = f64.inv_wss(window, n_frames, win_length, n_fft, hop_length, start, out_len)
     y = f64.istft(ctx, Dd, n_frames_used=n_frames, n_fft=n_fft, hop_length=hop_length, center=center, win=win,
                   inv=inv, out_len=out_len)
     if own:
-        ctx.synchronize()
         Dd.free()
     if on_device and out is None:
         return y
-    res = f64.fetch(ctx, y)
-    if res.dtype != dtype:
-        res = res.astype(dtype)
+    res = pl.finish(y, dtype)
     if out is None:
         return res
     out[...] = res
@@ -244,65 +190,29 @@ def istft(stft_matrix, *, hop_length: Optional[int] = None, win_length: Optional
     if dtype is None:
         dtype = dtype_c2r(in_dtype)
     dtype = pl.check_real_dtype(dtype, "istft dtype")
-    full_len = n_fft + hop_length * (n_frames - 1)
-    if length:
-        out_len = int(length)
-    elif center:
-        out_len = full_len - 2 * (n_fft // 2)
-    else:
-        out_len = full_len
+    out_len = _istft_out_len(n_fft, hop_length, n_frames, center, length)
     lead = tuple(stft_matrix.shape[:-2])
-    shape = lead + (out_len,)
-    if out is not None:
-        if isinstance(out, nat.DeviceArray):
-            raise ParameterError("out= must be a NumPy array")
-        if tuple(out.shape) != shape:
-            raise ParameterError(f"Shape mismatch for provided output array out.shape={out.shape} != {list(shape)}")
+    _check_istft_out(out, lead + (out_len,))
     pl.require_supported_n_fft(n_fft, inverse=True)
-    ctx = stft_matrix.ctx if on_device else nat.default_context()
-    n_clips = int(np.prod(lead, dtype=np.int64)) if lead else 1
+    ctx = pl.context_for(stft_matrix)
     key = ("stft", n_fft, hop_length, bool(center), "constant", wkey)
     plan = nat.make_plan(ctx, key, n_fft=n_fft, hop_length=hop_length, center=center, pad_mode="constant",
                          window=win)
-    L = nat.lib()
-    tmp = None
-    if on_device:
-        if stft_matrix.dtype != np.complex64:
-            raise ParameterError("device stft_matrix must be complex64")
-        if stft_matrix.layout == "ft":
-            d_ptr = stft_matrix.ptr
-        else:   # C-ordered (..., bin, frame) on the device -> native [frame][bin]
-            tmp = nat.DeviceArray.empty(ctx, stft_matrix.shape, np.complex64, layout="ft")
-            nat.check(L.b2l_transpose(ctx.handle, _vp(stft_matrix.ptr), n_clips, F, T_stored, 8, _vp(tmp.ptr)))
-            d_ptr = tmp.ptr
-    else:
-        Dt = np.swapaxes(stft_matrix, -1, -2)
-        if Dt.flags.c_contiguous and Dt.dtype == np.complex64:
-            host = Dt                                   # already [.., frame, bin] in memory
-            tmp = nat.DeviceArray.empty(ctx, stft_matrix.shape, np.complex64, layout="ft")
-            nat.check(L.b2l_h2d(ctx.handle, _vp(tmp.ptr), host.ctypes.data_as(_vp), host.nbytes))
-        else:
-            host = np.ascontiguousarray(stft_matrix, dtype=np.complex64)
-            raw = nat.DeviceArray.empty(ctx, stft_matrix.shape, np.complex64)
-            nat.check(L.b2l_h2d(ctx.handle, _vp(raw.ptr), host.ctypes.data_as(_vp), host.nbytes))
-            tmp = nat.DeviceArray.empty(ctx, stft_matrix.shape, np.complex64, layout="ft")
-            nat.check(L.b2l_transpose(ctx.handle, _vp(raw.ptr), n_clips, F, T_stored, 8, _vp(tmp.ptr)))
-            ctx.synchronize()
-            raw.free()
-        d_ptr = tmp.ptr
+    if on_device and stft_matrix.dtype != np.complex64:
+        raise ParameterError("device stft_matrix must be complex64")
+    # a host matrix whose memory already is [.., frame, bin] complex64 (stft's own output) uploads as it is
+    zero_copy = not on_device and in_dtype == np.complex64 and np.swapaxes(stft_matrix, -1, -2).flags.c_contiguous
+    Dd, own = pl.to_native(stft_matrix, np.complex64, host_transpose=zero_copy)
     start = n_fft // 2 if center else 0
     inv_ptr = _inv_wss(ctx, window, n_frames, win_length, n_fft, hop_length, start, out_len, wkey)
-    y = nat.DeviceArray.empty(ctx, shape, np.float32)
-    nat.check(L.b2l_istft(ctx.handle, plan.handle, _vp(d_ptr), n_clips, T_stored, n_frames, _vp(inv_ptr), out_len,
-                          _vp(y.ptr), out_len))
+    y = nat.DeviceArray.empty(ctx, lead + (out_len,), np.float32)
+    nat.check(nat.lib().b2l_istft(ctx.handle, plan.handle, _vp(Dd.ptr), pl.clip_count(lead), T_stored, n_frames,
+                                  _vp(inv_ptr), out_len, _vp(y.ptr), out_len))
+    if own:
+        Dd.free()   # stream-ordered pool: safe right after the launch
     if on_device and out is None:
-        if tmp is not None:
-            ctx.synchronize()
-            tmp.free()
         return y
-    res = pl.finish(ctx, y, True, dtype)
-    if tmp is not None:
-        tmp.free()
+    res = pl.finish(y, dtype)
     if out is None:
         return res
     out[...] = res
@@ -321,52 +231,25 @@ def _spectrogram(*, y=None, S=None, n_fft: Optional[int] = 2048, hop_length: Opt
         raise ParameterError(f"Unable to compute spectrogram with n_fft={n_fft}")
     if y is None:
         raise ParameterError("Input signal must be provided to compute a spectrogram")
-    hop_length, win_length = pl.frame_params(n_fft, hop_length, win_length)
-    n, req_dtype = pl.precheck_signal(y, native_ok=True)
-    win, wkey = pl.resolve_window(window, win_length, n_fft)
-    mode = pl.check_stft_geometry(n, n_fft, center, pad_mode)
-    if pl.wide_route(y, req_dtype, n_fft):
-        f64.require_supported(n_fft)
-        on_device = isinstance(y, nat.DeviceArray)
-        ctx = y.ctx if on_device else nat.default_context()
-        if not on_device:
-            nat.check(nat.lib().b2l_status_reset(ctx.handle))
-        yd = y if on_device else f64.to_device(ctx, y)
-        D = f64.stft(ctx, yd, n_fft=n_fft, hop_length=hop_length, center=center, mode=mode, win=win)
-        Sd = f64.abs_pow(ctx, D, power)
+    fr = pl.forward_front(y, n_fft, hop_length, win_length, window, center, pad_mode)
+    if pl.wide_route(y, fr.dtype, n_fft):
+        staged, D = f64.stft(y, n_fft=n_fft, hop_length=fr.hop, center=center, mode=fr.mode, win=fr.window)
+        Sd = f64.abs_pow(staged.ctx, D, power)
         D.free()
-        if not on_device:
-            yd.free()
-            res = f64.fetch(ctx, Sd, validate=True)
-            return (res if res.dtype == req_dtype else res.astype(req_dtype)), n_fft
-        return Sd, n_fft
+        return staged.result(Sd, fr.dtype), n_fft
     pl.require_supported_n_fft(n_fft)
-    key = ("spec", n_fft, hop_length, bool(center), mode, wkey, float(power))
-    F = 1 + n_fft // 2
-    T = 1 + (n + (2 * (n_fft // 2) if center else 0) - n_fft) // hop_length
-
-    def make_plan(ctx):
-        return nat.make_plan(ctx, key, n_fft=n_fft, hop_length=hop_length, center=center, pad_mode=mode, window=win,
-                             power=float(power))
-
-    if isinstance(y, nat.DeviceArray):
-        ctx = y.ctx
-        staged = pl.StagedInput(ctx, y)
-        plan = make_plan(ctx)
-        Sd = nat.DeviceArray.empty(ctx, staged.lead + (F, T), np.float32, layout="ft")
-        nat.check(nat.lib().b2l_spectrogram(ctx.handle, plan.handle, _vp(staged.dev.ptr), staged.n_clips, staged.n,
-                                            staged.n, _vp(Sd.ptr)))
-        return Sd, n_fft
 
     def launch(ctx, plan, d_in, m, n_, d_out, d_scr):
         nat.check(nat.lib().b2l_spectrogram(ctx.handle, plan.handle, _vp(d_in), m, n_, n_, _vp(d_out)))
 
-    mem = pl.run_host_forward(y, n_fft=n_fft, hop_length=hop_length, center=center, n_frames=T,
-                              out_mem_tail=(T, F), out_dtype=np.float32, make_plan=make_plan, launch=launch)
-    res = np.swapaxes(mem, -1, -2)
-    if res.dtype != req_dtype:
-        res = res.astype(req_dtype)
-    return res, n_fft
+    res = pl.run_forward(y, plan_key=("spec", n_fft, fr.hop, bool(center), fr.mode, fr.wkey, float(power)),
+                         plan_kw=dict(n_fft=n_fft, hop_length=fr.hop, center=center, pad_mode=fr.mode, window=fr.window,
+                                      power=float(power)),
+                         n_frames=fr.n_frames, out_tail=(1 + n_fft // 2, fr.n_frames), dtype=np.float32, layout="ft",
+                         launch=launch)
+    if isinstance(res, nat.DeviceArray) or res.dtype == fr.dtype:
+        return res, n_fft
+    return res.astype(fr.dtype), n_fft
 
 
 def power_to_db(S, *, ref=1.0, amin: float = 1e-10, top_db: Optional[float] = 80.0, axes="auto"):
@@ -411,7 +294,7 @@ def _to_db(S, ref, amin, top_db, axes, amplitude: bool):
         kept = [i for i in range(S.ndim) if i not in ax]
         perm = kept + list(ax)
         Sp = np.transpose(S, perm)
-        n_keep = int(np.prod([S.shape[i] for i in kept], dtype=np.int64)) if kept else 1
+        n_keep = pl.clip_count(tuple(S.shape[i] for i in kept))
         flat = np.ascontiguousarray(Sp).reshape(n_keep, 1, -1)
         res = _to_db(flat, ref, amin, top_db, "auto", amplitude)
         return np.transpose(np.asarray(res).reshape(Sp.shape), np.argsort(perm))[()]
@@ -435,7 +318,7 @@ def _to_db(S, ref, amin, top_db, axes, amplitude: bool):
     else:
         lead = ()
         per = dev.size
-    n_lead = int(np.prod(lead, dtype=np.int64)) if lead else 1
+    n_lead = pl.clip_count(lead)
     out = nat.DeviceArray.empty(ctx, dev.shape, np.float32, layout=dev.layout)
     tdb = -1.0 if top_db is None else float(top_db)
     L = nat.lib()
@@ -466,16 +349,14 @@ def _to_db(S, ref, amin, top_db, axes, amplitude: bool):
                                     _vp(out.ptr)))
     if on_device:
         return out
-    res = pl.finish(ctx, out, True, req)
-    return res[()]
+    return pl.finish(out, req)[()]
 
 
 def _to_db_f64(ctx, S, ref, amin, top_db, amplitude):
     """power_to_db / amplitude_to_db of a float64 host array in FP64 (core/spectrum.py:1866-1881, :1990-2038)."""
     shape = S.shape
     work = S if S.ndim >= 2 else S.reshape(1, -1)
-    lead = work.shape[:-2]
-    n_lead = int(np.prod(lead, dtype=np.int64)) if lead else 1
+    n_lead = pl.clip_count(work.shape[:-2])
     mag = np.abs(work) if amplitude else work
     if callable(ref):
         try:
@@ -496,9 +377,9 @@ def _to_db_f64(ctx, S, ref, amin, top_db, amplitude):
             one = nat.DeviceArray(ctx, dev.ptr + 8 * i * work.shape[-2] * work.shape[-1], (1,) + work.shape[-2:], np.float64,
                                   owner=False)
             parts.append(f64.power_to_db(ctx, one, ref_value=float(ref_value[i]), amin=amin, top_db=top_db))
-        res = np.concatenate([f64.fetch(ctx, p) for p in parts], axis=0)
+        res = np.concatenate([pl.finish(p) for p in parts], axis=0)
     else:
-        res = f64.fetch(ctx, f64.power_to_db(ctx, dev, ref_value=float(ref_value[0]), amin=amin, top_db=top_db))
+        res = pl.finish(f64.power_to_db(ctx, dev, ref_value=float(ref_value[0]), amin=amin, top_db=top_db))
     dev.free()
     return res.reshape(shape)[()]
 
@@ -521,7 +402,7 @@ def _db_inverse(S_db, op, param):
     nat.check(nat.lib().b2l_unary(ctx.handle, op, _vp(dev.ptr), dev.size, float(param), _vp(out.ptr)))
     if on_device:
         return out
-    return pl.finish(ctx, out, True, req)[()]
+    return pl.finish(out, req)[()]
 
 
 def db_to_power(S_db, *, ref: float = 1.0):
@@ -591,7 +472,7 @@ def pcen(S, *, sr: float = 22050, hop_length: int = 512, gain: float = 0.98, bia
     T = dev.shape[-1]
     rows = dev.shape[-2] if ndim >= 2 else 1
     lead = dev.shape[:-2] if ndim >= 2 else ()
-    n_lead = int(np.prod(lead, dtype=np.int64)) if lead else 1
+    n_lead = pl.clip_count(lead)
     state_shape = dev.shape[:-1] + (1,)
     d_zi = None
     if zi is not None:
@@ -618,9 +499,9 @@ def pcen(S, *, sr: float = 22050, hop_length: int = 512, gain: float = 0.98, bia
         return (out, d_zf) if return_zf else out
     dev.free()
     res_dtype = np.result_type(req, np.float64)
-    res = pl.finish(ctx, out, True, res_dtype)
+    res = pl.finish(out, res_dtype)
     if return_zf:
-        return res, pl.finish(ctx, d_zf, True, res_dtype)
+        return res, pl.finish(d_zf, res_dtype)
     return res
 
 
@@ -649,25 +530,15 @@ def reassigned_spectrogram(y, *, sr: float = 22050, S=None, n_fft: int = 2048, h
         hop_length = int(win_length // 4)
     n, req = pl.precheck_signal(y)
     w = pad_center(filters.get_window(window, win_length, fftbins=True), size=n_fft)
-    on_device = isinstance(y, nat.DeviceArray)
-    if on_device:
-        ctx, yd = y.ctx, y
-    else:
-        ctx = nat.default_context()
-        staged = pl.StagedInput(ctx, y)
-        yd = staged.dev
+    staged = pl.StagedInput(y)
+    ctx, yd = staged.ctx, staged.dev
     kw = dict(n_fft=n_fft, hop_length=hop_length, center=center, pad_mode=pad_mode)
     if S is None:
         Sh = stft(yd, window=w, **kw)
     else:
-        S = np.asarray(S)
-        Sh_host = np.ascontiguousarray(np.swapaxes(S, -1, -2), dtype=np.complex64)       # memory [.., frame, bin]
-        Sh = nat.DeviceArray.empty(ctx, S.shape, np.complex64, layout="ft")
-        nat.check(nat.lib().b2l_h2d(ctx.handle, _vp(Sh.ptr), Sh_host.ctypes.data_as(_vp), Sh_host.nbytes))
-        ctx.synchronize()
+        Sh, _ = pl.to_native(np.asarray(S), np.complex64, host_transpose=True, ctx=ctx)
     F, T = Sh.shape[-2], Sh.shape[-1]
-    if not on_device:
-        staged.scan_uncovered(n_fft, hop_length, center, T)
+    staged.scan_uncovered(n_fft, hop_length, win_length, center, T)
     Sdh = stft(yd, window=cyclic_gradient(w), **kw) if reassign_frequencies else None
     Sth = None
     if reassign_times:
@@ -676,13 +547,11 @@ def reassigned_spectrogram(y, *, sr: float = 22050, S=None, n_fft: int = 2048, h
         Sth = stft(yd, window=w * window_times, **kw)
     offset = 0 if center else int(n_fft // 2)
     frame_times = (np.arange(T) * hop_length + offset).astype(int) / float(sr)
-    from ..feature.stats import _device_table
     from .convert import fft_frequencies
 
-    d_bf = _device_table(ctx, ("fftfreq", float(sr), int(n_fft)), fft_frequencies(sr=sr, n_fft=n_fft))
-    d_ft = _device_table(ctx, ("frametimes", float(sr), int(hop_length), int(offset), int(T)), frame_times)
-    lead = Sh.shape[:-2]
-    n_clips = int(np.prod(lead, dtype=np.int64)) if lead else 1
+    d_bf = ctx.constant(("fftfreq", float(sr), int(n_fft)), lambda: fft_frequencies(sr=sr, n_fft=n_fft))
+    d_ft = ctx.constant(("frametimes", float(sr), int(hop_length), int(offset), int(T)), lambda: frame_times)
+    n_clips = pl.clip_count(Sh.shape[:-2])
     outs = [nat.DeviceArray.empty(ctx, Sh.shape, np.float32, layout="ft") for _ in range(3)]
     desc = nat.ReassignDesc(sr=float(sr), mag_threshold=float(ref_power) ** 0.5, max_time=float(n) / float(sr),
                             reassign_frequencies=int(bool(reassign_frequencies)), reassign_times=int(bool(reassign_times)),
@@ -693,13 +562,10 @@ def reassigned_spectrogram(y, *, sr: float = 22050, S=None, n_fft: int = 2048, h
     for tmp in (Sh, Sdh, Sth):
         if tmp is not None:
             tmp.free()
-    if on_device:
+    if staged.on_device:
         return tuple(outs)
     wide = np.result_type(req, np.float64)
-    freqs = pl.finish(ctx, outs[0], True, wide, validate=True)
-    times = pl.finish(ctx, outs[1], True, wide)
-    mags = pl.finish(ctx, outs[2], True, req)
-    return freqs, times, mags
+    return staged.result(outs[0], wide), pl.finish(outs[1], wide), pl.finish(outs[2], req)
 
 
 class _Deprecated:
@@ -738,13 +604,7 @@ def phase_vocoder(D, *, rate: Optional[float] = None, t_out=None, kind="linear",
     if on_device:
         if D.dtype != np.complex64:
             raise ParameterError("device STFT must be complex64")
-        ctx, res_dtype = D.ctx, np.dtype(np.complex64)
-        if D.layout == "ft":
-            src = D
-        else:
-            src = nat.DeviceArray.empty(ctx, D.shape, np.complex64, layout="ft")
-            lead0 = int(np.prod(D.shape[:-2], dtype=np.int64)) if D.ndim > 2 else 1
-            nat.check(nat.lib().b2l_transpose(ctx.handle, _vp(D.ptr), lead0, D.shape[-2], n_frames, 8, _vp(src.ptr)))
+        res_dtype = np.dtype(np.complex64)
     else:
         D = np.asarray(D)
         if not np.iscomplexobj(D):
@@ -752,15 +612,11 @@ def phase_vocoder(D, *, rate: Optional[float] = None, t_out=None, kind="linear",
         res_dtype = np.dtype(D.dtype)
         if res_dtype == np.complex128 and not pl.wide_complex_ok("phase_vocoder input"):
             raise ParameterError("complex128 input refused (B2L_FLOAT64=error)")
-        ctx = nat.default_context()
-        mem = np.ascontiguousarray(np.swapaxes(D, -1, -2), dtype=np.complex64)     # [.., frame, bin]
-        src = nat.DeviceArray.empty(ctx, D.shape, np.complex64, layout="ft")
-        if mem.nbytes:
-            nat.check(nat.lib().b2l_h2d(ctx.handle, _vp(src.ptr), mem.ctypes.data_as(_vp), mem.nbytes))
-            ctx.synchronize()
+    src, own = pl.to_native(D, np.complex64, host_transpose=True)
+    ctx = src.ctx
     F = D.shape[-2]
     lead = tuple(D.shape[:-2])
-    n_clips = int(np.prod(lead, dtype=np.int64)) if lead else 1
+    n_clips = pl.clip_count(lead)
     n_out = int(t_out.shape[0])
     # phase increments: frames floor(t), floor(t) + 1 (:1498-1512); magnitudes: the segment scipy's interp1d
     # picks — searchsorted(x, t) clipped to [1, n - 1], minus one — and the offset inside it (:1517-1527)
@@ -775,11 +631,11 @@ def phase_vocoder(D, *, rate: Optional[float] = None, t_out=None, kind="linear",
                                           _vp(tables[1].ptr), _vp(tables[2].ptr), _vp(tables[3].ptr), _vp(out.ptr)))
     for tb in tables:
         tb.free()
-    if src is not D:
+    if own:
         src.free()
     if on_device:
         return out
-    return pl.finish(ctx, out, True, res_dtype)
+    return pl.finish(out, res_dtype)
 
 
 def griffinlim(S, *, n_iter: int = 32, hop_length: Optional[int] = None, win_length: Optional[int] = None,
@@ -807,33 +663,21 @@ def griffinlim(S, *, n_iter: int = 32, hop_length: Optional[int] = None, win_len
     cdtype = dtype_r2c(np.float32)
     eps = float(tiny(np.zeros(1, dtype=cdtype)))
     F, T = S.shape[-2], S.shape[-1]
-    lead = tuple(S.shape[:-2])
-    n_clips = int(np.prod(lead, dtype=np.int64)) if lead else 1
+    n_clips = pl.clip_count(S.shape[:-2])
     pl.require_supported_n_fft(n_fft, inverse=True)
-    ctx = S.ctx if on_device else nat.default_context()
+    ctx = pl.context_for(S)
     L = nat.lib()
-
-    def to_ft(dev_c, itemsize, np_dtype):
-        out = nat.DeviceArray.empty(ctx, dev_c.shape, np_dtype, layout="ft")
-        nat.check(L.b2l_transpose(ctx.handle, _vp(dev_c.ptr), n_clips, F, T, itemsize, _vp(out.ptr)))
-        return out
-
-    if on_device:
-        S_ft = S if S.layout == "ft" else to_ft(S, 4, np.float32)
-        S_host_shape = S.shape
-    else:
-        S_c = ctx.to_device(np.ascontiguousarray(S, dtype=np.float32))
-        S_ft = to_ft(S_c, 4, np.float32)
-        S_host_shape = S.shape
+    S_ft, _ = pl.to_native(S, np.float32, ctx=ctx)
+    S_host_shape = S.shape
     if init == "random":
         # same generator calls as the reference, so a given seed gives the same starting phases
         ph = 2 * np.pi * rng.random(size=S_host_shape)
         a0 = (np.cos(ph) + 1j * np.sin(ph)).astype(np.complex64)
         a0 = a0 * (np.asarray(S.get()) if on_device else S.astype(np.float32))
-        angles = to_ft(ctx.to_device(np.ascontiguousarray(a0, dtype=np.complex64)), 8, np.complex64)
+        angles, _ = pl.to_native(a0, np.complex64, ctx=ctx)
     else:
         angles = nat.DeviceArray.empty(ctx, S_host_shape, np.complex64, layout="ft")
-        ones = to_ft(ctx.to_device(np.ones(S_host_shape, dtype=np.complex64)), 8, np.complex64)
+        ones, _ = pl.to_native(np.ones(S_host_shape, dtype=np.complex64), np.complex64, ctx=ctx)
         nat.check(L.b2l_gl_update(ctx.handle, _vp(ones.ptr), None, _vp(S_ft.ptr), 0.0, 0.0, _vp(angles.ptr),
                                   n_clips * F * T))
     kw_i = dict(hop_length=hop_length, win_length=win_length, n_fft=n_fft, window=window, center=center, length=length)
@@ -859,5 +703,4 @@ def griffinlim(S, *, n_iter: int = 32, hop_length: Optional[int] = None, win_len
     y = istft(angles, **kw_i)
     if on_device:
         return y
-    out_dtype = np.dtype(dtype) if dtype is not None else s_dtype
-    return pl.finish(ctx, y, True, out_dtype)
+    return pl.finish(y, np.dtype(dtype) if dtype is not None else s_dtype)

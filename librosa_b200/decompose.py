@@ -20,7 +20,7 @@ def _pair(v):
     return (v[0], v[1]) if isinstance(v, (tuple, list)) else (v, v)
 
 
-def _hpss_device(ctx, Sd, *, kernel_size, power, mask, margin):
+def _hpss_device(Sd, *, kernel_size, power, mask, margin):
     """Sd: DeviceArray (..., bins, frames), complex64 or float32, layout "ft" or "c".  Returns two DeviceArrays in
     layout "ft"."""
     win_harm, win_perc = _pair(kernel_size)
@@ -35,15 +35,10 @@ def _hpss_device(ctx, Sd, *, kernel_size, power, mask, margin):
         raise ParameterError("hpss needs an input of shape (..., bins, frames)")
     is_complex = Sd.dtype == np.complex64
     F, T = Sd.shape[-2], Sd.shape[-1]
-    lead = Sd.shape[:-2]
-    n_clips = int(np.prod(lead, dtype=np.int64)) if lead else 1
+    ctx = Sd.ctx
+    n_clips = pl.clip_count(Sd.shape[:-2])
     L = nat.lib()
-    if Sd.layout == "ft":
-        src = Sd
-    else:
-        src = nat.DeviceArray.empty(ctx, Sd.shape, Sd.dtype, layout="ft")
-        if Sd.size:
-            nat.check(L.b2l_transpose(ctx.handle, _vp(Sd.ptr), n_clips, F, T, Sd.dtype.itemsize, _vp(src.ptr)))
+    src, own = pl.to_native(Sd)
     if is_complex:
         mag = nat.DeviceArray.empty(ctx, Sd.shape, np.float32, layout="ft")
         nat.check(L.b2l_cabs(ctx.handle, _vp(src.ptr), src.size, _vp(mag.ptr)))
@@ -58,16 +53,9 @@ def _hpss_device(ctx, Sd, *, kernel_size, power, mask, margin):
                          _vp(harm.ptr), _vp(perc.ptr)))
     if mag is not src:
         mag.free()
-    if src is not Sd:
+    if own:
         src.free()
     return harm, perc
-
-
-def _to_host(ctx, arr, res_dtype):
-    """layout-"ft" DeviceArray (..., bins, frames) -> NumPy array of the logical shape."""
-    mem = arr.get()                     # DeviceArray.get returns the logical (..., bins, frames) view
-    arr.free()
-    return mem if mem.dtype == res_dtype else mem.astype(res_dtype)
 
 
 def hpss(S, *, kernel_size=31, power: float = 2.0, mask: bool = False, margin=1.0):
@@ -76,7 +64,7 @@ def hpss(S, *, kernel_size=31, power: float = 2.0, mask: bool = False, margin=1.
     if isinstance(S, nat.DeviceArray):
         if S.dtype not in (np.dtype(np.float32), np.dtype(np.complex64)):
             raise ParameterError("device spectrogram must be float32 or complex64")
-        return _hpss_device(S.ctx, S, kernel_size=kernel_size, power=power, mask=mask, margin=margin)
+        return _hpss_device(S, kernel_size=kernel_size, power=power, mask=mask, margin=margin)
     S = np.asarray(S)
     ctx = nat.default_context()
     if np.iscomplexobj(S):
@@ -90,7 +78,7 @@ def hpss(S, *, kernel_size=31, power: float = 2.0, mask: bool = False, margin=1.
             S = S.astype(np.float32)
         res_dtype = mask_dtype = pl.check_real_dtype(S.dtype, "hpss input")
         dev = ctx.to_device(np.ascontiguousarray(S, dtype=np.float32))
-    harm, perc = _hpss_device(ctx, dev, kernel_size=kernel_size, power=power, mask=mask, margin=margin)
+    harm, perc = _hpss_device(dev, kernel_size=kernel_size, power=power, mask=mask, margin=margin)
     dev.free()
     out_dtype = mask_dtype if mask else res_dtype
-    return _to_host(ctx, harm, out_dtype), _to_host(ctx, perc, out_dtype)
+    return pl.finish(harm, out_dtype), pl.finish(perc, out_dtype)

@@ -22,24 +22,16 @@ def _separate(y, want, *, kernel_size, power, mask, margin, n_fft, hop_length, w
     if mask:
         raise nat.UnsupportedOnGPU("effects.hpss(mask=True) inverts the masks themselves; not supported on the GPU")
     n, req = pl.precheck_signal(y)
-    on_device = isinstance(y, nat.DeviceArray)
-    if on_device:
-        ctx, yd = y.ctx, y
-    else:
-        ctx = nat.default_context()
-        staged = pl.StagedInput(ctx, y)
-        yd = staged.dev
-    D = stft(yd, n_fft=n_fft, hop_length=hop_length, win_length=win_length, center=center, pad_mode=pad_mode)
-    if not on_device:
-        hop_eff, _ = pl.frame_params(n_fft, hop_length, win_length)
-        staged.scan_uncovered(n_fft, hop_eff, center, D.shape[-1])
-    harm, perc = _hpss_device(ctx, D, kernel_size=kernel_size, power=power, mask=False, margin=margin)
+    staged = pl.StagedInput(y)
+    D = stft(staged.dev, n_fft=n_fft, hop_length=hop_length, win_length=win_length, center=center, pad_mode=pad_mode)
+    staged.scan_uncovered(n_fft, hop_length, win_length, center, D.shape[-1])
+    harm, perc = _hpss_device(D, kernel_size=kernel_size, power=power, mask=False, margin=margin)
     D.free()
     outs = []
     for name, comp in (("harm", harm), ("perc", perc)):
         if name in want:
             yd_out = istft(comp, n_fft=n_fft, hop_length=hop_length, win_length=win_length, center=center, length=n)
-            outs.append(yd_out if on_device else pl.finish(ctx, yd_out, True, req, validate=True))
+            outs.append(staged.result(yd_out, req))
         comp.free()
     return outs
 
@@ -75,24 +67,16 @@ def time_stretch(y, *, rate: float, **kwargs):
     if rate <= 0:
         raise ParameterError("rate must be a positive number")
     n, req = pl.precheck_signal(y)
-    on_device = isinstance(y, nat.DeviceArray)
-    if on_device:
-        ctx, yd = y.ctx, y
-    else:
-        ctx = nat.default_context()
-        staged = pl.StagedInput(ctx, y)
-        yd = staged.dev
-    D = stft(yd, **kwargs)
-    if not on_device:
-        n_fft = kwargs.get("n_fft", 2048)
-        hop_eff, _ = pl.frame_params(n_fft, kwargs.get("hop_length"), kwargs.get("win_length"))
-        staged.scan_uncovered(n_fft, hop_eff, kwargs.get("center", True), D.shape[-1])
+    staged = pl.StagedInput(y)
+    D = stft(staged.dev, **kwargs)
+    staged.scan_uncovered(kwargs.get("n_fft", 2048), kwargs.get("hop_length"), kwargs.get("win_length"),
+                          kwargs.get("center", True), D.shape[-1])
     # the reference forwards these two (deprecated, unused) arguments, so its call always warns; same here
     Ds = phase_vocoder(D, rate=rate, hop_length=kwargs.get("hop_length"), n_fft=kwargs.get("n_fft"))
     D.free()
     out = istft(Ds, length=round(n / rate), **kwargs)
     Ds.free()
-    return out if on_device else pl.finish(ctx, out, True, req, validate=True)
+    return staged.result(out, req)
 
 
 def pitch_shift(y, *, sr: float, n_steps: float, bins_per_octave: int = 12, res_type: str = "soxr_hq",
@@ -109,22 +93,15 @@ def pitch_shift(y, *, sr: float, n_steps: float, bins_per_octave: int = 12, res_
         raise ParameterError(f"bins_per_octave={bins_per_octave} must be a positive integer.")
     rate = 2.0 ** (-float(n_steps) / bins_per_octave)
     n, req = pl.precheck_signal(y)
-    on_device = isinstance(y, nat.DeviceArray)
-    yd = y if on_device else nat.default_context().to_device(np.ascontiguousarray(y, dtype=np.float32))
-    if not on_device:
-        ctx = yd.ctx
-        nat.check(nat.lib().b2l_status_reset(ctx.handle))
-        lead = yd.shape[:-1]
-        n_clips = int(np.prod(lead, dtype=np.int64)) if lead else 1
-        if n_clips and n:
-            nat.check(nat.lib().b2l_scan_finite(ctx.handle, C.c_void_p(yd.ptr), n_clips, n, n, 0))
-    stretched = time_stretch(yd, rate=rate, **kwargs)
+    staged = pl.StagedInput(y)
+    staged.scan_all()
+    stretched = time_stretch(staged.dev, rate=rate, **kwargs)
     try:
         shifted = resample(stretched, orig_sr=float(sr) / rate, target_sr=sr, res_type=res_type, scale=scale)
     finally:
         stretched.free()
-        if not on_device and "shifted" not in locals():
-            yd.free()
+        if "shifted" not in locals():
+            staged.release()
     # util.fix_length(y_shift, size=y.shape[-1]) on the device
     m = shifted.shape[-1]
     if m == n:
@@ -132,7 +109,7 @@ def pitch_shift(y, *, sr: float, n_steps: float, bins_per_octave: int = 12, res_
     else:
         ctx = shifted.ctx
         lead = shifted.shape[:-1]
-        rows = int(np.prod(lead, dtype=np.int64)) if lead else 1
+        rows = pl.clip_count(lead)
         out = nat.DeviceArray.empty(ctx, tuple(lead) + (n,), np.float32)
         L = nat.lib()
         if m < n:
@@ -141,6 +118,5 @@ def pitch_shift(y, *, sr: float, n_steps: float, bins_per_octave: int = 12, res_
             nat.check(L.b2l_copy2d(ctx.handle, C.c_void_p(out.ptr), n * 4, C.c_void_p(shifted.ptr), m * 4,
                                    min(m, n) * 4, rows))
         shifted.free()
-    if not on_device:
-        yd.free()
-    return out if on_device else pl.finish(out.ctx, out, True, req, validate=True)
+    staged.release()
+    return staged.result(out, req)

@@ -68,14 +68,13 @@ def mel_to_stft(M, *, sr: float = 22050, n_fft: int = 2048, power: float = 2.0, 
     else:
         Md = ctx.to_device(np.ascontiguousarray(M, dtype=np.float32))
     lead = tuple(M.shape[:-2])
-    n_clips = int(np.prod(lead, dtype=np.int64)) if lead else 1
     out = nat.DeviceArray.empty(ctx, lead + (F, T), np.float32)
-    nat.check(nat.lib().b2l_nnls_mel(ctx.handle, _vp(Md.ptr), n_clips, T, n_mels, F, basis.ctypes.data_as(_fp),
-                                     pinv.ctypes.data_as(_fp), float(step), NNLS_ITERATIONS, float(1.0 / power),
-                                     _vp(out.ptr)))
+    nat.check(nat.lib().b2l_nnls_mel(ctx.handle, _vp(Md.ptr), pl.clip_count(lead), T, n_mels, F,
+                                     basis.ctypes.data_as(_fp), pinv.ctypes.data_as(_fp), float(step), NNLS_ITERATIONS,
+                                     float(1.0 / power), _vp(out.ptr)))
     if on_device:
         return out
-    res = pl.finish(ctx, out, True, req)
+    res = pl.finish(out, req)
     Md.free()
     return res
 
@@ -133,15 +132,15 @@ def mfcc_to_mel(mfcc, *, n_mels: int = 128, dct_type: int = 2, norm="ortho", ref
                          pad_mode="constant", window=np.ones(8),
                          mel_basis=np.zeros((n_mfcc, 5), dtype=np.float32), dct_basis=basis)
     lead = tuple(mfcc.shape[:-2])
-    n_clips = int(np.prod(lead, dtype=np.int64)) if lead else 1
     logmel = nat.DeviceArray.empty(ctx, lead + (n_mels, T), np.float32)
-    nat.check(nat.lib().b2l_dct_project(ctx.handle, plan.handle, _vp(Cd.ptr), n_clips, T, _vp(logmel.ptr)))
+    nat.check(nat.lib().b2l_dct_project(ctx.handle, plan.handle, _vp(Cd.ptr), pl.clip_count(lead), T,
+                                        _vp(logmel.ptr)))
     mel = db_to_power(logmel, ref=ref)
     logmel.free()
     if on_device:
         return mel
     Cd.free()
-    return pl.finish(ctx, mel, True, req)
+    return pl.finish(mel, req)
 
 
 def mfcc_to_audio(mfcc, *, n_mels: int = 128, dct_type: int = 2, norm="ortho", ref: float = 1.0, lifter: float = 0,

@@ -22,19 +22,6 @@ from ..util.exceptions import ParameterError
 _vp = C.c_void_p
 
 
-def _spec_to_device(ctx, S):
-    """Host/device spectrogram-like array (..., rows, frames) -> DeviceArray (C layout or native "ft")."""
-    if isinstance(S, nat.DeviceArray):
-        if S.dtype != np.float32:
-            raise ParameterError("device spectrogram must be float32")
-        return S, np.dtype(np.float32), True
-    S = np.asarray(S)
-    if np.iscomplexobj(S):
-        raise ParameterError("spectrogram input must be real")
-    req = pl.check_real_dtype(S.dtype if np.issubdtype(S.dtype, np.floating) else np.float32, "S")
-    return ctx.to_device(np.ascontiguousarray(S, dtype=np.float32)), req, False
-
-
 def melspectrogram(*, y=None, sr: float = 22050, S=None, n_fft: int = 2048, hop_length: int = 512,
                    win_length: Optional[int] = None, window="hann", center: bool = True,
                    pad_mode="constant", power: float = 2.0, **kwargs):
@@ -42,95 +29,59 @@ def melspectrogram(*, y=None, sr: float = 22050, S=None, n_fft: int = 2048, hop_
     ``librosa.feature.melspectrogram``.  ``kwargs`` go to ``filters.mel`` (n_mels, fmin, fmax, htk, norm, dtype)."""
     if S is not None:
         # mel_basis . S for a caller-supplied spectrogram (feature/spectral.py:2158-2160)
-        ctx = S.ctx if isinstance(S, nat.DeviceArray) else nat.default_context()
-        Sd, req, on_device = _spec_to_device(ctx, S)
+        Sd, req, on_device = pl.spectrogram_input(S)
         F, T = Sd.shape[-2], Sd.shape[-1]
         if n_fft is None or n_fft // 2 + 1 != F:
             n_fft = 2 * (F - 1)
         basis, bkey = pl.mel_basis(sr, n_fft, kwargs)
+        ctx = Sd.ctx
         plan = nat.make_plan(ctx, ("melproj", n_fft, bkey), n_fft=n_fft, hop_length=1, center=True,
                              pad_mode="constant", window=np.ones(n_fft), mel_basis=basis)
         lead = Sd.shape[:-2]
-        n_clips = int(np.prod(lead, dtype=np.int64)) if lead else 1
-        L = nat.lib()
-        if Sd.layout == "ft":
-            src = Sd
-        else:
-            src = nat.DeviceArray.empty(ctx, Sd.shape, np.float32, layout="ft")
-            nat.check(L.b2l_transpose(ctx.handle, _vp(Sd.ptr), n_clips, F, T, 4, _vp(src.ptr)))
+        src, own = pl.to_native(Sd)
         out = nat.DeviceArray.empty(ctx, lead + (basis.shape[0], T), np.float32)
-        nat.check(L.b2l_mel_project(ctx.handle, plan.handle, _vp(src.ptr), n_clips, T, _vp(out.ptr)))
-        res = pl.finish(ctx, out, not on_device, np.result_type(req, basis.dtype))
-        if src is not Sd:
-            ctx.synchronize()
+        nat.check(nat.lib().b2l_mel_project(ctx.handle, plan.handle, _vp(src.ptr), pl.clip_count(lead), T,
+                                            _vp(out.ptr)))
+        if own:
             src.free()
-        return res
+        return out if on_device else pl.finish(out, np.result_type(req, basis.dtype))
     if n_fft is None:
         raise ParameterError(f"Unable to compute spectrogram with n_fft={n_fft}")
     if y is None:
         raise ParameterError("Input signal must be provided to compute a spectrogram")
-    hop_length, win_length = pl.frame_params(n_fft, hop_length, win_length)
-    n, req_dtype = pl.precheck_signal(y, native_ok=True)
-    win, wkey = pl.resolve_window(window, win_length, n_fft)
-    mode = pl.check_stft_geometry(n, n_fft, center, pad_mode)
+    fr = pl.forward_front(y, n_fft, hop_length, win_length, window, center, pad_mode)
     basis, bkey = pl.mel_basis(sr, n_fft, kwargs)
-    if pl.wide_route(y, req_dtype, n_fft):
-        ctx, mel_d, on_device = _mel_f64(y, n_fft, hop_length, center, mode, win, power, basis)
-        if on_device:
-            return mel_d
-        res = f64.fetch(ctx, mel_d, validate=True)
-        res_dtype = np.result_type(req_dtype, basis.dtype)
-        return res if res.dtype == res_dtype else res.astype(res_dtype)
+    res_dtype = np.result_type(fr.dtype, basis.dtype)
+    if pl.wide_route(y, fr.dtype, n_fft):
+        staged, mel_d = _mel_f64(y, n_fft, fr, center, power, basis)
+        return staged.result(mel_d, res_dtype)
     pl.require_supported_n_fft(n_fft)
     if not pl.fused_front_end(n_fft):
         # chirp-z frames: |STFT|**power on the device, then the band-sparse projection (two kernels)
-        res_dtype = np.result_type(req_dtype, basis.dtype)
         return _compose_nonpow2(y, lambda Sd: melspectrogram(S=Sd, sr=sr, n_fft=n_fft, **kwargs), res_dtype,
-                                n_fft=n_fft, hop_length=hop_length, power=power, win_length=win_length,
+                                n_fft=n_fft, hop_length=fr.hop, power=power, win_length=win_length,
                                 window=window, center=center, pad_mode=pad_mode)
-    key = ("mel", n_fft, hop_length, bool(center), mode, wkey, bkey, float(power))
-    n_mels = basis.shape[0]
-    T = 1 + (n + (2 * (n_fft // 2) if center else 0) - n_fft) // hop_length
-    res_dtype = np.result_type(req_dtype, basis.dtype)
-
-    def make_plan(ctx):
-        return nat.make_plan(ctx, key, n_fft=n_fft, hop_length=hop_length, center=center, pad_mode=mode, window=win,
-                             mel_basis=basis, power=float(power))
-
-    if isinstance(y, nat.DeviceArray):
-        ctx = y.ctx
-        staged = pl.StagedInput(ctx, y)
-        plan = make_plan(ctx)
-        out = nat.DeviceArray.empty(ctx, staged.lead + (n_mels, T), np.float32)
-        nat.check(nat.lib().b2l_melspectrogram(ctx.handle, plan.handle, _vp(staged.dev.ptr), staged.n_clips,
-                                               staged.n, staged.n, _vp(out.ptr)))
-        return out
 
     def launch(ctx, plan, d_in, m, n_, d_out, d_scr):
         nat.check(nat.lib().b2l_melspectrogram(ctx.handle, plan.handle, _vp(d_in), m, n_, n_, _vp(d_out)))
 
-    res = pl.run_host_forward(y, n_fft=n_fft, hop_length=hop_length, center=center, n_frames=T,
-                              out_mem_tail=(n_mels, T), out_dtype=np.float32, make_plan=make_plan, launch=launch)
-    return res if res.dtype == res_dtype else res.astype(res_dtype)
+    res = pl.run_forward(y, plan_key=("mel", n_fft, fr.hop, bool(center), fr.mode, fr.wkey, bkey, float(power)),
+                         plan_kw=dict(n_fft=n_fft, hop_length=fr.hop, center=center, pad_mode=fr.mode, window=fr.window,
+                                      mel_basis=basis, power=float(power)),
+                         n_frames=fr.n_frames, out_tail=(basis.shape[0], fr.n_frames), dtype=np.float32,
+                         launch=launch)
+    return res if isinstance(res, nat.DeviceArray) or res.dtype == res_dtype else res.astype(res_dtype)
 
 
-def _mel_f64(y, n_fft, hop_length, center, mode, win, power, basis):
+def _mel_f64(y, n_fft, fr, center, power, basis):
     """float64 signal -> float64 mel spectrogram on the device in FP64: stft, |.|**power, band projection
-    (feature/spectral.py:2145-2160 in the input's precision).  Returns (ctx, DeviceArray, input was on device)."""
-    f64.require_supported(n_fft)
-    on_device = isinstance(y, nat.DeviceArray)
-    ctx = y.ctx if on_device else nat.default_context()
-    if not on_device:
-        nat.check(nat.lib().b2l_status_reset(ctx.handle))
-    yd = y if on_device else f64.to_device(ctx, y)
-    D = f64.stft(ctx, yd, n_fft=n_fft, hop_length=hop_length, center=center, mode=mode, win=win)
-    Sd = f64.abs_pow(ctx, D, power)
+    (feature/spectral.py:2145-2160 in the input's precision).  Returns (StagedInput, DeviceArray)."""
+    staged, D = f64.stft(y, n_fft=n_fft, hop_length=fr.hop, center=center, mode=fr.mode, win=fr.window)
+    Sd = f64.abs_pow(staged.ctx, D, power)
     D.free()
-    mel_d = f64.mel(ctx, Sd, basis)
+    mel_d = f64.mel(staged.ctx, Sd, basis)
     Sd.free()
-    if not on_device:
-        yd.free()
-    return ctx, mel_d, on_device
+    return staged, mel_d
 
 
 def _compose_nonpow2(y, tail, res_dtype, **spec_kw):
@@ -138,24 +89,11 @@ def _compose_nonpow2(y, tail, res_dtype, **spec_kw):
     the S= kernels, all on the device; host inputs get the device-side valid_audio verdict at the end."""
     from ..core.spectrum import _spectrogram
 
-    if isinstance(y, nat.DeviceArray):
-        Sd, _ = _spectrogram(y=y, **spec_kw)
-        return tail(Sd)
-    ctx = nat.default_context()
-    L = nat.lib()
-    host = np.ascontiguousarray(y, dtype=np.float32)
-    nat.check(L.b2l_status_reset(ctx.handle))
-    yd = ctx.to_device(host)
-    n_fft, hop, center = spec_kw["n_fft"], spec_kw["hop_length"], spec_kw["center"]
-    n = host.shape[-1]
-    T = 1 + (n + (2 * (n_fft // 2) if center else 0) - n_fft) // hop
-    staged = pl.StagedInput(ctx, yd)
-    begin = 0 if hop > n_fft else max(0, (T - 1) * hop + n_fft - (n_fft // 2 if center else 0))
-    if begin < n and staged.n_clips:
-        nat.check(L.b2l_scan_finite(ctx.handle, _vp(yd.ptr), staged.n_clips, n, n, begin))
-    Sd, _ = _spectrogram(y=yd, **spec_kw)
-    out = tail(Sd)
-    return pl.finish(ctx, out, True, res_dtype, validate=True)
+    staged = pl.StagedInput(y)
+    Sd, _ = _spectrogram(y=staged.dev, **spec_kw)
+    staged.scan_uncovered(spec_kw["n_fft"], spec_kw["hop_length"], spec_kw["win_length"], spec_kw["center"],
+                          Sd.shape[-1])
+    return staged.result(tail(Sd), res_dtype)
 
 
 def chroma_stft(*, y=None, sr: float = 22050, S=None, norm=np.inf, n_fft: int = 2048, hop_length: int = 512,
@@ -169,42 +107,26 @@ def chroma_stft(*, y=None, sr: float = 22050, S=None, norm=np.inf, n_fft: int = 
     from ..core.pitch import _tuning_from_device_spec
     from ..core.spectrum import _spectrogram
 
-    to_host, validate, own = True, False, False
+    staged = None
     if S is None:
         if y is None:
             raise ParameterError("Input signal must be provided to compute a spectrogram")
         _, req = pl.precheck_signal(y)
-        if isinstance(y, nat.DeviceArray):
-            ctx, yd, to_host = y.ctx, y, False
-        else:
-            ctx = nat.default_context()
-            staged = pl.StagedInput(ctx, y)
-            yd, validate = staged.dev, True
-        Sd, n_fft = _spectrogram(y=yd, n_fft=n_fft, hop_length=hop_length, power=2, win_length=win_length,
+        staged = pl.StagedInput(y)
+        Sd, n_fft = _spectrogram(y=staged.dev, n_fft=n_fft, hop_length=hop_length, power=2, win_length=win_length,
                                  window=window, center=center, pad_mode=pad_mode)
-        own = True
-        if validate:
-            hop_eff, _ = pl.frame_params(n_fft, hop_length, win_length)
-            staged.scan_uncovered(n_fft, hop_eff, center, Sd.shape[-1])
+        staged.scan_uncovered(n_fft, hop_length, win_length, center, Sd.shape[-1])
+        src, own = Sd, True
     else:
-        ctx = S.ctx if isinstance(S, nat.DeviceArray) else nat.default_context()
-        Sd, req, on_device = _spec_to_device(ctx, S)
-        to_host, own = not on_device, not on_device
+        Sd, req, on_device = pl.spectrogram_input(S)
         if n_fft is None or n_fft // 2 + 1 != Sd.shape[-2]:
             n_fft = 2 * (Sd.shape[-2] - 1)
-    F, T = Sd.shape[-2], Sd.shape[-1]
-    lead = Sd.shape[:-2]
-    n_clips = int(np.prod(lead, dtype=np.int64)) if lead else 1
+        src, own = pl.to_native(Sd)
+    ctx = src.ctx
+    F, T = src.shape[-2], src.shape[-1]
+    lead = src.shape[:-2]
+    n_clips = pl.clip_count(lead)
     L = nat.lib()
-    if Sd.layout == "ft":
-        src = Sd
-    else:
-        src = nat.DeviceArray.empty(ctx, Sd.shape, np.float32, layout="ft")
-        if n_clips and F and T:
-            nat.check(L.b2l_transpose(ctx.handle, _vp(Sd.ptr), n_clips, F, T, 4, _vp(src.ptr)))
-        if own:
-            Sd.free()
-        own = True
     try:
         if tuning is None:
             tuning = _tuning_from_device_spec(ctx, src, sr, n_fft, resolution=0.01, bins_per_octave=n_chroma,
@@ -235,9 +157,10 @@ def chroma_stft(*, y=None, sr: float = 22050, S=None, norm=np.inf, n_fft: int = 
         out = nat.DeviceArray.empty(ctx, raw.shape, np.float32)
         nat.check(L.b2l_normalize_rows(ctx.handle, _vp(raw.ptr), n_clips, fb.shape[0], T, kind, p, _vp(out.ptr)))
         raw.free()
-    if not to_host:
-        return out
-    return pl.finish(ctx, out, True, np.result_type(req, fb.dtype), validate=validate)
+    res_dtype = np.result_type(req, fb.dtype)
+    if staged is not None:
+        return staged.result(out, res_dtype)
+    return out if on_device else pl.finish(out, res_dtype)
 
 
 def _dct_basis(n_mels: int, n_mfcc: int, dct_type: int, norm, lifter: float, dtype=np.float32) -> np.ndarray:
@@ -259,20 +182,20 @@ def mfcc(*, y=None, sr: float = 22050, S=None, n_mfcc: int = 20, dct_type: int =
     if not (lifter >= 0):   # also catches NaN, like the reference's final else-branch
         raise ParameterError(f"MFCC lifter={lifter} must be a non-negative number")
     if S is not None:
-        ctx = S.ctx if isinstance(S, nat.DeviceArray) else nat.default_context()
-        Sd, req, on_device = _spec_to_device(ctx, S)
+        Sd, req, on_device = pl.spectrogram_input(S)
         if Sd.layout != "c":
             raise ParameterError("device log-mel input must be C-ordered (..., n_mels, frames)")
+        ctx = Sd.ctx
         n_mels, T = Sd.shape[-2], Sd.shape[-1]
         dct = _dct_basis(n_mels, n_mfcc, dct_type, norm, lifter)
         plan = nat.make_plan(ctx, ("dct", n_mels, pl.digest(dct)), n_fft=8, hop_length=1, center=True,
                              pad_mode="constant", window=np.ones(8),
                              mel_basis=np.zeros((n_mels, 5), dtype=np.float32), dct_basis=dct)
         lead = Sd.shape[:-2]
-        n_clips = int(np.prod(lead, dtype=np.int64)) if lead else 1
         out = nat.DeviceArray.empty(ctx, lead + (dct.shape[0], T), np.float32)
-        nat.check(nat.lib().b2l_dct_project(ctx.handle, plan.handle, _vp(Sd.ptr), n_clips, T, _vp(out.ptr)))
-        return pl.finish(ctx, out, not on_device, req)
+        nat.check(nat.lib().b2l_dct_project(ctx.handle, plan.handle, _vp(Sd.ptr), pl.clip_count(lead), T,
+                                            _vp(out.ptr)))
+        return out if on_device else pl.finish(out, req)
     # y path: fused stft -> |.|^power -> mel -> dB (+ per-clip max), then clamp + DCT
     n_fft = kwargs.pop("n_fft", 2048)
     hop_length = kwargs.pop("hop_length", 512)
@@ -285,63 +208,41 @@ def mfcc(*, y=None, sr: float = 22050, S=None, n_mfcc: int = 20, dct_type: int =
         raise ParameterError(f"Unable to compute spectrogram with n_fft={n_fft}")
     if y is None:
         raise ParameterError("Input signal must be provided to compute a spectrogram")
-    hop_length, win_length = pl.frame_params(n_fft, hop_length, win_length)
-    n, req_dtype = pl.precheck_signal(y, native_ok=True)
-    win, wkey = pl.resolve_window(window, win_length, n_fft)
-    mode = pl.check_stft_geometry(n, n_fft, center, pad_mode)
+    fr = pl.forward_front(y, n_fft, hop_length, win_length, window, center, pad_mode)
     mel_kwargs = dict(kwargs)
     mel_kwargs["norm"] = mel_norm
     basis, bkey = pl.mel_basis(sr, n_fft, mel_kwargs)
     n_mels = basis.shape[0]
-    if pl.wide_route(y, req_dtype, n_fft):
+    res_dtype = np.result_type(fr.dtype, basis.dtype)
+    if pl.wide_route(y, fr.dtype, n_fft):
         # float64 signal (or a frame length only the FP64 kernels cover): mel -> power_to_db (ref 1.0, amin 1e-10,
         # top_db 80) -> DCT, all in FP64
-        ctx, mel_d, on_device = _mel_f64(y, n_fft, hop_length, center, mode, win, power, basis)
-        db_d = f64.power_to_db(ctx, mel_d, ref_value=1.0, amin=1e-10, top_db=80.0)
+        staged, mel_d = _mel_f64(y, n_fft, fr, center, power, basis)
+        db_d = f64.power_to_db(staged.ctx, mel_d, ref_value=1.0, amin=1e-10, top_db=80.0)
         mel_d.free()
-        out = f64.dct(ctx, db_d, _dct_basis(n_mels, n_mfcc, dct_type, norm, lifter, dtype=np.float64))
+        out = f64.dct(staged.ctx, db_d, _dct_basis(n_mels, n_mfcc, dct_type, norm, lifter, dtype=np.float64))
         db_d.free()
-        if on_device:
-            return out
-        res = f64.fetch(ctx, out, validate=True)
-        res_dtype = np.result_type(req_dtype, basis.dtype)
-        return res if res.dtype == res_dtype else res.astype(res_dtype)
+        return staged.result(out, res_dtype)
     dct = _dct_basis(n_mels, n_mfcc, dct_type, norm, lifter)
     pl.require_supported_n_fft(n_fft)
     if not pl.fused_front_end(n_fft):
-        res_dtype = np.result_type(req_dtype, basis.dtype)
-
         def tail(Sd):
             mel_d = melspectrogram(S=Sd, sr=sr, n_fft=n_fft, norm=mel_norm, **kwargs)
             return mfcc(S=power_to_db(mel_d), n_mfcc=n_mfcc, dct_type=dct_type, norm=norm, lifter=lifter)
 
-        return _compose_nonpow2(y, tail, res_dtype, n_fft=n_fft, hop_length=hop_length, power=power,
+        return _compose_nonpow2(y, tail, res_dtype, n_fft=n_fft, hop_length=fr.hop, power=power,
                                 win_length=win_length, window=window, center=center, pad_mode=pad_mode)
-    key = ("mfcc", n_fft, hop_length, bool(center), mode, wkey, bkey, float(power), pl.digest(dct))
-    T = 1 + (n + (2 * (n_fft // 2) if center else 0) - n_fft) // hop_length
-    res_dtype = np.result_type(req_dtype, basis.dtype)
-
-    def make_plan(ctx):
-        # power_to_db defaults used by mfcc: ref=1.0, amin=1e-10, top_db=80 (feature/spectral.py:2001)
-        return nat.make_plan(ctx, key, n_fft=n_fft, hop_length=hop_length, center=center, pad_mode=mode, window=win,
-                             mel_basis=basis, power=float(power), dct_basis=dct, amin=1e-10, ref_value=1.0,
-                             top_db=80.0)
-
-    if isinstance(y, nat.DeviceArray):
-        ctx = y.ctx
-        staged = pl.StagedInput(ctx, y)
-        plan = make_plan(ctx)
-        out = nat.DeviceArray.empty(ctx, staged.lead + (dct.shape[0], T), np.float32)
-        scratch = nat.DeviceArray.empty(ctx, (staged.n_clips, n_mels, (T + 63) // 64 * 64), np.float32)
-        nat.check(nat.lib().b2l_mfcc(ctx.handle, plan.handle, _vp(staged.dev.ptr), staged.n_clips, staged.n,
-                                     staged.n, _vp(out.ptr), _vp(scratch.ptr)))
-        scratch.free()   # stream-ordered pool: the block can be handed out again without a sync
-        return out
 
     def launch(ctx, plan, d_in, m, n_, d_out, d_scr):
         nat.check(nat.lib().b2l_mfcc(ctx.handle, plan.handle, _vp(d_in), m, n_, n_, _vp(d_out), _vp(d_scr)))
 
-    res = pl.run_host_forward(y, n_fft=n_fft, hop_length=hop_length, center=center, n_frames=T,
-                              out_mem_tail=(dct.shape[0], T), out_dtype=np.float32, make_plan=make_plan,
-                              launch=launch, scratch_per_clip=n_mels * ((T + 63) // 64 * 64))
-    return res if res.dtype == res_dtype else res.astype(res_dtype)
+    T = fr.n_frames
+    # power_to_db defaults used by mfcc: ref=1.0, amin=1e-10, top_db=80 (feature/spectral.py:2001)
+    res = pl.run_forward(y, plan_key=("mfcc", n_fft, fr.hop, bool(center), fr.mode, fr.wkey, bkey, float(power),
+                                      pl.digest(dct)),
+                         plan_kw=dict(n_fft=n_fft, hop_length=fr.hop, center=center, pad_mode=fr.mode, window=fr.window,
+                                      mel_basis=basis, power=float(power), dct_basis=dct, amin=1e-10, ref_value=1.0,
+                                      top_db=80.0),
+                         n_frames=T, out_tail=(dct.shape[0], T), dtype=np.float32, launch=launch,
+                         scratch_per_clip=n_mels * ((T + 63) // 64 * 64))
+    return res if isinstance(res, nat.DeviceArray) or res.dtype == res_dtype else res.astype(res_dtype)

@@ -25,21 +25,6 @@ _vp = C.c_void_p
 _NP_PAD_ONLY = ("maximum", "mean", "median", "minimum", "wrap")
 
 
-def _device_table(ctx, key, values: np.ndarray) -> int:
-    """Small float32 constant (bin frequencies) cached on the device per context."""
-    ptr = ctx._wss.fetch(key)
-    if ptr is None:
-        arr = np.ascontiguousarray(values, dtype=np.float32)
-        while len(ctx._wss) >= 32:                 # least recently used first: a table fetched earlier in
-            _, old = ctx._wss.evict_oldest()       # the same call is the youngest entry and stays
-            ctx.free(old)
-        ptr = ctx.alloc(max(arr.nbytes, 16))
-        nat.check(nat.lib().b2l_h2d(ctx.handle, _vp(ptr), arr.ctypes.data_as(_vp), arr.nbytes))
-        ctx.synchronize()
-        ctx._wss[key] = ptr
-    return ptr
-
-
 def _freq_table(freq, sr, n_fft, n_bins):
     """``freq`` argument of the spectral statistics -> (float32-able table, cache key, result dtype)."""
     if freq is None:
@@ -60,7 +45,7 @@ def _desc(row, *, roll_percent=0.85, amin=1e-10, power=2.0, p=2.0, norm=True, fr
 
 def _take_row(ctx, stats, lead, T, row, on_device, res_dtype):
     """Row ``row`` of a [clip][N_STATS][T] block -> array of shape lead + (1, T)."""
-    n_clips = int(np.prod(lead, dtype=np.int64)) if lead else 1
+    n_clips = pl.clip_count(lead)
     if isinstance(stats, np.ndarray):
         out = stats.reshape(n_clips, nat.N_STATS, T)[:, row:row + 1, :].reshape(tuple(lead) + (1, T))
         return np.ascontiguousarray(out).astype(res_dtype, copy=False)
@@ -69,52 +54,38 @@ def _take_row(ctx, stats, lead, T, row, on_device, res_dtype):
         nat.check(nat.lib().b2l_copy2d(ctx.handle, _vp(dst.ptr), T * 4, _vp(stats.ptr + row * T * 4),
                                        nat.N_STATS * T * 4, T * 4, n_clips))
     stats.free()                      # stream-ordered pool: safe right after the copy has been enqueued
-    if on_device:
-        return dst
-    return pl.finish(ctx, dst, True, res_dtype)
+    return dst if on_device else pl.finish(dst, res_dtype)
 
 
 def _stats_from_S(S, desc, freq, sr, n_fft, what, check_negative=True):
     """S= form: stats_kernel over a stored spectrogram.  Returns (stats block, ctx, lead, T, on_device,
     S dtype, freq dtype).  ``check_negative``: fetch the kernel's "negative entry" verdict and raise like the
     reference (skipped for spectrograms this package has just computed itself)."""
-    from .spectral import _spec_to_device
-
     if not isinstance(S, nat.DeviceArray) and np.iscomplexobj(S):
         raise ParameterError(f"{what} is only defined with real-valued input")
-    ctx = S.ctx if isinstance(S, nat.DeviceArray) else nat.default_context()
+    ctx = pl.context_for(S)
     if check_negative:
         nat.check(nat.lib().b2l_status_reset(ctx.handle))
-    Sd, req, on_device = _spec_to_device(ctx, S)
+    Sd, req, on_device = pl.spectrogram_input(S)
     if Sd.ndim < 2:
         raise ParameterError("spectrogram input must have at least two dimensions")
     F, T = Sd.shape[-2], Sd.shape[-1]
     if n_fft is None or n_fft // 2 + 1 != F:
         n_fft = 2 * (F - 1)
     table, fkey, fdtype = _freq_table(freq, sr, n_fft, F)
-    d_freq = _device_table(ctx, fkey, table)
+    d_freq = ctx.constant(fkey, lambda: table)
     lead = Sd.shape[:-2]
-    n_clips = int(np.prod(lead, dtype=np.int64)) if lead else 1
-    L = nat.lib()
-    if Sd.layout == "ft":
-        src = Sd
-    else:
-        src = nat.DeviceArray.empty(ctx, Sd.shape, np.float32, layout="ft")
-        if n_clips and F and T:
-            nat.check(L.b2l_transpose(ctx.handle, _vp(Sd.ptr), n_clips, F, T, 4, _vp(src.ptr)))
+    src, own = pl.to_native(Sd)
     stats = nat.DeviceArray.empty(ctx, tuple(lead) + (nat.N_STATS, T), np.float32)
-    nat.check(L.b2l_spectral_stats_from_spec(ctx.handle, C.byref(desc), _vp(src.ptr), n_clips, T, F, _vp(d_freq),
-                                             _vp(stats.ptr)))
-    if src is not Sd:
+    nat.check(nat.lib().b2l_spectral_stats_from_spec(ctx.handle, C.byref(desc), _vp(src.ptr), pl.clip_count(lead), T,
+                                                     F, _vp(d_freq), _vp(stats.ptr)))
+    if own:
         src.free()
     if not on_device:
         Sd.free()
-    if check_negative:
-        flag = C.c_int(0)
-        nat.check(L.b2l_status_read(ctx.handle, C.byref(flag)))
-        if flag.value & 2:
-            stats.free()
-            raise ParameterError(f"{what} is only defined with non-negative energies")
+    if check_negative and pl.status_word(ctx) & 2:
+        stats.free()
+        raise ParameterError(f"{what} is only defined with non-negative energies")
     return stats, ctx, lead, T, on_device, req, fdtype
 
 
@@ -124,14 +95,9 @@ def _stats_from_y(y, desc, freq, sr, *, n_fft, hop_length, win_length, window, c
         raise ParameterError(f"Unable to compute spectrogram with n_fft={n_fft}")
     if y is None:
         raise ParameterError("Input signal must be provided to compute a spectrogram")
-    hop_length, win_length = pl.frame_params(n_fft, hop_length, win_length)
-    n, req_dtype = pl.precheck_signal(y)
-    win, wkey = pl.resolve_window(window, win_length, n_fft)
-    mode = pl.check_stft_geometry(n, n_fft, center, pad_mode)
+    fr = pl.forward_front(y, n_fft, hop_length, win_length, window, center, pad_mode, native_ok=False)
     pl.require_supported_n_fft(n_fft)
-    F = 1 + n_fft // 2
-    table, fkey, fdtype = _freq_table(freq, sr, n_fft, F)
-    T = 1 + (n + (2 * (n_fft // 2) if center else 0) - n_fft) // hop_length
+    table, fkey, fdtype = _freq_table(freq, sr, n_fft, 1 + n_fft // 2)
     if not pl.is_pow2(n_fft):
         from .spectral import _compose_nonpow2
 
@@ -143,33 +109,22 @@ def _stats_from_y(y, desc, freq, sr, *, n_fft, hop_length, win_length, window, c
             return stats
 
         on_device = isinstance(y, nat.DeviceArray)
-        stats = _compose_nonpow2(y, tail, np.float32, n_fft=n_fft, hop_length=hop_length, power=1, win_length=win_length,
+        stats = _compose_nonpow2(y, tail, np.float32, n_fft=n_fft, hop_length=fr.hop, power=1, win_length=win_length,
                                  window=window, center=center, pad_mode=pad_mode)
         ctx, lead, T_ = box["v"]
-        return stats, ctx, lead, T_, on_device, req_dtype, fdtype
-    key = ("stats", n_fft, hop_length, bool(center), mode, wkey)
-
-    def make_plan(ctx):
-        return nat.make_plan(ctx, key, n_fft=n_fft, hop_length=hop_length, center=center, pad_mode=mode, window=win,
-                             power=1.0)
-
-    L = nat.lib()
-    if isinstance(y, nat.DeviceArray):
-        ctx = y.ctx
-        staged = pl.StagedInput(ctx, y)
-        plan = make_plan(ctx)
-        stats = nat.DeviceArray.empty(ctx, staged.lead + (nat.N_STATS, T), np.float32)
-        nat.check(L.b2l_spectral_stats(ctx.handle, plan.handle, C.byref(desc), _vp(staged.dev.ptr), staged.n_clips,
-                                       staged.n, staged.n, _vp(_device_table(ctx, fkey, table)), _vp(stats.ptr)))
-        return stats, ctx, staged.lead, T, True, req_dtype, fdtype
+        return stats, ctx, lead, T_, on_device, fr.dtype, fdtype
 
     def launch(ctx, plan, d_in, m, n_, d_out, d_scr):
-        nat.check(L.b2l_spectral_stats(ctx.handle, plan.handle, C.byref(desc), _vp(d_in), m, n_, n_,
-                                       _vp(_device_table(ctx, fkey, table)), _vp(d_out)))
+        nat.check(nat.lib().b2l_spectral_stats(ctx.handle, plan.handle, C.byref(desc), _vp(d_in), m, n_, n_,
+                                               _vp(ctx.constant(fkey, lambda: table)), _vp(d_out)))
 
-    host = pl.run_host_forward(y, n_fft=n_fft, hop_length=hop_length, center=center, n_frames=T,
-                               out_mem_tail=(nat.N_STATS, T), out_dtype=np.float32, make_plan=make_plan, launch=launch)
-    return host, nat.default_context(), y.shape[:-1], T, False, req_dtype, fdtype
+    T = fr.n_frames
+    stats = pl.run_forward(y, plan_key=("stats", n_fft, fr.hop, bool(center), fr.mode, fr.wkey),
+                           plan_kw=dict(n_fft=n_fft, hop_length=fr.hop, center=center, pad_mode=fr.mode,
+                                        window=fr.window, power=1.0),
+                           n_frames=T, out_tail=(nat.N_STATS, T), dtype=np.float32, launch=launch)
+    on_device = isinstance(y, nat.DeviceArray)
+    return stats, pl.context_for(y), tuple(y.shape[:-1]), T, on_device, fr.dtype, fdtype
 
 
 def _statistic(row, what, desc, res_of, *, y, S, sr, n_fft, hop_length, freq, win_length, window, center, pad_mode):
@@ -237,33 +192,25 @@ def spectral_contrast(*, y=None, sr: float = 22050, S=None, n_fft: int = 2048, h
     ``librosa.feature.spectral_contrast`` (the bins of every octave band must be contiguous, which holds for
     any increasing ``freq``)."""
     from ..core.spectrum import _spectrogram, power_to_db
-    from .spectral import _spec_to_device
 
-    to_host, validate = True, False
+    staged = None
     if S is None:
         if y is None:
             raise ParameterError("Input signal must be provided to compute a spectrogram")
         _, req = pl.precheck_signal(y)
-        if isinstance(y, nat.DeviceArray):
-            ctx, yd, to_host = y.ctx, y, False
-        else:
-            ctx = nat.default_context()
-            staged = pl.StagedInput(ctx, y)
-            yd, validate = staged.dev, True
-        Sd, n_fft = _spectrogram(y=yd, n_fft=n_fft, hop_length=hop_length, power=1, win_length=win_length,
+        staged = pl.StagedInput(y)
+        Sd, n_fft = _spectrogram(y=staged.dev, n_fft=n_fft, hop_length=hop_length, power=1, win_length=win_length,
                                  window=window, center=center, pad_mode=pad_mode)
-        if validate:
-            hop_eff, _ = pl.frame_params(n_fft, hop_length, win_length)
-            staged.scan_uncovered(n_fft, hop_eff, center, Sd.shape[-1])
+        staged.scan_uncovered(n_fft, hop_length, win_length, center, Sd.shape[-1])
         own_S = True
     else:
         if not isinstance(S, nat.DeviceArray) and np.iscomplexobj(S):
             raise nat.UnsupportedOnGPU("spectral_contrast of a complex S is not supported on the GPU: pass np.abs(S)")
-        ctx = S.ctx if isinstance(S, nat.DeviceArray) else nat.default_context()
-        Sd, req, on_device = _spec_to_device(ctx, S)
-        to_host, own_S = not on_device, not on_device
+        Sd, req, on_device = pl.spectrogram_input(S)
+        own_S = not on_device
         if n_fft is None or n_fft // 2 + 1 != Sd.shape[-2]:
             n_fft = 2 * (Sd.shape[-2] - 1)
+    ctx = Sd.ctx
     F, T = Sd.shape[-2], Sd.shape[-1]
     if freq is None:
         freq = fft_frequencies(sr=sr, n_fft=n_fft)
@@ -299,20 +246,15 @@ def spectral_contrast(*, y=None, sr: float = 22050, S=None, n_fft: int = 2048, h
         desc.count[k] = max(int(count), 0)
         desc.k[k] = int(max(np.rint(quantile * np.sum(band)), 1))
     lead = Sd.shape[:-2]
-    n_clips = int(np.prod(lead, dtype=np.int64)) if lead else 1
+    n_clips = pl.clip_count(lead)
     L = nat.lib()
-    if Sd.layout == "ft":
-        src = Sd
-    else:
-        src = nat.DeviceArray.empty(ctx, Sd.shape, np.float32, layout="ft")
-        if n_clips and F and T:
-            nat.check(L.b2l_transpose(ctx.handle, _vp(Sd.ptr), n_clips, F, T, 4, _vp(src.ptr)))
+    src, own = pl.to_native(Sd)
     shape = tuple(lead) + (n_bands + 1, T)
     peak = nat.DeviceArray.empty(ctx, shape, np.float32)
     valley = nat.DeviceArray.empty(ctx, shape, np.float32)
     nat.check(L.b2l_spectral_contrast(ctx.handle, C.byref(desc), _vp(src.ptr), n_clips, T, F, _vp(peak.ptr),
                                       _vp(valley.ptr)))
-    if src is not Sd:
+    if own:
         src.free()
     if own_S:
         Sd.free()
@@ -325,9 +267,10 @@ def spectral_contrast(*, y=None, sr: float = 22050, S=None, n_fft: int = 2048, h
     nat.check(L.b2l_sub(ctx.handle, _vp(peak.ptr), _vp(valley.ptr), peak.size, _vp(out.ptr)))
     peak.free()
     valley.free()
-    if not to_host:
-        return out
-    return pl.finish(ctx, out, True, np.result_type(req, np.float64), validate=validate)
+    res_dtype = np.result_type(req, np.float64)
+    if staged is not None:
+        return staged.result(out, res_dtype)
+    return out if on_device else pl.finish(out, res_dtype)
 
 
 # --------------------------------------------------------------------------------------------- time-domain framings
@@ -342,9 +285,9 @@ def _frame_feature(what, y, frame_length, hop_length, center, pad_mode, *, thres
         raise ParameterError(f"Input is too short (n={padded}) for frame_length={frame_length}")
     if hop_length < 1:
         raise ParameterError(f"Invalid hop_length: {hop_length}")
-    T = 1 + (padded - frame_length) // hop_length
-    ctx = pl.context_for(y)
-    staged = pl.StagedInput(ctx, y)
+    T = pl.frame_count(n, frame_length, hop_length, center)
+    staged = pl.StagedInput(y)
+    ctx = staged.ctx
     out = nat.DeviceArray.empty(ctx, staged.lead + (1, T), np.float32)
     nat.check(nat.lib().b2l_frame_feature(ctx.handle, what, _vp(staged.dev.ptr), staged.n_clips, staged.n, staged.n,
                                           frame_length, hop_length, int(bool(center)), nat.PAD_MODES[pad_mode],
@@ -353,9 +296,9 @@ def _frame_feature(what, y, frame_length, hop_length, center, pad_mode, *, thres
     if staged.on_device:
         return out, True
     if validate:
-        staged.scan_uncovered(frame_length, hop_length, center, T)
-    res = pl.finish(ctx, out, True, None, validate=validate)
-    staged.dev.free()
+        staged.scan_uncovered(frame_length, hop_length, None, center, T)
+    res = pl.finish(out, validate=validate)
+    staged.release()
     return res, False
 
 

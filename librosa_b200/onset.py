@@ -59,35 +59,23 @@ def onset_strength_multi(*, y=None, sr: float = 22050, S=None, n_fft: int = 2048
     if ref is not None:
         raise nat.UnsupportedOnGPU("a caller-supplied reference spectrum is not supported on the GPU")
 
-    to_host = True
-    validate = False
+    staged = None
     if S is None:
         if y is None:
             raise ParameterError("Input signal must be provided to compute a spectrogram")
-        n, req = pl.precheck_signal(y)
-        if isinstance(y, nat.DeviceArray):
-            ctx, yd, to_host = y.ctx, y, False
-        else:
-            # host signal: upload once, keep every intermediate on the device; util.valid_audio's finite
-            # check is the kernels' status word, read when the envelope is copied back
-            ctx = nat.default_context()
-            staged = pl.StagedInput(ctx, y)
-            yd, validate = staged.dev, True
-            hop_eff, _ = pl.frame_params(n_fft, hop_length, kwargs.get("win_length"))
-            T_ = 1 + (n + 2 * (n_fft // 2) - n_fft) // hop_eff
-            staged.scan_uncovered(n_fft, hop_eff, True, T_)
-        mel = melspectrogram(y=yd, sr=sr, n_fft=n_fft, hop_length=hop_length, **kwargs)
+        _, req = pl.precheck_signal(y)
+        # one upload, every intermediate on the device; the mel frames are always centred (``center`` only
+        # sets the pad width below)
+        staged = pl.StagedInput(y)
+        mel = melspectrogram(y=staged.dev, sr=sr, n_fft=n_fft, hop_length=hop_length, **kwargs)
+        staged.scan_uncovered(n_fft, hop_length, kwargs.get("win_length"), True, mel.shape[-1])
         Sd = power_to_db(mel)
         mel.free()
         res_dtype = np.dtype(req)
     else:
-        from .feature.spectral import _spec_to_device
-
-        ctx = S.ctx if isinstance(S, nat.DeviceArray) else nat.default_context()
         if not isinstance(S, nat.DeviceArray):
             S = np.atleast_2d(np.asarray(S))
-        Sd, res_dtype, on_device = _spec_to_device(ctx, S)
-        to_host = not on_device
+        Sd, res_dtype, on_device = pl.spectrogram_input(S)
         if Sd.layout != "c":
             raise ParameterError("device spectrogram must be C-ordered (..., rows, frames)")
     if Sd.ndim < 2:
@@ -95,8 +83,8 @@ def onset_strength_multi(*, y=None, sr: float = 22050, S=None, n_fft: int = 2048
     rows, T = Sd.shape[-2], Sd.shape[-1]
     if T <= lag:
         raise ParameterError(f"lag={lag} needs more than {T} frames")
+    ctx = Sd.ctx
     lead = Sd.shape[:-2]
-    n_clips = int(np.prod(lead, dtype=np.int64)) if lead else 1
     desc = nat.OnsetDesc(lag=int(lag), max_size=int(max_size), detrend=int(bool(detrend)),
                          pad_width=int(lag) + (n_fft // (2 * hop_length) if center else 0))
     if callable(aggregate):
@@ -111,14 +99,15 @@ def onset_strength_multi(*, y=None, sr: float = 22050, S=None, n_fft: int = 2048
         desc.n_channels = 0
         n_out = rows
     out = nat.DeviceArray.empty(ctx, tuple(lead) + (n_out, T), np.float32)
-    nat.check(nat.lib().b2l_onset_from_spec(ctx.handle, C.byref(desc), _vp(Sd.ptr), n_clips, rows, T, _vp(out.ptr)))
-    if S is None or to_host:
+    nat.check(nat.lib().b2l_onset_from_spec(ctx.handle, C.byref(desc), _vp(Sd.ptr), pl.clip_count(lead), rows, T,
+                                            _vp(out.ptr)))
+    if staged is not None or not on_device:
         Sd.free()
-    if not to_host:
-        return out
     if detrend:   # scipy.signal.lfilter with float64 coefficients returns float64
         res_dtype = np.result_type(res_dtype, np.float64)
-    return pl.finish(ctx, out, True, res_dtype, validate=validate)
+    if staged is not None:
+        return staged.result(out, res_dtype)
+    return out if on_device else pl.finish(out, res_dtype)
 
 
 def onset_strength(*, y=None, sr: float = 22050, S=None, lag: int = 1, max_size: int = 1, ref=None,

@@ -489,13 +489,64 @@ def test_pinned_host_end_to_end(lb, oracle):
     close(M, oracle.melspectrogram(y=np.array(y), sr=22050), **TOL["mel"])
 
 
+def _y(lb):
+    y = 0.1 * np.random.default_rng(5).standard_normal((2, 12000))
+    return lb.default_context().to_device(y.astype(np.float32))
+
+
+def _dev_c(lb, a):
+    """A C-ordered device copy of a logical (..., bins, frames) array."""
+    return lb.default_context().to_device(np.ascontiguousarray(a))
+
+
+# (input builder, call, kernel launches of the call): every spectrogram input in the native [frame][bin] layout goes
+# straight to its kernel, a C-ordered one costs exactly one transpose; host batches take no extra kernel
+LAUNCHES = {
+    "stft host": (lambda lb: np.zeros(4096, dtype=np.float32), lambda lb, x: lb.stft(x), 1),
+    "mfcc host": (lambda lb: np.zeros(4096, dtype=np.float32), lambda lb, x: lb.feature.mfcc(y=x), 2),
+    "stft": (_y, lambda lb, x: lb.stft(x), 1),
+    "istft ft": (lambda lb: lb.stft(_y(lb)), lambda lb, x: lb.istft(x), 1),
+    "istft c": (lambda lb: _dev_c(lb, lb.stft(_y(lb)).get()), lambda lb, x: lb.istft(x), 2),
+    "_spectrogram": (_y, lambda lb, x: lb._spectrogram(y=x), 1),
+    "melspectrogram": (_y, lambda lb, x: lb.feature.melspectrogram(y=x), 1),
+    "melspectrogram S ft": (lambda lb: lb._spectrogram(y=_y(lb), power=2)[0],
+                            lambda lb, x: lb.feature.melspectrogram(S=x), 1),
+    "melspectrogram S c": (lambda lb: _dev_c(lb, lb._spectrogram(y=_y(lb), power=2)[0].get()),
+                           lambda lb, x: lb.feature.melspectrogram(S=x), 2),
+    "mfcc": (_y, lambda lb, x: lb.feature.mfcc(y=x), 2),   # fused mel kernel + clamp/DCT kernel
+    "spectral_centroid": (_y, lambda lb, x: lb.feature.spectral_centroid(y=x), 1),
+    "spectral_centroid S ft": (lambda lb: lb._spectrogram(y=_y(lb))[0],
+                               lambda lb, x: lb.feature.spectral_centroid(S=x), 1),
+    "spectral_centroid S c": (lambda lb: _dev_c(lb, lb._spectrogram(y=_y(lb))[0].get()),
+                              lambda lb, x: lb.feature.spectral_centroid(S=x), 2),
+    "spectral_contrast": (_y, lambda lb, x: lb.feature.spectral_contrast(y=x), 7),
+    "spectral_contrast S ft": (lambda lb: lb._spectrogram(y=_y(lb))[0],
+                               lambda lb, x: lb.feature.spectral_contrast(S=x), 6),
+    "spectral_contrast S c": (lambda lb: _dev_c(lb, lb._spectrogram(y=_y(lb))[0].get()),
+                              lambda lb, x: lb.feature.spectral_contrast(S=x), 7),
+    "chroma_stft": (_y, lambda lb, x: lb.feature.chroma_stft(y=x, tuning=0.0), 3),
+    "chroma_stft S ft": (lambda lb: lb._spectrogram(y=_y(lb), power=2)[0],
+                         lambda lb, x: lb.feature.chroma_stft(S=x, tuning=0.0), 2),
+    "chroma_stft S c": (lambda lb: _dev_c(lb, lb._spectrogram(y=_y(lb), power=2)[0].get()),
+                        lambda lb, x: lb.feature.chroma_stft(S=x, tuning=0.0), 3),
+    "onset_strength": (_y, lambda lb, x: lb.onset.onset_strength(y=x), 4),
+    "decompose.hpss ft": (lambda lb: lb.stft(_y(lb)), lambda lb, x: lb.decompose.hpss(x), 2),
+    "decompose.hpss c": (lambda lb: _dev_c(lb, lb.stft(_y(lb)).get()), lambda lb, x: lb.decompose.hpss(x), 3),
+    "effects.harmonic": (_y, lambda lb, x: lb.effects.harmonic(x), 4),
+    "phase_vocoder ft": (lambda lb: lb.stft(_y(lb)), lambda lb, x: lb.phase_vocoder(x, rate=1.25), 1),
+    "phase_vocoder c": (lambda lb: _dev_c(lb, lb.stft(_y(lb)).get()), lambda lb, x: lb.phase_vocoder(x, rate=1.25), 2),
+}
+
+
 def test_launch_counter_and_no_fallback(lb):
     ctx = lb.default_context()
-    before = ctx.launch_count
-    lb.stft(np.zeros(4096, dtype=np.float32))
-    assert ctx.launch_count == before + 1
-    lb.feature.mfcc(y=np.zeros(4096, dtype=np.float32))
-    assert ctx.launch_count == before + 3   # fused mel kernel + clamp/DCT kernel
+    counted = {}
+    for name, (build, call, _) in LAUNCHES.items():
+        x = build(lb)
+        before = ctx.launch_count
+        call(lb, x)
+        counted[name] = ctx.launch_count - before
+    assert counted == {name: expected for name, (_, _, expected) in LAUNCHES.items()}
 
 
 def test_single_rank_communicator_roundtrip(lb, oracle):
