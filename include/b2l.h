@@ -324,6 +324,57 @@ int b2l_frame_feature(b2l_ctx* ctx, int32_t what, const float* d_y, int64_t n_cl
                       int32_t frame_length, int32_t hop_length, int32_t center, int32_t pad_mode, float threshold,
                       int32_t zero_pos, int32_t pad_first, float out_scale, float* d_out);
 
+/* ---- pitch tracking: librosa.yin / librosa.pyin (core/pitch.py:369-931, sequence.py:1174-1259) ---------------
+ * A row is one (clip, frame) pair; n_lags = max_period - min_period + 1; max_cand = (n_lags + 1) / 2.
+ * b2l_yin_cmnd: frames (frame_length, hop_length, center / pad_mode as librosa.util.frame after np.pad) -> the
+ *   cumulative mean normalised difference, float32 d_cmnd [n_clips][n_frames][n_lags]; the autocorrelation comes
+ *   from the register FFT at N = the smallest power of two >= frame_length + max_period + 1 (up to 8192, else
+ *   B2L_ERR_UNSUPPORTED).  Sets bit 0 of the status word when a frame reads a non-finite sample.
+ * b2l_yin_pick: CMND rows -> f0 of yin, float64 [n_rows]. */
+typedef struct b2l_yin_desc {
+  int32_t frame_length, hop_length, center, pad_mode;
+  int32_t min_period, max_period;
+  double sr, trough_threshold;
+} b2l_yin_desc;
+int b2l_yin_cmnd(b2l_ctx* ctx, const b2l_yin_desc* desc, const float* d_y, int64_t n_clips, int64_t n,
+                 int64_t y_stride, float* d_cmnd);
+int b2l_yin_pick(b2l_ctx* ctx, const b2l_yin_desc* desc, const float* d_cmnd, int64_t n_rows, double* d_f0);
+/* pyin's decision stages.  Tables are device arrays built by the caller:
+ *   d_thresholds [n_thresholds + 1] np.linspace(0, 1, n_thresholds + 1); d_beta [n_thresholds] the beta weights;
+ *   d_beta_cum [n_thresholds + 1] np.sum(beta[:c]); d_pmf: scipy.stats.boltzmann.pmf(pos, lambda, n) at
+ *   n (n - 1) / 2 + pos for n = 1 .. max_cand;
+ *   the Viterbi's log(T + tiny) of T = kron(transition_loop(2, 1 - switch_prob), transition_local(n_pitch_bins,
+ *   2 half_width + 1)) for source state (a, p) and target (b, q): d_ltab[(d_cls[p] * 2 + (a != b)) * (2 half_width
+ *   + 1) + q - p + half_width] for |q - p| <= half_width (d_cls[p]: class of the row sum of transition_local's row p),
+ *   log(tiny) elsewhere; a transition is searched when its value is >= log_thr, or always when full;
+ *   d_freqs [n_pitch_bins] the bin frequencies.
+ * b2l_pyin_obs: CMND rows -> per row the voiced candidates (count, pitch bins ascending, probabilities; at most
+ *   max_cand) and voiced_prob.
+ * b2l_viterbi: candidates of [n_clips][n_frames] rows -> decoded states (uint16) and, when d_f0 is given, f0 and the
+ *   voiced flag (d_voiced, one byte per frame; unvoiced f0 = fill_na when fill).  2 * n_pitch_bins states, at most
+ *   what fits in shared memory at 18 bytes per state. */
+typedef struct b2l_pyin_desc {
+  int32_t min_period, max_period;
+  int32_t n_thresholds, n_pitch_bins, n_bins_per_semitone;
+  double sr, fmin, no_trough_prob;
+  const double* d_thresholds;
+  const double* d_beta;
+  const double* d_beta_cum;
+  const double* d_pmf;
+  double log_p_init, fill_na;
+  int32_t fill;
+  int32_t half_width, full;
+  double log_thr;
+  const int32_t* d_cls;
+  const double* d_ltab;
+  const double* d_freqs;
+} b2l_pyin_desc;
+int b2l_pyin_obs(b2l_ctx* ctx, const b2l_pyin_desc* desc, const float* d_cmnd, int64_t n_rows, int32_t* d_count,
+                 int32_t* d_cand_bin, double* d_cand_prob, double* d_voiced_prob);
+int b2l_viterbi(b2l_ctx* ctx, const b2l_pyin_desc* desc, const int32_t* d_count, const int32_t* d_cand_bin,
+                const double* d_cand_prob, const double* d_voiced_prob, int64_t n_clips, int64_t n_frames,
+                uint16_t* d_states, double* d_f0, uint8_t* d_voiced);
+
 /* ---- double-precision path: float64 audio / complex128 spectra ---------------------------------
  * librosa computes a float64 signal in float64 (dtype_r2c, core/spectrum.py:341; the window product :388 and the
  * irfft :598 follow the input's precision; the mel einsum feature/spectral.py:2160 and scipy.fft.dct :2005

@@ -110,6 +110,22 @@ class ReassignDesc(C.Structure):
                 ("fill_nan", C.c_int32), ("clip", C.c_int32)]
 
 
+class YinDesc(C.Structure):
+    """struct b2l_yin_desc (include/b2l.h)."""
+    _fields_ = [("frame_length", C.c_int32), ("hop_length", C.c_int32), ("center", C.c_int32), ("pad_mode", C.c_int32),
+                ("min_period", C.c_int32), ("max_period", C.c_int32), ("sr", C.c_double), ("trough_threshold", C.c_double)]
+
+
+class PyinDesc(C.Structure):
+    """struct b2l_pyin_desc (include/b2l.h); the d_* fields are device pointers."""
+    _fields_ = [("min_period", C.c_int32), ("max_period", C.c_int32), ("n_thresholds", C.c_int32),
+                ("n_pitch_bins", C.c_int32), ("n_bins_per_semitone", C.c_int32), ("sr", C.c_double),
+                ("fmin", C.c_double), ("no_trough_prob", C.c_double), ("d_thresholds", C.c_void_p),
+                ("d_beta", C.c_void_p), ("d_beta_cum", C.c_void_p), ("d_pmf", C.c_void_p), ("log_p_init", C.c_double),
+                ("fill_na", C.c_double), ("fill", C.c_int32), ("half_width", C.c_int32), ("full", C.c_int32),
+                ("log_thr", C.c_double), ("d_cls", C.c_void_p), ("d_ltab", C.c_void_p), ("d_freqs", C.c_void_p)]
+
+
 N_STATS = 6
 STAT_CENTROID, STAT_BANDWIDTH, STAT_ROLLOFF, STAT_FLATNESS, STAT_RMS, STAT_TOTAL = range(6)
 FRAME_RMS, FRAME_ZERO_CROSSINGS = 0, 1
@@ -181,6 +197,10 @@ def _declare(lib):
         "b2l_spectral_stats_from_spec": (C.c_int, [_vp, P(StatsDesc), _vp, _i64, _i64, C.c_int32, _vp, _vp]),
         "b2l_frame_feature": (C.c_int, [_vp, C.c_int32, _vp, _i64, _i64, _i64, C.c_int32, C.c_int32, C.c_int32,
                                         C.c_int32, C.c_float, C.c_int32, C.c_int32, C.c_float, _vp]),
+        "b2l_yin_cmnd": (C.c_int, [_vp, P(YinDesc), _vp, _i64, _i64, _i64, _vp]),
+        "b2l_yin_pick": (C.c_int, [_vp, P(YinDesc), _vp, _i64, _vp]),
+        "b2l_pyin_obs": (C.c_int, [_vp, P(PyinDesc), _vp, _i64, _vp, _vp, _vp, _vp]),
+        "b2l_viterbi": (C.c_int, [_vp, P(PyinDesc), _vp, _vp, _vp, _vp, _i64, _i64, _vp, _vp, _vp]),
         "b2l_stft_f64": (C.c_int, [_vp, _vp, _i64, _i64, _i64, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                    P(C.c_double), _vp]),
         "b2l_istft_f64": (C.c_int, [_vp, _vp, _i64, _i64, _i64, C.c_int32, C.c_int32, C.c_int32, P(C.c_double),

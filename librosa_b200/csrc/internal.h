@@ -217,6 +217,8 @@ int launch(b2l_ctx* c, void (*fn)(P...), dim3 grid, int threads, size_t smem, co
 
 // ------------------------------------------------------------------ plans (plan.cu)
 long long plan_frames(const b2l_plan* p, long long n);
+// Inter-pass twiddles of the register FFT of complex size 2^cfg.log2m (FftCfg::tw_offset layout; split: fwd_kernel's table).
+std::vector<float2> engine_twiddles(const HostFftCfg& cfg, bool split = false);
 // MelRow table for warps that process H mel rows at a time (see MelRow / MelLayout in common.cuh), built on first use.
 int get_row_table(const b2l_plan* p, int H, const b2l_plan::RowTable** out);
 

@@ -25,7 +25,7 @@ static int upload(const b2l_plan* p, const std::vector<T>& h, T** d) {
 
 // inter-pass twiddles of the register FFT for a complex size 2^log2m (FftCfg::tw_offset layout): the full table, or
 // the split one of fwd_kernel (radix-32 passes as the factors of tw_row_exponent)
-static std::vector<float2> engine_twiddles(const HostFftCfg& cfg, bool split = false) {
+std::vector<float2> b2l::engine_twiddles(const HostFftCfg& cfg, bool split) {
   const double two_pi = 6.283185307179586476925286766559;
   std::vector<float2> tw((size_t)cfg.tw_count(split));
   for (int s = 1; s < cfg.npass; ++s) {

@@ -1,5 +1,6 @@
 """Device-resident timings of the frame-wise features (SURVEY 8f rank 2) on a cfg-2 shaped batch, next to the
-oracle (CPU, one process) on a small sample.  CUDA events around `reps` calls after warm-up.
+oracle (CPU, one process) on a small sample.  CUDA events around `reps` calls after warm-up.  The pitch trackers
+run with fmin C2, fmax C7 and their other defaults (frame_length 2048, hop 512); their oracle sample is one clip.
 
     python tools/feature_timing.py [clips=1024] [reps=10] > gpurun_out/feature_timing.json
 """
@@ -16,6 +17,7 @@ import numpy as np
 
 import bench
 import librosa_b200 as lb
+import pitch_oracle as PO
 from oracle import ref_np as O
 
 clips = int(sys.argv[1]) if len(sys.argv) > 1 else 1024
@@ -30,6 +32,9 @@ frames = clips * T
 mel_db = lb.power_to_db(lb.feature.melspectrogram(y=dev, sr=sr))
 mel_pw = lb.feature.melspectrogram(y=dev, sr=sr)
 dev128 = ctx.to_device(host[:128])
+
+
+C2, C7 = 65.40639132514966, 2093.004522404789
 
 
 def free(x):
@@ -52,7 +57,10 @@ FEATURES = {
     "effects.hpss (128 clips)": (lambda: lb.effects.hpss(dev128), None),
     "pcen(mel)": (lambda: lb.pcen(mel_pw, sr=sr), None),
     "amplitude_to_db(mel)": (lambda: lb.amplitude_to_db(mel_pw), None),
+    "yin(C2-C7)": (lambda: lb.yin(dev, fmin=C2, fmax=C7, sr=sr), lambda y: PO.yin(y, fmin=C2, fmax=C7, sr=sr)),
+    "pyin(C2-C7)": (lambda: lb.pyin(dev, fmin=C2, fmax=C7, sr=sr), lambda y: PO.pyin(y, fmin=C2, fmax=C7, sr=sr)),
 }
+CPU_SAMPLE = {"yin(C2-C7)": 1, "pyin(C2-C7)": 1}   # clips in the oracle sample (default 8)
 out = {"clips": clips, "frames": frames, "reps": reps, "features": {}}
 with warnings.catch_warnings():
     warnings.simplefilter("ignore")
@@ -72,12 +80,13 @@ with warnings.catch_warnings():
         row = {"gpu_ms": round(ms, 3), "frames": nfr, "gpu_frames_per_s": round(nfr / ms * 1e3),
                "launches_per_call": (ctx.launch_count - l0) / reps}
         if cpu is not None:
-            sample = host[:8]
+            sample = host[:CPU_SAMPLE.get(name, 8)]
             cpu(sample[:1])
             t0 = time.perf_counter()
             cpu(sample)
             dt = time.perf_counter() - t0
             row["cpu_oracle_frames_per_s_1proc"] = round(sample.shape[0] * T / dt)
+            row["cpu_oracle_s_per_clip"] = round(dt / sample.shape[0], 4)
         out["features"][name] = row
         print(name, row, file=sys.stderr)
 print(json.dumps(out, indent=1))

@@ -1,12 +1,14 @@
 """Generate tests/golden/hotpath_v1.npz (tests/cases.py), tests/golden/features_v1.npz
 (tests/feature_cases.py) and tests/golden/reference_pins_v1.npz (tests/reference_pins.py) by running the
-cases through the UNMODIFIED reference.
+cases through the UNMODIFIED reference; ``--pitch`` writes only tests/golden/pitch_v1.npz (tests/pitch_cases.py)
+and leaves the other fixtures as they are.
 
 Needs a checkout of the reference (see tools/ref_shim.py); the tests only read the stored fixtures.  Also
 stores a handful of constant tables (mel bases, window sum-square, mel-scale known answers) produced by the
 reference.
 
     python tools/make_golden.py
+    python tools/make_golden.py --pitch
 """
 from __future__ import annotations
 
@@ -101,5 +103,25 @@ def write_reference_pins(ref):
     print("wrote", path, os.path.getsize(path), "bytes")
 
 
+def write_pitch():
+    """tests/golden/pitch_v1.npz: yin / pyin of every case of tests/pitch_cases.py."""
+    from pitch_cases import PITCH_CASES, outputs, run
+
+    ref = ref_shim.load_reference()
+    store = {}
+    for case in PITCH_CASES:
+        with warnings.catch_warnings():
+            warnings.simplefilter("ignore")
+            for key, arr in outputs(case, run(ref, case)).items():
+                store[key] = np.ascontiguousarray(arr)
+                print(f"{key:40s} {arr.shape} {arr.dtype}")
+    path = os.path.join(ROOT, "tests", "golden", "pitch_v1.npz")
+    np.savez_compressed(path, **store)
+    print("wrote", path, os.path.getsize(path), "bytes")
+
+
 if __name__ == "__main__":
-    main()
+    if "--pitch" in sys.argv[1:]:
+        write_pitch()
+    else:
+        main()
