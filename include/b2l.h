@@ -375,6 +375,38 @@ int b2l_viterbi(b2l_ctx* ctx, const b2l_pyin_desc* desc, const int32_t* d_count,
                 const double* d_cand_prob, const double* d_voiced_prob, int64_t n_clips, int64_t n_frames,
                 uint16_t* d_states, double* d_f0, uint8_t* d_voiced);
 
+/* ---- rhythm: librosa.feature.tempogram / tempo (feature/rhythm.py:38-470) ---------------------------------------
+ * b2l_tempogram: onset envelopes d_env [n_rows][n] (float32, or float64 when env_f64) -> the normalised local
+ *   autocorrelation, float64 d_out [n_rows][n_frames][win_length] (lags contiguous); n_frames = n when centred
+ *   (np.pad mode "linear_ramp", then the first n frames), n - win_length + 1 otherwise.  d_window [win_length] is
+ *   the float64 window.  The arithmetic is FP64 for both envelope types.  win_length up to 4096
+ *   (else B2L_ERR_UNSUPPORTED).  util.normalize along the lags with `norm` (B2L_TG_NORM_*; norm_p the exponent of
+ *   B2L_TG_NORM_P) and threshold tiny(float64); sets bit 2 of the status word when an autocorrelation value is not
+ *   finite (normalize's "Input must be finite").
+ * b2l_tempo: tempograms -> the BPM d_bpms[k] of the first lag k maximising log1p(1e6 tg) + d_logprior[k]
+ *   (NaN counts as the maximum), float64.  Element (row, lag, frame) of d_tg (float32, or float64 when tg_f64)
+ *   is at row * row_stride + lag * lag_stride + frame * frame_stride.  With mean != 0 the tempogram is first
+ *   averaged over the frames (d_out [n_rows]), else every frame is scored (d_out [n_rows][n_frames]). */
+enum b2l_tempogram_norm {
+  B2L_TG_NORM_NONE = 0,
+  B2L_TG_NORM_MAX = 1,     /* np.inf */
+  B2L_TG_NORM_MIN = 2,     /* -np.inf */
+  B2L_TG_NORM_COUNT = 3,   /* 0 */
+  B2L_TG_NORM_P = 4        /* p > 0 */
+};
+typedef struct b2l_tempogram_desc {
+  int32_t win_length, center, norm, env_f64;
+  double norm_p;
+} b2l_tempogram_desc;
+int b2l_tempogram(b2l_ctx* ctx, const b2l_tempogram_desc* desc, const void* d_env, int64_t n_rows, int64_t n,
+                  const double* d_window, double* d_out);
+typedef struct b2l_tempo_desc {
+  int32_t n_lags, mean, tg_f64;
+  int64_t n_frames, row_stride, lag_stride, frame_stride;
+} b2l_tempo_desc;
+int b2l_tempo(b2l_ctx* ctx, const b2l_tempo_desc* desc, const void* d_tg, int64_t n_rows, const double* d_logprior,
+              const double* d_bpms, double* d_out);
+
 /* ---- double-precision path: float64 audio / complex128 spectra ---------------------------------
  * librosa computes a float64 signal in float64 (dtype_r2c, core/spectrum.py:341; the window product :388 and the
  * irfft :598 follow the input's precision; the mel einsum feature/spectral.py:2160 and scipy.fft.dct :2005

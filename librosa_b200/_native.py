@@ -126,6 +126,19 @@ class PyinDesc(C.Structure):
                 ("log_thr", C.c_double), ("d_cls", C.c_void_p), ("d_ltab", C.c_void_p), ("d_freqs", C.c_void_p)]
 
 
+class TempogramDesc(C.Structure):
+    """struct b2l_tempogram_desc (include/b2l.h)."""
+    _fields_ = [("win_length", C.c_int32), ("center", C.c_int32), ("norm", C.c_int32), ("env_f64", C.c_int32),
+                ("norm_p", C.c_double)]
+
+
+class TempoDesc(C.Structure):
+    """struct b2l_tempo_desc (include/b2l.h)."""
+    _fields_ = [("n_lags", C.c_int32), ("mean", C.c_int32), ("tg_f64", C.c_int32), ("n_frames", C.c_int64),
+                ("row_stride", C.c_int64), ("lag_stride", C.c_int64), ("frame_stride", C.c_int64)]
+
+
+TG_NORM_NONE, TG_NORM_MAX, TG_NORM_MIN, TG_NORM_COUNT, TG_NORM_P = range(5)   # enum b2l_tempogram_norm
 N_STATS = 6
 STAT_CENTROID, STAT_BANDWIDTH, STAT_ROLLOFF, STAT_FLATNESS, STAT_RMS, STAT_TOTAL = range(6)
 FRAME_RMS, FRAME_ZERO_CROSSINGS = 0, 1
@@ -201,6 +214,8 @@ def _declare(lib):
         "b2l_yin_pick": (C.c_int, [_vp, P(YinDesc), _vp, _i64, _vp]),
         "b2l_pyin_obs": (C.c_int, [_vp, P(PyinDesc), _vp, _i64, _vp, _vp, _vp, _vp]),
         "b2l_viterbi": (C.c_int, [_vp, P(PyinDesc), _vp, _vp, _vp, _vp, _i64, _i64, _vp, _vp, _vp]),
+        "b2l_tempogram": (C.c_int, [_vp, P(TempogramDesc), _vp, _i64, _i64, _vp, _vp]),
+        "b2l_tempo": (C.c_int, [_vp, P(TempoDesc), _vp, _i64, _vp, _vp, _vp]),
         "b2l_stft_f64": (C.c_int, [_vp, _vp, _i64, _i64, _i64, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                    P(C.c_double), _vp]),
         "b2l_istft_f64": (C.c_int, [_vp, _vp, _i64, _i64, _i64, C.c_int32, C.c_int32, C.c_int32, P(C.c_double),

@@ -239,6 +239,12 @@ def context_for(x):
     return x.ctx if isinstance(x, nat.DeviceArray) else nat.default_context()
 
 
+def f64_constant(ctx, key, arr) -> int:
+    """Device copy of a float64 / integer table cached by the context (Context.constant stores raw 4-byte words)."""
+    arr = np.ascontiguousarray(arr)
+    return ctx.constant(key, lambda: arr.reshape(-1).view(np.float32))
+
+
 def clip_count(lead) -> int:
     """Number of clips in a batch with leading dimensions ``lead`` (one for a single clip)."""
     return int(np.prod(lead, dtype=np.int64)) if lead else 1

@@ -1,7 +1,8 @@
 """Frequency-scale conversions feeding ``filters.mel`` (host side, float64).
 
 Mirrors librosa/core/convert.py: hz_to_mel (:1004-1058), mel_to_hz (:1069-1121),
-mel_frequencies (:1432-1508), fft_frequencies (:1369).
+mel_frequencies (:1432-1508), fft_frequencies (:1369), tempo_frequencies (:1514-1548) and
+fourier_tempo_frequencies (:1551-1579).
 """
 from __future__ import annotations
 
@@ -59,3 +60,16 @@ def hz_to_octs(frequencies, *, tuning: float = 0.0, bins_per_octave: int = 12):
     a440 = 440.0 * 2.0 ** (tuning / bins_per_octave)
     octs = np.log2(np.asanyarray(frequencies) / (float(a440) / 16))
     return octs[()]
+
+
+def tempo_frequencies(n_bins: int, *, hop_length: int = 512, sr: float = 22050):
+    """BPM of each lag of a tempogram: lag k spans k * hop_length / sr seconds; the zero lag is ``inf``."""
+    bpm = np.empty(int(n_bins), dtype=np.float64)
+    bpm[0] = np.inf                    # an IndexError for n_bins < 1, like the reference's
+    bpm[1:] = 60.0 * sr / (hop_length * np.arange(1.0, n_bins))
+    return bpm
+
+
+def fourier_tempo_frequencies(*, sr: float = 22050, win_length: int = 384, hop_length: int = 512):
+    """BPM of each bin of a Fourier tempogram."""
+    return fft_frequencies(sr=sr * 60 / float(hop_length), n_fft=win_length)

@@ -332,12 +332,6 @@ def _obs_tables(n_thresholds, beta_parameters, boltzmann_parameter, max_cand):
     return thresholds, beta, beta_cum, pmf
 
 
-def _f64_constant(ctx, key, arr):
-    """Device copy of a float64 / integer table cached by the context (Context.constant stores raw 4-byte words)."""
-    arr = np.ascontiguousarray(arr)
-    return ctx.constant(key, lambda: arr.reshape(-1).view(np.float32))
-
-
 # 18 bytes of shared memory per Viterbi state (csrc/pitch_kernels.cuh viterbi_smem) within the 227 KiB an H100 CTA
 # may opt into; checked here before the host builds the transition tables of an oversized configuration
 _VITERBI_MAX_STATES = min(65535, (227 * 1024) // 18)
@@ -370,11 +364,11 @@ def _pyin_setup(where, *, min_period, max_period, hop_length, sr, fmin, fmax, n_
                         fill_na=float(fill_na) if fill_na is not None else 0.0, fill=int(fill_na is not None),
                         half_width=vt["half_width"], full=vt["full"], log_thr=vt["log_thr"])
     for name, arr in (("thresholds", thresholds), ("beta", beta), ("beta_cum", beta_cum), ("pmf", pmf)):
-        setattr(desc, "d_" + name, _f64_constant(ctx, okey + (name,), arr))
+        setattr(desc, "d_" + name, pl.f64_constant(ctx, okey + (name,), arr))
     for name in ("cls", "ltab"):
-        setattr(desc, "d_" + name, _f64_constant(ctx, vkey + (name,), vt[name]))
+        setattr(desc, "d_" + name, pl.f64_constant(ctx, vkey + (name,), vt[name]))
     freqs = fmin * 2 ** (np.arange(n_pitch_bins) / (12 * n_bins_per_semitone))
-    desc.d_freqs = _f64_constant(ctx, vkey + ("freqs", float(fmin), n_bins_per_semitone), freqs)
+    desc.d_freqs = pl.f64_constant(ctx, vkey + ("freqs", float(fmin), n_bins_per_semitone), freqs)
     return ctx, desc, max_cand
 
 

@@ -12,10 +12,7 @@
 
 using namespace b2l;
 
-namespace {
-
-// exp(-2*pi*i*j/n), j < count, octant-reduced in long double
-std::vector<double2> twiddles(int n, int count) {
+std::vector<double2> b2l::f64_twiddles(int n, int count) {
   std::vector<double2> tw((size_t)count);
   const long double two_pi = 6.283185307179586476925286766559005768L;
   for (int j = 0; j < count; ++j) {
@@ -24,6 +21,8 @@ std::vector<double2> twiddles(int n, int count) {
   }
   return tw;
 }
+
+namespace {
 
 const int kMaxFft64 = 1 << 20;   // power-of-two n_fft (work area in shared memory up to 16384, else in global memory)
 const int kMaxDft64 = 1 << 16;   // any other n_fft: direct O(n_fft^2) DFT
@@ -46,7 +45,7 @@ extern "C" int b2l_stft_f64(b2l_ctx* c, const double* d_y, int64_t n_clips, int6
   const int l2 = ilog2_exact(n_fft);
   const bool fft = l2 >= 2 && n_fft <= kMaxFft64;
   if (!fft && n_fft > kMaxDft64) return fail(B2L_ERR_UNSUPPORTED, "float64 stft: n_fft=%d (direct DFT path is limited to %d)", n_fft, kMaxDft64);
-  std::vector<double2> tw = twiddles(n_fft, fft ? n_fft / 2 + 1 : n_fft);
+  std::vector<double2> tw = f64_twiddles(n_fft, fft ? n_fft / 2 + 1 : n_fft);
   Temp d_tw(st), d_win(st), d_z(st);
   CUDA_TRY(upload(d_tw, tw.data(), tw.size()));
   CUDA_TRY(upload(d_win, h_window, (size_t)n_fft));
@@ -92,7 +91,7 @@ extern "C" int b2l_istft_f64(b2l_ctx* c, const void* d_D, int64_t n_clips, int64
   const bool fft = l2 >= 2 && n_fft <= kMaxFft64;
   if (!fft && n_fft > kMaxDft64) return fail(B2L_ERR_UNSUPPORTED, "float64 istft: n_fft=%d (direct DFT path is limited to %d)", n_fft, kMaxDft64);
   const int F = n_fft / 2 + 1;
-  std::vector<double2> tw = twiddles(n_fft, fft ? n_fft / 2 + 1 : n_fft);
+  std::vector<double2> tw = f64_twiddles(n_fft, fft ? n_fft / 2 + 1 : n_fft);
   Temp d_tw(st), d_win(st), d_wss(st), d_frames(st), d_z(st);
   CUDA_TRY(upload(d_tw, tw.data(), tw.size()));
   CUDA_TRY(upload(d_win, h_window, (size_t)n_fft));

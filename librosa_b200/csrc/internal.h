@@ -1,5 +1,5 @@
 // internal.h — host-side state and helpers shared by the C ABI units (runtime.cu, plan.cu, api.cu, f64_api.cu,
-// inverse_api.cu) and the per-size kernel instantiations (fwd_inst.cu, inv_inst.cu, czt_inst.cu).
+// inverse_api.cu, rhythm_api.cu) and the per-size kernel instantiations (fwd_inst.cu, inv_inst.cu, czt_inst.cu).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -191,6 +191,9 @@ cudaError_t upload(Temp& t, const T* h, size_t count) {
   if (e != cudaSuccess) return e;
   return cudaMemcpyAsync(t.p, h, count * sizeof(T), cudaMemcpyHostToDevice, t.st);   // pageable source: returns after the copy is staged
 }
+
+// exp(-2*pi*i*j/n) for j < count, in long double rounded to double (the FP64 transforms' twiddles; f64_api.cu)
+std::vector<double2> f64_twiddles(int n, int count);
 
 // Grows the context's per-clip maximum scratch to at least n_clips entries.
 int ensure_clip_max(b2l_ctx* c, size_t n_clips);

@@ -1,11 +1,15 @@
 """Device-resident timings of the frame-wise features (SURVEY 8f rank 2) on a cfg-2 shaped batch, next to the
 oracle (CPU, one process) on a small sample.  CUDA events around `reps` calls after warm-up.  The pitch trackers
 run with fmin C2, fmax C7 and their other defaults (frame_length 2048, hop 512); their oracle sample is one clip.
+The rhythm features take the device onset envelope of the batch (431 frames per 10 s clip) and their defaults;
+``rhythm_bounds`` holds the tempogram kernel's least time on the card (output bytes at 3.35 TB/s, two packed FP64
+transforms per frame at 34 TFLOP/s), and ``card`` the GPU's name and power limit read in the same run.
 
     python tools/feature_timing.py [clips=1024] [reps=10] > gpurun_out/feature_timing.json
 """
 import json
 import os
+import subprocess
 import sys
 import time
 import warnings
@@ -18,6 +22,7 @@ import numpy as np
 import bench
 import librosa_b200 as lb
 import pitch_oracle as PO
+import rhythm_oracle as RO
 from oracle import ref_np as O
 
 clips = int(sys.argv[1]) if len(sys.argv) > 1 else 1024
@@ -32,6 +37,9 @@ frames = clips * T
 mel_db = lb.power_to_db(lb.feature.melspectrogram(y=dev, sr=sr))
 mel_pw = lb.feature.melspectrogram(y=dev, sr=sr)
 dev128 = ctx.to_device(host[:128])
+oenv = lb.onset.onset_strength(y=dev, sr=sr)
+oenv_host = oenv.get().copy()
+tg_dev = lb.feature.tempogram(onset_envelope=oenv)
 
 
 C2, C7 = 65.40639132514966, 2093.004522404789
@@ -59,9 +67,36 @@ FEATURES = {
     "amplitude_to_db(mel)": (lambda: lb.amplitude_to_db(mel_pw), None),
     "yin(C2-C7)": (lambda: lb.yin(dev, fmin=C2, fmax=C7, sr=sr), lambda y: PO.yin(y, fmin=C2, fmax=C7, sr=sr)),
     "pyin(C2-C7)": (lambda: lb.pyin(dev, fmin=C2, fmax=C7, sr=sr), lambda y: PO.pyin(y, fmin=C2, fmax=C7, sr=sr)),
+    "tempogram(onset_envelope)": (lambda: lb.feature.tempogram(onset_envelope=oenv),
+                                  lambda y: RO.tempogram(onset_envelope=oenv_host[:len(y)])),
+    "fourier_tempogram(onset_envelope)": (lambda: lb.feature.fourier_tempogram(onset_envelope=oenv),
+                                          lambda y: RO.fourier_tempogram(onset_envelope=oenv_host[:len(y)])),
+    "tempo(onset_envelope)": (lambda: lb.feature.tempo(onset_envelope=oenv),
+                              lambda y: RO.tempo(onset_envelope=oenv_host[:len(y)])),
+    "tempo(tg, aggregate=None)": (lambda: lb.feature.tempo(tg=tg_dev, aggregate=None), None),
 }
 CPU_SAMPLE = {"yin(C2-C7)": 1, "pyin(C2-C7)": 1}   # clips in the oracle sample (default 8)
-out = {"clips": clips, "frames": frames, "reps": reps, "features": {}}
+
+
+def rhythm_bounds(rows, n_frames, win=384):
+    """Least time of the tempogram kernel on an H100 SXM from the data sheet: float64 output bytes at 3.35 TB/s,
+    and 2 packed real transforms of N = 2^ceil(log2(2 win - 1)) points per frame (5 (N/2) log2(N/2) flops each,
+    plus the un-mix) at 34 TFLOP/s FP64."""
+    N = 1 << int(np.ceil(np.log2(2 * win - 1)))
+    M = N // 2
+    flops = rows * n_frames * 2 * (5 * M * np.log2(M) + 10 * M)
+    nbytes = rows * n_frames * win * 8
+    return {"bytes": nbytes, "flop": flops, "bytes_ms": nbytes / 3.35e12 * 1e3, "flop_ms": flops / 34e12 * 1e3}
+
+
+def card():
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                       capture_output=True, text=True)
+    return q.stdout.strip().splitlines()[lb.default_context().device] if q.returncode == 0 else "unknown"
+
+
+out = {"clips": clips, "frames": frames, "reps": reps, "card": card(),
+       "rhythm_bounds": rhythm_bounds(clips, oenv.shape[-1]), "features": {}}
 with warnings.catch_warnings():
     warnings.simplefilter("ignore")
     for name, (gpu, cpu) in FEATURES.items():

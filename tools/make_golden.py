@@ -1,7 +1,8 @@
 """Generate tests/golden/hotpath_v1.npz (tests/cases.py), tests/golden/features_v1.npz
 (tests/feature_cases.py) and tests/golden/reference_pins_v1.npz (tests/reference_pins.py) by running the
 cases through the UNMODIFIED reference; ``--pitch`` writes only tests/golden/pitch_v1.npz (tests/pitch_cases.py)
-and leaves the other fixtures as they are.
+and leaves the other fixtures as they are; ``--rhythm`` likewise writes only tests/golden/rhythm_v1.npz
+(tests/rhythm_cases.py).
 
 Needs a checkout of the reference (see tools/ref_shim.py); the tests only read the stored fixtures.  Also
 stores a handful of constant tables (mel bases, window sum-square, mel-scale known answers) produced by the
@@ -9,6 +10,7 @@ reference.
 
     python tools/make_golden.py
     python tools/make_golden.py --pitch
+    python tools/make_golden.py --rhythm
 """
 from __future__ import annotations
 
@@ -120,8 +122,27 @@ def write_pitch():
     print("wrote", path, os.path.getsize(path), "bytes")
 
 
+def write_rhythm():
+    """tests/golden/rhythm_v1.npz: tempogram / fourier_tempogram / tempo of every case of tests/rhythm_cases.py."""
+    from rhythm_cases import RHYTHM_CASES, outputs, run
+
+    ref = ref_shim.load_reference()
+    store = {}
+    for case in RHYTHM_CASES:
+        with warnings.catch_warnings():
+            warnings.simplefilter("ignore")
+            for key, arr in outputs(case, run(ref, case)).items():
+                store[key] = np.ascontiguousarray(arr)
+                print(f"{key:48s} {arr.shape} {arr.dtype}")
+    path = os.path.join(ROOT, "tests", "golden", "rhythm_v1.npz")
+    np.savez_compressed(path, **store)
+    print("wrote", path, os.path.getsize(path), "bytes")
+
+
 if __name__ == "__main__":
     if "--pitch" in sys.argv[1:]:
         write_pitch()
+    elif "--rhythm" in sys.argv[1:]:
+        write_rhythm()
     else:
         main()
