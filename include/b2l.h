@@ -82,13 +82,16 @@ int b2l_ctx_launch_count(const b2l_ctx* ctx, uint64_t* launches);
 
 /* ---- util.valid_audio on the device (librosa/util/utils.py:246-308) ----------------------------
  * The forward kernels set bit 0 of a per-context status word when a non-finite sample reaches a frame;
- * b2l_scan_finite covers samples [begin, n) that no frame reads (tail / hop > n_fft gaps).  The Python
- * layer resets the word before a call on host data, reads it with the results and raises
- * ParameterError("Audio buffer is not finite everywhere") exactly as the reference does. */
+ * b2l_scan_finite covers samples [begin, n) that no frame reads (tail / hop > n_fft gaps);
+ * b2l_scan_finite_f64 does the same for the float64 signals of the FP64 path and flags exactly the samples
+ * np.isfinite rejects.  The Python layer resets the word before a call on host data, reads it with the
+ * results and raises ParameterError("Audio buffer is not finite everywhere") exactly as the reference does. */
 int b2l_status_reset(b2l_ctx* ctx);
 int b2l_status_read(b2l_ctx* ctx, int* status); /* synchronises the ctx stream */
 int b2l_scan_finite(b2l_ctx* ctx, const float* d_y, int64_t n_clips, int64_t n, int64_t y_stride,
                     int64_t begin);
+int b2l_scan_finite_f64(b2l_ctx* ctx, const double* d_y, int64_t n_clips, int64_t n, int64_t y_stride,
+                        int64_t begin);
 
 /* ---- memory --------------------------------------------------------------------------------- */
 int b2l_alloc(b2l_ctx* ctx, size_t bytes, void** d_ptr);

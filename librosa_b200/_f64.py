@@ -43,12 +43,13 @@ def stft(y, *, n_fft, hop_length, center, mode, win: np.ndarray):
     require_supported(n_fft)
     staged = pl.StagedInput(y, np.float64)
     ctx, n = staged.ctx, staged.n
-    D = nat.DeviceArray.empty(ctx, staged.lead + (1 + n_fft // 2, pl.frame_count(n, n_fft, hop_length, center)),
-                              np.complex128, layout="ft")
+    n_frames = pl.frame_count(n, n_fft, hop_length, center)
+    D = nat.DeviceArray.empty(ctx, staged.lead + (1 + n_fft // 2, n_frames), np.complex128, layout="ft")
     w = np.ascontiguousarray(win, dtype=np.float64)
     nat.check(nat.lib().b2l_stft_f64(ctx.handle, _vp(staged.dev.ptr), staged.n_clips, n, n, int(n_fft),
                                      int(hop_length), 1 if center else 0, nat.PAD_MODES[mode], w.ctypes.data_as(_dp),
                                      _vp(D.ptr)))
+    staged.scan_uncovered(n_fft, hop_length, None, center, n_frames)   # samples no frame reads (host signals only)
     staged.release()
     return staged, D
 

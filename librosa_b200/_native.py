@@ -166,6 +166,7 @@ def _declare(lib):
         "b2l_status_reset": (C.c_int, [_vp]),
         "b2l_status_read": (C.c_int, [_vp, P(C.c_int)]),
         "b2l_scan_finite": (C.c_int, [_vp, _vp, _i64, _i64, _i64, _i64]),
+        "b2l_scan_finite_f64": (C.c_int, [_vp, _vp, _i64, _i64, _i64, _i64]),
         "b2l_alloc": (C.c_int, [_vp, C.c_size_t, P(_vp)]),
         "b2l_free": (C.c_int, [_vp, _vp]),
         "b2l_memset": (C.c_int, [_vp, _vp, C.c_int, C.c_size_t]),

@@ -330,8 +330,8 @@ class StagedInput:
 
     def _scan(self, begin: int):
         if not self.on_device and self.n_clips and begin < self.n:
-            nat.check(nat.lib().b2l_scan_finite(self.ctx.handle, C.c_void_p(self.dev.ptr), self.n_clips, self.n,
-                                                self.n, begin))
+            scan = nat.lib().b2l_scan_finite_f64 if self.dev.dtype == np.float64 else nat.lib().b2l_scan_finite
+            nat.check(scan(self.ctx.handle, C.c_void_p(self.dev.ptr), self.n_clips, self.n, self.n, begin))
 
     def scan_uncovered(self, n_fft: int, hop_length, win_length, center: bool, n_frames: int):
         """Scan the samples that no STFT frame reads (the tail after the last frame, or everything when the hop

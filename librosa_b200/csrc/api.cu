@@ -372,8 +372,9 @@ extern "C" int b2l_spectrogram(b2l_ctx* c, const b2l_plan* p, const float* d_y, 
 }
 
 // ------------------------------------------------------------------ device-side input validation
-extern "C" int b2l_scan_finite(b2l_ctx* c, const float* d_y, int64_t n_clips, int64_t n, int64_t y_stride,
-                               int64_t begin) {
+template <typename T, typename Kernel>
+static int scan_finite(b2l_ctx* c, Kernel kernel, const T* d_y, int64_t n_clips, int64_t n, int64_t y_stride,
+                       int64_t begin) {
   if (!c || !d_y) return fail(B2L_ERR_INVALID, "NULL argument");
   if (n_clips <= 0 || begin >= n) return B2L_OK;
   if (n > 0x7fffffffLL) return fail(B2L_ERR_UNSUPPORTED, "scan_finite: clips longer than 2^31-1 samples");
@@ -381,11 +382,18 @@ extern "C" int b2l_scan_finite(b2l_ctx* c, const float* d_y, int64_t n_clips, in
   long long bx = ((n - begin) + 1023) / 1024;
   if (bx > 64) bx = 64;
   dim3 grid((unsigned)bx, (unsigned)(n_clips > 65535 ? 65535 : n_clips));
-  finite_scan_kernel<<<grid, 256, 0, c->stream>>>(d_y, y_stride, (int)n, (int)(begin < 0 ? 0 : begin), n_clips,
-                                                  c->d_status);
+  kernel<<<grid, 256, 0, c->stream>>>(d_y, y_stride, (int)n, (int)(begin < 0 ? 0 : begin), n_clips, c->d_status);
   CUDA_TRY(cudaGetLastError());
   c->launches++;
   return B2L_OK;
+}
+extern "C" int b2l_scan_finite(b2l_ctx* c, const float* d_y, int64_t n_clips, int64_t n, int64_t y_stride,
+                               int64_t begin) {
+  return scan_finite(c, finite_scan_kernel, d_y, n_clips, n, y_stride, begin);
+}
+extern "C" int b2l_scan_finite_f64(b2l_ctx* c, const double* d_y, int64_t n_clips, int64_t n, int64_t y_stride,
+                                   int64_t begin) {
+  return scan_finite(c, finite_scan64_kernel, d_y, n_clips, n, y_stride, begin);
 }
 // ------------------------------------------------------------------ frame-wise spectral statistics / framings
 static int check_stats_desc(const b2l_stats_desc* d, StatsParams* sp) {

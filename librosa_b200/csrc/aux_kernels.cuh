@@ -329,6 +329,18 @@ __global__ void finite_scan_kernel(const float* __restrict__ y, long long stride
   }
   if (bad) *status = 1;
 }
+// The same scan over float64 signals (the FP64 path): flags exactly what np.isfinite rejects.
+__global__ void finite_scan64_kernel(const double* __restrict__ y, long long stride, int n, int begin,
+                                     long long n_clips, int* status) {
+  bool bad = false;
+  for (long long clip = blockIdx.y; clip < n_clips; clip += gridDim.y) {
+    const double* yc = y + clip * stride;
+    for (long long i = begin + (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n;
+         i += (long long)gridDim.x * blockDim.x)
+      bad |= !isfinite(yc[i]);
+  }
+  if (bad) *status = 1;
+}
 
 // ------------------------------------------------------------------ Griffin-Lim phase update
 // angles <- rebuilt - scale * tprev ;  angles <- angles / (|angles| + eps) * S      (elementwise)

@@ -5,6 +5,7 @@
 #include <stdint.h>
 #include <string.h>
 
+#include <algorithm>
 #include <vector>
 
 #include "f64_kernels.cuh"
@@ -26,6 +27,7 @@ namespace {
 
 const int kMaxFft64 = 1 << 20;   // power-of-two n_fft (work area in shared memory up to 16384, else in global memory)
 const int kMaxDft64 = 1 << 16;   // any other n_fft: direct O(n_fft^2) DFT
+const int64_t kMaxGridY = 65535; // kernels that carry the clip index in grid.y run in slices of this many clips
 
 }  // namespace
 
@@ -83,7 +85,7 @@ extern "C" int b2l_istft_f64(b2l_ctx* c, const void* d_D, int64_t n_clips, int64
     return fail(B2L_ERR_INVALID, "bad istft geometry");
   if (n_clips == 0 || out_len == 0) return B2L_OK;
   if (!d_D || !d_y) return fail(B2L_ERR_INVALID, "NULL device pointer");
-  if (n_clips * n_frames_used > 0x7fffffffLL || out_len > 0x7fffffffLL || n_clips > 65535)
+  if (n_clips * n_frames_used > 0x7fffffffLL || out_len > 0x7fffffffLL)
     return fail(B2L_ERR_UNSUPPORTED, "float64 istft: batch too large for one call");
   DeviceGuard g(c->device);
   cudaStream_t st = c->stream;
@@ -122,13 +124,20 @@ extern "C" int b2l_istft_f64(b2l_ctx* c, const void* d_D, int64_t n_clips, int64
   }
   int rc = blocks_per_sm(c, istft64_frames_kernel, 256, smem, nullptr);
   if (rc || (rc = launch(c, istft64_frames_kernel, (unsigned)(n_clips * n_frames_used), 256, smem, a))) return rc;
-  long long bx = (out_len + 255) / 256;
-  const long long cap = (8LL * c->sm_count + n_clips - 1) / n_clips;
-  if (bx > cap) bx = cap;
-  if (bx < 1) bx = 1;
-  ola64_kernel<<<dim3((unsigned)bx, (unsigned)n_clips), 256, 0, st>>>(a);
-  CUDA_TRY(cudaGetLastError());
-  c->launches++;
+  // the overlap-add carries the clip index in grid.y (at most 65535): larger batches go in slices
+  for (int64_t c0 = 0; c0 < n_clips; c0 += kMaxGridY) {
+    const int64_t m = std::min<int64_t>(kMaxGridY, n_clips - c0);
+    F64InvArgs s = a;
+    s.frames += c0 * n_frames_used * n_fft;
+    s.y += c0 * y_stride;
+    long long bx = (out_len + 255) / 256;
+    const long long cap = (8LL * c->sm_count + m - 1) / m;
+    if (bx > cap) bx = cap;
+    if (bx < 1) bx = 1;
+    ola64_kernel<<<dim3((unsigned)bx, (unsigned)m), 256, 0, st>>>(s);
+    CUDA_TRY(cudaGetLastError());
+    c->launches++;
+  }
   return B2L_OK;
 }
 
@@ -189,24 +198,29 @@ extern "C" int b2l_f64_db(b2l_ctx* c, const double* d_in, int64_t n_clips, int64
   if (!c || !d_in || !d_out) return fail(B2L_ERR_INVALID, "NULL argument");
   if (!(amin > 0.0)) return fail(B2L_ERR_INVALID, "amin must be strictly positive");
   if (n_clips <= 0 || per_clip <= 0) return B2L_OK;
-  if (n_clips > 65535) return fail(B2L_ERR_UNSUPPORTED, "float64 power_to_db: more than 65535 leading indices");
   DeviceGuard g(c->device);
   cudaStream_t st = c->stream;
-  Temp d_max(st);
+  Temp d_max(st);   // one maximum per clip of the whole batch
   CUDA_TRY(d_max.alloc((size_t)n_clips * sizeof(unsigned long long)));
   CUDA_TRY(cudaMemsetAsync(d_max.p, 0, (size_t)n_clips * sizeof(unsigned long long), st));
-  long long bx = (per_clip + 255) / 256;
-  const long long cap = (8LL * c->sm_count + n_clips - 1) / n_clips;
-  if (bx > cap) bx = cap;
-  if (bx < 1) bx = 1;
+  unsigned long long* clip_max = (unsigned long long*)d_max.p;
   const double db_sub = 10.0 * log10(fmax(amin, fabs(ref_value)));
-  db64_kernel<<<dim3((unsigned)bx, (unsigned)n_clips), 256, 0, st>>>(d_in, per_clip, amin, db_sub, d_out, (unsigned long long*)d_max.p);
-  CUDA_TRY(cudaGetLastError());
-  c->launches++;
-  if (top_db >= 0.0) {
-    db64_clamp_kernel<<<dim3((unsigned)bx, (unsigned)n_clips), 256, 0, st>>>(d_out, per_clip, top_db, (const unsigned long long*)d_max.p);
+  // the clip index rides in grid.y (at most 65535): larger batches go in slices
+  for (int64_t c0 = 0; c0 < n_clips; c0 += kMaxGridY) {
+    const int64_t m = std::min<int64_t>(kMaxGridY, n_clips - c0);
+    long long bx = (per_clip + 255) / 256;
+    const long long cap = (8LL * c->sm_count + m - 1) / m;
+    if (bx > cap) bx = cap;
+    if (bx < 1) bx = 1;
+    const dim3 grid((unsigned)bx, (unsigned)m);
+    db64_kernel<<<grid, 256, 0, st>>>(d_in + c0 * per_clip, per_clip, amin, db_sub, d_out + c0 * per_clip, clip_max + c0);
     CUDA_TRY(cudaGetLastError());
     c->launches++;
+    if (top_db >= 0.0) {
+      db64_clamp_kernel<<<grid, 256, 0, st>>>(d_out + c0 * per_clip, per_clip, top_db, clip_max + c0);
+      CUDA_TRY(cudaGetLastError());
+      c->launches++;
+    }
   }
   return B2L_OK;
 }
@@ -215,7 +229,6 @@ extern "C" int b2l_f64_dct(b2l_ctx* c, const double* d_L, int64_t n_clips, int32
                            const double* h_dct, int32_t n_mfcc, double* d_out) {
   if (!c || !d_L || !h_dct || !d_out) return fail(B2L_ERR_INVALID, "NULL argument");
   if (n_clips <= 0 || n_frames <= 0 || n_mfcc <= 0) return B2L_OK;
-  if (n_clips > 65535) return fail(B2L_ERR_UNSUPPORTED, "float64 dct: more than 65535 leading indices");
   DeviceGuard g(c->device);
   cudaStream_t st = c->stream;
   const size_t smem = (size_t)n_mfcc * n_mels * sizeof(double);
@@ -226,6 +239,11 @@ extern "C" int b2l_f64_dct(b2l_ctx* c, const double* d_L, int64_t n_clips, int32
   if (rc) return rc;
   long long bx = (n_frames + 127) / 128;
   if (bx < 1) bx = 1;
-  return launch(c, dct64_kernel, dim3((unsigned)bx, (unsigned)n_clips), 128, smem, d_L, (const double*)d_dct.p, n_mels,
-                n_mfcc, (int)n_frames, d_out);
+  // the clip index rides in grid.y (at most 65535): larger batches go in slices
+  for (int64_t c0 = 0; c0 < n_clips && !rc; c0 += kMaxGridY) {
+    const int64_t m = std::min<int64_t>(kMaxGridY, n_clips - c0);
+    rc = launch(c, dct64_kernel, dim3((unsigned)bx, (unsigned)m), 128, smem, d_L + c0 * n_mels * n_frames,
+                (const double*)d_dct.p, n_mels, n_mfcc, (int)n_frames, d_out + c0 * n_mfcc * n_frames);
+  }
+  return rc;
 }

@@ -59,7 +59,9 @@ struct F64FwdArgs {
                             // (n_fft/2 double2 per frame for the FFT, n_fft doubles for the DFT); NULL: shared memory
 };
 
-// One CTA per (frame, clip): windowed frame -> complex spectrum.
+// One CTA per (frame, clip): windowed frame -> complex spectrum.  A sample np.isfinite rejects sets the status word
+// (tested before the window product, so a zero window tap does not hide it); samples no frame reads are left to
+// finite_scan64_kernel.
 __global__ void stft64_kernel(const F64FwdArgs a) {
   extern __shared__ __align__(16) unsigned char smem64[];
   const long long item = blockIdx.x;
@@ -73,10 +75,10 @@ __global__ void stft64_kernel(const F64FwdArgs a) {
     const int M = N / 2;
     double2* z = a.zscratch ? a.zscratch + item * M : reinterpret_cast<double2*>(smem64);
     for (int e = threadIdx.x; e < M; e += blockDim.x) {
-      const double x0 = load_padded64(yc, a.n, s0 + 2 * e, a.pad_mode, a.pad) * a.window[2 * e];
-      const double x1 = load_padded64(yc, a.n, s0 + 2 * e + 1, a.pad_mode, a.pad) * a.window[2 * e + 1];
-      bad |= !(fabs(x0) <= 1.0e300) || !(fabs(x1) <= 1.0e300);
-      z[bitrev_rt(e, a.log2m)] = make_double2(x0, x1);
+      const double v0 = load_padded64(yc, a.n, s0 + 2 * e, a.pad_mode, a.pad);
+      const double v1 = load_padded64(yc, a.n, s0 + 2 * e + 1, a.pad_mode, a.pad);
+      bad |= !isfinite(v0) || !isfinite(v1);
+      z[bitrev_rt(e, a.log2m)] = make_double2(v0 * a.window[2 * e], v1 * a.window[2 * e + 1]);
     }
     __syncthreads();
     fft64_inplace(z, a.log2m, a.tw);
@@ -91,9 +93,9 @@ __global__ void stft64_kernel(const F64FwdArgs a) {
   } else {
     double* xw = a.zscratch ? reinterpret_cast<double*>(a.zscratch) + item * N : reinterpret_cast<double*>(smem64);
     for (int i = threadIdx.x; i < N; i += blockDim.x) {
-      const double x = load_padded64(yc, a.n, s0 + i, a.pad_mode, a.pad) * a.window[i];
-      bad |= !(fabs(x) <= 1.0e300);
-      xw[i] = x;
+      const double v = load_padded64(yc, a.n, s0 + i, a.pad_mode, a.pad);
+      bad |= !isfinite(v);
+      xw[i] = v * a.window[i];
     }
     __syncthreads();
     for (int k = threadIdx.x; k < F; k += blockDim.x) {
