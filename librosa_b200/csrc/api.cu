@@ -209,12 +209,9 @@ static int run_forward(b2l_ctx* c, const b2l_plan* p, int mode, int log_mode, co
   const FwdKernel fn = fwd_kernel_for(p->log2m, variant, mode);
   if (!fn) return fail(B2L_ERR_CUDA, "no forward kernel variant %d for n_fft=%d", variant, N);
   const int threads = variant_threads(variant);
-  int occ = 0;
-  if ((rc = blocks_per_sm(c, fn, threads, smem, &occ))) return rc;
-  if (occ < 1) return fail(B2L_ERR_CUDA, "forward kernel does not fit on an SM (smem %zu)", smem);
-  long long grid = (long long)c->sm_count * occ;
-  const long long ctas_needed = (a.total_tiles + halves - 1) / halves;
-  if (grid > ctas_needed) grid = ctas_needed;
+  long long grid = 0;
+  if ((rc = resident_grid(c, fn, threads, smem, (a.total_tiles + halves - 1) / halves, &grid))) return rc;
+  if (!grid) return fail(B2L_ERR_CUDA, "forward kernel does not fit on an SM (smem %zu)", smem);
   return launch(c, fn, (unsigned)grid, threads, smem, a);
 }
 
@@ -261,13 +258,11 @@ static int run_czt(b2l_ctx* c, const b2l_plan* p, int mode, const float* d_y, in
   const CztKernel fn = czt_kernel_for(p->log2p);
   // the table part of the shared memory depends on n_fft, not only on P: size the grid for the largest case (the
   // kernels run one block per SM anyway)
-  int occ = 0;
-  if ((rc = blocks_per_sm(c, fn, nw * 32, c->smem_optin / 2 + 1, &occ))) return rc;
-  if (smem > c->smem_optin) return fail(B2L_ERR_UNSUPPORTED, "n_fft=%d needs more shared memory than one SM has", p->n_fft);
-  if (occ < 1) return fail(B2L_ERR_CUDA, "chirp-z kernel does not fit on an SM (smem %zu)", smem);
   const long long steps = ((long long)n_clips * ((T + 1) / 2) + G - 1) / G;   // frames go in pairs inside a clip
-  long long grid = (long long)c->sm_count * occ;
-  if (grid > steps) grid = steps;
+  long long grid = 0;
+  if ((rc = resident_grid(c, fn, nw * 32, c->smem_optin / 2 + 1, steps, &grid))) return rc;
+  if (smem > c->smem_optin) return fail(B2L_ERR_UNSUPPORTED, "n_fft=%d needs more shared memory than one SM has", p->n_fft);
+  if (!grid) return fail(B2L_ERR_CUDA, "chirp-z kernel does not fit on an SM (smem %zu)", smem);
   return launch(c, fn, (unsigned)grid, nw * 32, smem, a);
 }
 
@@ -342,13 +337,11 @@ static int run_mr(b2l_ctx* c, const b2l_plan* p, int mode, int log_mode, const f
   if ((rc = mr_block(c, p, a.n_mels, a.mel_w_count, fpw, &nw, &smem))) return rc;
   auto kern = fpw == 2 ? (mode == 0 ? mr_kernel<0, 16> : (mode == 1 ? mr_kernel<1, 16> : mr_kernel<2, 16>))
                        : (mode == 0 ? mr_kernel<0, 32> : (mode == 1 ? mr_kernel<1, 32> : mr_kernel<2, 32>));
-  int occ = 0;
-  if ((rc = blocks_per_sm(c, kern, nw * 32, smem, &occ))) return rc;
-  if (occ < 1) return fail(B2L_ERR_CUDA, "mixed-radix kernel does not fit on an SM (smem %zu)", smem);
   const long long total = (long long)n_clips * T;
-  long long grid = (long long)c->sm_count * occ;
-  const long long need = (total + (long long)nw * fpw - 1) / ((long long)nw * fpw);
-  if (grid > need) grid = need;
+  long long grid = 0;
+  if ((rc = resident_grid(c, kern, nw * 32, smem, (total + (long long)nw * fpw - 1) / ((long long)nw * fpw), &grid)))
+    return rc;
+  if (!grid) return fail(B2L_ERR_CUDA, "mixed-radix kernel does not fit on an SM (smem %zu)", smem);
   return launch(c, kern, (unsigned)grid, nw * 32, smem, a);
 }
 
@@ -381,11 +374,8 @@ static int scan_finite(b2l_ctx* c, Kernel kernel, const T* d_y, int64_t n_clips,
   DeviceGuard g(c->device);
   long long bx = ((n - begin) + 1023) / 1024;
   if (bx > 64) bx = 64;
-  dim3 grid((unsigned)bx, (unsigned)(n_clips > 65535 ? 65535 : n_clips));
-  kernel<<<grid, 256, 0, c->stream>>>(d_y, y_stride, (int)n, (int)(begin < 0 ? 0 : begin), n_clips, c->d_status);
-  CUDA_TRY(cudaGetLastError());
-  c->launches++;
-  return B2L_OK;
+  const dim3 grid((unsigned)bx, (unsigned)std::min(n_clips, kMaxGridY));
+  return launch(c, kernel, grid, 256, 0, d_y, y_stride, (int)n, (int)(begin < 0 ? 0 : begin), n_clips, c->d_status);
 }
 extern "C" int b2l_scan_finite(b2l_ctx* c, const float* d_y, int64_t n_clips, int64_t n, int64_t y_stride,
                                int64_t begin) {
@@ -431,9 +421,7 @@ extern "C" int b2l_spectral_stats_from_spec(b2l_ctx* c, const b2l_stats_desc* d,
   rc = blocks_per_sm(c, stats_kernel, nw * 32, smem, nullptr);
   if (rc) return rc;
   const long long rows = (long long)n_clips * n_frames;
-  long long grid = (rows + nw - 1) / nw;
-  const long long cap = (long long)c->sm_count * 8;
-  if (grid > cap) grid = cap;
+  const long long grid = grid_stride_blocks(rows, nw, 8LL * c->sm_count);
   return launch(c, stats_kernel, (unsigned)grid, nw * 32, smem, d_S, rows, (int)n_frames, n_bins, d_freq, sc.sp, d_out,
                 c->d_status);
 }
@@ -474,27 +462,18 @@ extern "C" int b2l_frame_feature(b2l_ctx* c, int32_t what, const float* d_y, int
   // frame_length a multiple of hop_length: block form, every sample read once (feat_kernels.cuh)
   {
     const long long tiles = (T + TD_FRAMES - 1) / TD_FRAMES;
-    if (frame_length % hop_length == 0 && frame_length / hop_length <= 64 && n_clips <= 65535 && tiles <= 0x7fffffffLL) {
+    if (frame_length % hop_length == 0 && frame_length / hop_length <= 64 && n_clips <= kMaxGridY && tiles <= 0x7fffffffLL) {
       const int R = frame_length / hop_length;
       const size_t smem = (size_t)(TD_FRAMES + R - 1) * 8;
-      frame_td_block_kernel<<<dim3((unsigned)tiles, (unsigned)n_clips), 256, smem, c->stream>>>(
-          d_y, y_stride, (int)n, frame_length, hop_length, pad, pad_mode, (int)T, what, threshold, zero_pos, pad_first,
-          out_scale, d_out, c->d_status);
-      CUDA_TRY(cudaGetLastError());
-      c->launches++;
-      return B2L_OK;
+      return launch(c, frame_td_block_kernel, dim3((unsigned)tiles, (unsigned)n_clips), 256, smem, d_y, y_stride, (int)n,
+                    frame_length, hop_length, pad, pad_mode, (int)T, what, threshold, zero_pos, pad_first, out_scale, d_out,
+                    c->d_status);
     }
   }
   const long long rows = (long long)n_clips * T;
-  long long grid = (rows + 7) / 8;
-  const long long cap = (long long)c->sm_count * 8;
-  if (grid > cap) grid = cap;
-  frame_td_kernel<<<(int)grid, 256, 0, c->stream>>>(d_y, y_stride, (int)n, n_clips, frame_length, hop_length, pad,
-                                                    pad_mode, (int)T, what, threshold, zero_pos, pad_first, out_scale,
-                                                    d_out,                                                    c->d_status);
-  CUDA_TRY(cudaGetLastError());
-  c->launches++;
-  return B2L_OK;
+  const long long grid = grid_stride_blocks(rows, 8, 8LL * c->sm_count);
+  return launch(c, frame_td_kernel, (unsigned)grid, 256, 0, d_y, y_stride, (int)n, n_clips, frame_length, hop_length, pad,
+                pad_mode, (int)T, what, threshold, zero_pos, pad_first, out_scale, d_out, c->d_status);
 }
 
 extern "C" int b2l_melspectrogram(b2l_ctx* c, const b2l_plan* p, const float* d_y, int64_t n_clips, int64_t n,
@@ -518,13 +497,9 @@ static int launch_dct(b2l_ctx* c, const b2l_plan* p, const float* d_L, int64_t n
   if (smem > c->smem_optin) {
     // too many input rows for the shared-memory tile (e.g. mfcc(S=...) of a 1025-bin spectrogram): generic kernel
     if (tiled) return fail(B2L_ERR_UNSUPPORTED, "n_mels=%d is too large for the fused mfcc path", p->n_mels);
-    if (n_clips > 65535) return fail(B2L_ERR_UNSUPPORTED, "dct: more than 65535 leading indices");
-    dct_generic_kernel<<<dim3((unsigned)((T + 127) / 128), (unsigned)n_clips), 128, 0, c->stream>>>(
-        d_L, p->d_dct, clamp ? c->d_clip_max : nullptr, clamp ? p->top_db : -1.0f, p->n_mels, p->n_mfcc, 8 * KG, (int)T,
-        d_out);
-    CUDA_TRY(cudaGetLastError());
-    c->launches++;
-    return B2L_OK;
+    if (n_clips > kMaxGridY) return fail(B2L_ERR_UNSUPPORTED, "dct: more than 65535 leading indices");
+    return launch(c, dct_generic_kernel, dim3((unsigned)((T + 127) / 128), (unsigned)n_clips), 128, 0, d_L, p->d_dct,
+                  clamp ? c->d_clip_max : nullptr, clamp ? p->top_db : -1.0f, p->n_mels, p->n_mfcc, 8 * KG, (int)T, d_out);
   }
   // two warp sets over the mel rows when the partial sums fit in the tile buffer
   const int ks = KG <= 10 && p->n_mels >= 8 * KG ? 2 : 1;   // 640 threads at most; 32*KG*32 partial sums <= 2*n_mels*64 tile words
@@ -532,12 +507,9 @@ static int launch_dct(b2l_ctx* c, const b2l_plan* p, const float* d_L, int64_t n
   const int threads = KG * 32 * ks;
   const int tiles = (int)((T + DCT4_TILE - 1) / DCT4_TILE);
   const long long total = (long long)tiles * n_clips;
-  int occ = 0;
-  const int rc = blocks_per_sm(c, kern, threads, smem, &occ);
-  if (rc) return rc;
-  if (occ < 1) return fail(B2L_ERR_CUDA, "DCT kernel does not fit on an SM");
-  long long grid = (long long)c->sm_count * occ;
-  if (grid > total) grid = total;
+  long long grid = 0;
+  if (int rc = resident_grid(c, kern, threads, smem, total, &grid)) return rc;
+  if (!grid) return fail(B2L_ERR_CUDA, "DCT kernel does not fit on an SM");
   return launch(c, kern, (unsigned)grid, threads, smem, d_L, p->d_dct, clamp ? c->d_clip_max : nullptr,
                 clamp ? p->top_db : -1.0f, p->n_mels, p->n_mfcc, (int)T, tiles, total, tiled, d_out);
 }
@@ -557,19 +529,18 @@ extern "C" int b2l_mfcc(b2l_ctx* c, const b2l_plan* p, const float* d_y, int64_t
   int rc = ensure_clip_max(c, (size_t)n_clips);
   if (rc) return rc;
   CUDA_TRY(cudaMemsetAsync(c->d_clip_max, 0, (size_t)n_clips * sizeof(unsigned int), c->stream));
+  Temp own(c->stream);
   float* scratch = d_logmel;
   // the log-mel scratch is tiled: [clip][ceil(T/64)][n_mels][64] (see dct_clamp4_kernel)
-  if (!scratch) CUDA_TRY(cudaMalloc((void**)&scratch, (size_t)n_clips * p->n_mels * ((T + 63) / 64 * 64) * sizeof(float)));
+  if (!scratch) {
+    CUDA_TRY(own.alloc((size_t)n_clips * p->n_mels * ((T + 63) / 64 * 64) * sizeof(float)));
+    scratch = (float*)own.p;
+  }
   // mixed-radix frames (mr_kernel): the dB rows go to the scratch in the plain [clip][mel][frame] layout
   const int tiled = path == PATH_POW2 ? 1 : 0;
   rc = path == PATH_MR ? run_mr(c, p, 2, 1, d_y, n_clips, n, y_stride, nullptr, scratch)
                        : run_forward(c, p, MODE_MEL, 2, d_y, n_clips, n, y_stride, nullptr, scratch);
-  if (rc == B2L_OK) rc = launch_dct(c, p, scratch, n_clips, T, 1, d_mfcc, tiled);
-  if (!d_logmel) {
-    cudaStreamSynchronize(c->stream);
-    cudaFree(scratch);
-  }
-  return rc;
+  return rc ? rc : launch_dct(c, p, scratch, n_clips, T, 1, d_mfcc, tiled);
 }
 
 // ------------------------------------------------------------------ inverse launches
@@ -685,15 +656,13 @@ static int run_mr_inverse(b2l_ctx* c, const b2l_plan* p, const void* d_D, int64_
   a.tw = p->d_mr_tw;
   a.twn = p->d_mr_twn;
   a.ytmp = c->d_scratch;
-  int nw = 0, occ = 0;
+  int nw = 0;
   size_t smem = 0;
-  int rc = mr_block(c, p, 0, 0, 1, &nw, &smem);
-  if (rc || (rc = blocks_per_sm(c, mr_inv_kernel, nw * 32, smem, &occ))) return rc;
-  if (occ < 1) return fail(B2L_ERR_CUDA, "mixed-radix inverse kernel does not fit on an SM (smem %zu)", smem);
+  long long grid = 0;
   const long long total = (long long)n_clips * n_frames_used;
-  long long grid = (long long)c->sm_count * occ;
-  const long long need_blocks = (total + nw - 1) / nw;
-  if (grid > need_blocks) grid = need_blocks;
+  int rc = mr_block(c, p, 0, 0, 1, &nw, &smem);
+  if (rc || (rc = resident_grid(c, mr_inv_kernel, nw * 32, smem, (total + nw - 1) / nw, &grid))) return rc;
+  if (!grid) return fail(B2L_ERR_CUDA, "mixed-radix inverse kernel does not fit on an SM (smem %zu)", smem);
   return launch(c, mr_inv_kernel, (unsigned)grid, nw * 32, smem, a);
 }
 
@@ -719,13 +688,11 @@ static int run_czt_inverse(b2l_ctx* c, const b2l_plan* p, const void* d_D, int64
   const size_t smem = czt_smem(p, cfg, G, false);
   if (smem > c->smem_optin) return fail(B2L_ERR_UNSUPPORTED, "n_fft=%d needs more shared memory than one SM has", L);
   const CztInvKernel fn = czt_inv_kernel_for(p->log2p);
-  int occ = 0;
-  int rc = blocks_per_sm(c, fn, nw * 32, c->smem_optin / 2 + 1, &occ);   // sized like the forward (run_czt)
-  if (rc) return rc;
-  if (occ < 1) return fail(B2L_ERR_CUDA, "chirp-z inverse kernel does not fit on an SM");
   const long long steps = ((long long)n_clips * ((n_frames_used + 1) / 2) + G - 1) / G;   // frames go in pairs inside a clip
-  long long grid = (long long)c->sm_count * occ;
-  if (grid > steps) grid = steps;
+  long long grid = 0;
+  // sized like the forward (run_czt)
+  if (int rc = resident_grid(c, fn, nw * 32, c->smem_optin / 2 + 1, steps, &grid)) return rc;
+  if (!grid) return fail(B2L_ERR_CUDA, "chirp-z inverse kernel does not fit on an SM");
   return launch(c, fn, (unsigned)grid, nw * 32, smem, a);
 }
 
@@ -742,7 +709,7 @@ extern "C" int b2l_istft(b2l_ctx* c, const b2l_plan* p, const void* d_D, int64_t
   if (path == PATH_POW2)
     return run_inverse(c, p, d_D, n_clips, n_frames_stored, n_frames_used, d_inv_wss, out_len, d_y, y_stride);
   // mixed-radix or chirp-z frames into the scratch array, then a gather overlap-add
-  if (out_len > 0x7fffffffLL || n_clips > 65535) return fail(B2L_ERR_UNSUPPORTED, "istft batch too large");
+  if (out_len > 0x7fffffffLL || n_clips > kMaxGridY) return fail(B2L_ERR_UNSUPPORTED, "istft batch too large");
   DeviceGuard g(c->device);
   const int L = p->n_fft;
   int rc = ensure_scratch(c, (size_t)n_clips * (size_t)n_frames_used * L * sizeof(float));
@@ -750,16 +717,9 @@ extern "C" int b2l_istft(b2l_ctx* c, const b2l_plan* p, const void* d_D, int64_t
     rc = path == PATH_MR ? run_mr_inverse(c, p, d_D, n_clips, n_frames_stored, n_frames_used)
                          : run_czt_inverse(c, p, d_D, n_clips, n_frames_stored, n_frames_used);
   if (rc) return rc;
-  long long bx = (out_len + 255) / 256;
-  const long long cap = (8LL * c->sm_count + n_clips - 1) / n_clips;
-  if (bx > cap) bx = cap;
-  if (bx < 1) bx = 1;
-  dim3 og((unsigned)bx, (unsigned)n_clips);
-  ola_kernel<<<og, 256, 0, c->stream>>>(c->d_scratch, (int)n_frames_used, L, p->hop, p->center ? L / 2 : 0, (int)out_len,
-                                        y_stride, d_inv_wss, d_y);
-  CUDA_TRY(cudaGetLastError());
-  c->launches++;
-  return B2L_OK;
+  const dim3 og((unsigned)row_blocks(out_len, 256, 8LL * c->sm_count, n_clips), (unsigned)n_clips);
+  return launch(c, ola_kernel, og, 256, 0, c->d_scratch, (int)n_frames_used, L, p->hop, p->center ? L / 2 : 0,
+                (int)out_len, y_stride, d_inv_wss, d_y);
 }
 
 // ------------------------------------------------------------------ S= pieces
@@ -807,15 +767,9 @@ extern "C" int b2l_resample_poly(b2l_ctx* c, const float* d_x, int64_t n_clips, 
   if (n_clips <= 0 || n_total <= 0) return B2L_OK;
   if (n_in > 0x7fffffffLL || n_total > 0x7fffffffLL) return fail(B2L_ERR_UNSUPPORTED, "signals longer than 2^31-1 samples");
   DeviceGuard g(c->device);
-  const long long total = (long long)n_clips * n_total;
-  long long grid = (total + 255) / 256;
-  const long long cap = (long long)c->sm_count * 32;
-  if (grid > cap) grid = cap;
-  resample_poly_kernel<<<(int)grid, 256, 0, c->stream>>>(d_x, x_stride, (int)n_in, d_h, n_h, up, down, n_pre_remove,
-                                                          (int)n_keep, (int)n_total, n_clips, out_scale, d_out);
-  CUDA_TRY(cudaGetLastError());
-  c->launches++;
-  return B2L_OK;
+  const long long grid = grid_stride_blocks((long long)n_clips * n_total, 256, 32LL * c->sm_count);
+  return launch(c, resample_poly_kernel, (unsigned)grid, 256, 0, d_x, x_stride, (int)n_in, d_h, n_h, up, down,
+                n_pre_remove, (int)n_keep, (int)n_total, n_clips, out_scale, d_out);
 }
 
 extern "C" int b2l_power_to_db(b2l_ctx* c, const float* d_in, int64_t n_clips, int64_t per_clip, float amin,
@@ -828,24 +782,14 @@ extern "C" int b2l_power_to_db(b2l_ctx* c, const float* d_in, int64_t n_clips, i
   if (rc) return rc;
   CUDA_TRY(cudaMemsetAsync(c->d_clip_max, 0, (size_t)n_clips * sizeof(unsigned int), c->stream));
   const float db_sub = 10.0f * log10f(fmaxf(amin, fabsf(ref_value)));
-  // the clip index rides in grid.y (at most 65535): larger batches go in slices, like the kernels they accompany
-  for (int64_t c0 = 0; c0 < n_clips; c0 += 65535) {
-    const int64_t m = std::min<int64_t>(65535, n_clips - c0);
-    long long bx = (per_clip + 256LL * 8 - 1) / (256LL * 8);
-    long long cap = (4LL * c->sm_count + m - 1) / m;
-    if (bx > cap) bx = cap;
-    if (bx < 1) bx = 1;
-    dim3 grid((unsigned)bx, (unsigned)m);
-    db_kernel<<<grid, 256, 0, c->stream>>>(d_in + c0 * per_clip, per_clip, amin, db_sub, c->d_clip_max + c0, d_out + c0 * per_clip);
-    CUDA_TRY(cudaGetLastError());
-    c->launches++;
-    if (top_db >= 0.0f) {
-      db_clamp_kernel<<<grid, 256, 0, c->stream>>>(d_out + c0 * per_clip, per_clip, c->d_clip_max + c0, top_db);
-      CUDA_TRY(cudaGetLastError());
-      c->launches++;
-    }
-  }
-  return B2L_OK;
+  return for_clip_slices(n_clips, [&](int64_t c0, int64_t m) {
+    const dim3 grid((unsigned)row_blocks(per_clip, 256 * 8, 4LL * c->sm_count, m), (unsigned)m);
+    int rc = launch(c, db_kernel, grid, 256, 0, d_in + c0 * per_clip, per_clip, amin, db_sub, c->d_clip_max + c0,
+                    d_out + c0 * per_clip);
+    if (rc == B2L_OK && top_db >= 0.0f)
+      rc = launch(c, db_clamp_kernel, grid, 256, 0, d_out + c0 * per_clip, per_clip, c->d_clip_max + c0, top_db);
+    return rc;
+  });
 }
 
 extern "C" int b2l_onset_from_spec(b2l_ctx* c, const b2l_onset_desc* d, const float* d_S, int64_t n_clips,
@@ -856,7 +800,7 @@ extern "C" int b2l_onset_from_spec(b2l_ctx* c, const b2l_onset_desc* d, const fl
   if (d->pad_width < 0) return fail(B2L_ERR_INVALID, "negative pad_width");
   if (d->n_channels < 0 || d->n_channels > 32) return fail(B2L_ERR_UNSUPPORTED, "at most 32 onset channels");
   if (n_clips <= 0 || n_rows <= 0 || n_frames <= 0) return B2L_OK;
-  if (n_clips > 65535 || n_rows > 0x7fffffffLL || n_frames > 0x7fffffffLL)
+  if (n_clips > kMaxGridY || n_rows > 0x7fffffffLL || n_frames > 0x7fffffffLL)
     return fail(B2L_ERR_UNSUPPORTED, "onset: batch too large");
   OnsetArgs a;
   memset(&a, 0, sizeof(a));
@@ -872,17 +816,10 @@ extern "C" int b2l_onset_from_spec(b2l_ctx* c, const b2l_onset_desc* d, const fl
   a.n_rows = (int)n_rows;
   a.T = (int)n_frames;
   DeviceGuard g(c->device);
-  dim3 grid((unsigned)((n_frames + 127) / 128), (unsigned)n_clips);
-  onset_kernel<<<grid, 128, 0, c->stream>>>(d_S, a, d_out);
-  CUDA_TRY(cudaGetLastError());
-  c->launches++;
-  if (d->detrend) {
-    const long long rows = (long long)n_clips * (a.n_ch > 0 ? a.n_ch : a.n_rows);
-    detrend_kernel<<<(unsigned)((rows + 127) / 128), 128, 0, c->stream>>>(d_out, rows, a.T);
-    CUDA_TRY(cudaGetLastError());
-    c->launches++;
-  }
-  return B2L_OK;
+  int rc = launch(c, onset_kernel, dim3((unsigned)((n_frames + 127) / 128), (unsigned)n_clips), 128, 0, d_S, a, d_out);
+  if (rc || !d->detrend) return rc;
+  const long long rows = (long long)n_clips * (a.n_ch > 0 ? a.n_ch : a.n_rows);
+  return launch(c, detrend_kernel, (unsigned)((rows + 127) / 128), 128, 0, d_out, rows, a.T);
 }
 
 extern "C" int b2l_pcen(b2l_ctx* c, const b2l_pcen_desc* d, const float* d_S, int64_t n_clips, int64_t n_rows,
@@ -895,15 +832,15 @@ extern "C" int b2l_pcen(b2l_ctx* c, const b2l_pcen_desc* d, const float* d_S, in
   if (!(d->b >= 0.0f && d->b <= 1.0f)) return fail(B2L_ERR_INVALID, "b=%g must be between 0 and 1", d->b);
   if (d->max_size < 1) return fail(B2L_ERR_INVALID, "max_size=%d must be a positive integer", d->max_size);
   if (n_clips <= 0 || n_rows <= 0 || n_frames <= 0) return B2L_OK;
-  if (n_frames > 0x7fffffffLL || n_rows > 65535 || n_clips > 65535) return fail(B2L_ERR_UNSUPPORTED, "pcen: batch too large");
+  if (n_frames > 0x7fffffffLL || n_rows > kMaxGridY || n_clips > kMaxGridY)
+    return fail(B2L_ERR_UNSUPPORTED, "pcen: batch too large");
   DeviceGuard g(c->device);
   const float* ref = d_S;
   if (d->max_size > 1) {
     if (!d_scratch) return fail(B2L_ERR_INVALID, "max_size > 1 needs a scratch buffer of the size of S");
-    dim3 grid((unsigned)((n_frames + 127) / 128), (unsigned)n_rows, (unsigned)n_clips);
-    maxfilter_rows_kernel<<<grid, 128, 0, c->stream>>>(d_S, (int)n_rows, (int)n_frames, d->max_size, d_scratch);
-    CUDA_TRY(cudaGetLastError());
-    c->launches++;
+    const dim3 grid((unsigned)((n_frames + 127) / 128), (unsigned)n_rows, (unsigned)n_clips);
+    if (int rc = launch(c, maxfilter_rows_kernel, grid, 128, 0, d_S, (int)n_rows, (int)n_frames, d->max_size, d_scratch))
+      return rc;
     ref = d_scratch;
   }
   PcenArgs a;
@@ -914,11 +851,8 @@ extern "C" int b2l_pcen(b2l_ctx* c, const b2l_pcen_desc* d, const float* d_S, in
   a.b = d->b;
   a.mode = d->power == 0.0f ? 0 : (d->bias == 0.0f ? 1 : 2);
   const long long rows = (long long)n_clips * n_rows;
-  const long long blocks = (rows + 127) / 128;
-  pcen_kernel<<<(unsigned)blocks, 128, 0, c->stream>>>(d_S, ref, rows, (int)n_frames, a, d_zi, d_zf, d_out);
-  CUDA_TRY(cudaGetLastError());
-  c->launches++;
-  return B2L_OK;
+  return launch(c, pcen_kernel, (unsigned)((rows + 127) / 128), 128, 0, d_S, ref, rows, (int)n_frames, a, d_zi, d_zf,
+                d_out);
 }
 
 extern "C" int b2l_spectral_contrast(b2l_ctx* c, const b2l_contrast_desc* d, const float* d_S, int64_t n_clips,
@@ -949,9 +883,7 @@ extern "C" int b2l_spectral_contrast(b2l_ctx* c, const b2l_contrast_desc* d, con
   const int rc = blocks_per_sm(c, contrast_kernel, nw * 32, smem, nullptr);
   if (rc) return rc;
   const long long rows = (long long)n_clips * n_frames;
-  long long grid = (rows + nw - 1) / nw;
-  const long long lim = (long long)c->sm_count * 8;
-  if (grid > lim) grid = lim;
+  const long long grid = grid_stride_blocks(rows, nw, 8LL * c->sm_count);
   return launch(c, contrast_kernel, (unsigned)grid, nw * 32, smem, d_S, rows, (int)n_frames, n_bins, cap, a, d_peak,
                 d_valley);
 }
@@ -960,12 +892,7 @@ extern "C" int b2l_sub(b2l_ctx* c, const float* d_x, const float* d_y, int64_t n
   if (!c || !d_x || !d_y || !d_out) return fail(B2L_ERR_INVALID, "NULL argument");
   if (n <= 0) return B2L_OK;
   DeviceGuard g(c->device);
-  long long grid = (n + 256LL * 8 - 1) / (256LL * 8);
-  if (grid > 8LL * c->sm_count) grid = 8LL * c->sm_count;
-  sub_kernel<<<(int)grid, 256, 0, c->stream>>>(d_x, d_y, n, d_out);
-  CUDA_TRY(cudaGetLastError());
-  c->launches++;
-  return B2L_OK;
+  return launch(c, sub_kernel, (unsigned)grid_stride_blocks(n, 256 * 8, 8LL * c->sm_count), 256, 0, d_x, d_y, n, d_out);
 }
 
 extern "C" int b2l_pip_pass(b2l_ctx* c, const b2l_pip_desc* d, const float* d_S, int64_t n_rows, int32_t n_bins,
@@ -1004,9 +931,7 @@ extern "C" int b2l_pip_pass(b2l_ctx* c, const b2l_pip_desc* d, const float* d_S,
   if (smem + 8192 + 1024 > c->smem_optin) return fail(B2L_ERR_UNSUPPORTED, "n_bins=%d rows do not fit in shared memory", n_bins);
   // 8 KB of static shared memory (the block's histogram) and 1 KB reserved by the system
   if ((rc = blocks_per_sm(c, pip_pass_kernel, nw * 32, smem, nullptr, c->smem_optin - 8192 - 1024))) return rc;
-  long long grid = (n_rows + nw - 1) / nw;
-  const long long lim = (long long)c->sm_count * 4;
-  if (grid > lim) grid = lim;
+  const long long grid = grid_stride_blocks(n_rows, nw, 4LL * c->sm_count);
   if ((rc = launch(c, pip_pass_kernel, (unsigned)grid, nw * 32, smem, d_S, n_rows, n_bins, a, d_edges, d_hist))) return rc;
   CUDA_TRY(cudaMemcpyAsync(h_hist, d_hist, (size_t)n_hist * sizeof(unsigned long long), cudaMemcpyDeviceToHost, c->stream));
   CUDA_TRY(cudaStreamSynchronize(c->stream));
@@ -1019,25 +944,18 @@ extern "C" int b2l_normalize_rows(b2l_ctx* c, const float* d_in, int64_t n_clips
   if (norm_kind < 0 || norm_kind > 3) return fail(B2L_ERR_INVALID, "bad norm kind %d", norm_kind);
   if (norm_kind == 3 && !(norm_p > 0.0f)) return fail(B2L_ERR_INVALID, "Unsupported norm: %g", norm_p);
   if (n_clips <= 0 || n_rows <= 0 || n_frames <= 0) return B2L_OK;
-  if (n_clips > 65535 || n_rows > 0x7fffffffLL || n_frames > 0x7fffffffLL) return fail(B2L_ERR_UNSUPPORTED, "normalize: batch too large");
+  if (n_clips > kMaxGridY || n_rows > 0x7fffffffLL || n_frames > 0x7fffffffLL) return fail(B2L_ERR_UNSUPPORTED, "normalize: batch too large");
   DeviceGuard g(c->device);
-  dim3 grid((unsigned)((n_frames + 127) / 128), (unsigned)n_clips);
-  normalize_rows_kernel<<<grid, 128, 0, c->stream>>>(d_in, (int)n_rows, (int)n_frames, norm_kind, norm_p, d_out);
-  CUDA_TRY(cudaGetLastError());
-  c->launches++;
-  return B2L_OK;
+  return launch(c, normalize_rows_kernel, dim3((unsigned)((n_frames + 127) / 128), (unsigned)n_clips), 128, 0, d_in,
+                (int)n_rows, (int)n_frames, norm_kind, norm_p, d_out);
 }
 
 extern "C" int b2l_cabs(b2l_ctx* c, const void* d_complex, int64_t n, float* d_out) {
   if (!c || !d_complex || !d_out) return fail(B2L_ERR_INVALID, "NULL argument");
   if (n <= 0) return B2L_OK;
   DeviceGuard g(c->device);
-  long long grid = (n + 256LL * 8 - 1) / (256LL * 8);
-  if (grid > 8LL * c->sm_count) grid = 8LL * c->sm_count;
-  cabs_kernel<<<(int)grid, 256, 0, c->stream>>>((const float2*)d_complex, n, d_out);
-  CUDA_TRY(cudaGetLastError());
-  c->launches++;
-  return B2L_OK;
+  return launch(c, cabs_kernel, (unsigned)grid_stride_blocks(n, 256 * 8, 8LL * c->sm_count), 256, 0,
+                (const float2*)d_complex, n, d_out);
 }
 
 extern "C" int b2l_hpss(b2l_ctx* c, const b2l_hpss_desc* d, const float* d_mag, const void* d_S_complex,
@@ -1049,7 +967,8 @@ extern "C" int b2l_hpss(b2l_ctx* c, const b2l_hpss_desc* d, const float* d_mag, 
     return fail(B2L_ERR_INVALID, "Margins must be >= 1.0. A typical range is between 1 and 10.");
   if (!(d->power > 0.0f)) return fail(B2L_ERR_INVALID, "power must be strictly positive");
   if (n_clips <= 0 || n_frames <= 0 || n_bins <= 0) return B2L_OK;
-  if (n_frames > 65535 || n_clips > 65535 || n_bins > 0x7fffffffLL) return fail(B2L_ERR_UNSUPPORTED, "hpss: batch too large");
+  if (n_frames > kMaxGridY || n_clips > kMaxGridY || n_bins > 0x7fffffffLL)
+    return fail(B2L_ERR_UNSUPPORTED, "hpss: batch too large");
   HpssArgs a;
   a.T = (int)n_frames;
   a.F = (int)n_bins;
@@ -1062,15 +981,10 @@ extern "C" int b2l_hpss(b2l_ctx* c, const b2l_hpss_desc* d, const float* d_mag, 
   a.mode = d->mask_only ? 1 : 0;
   DeviceGuard g(c->device);
   const int w = std::max(d->win_harm, d->win_perc);
-  dim3 grid((unsigned)((n_bins + 127) / 128), (unsigned)n_frames, (unsigned)n_clips);
+  auto kern = w <= 8 ? hpss_kernel<8> : w <= 16 ? hpss_kernel<16> : w <= 32 ? hpss_kernel<32> : hpss_kernel<64>;
+  const dim3 grid((unsigned)((n_bins + 127) / 128), (unsigned)n_frames, (unsigned)n_clips);
   const float2* sc = d->mask_only ? nullptr : (const float2*)d_S_complex;
-  if (w <= 8) hpss_kernel<8><<<grid, 128, 0, c->stream>>>(d_mag, sc, a, (float*)d_out_harm, (float*)d_out_perc);
-  else if (w <= 16) hpss_kernel<16><<<grid, 128, 0, c->stream>>>(d_mag, sc, a, (float*)d_out_harm, (float*)d_out_perc);
-  else if (w <= 32) hpss_kernel<32><<<grid, 128, 0, c->stream>>>(d_mag, sc, a, (float*)d_out_harm, (float*)d_out_perc);
-  else hpss_kernel<64><<<grid, 128, 0, c->stream>>>(d_mag, sc, a, (float*)d_out_harm, (float*)d_out_perc);
-  CUDA_TRY(cudaGetLastError());
-  c->launches++;
-  return B2L_OK;
+  return launch(c, kern, grid, 128, 0, d_mag, sc, a, (float*)d_out_harm, (float*)d_out_perc);
 }
 
 extern "C" int b2l_reassign(b2l_ctx* c, const b2l_reassign_desc* d, const void* d_Sh, const void* d_Sdh,
@@ -1098,13 +1012,9 @@ extern "C" int b2l_reassign(b2l_ctx* c, const b2l_reassign_desc* d, const void* 
   a.clip = d->clip ? 1 : 0;
   DeviceGuard g(c->device);
   const long long n = (long long)n_clips * n_frames * n_bins;
-  long long grid = (n + 256LL * 4 - 1) / (256LL * 4);
-  if (grid > 16LL * c->sm_count) grid = 16LL * c->sm_count;
-  reassign_kernel<<<(int)grid, 256, 0, c->stream>>>((const float2*)d_Sh, (const float2*)d_Sdh, (const float2*)d_Sth,
-                                                    d_bin_freqs, d_frame_times, a, n, d_freqs, d_times, d_mags);
-  CUDA_TRY(cudaGetLastError());
-  c->launches++;
-  return B2L_OK;
+  return launch(c, reassign_kernel, (unsigned)grid_stride_blocks(n, 256 * 4, 16LL * c->sm_count), 256, 0,
+                (const float2*)d_Sh, (const float2*)d_Sdh, (const float2*)d_Sth, d_bin_freqs, d_frame_times, a, n, d_freqs,
+                d_times, d_mags);
 }
 
 extern "C" int b2l_phase_vocoder(b2l_ctx* c, const void* d_D, int64_t n_clips, int64_t n_frames, int64_t n_bins,
@@ -1117,11 +1027,8 @@ extern "C" int b2l_phase_vocoder(b2l_ctx* c, const void* d_D, int64_t n_clips, i
     return fail(B2L_ERR_UNSUPPORTED, "phase_vocoder: too large");
   DeviceGuard g(c->device);
   const long long threads = (long long)n_clips * n_bins;
-  phase_vocoder_kernel<<<(unsigned)((threads + 127) / 128), 128, 0, c->stream>>>(
-      (const float2*)d_D, (int)n_frames, (int)n_bins, n_clips, (int)n_out, d_i0, d_i1, d_lo, d_dx, (float2*)d_out);
-  CUDA_TRY(cudaGetLastError());
-  c->launches++;
-  return B2L_OK;
+  return launch(c, phase_vocoder_kernel, (unsigned)((threads + 127) / 128), 128, 0, (const float2*)d_D, (int)n_frames,
+                (int)n_bins, n_clips, (int)n_out, d_i0, d_i1, d_lo, d_dx, (float2*)d_out);
 }
 
 extern "C" int b2l_unary(b2l_ctx* c, int32_t op, const float* d_in, int64_t n, float param, float* d_out) {
@@ -1129,12 +1036,8 @@ extern "C" int b2l_unary(b2l_ctx* c, int32_t op, const float* d_in, int64_t n, f
   if (op < 0 || op > B2L_UNARY_DB_TO_AMPLITUDE) return fail(B2L_ERR_INVALID, "bad unary op %d", op);
   if (n <= 0) return B2L_OK;
   DeviceGuard g(c->device);
-  long long grid = (n + 256LL * 8 - 1) / (256LL * 8);
-  if (grid > 8LL * c->sm_count) grid = 8LL * c->sm_count;
-  unary_kernel<<<(int)grid, 256, 0, c->stream>>>(d_in, n, op, param, d_out);
-  CUDA_TRY(cudaGetLastError());
-  c->launches++;
-  return B2L_OK;
+  return launch(c, unary_kernel, (unsigned)grid_stride_blocks(n, 256 * 8, 8LL * c->sm_count), 256, 0, d_in, n, op, param,
+                d_out);
 }
 
 extern "C" int b2l_dct_project(b2l_ctx* c, const b2l_plan* p, const float* d_S, int64_t n_clips, int64_t n_frames,
@@ -1151,14 +1054,8 @@ extern "C" int b2l_gl_update(b2l_ctx* c, const void* d_rebuilt, const void* d_tp
   if (!c || !d_rebuilt || !d_S || !d_angles) return fail(B2L_ERR_INVALID, "NULL argument");
   if (n <= 0) return B2L_OK;
   DeviceGuard g(c->device);
-  long long blocks = (n + 255) / 256;
-  const long long cap = 8LL * c->sm_count;
-  if (blocks > cap) blocks = cap;
-  gl_update_kernel<<<(int)blocks, 256, 0, c->stream>>>((const float2*)d_rebuilt, (const float2*)d_tprev, d_S, scale, eps,
-                                                     (float2*)d_angles, n);
-  CUDA_TRY(cudaGetLastError());
-  c->launches++;
-  return B2L_OK;
+  return launch(c, gl_update_kernel, (unsigned)grid_stride_blocks(n, 256, 8LL * c->sm_count), 256, 0,
+                (const float2*)d_rebuilt, (const float2*)d_tprev, d_S, scale, eps, (float2*)d_angles, n);
 }
 
 extern "C" int b2l_transpose(b2l_ctx* c, const void* d_in, int64_t n_clips, int64_t rows, int64_t cols,
@@ -1167,19 +1064,14 @@ extern "C" int b2l_transpose(b2l_ctx* c, const void* d_in, int64_t n_clips, int6
   if (n_clips <= 0 || rows <= 0 || cols <= 0) return B2L_OK;
   if (elem_bytes != 4 && elem_bytes != 8) return fail(B2L_ERR_INVALID, "elem_bytes must be 4 or 8");
   DeviceGuard g(c->device);
-  dim3 block(32, 8);
-  for (int64_t c0 = 0; c0 < n_clips; c0 += 65535) {   // the clip index rides in grid.z: larger batches go in slices
-    const int64_t m = std::min<int64_t>(65535, n_clips - c0);
-    dim3 grid((unsigned)((cols + 31) / 32), (unsigned)((rows + 31) / 32), (unsigned)m);
+  return for_clip_slices(n_clips, [&](int64_t c0, int64_t m) {
+    const dim3 grid((unsigned)((cols + 31) / 32), (unsigned)((rows + 31) / 32), (unsigned)m), block(32, 8);
     const size_t off = (size_t)c0 * (size_t)rows * (size_t)cols;
-    if (elem_bytes == 4)
-      transpose_kernel<float><<<grid, block, 0, c->stream>>>((const float*)d_in + off, (int)rows, (int)cols, (float*)d_out + off);
-    else
-      transpose_kernel<float2><<<grid, block, 0, c->stream>>>((const float2*)d_in + off, (int)rows, (int)cols, (float2*)d_out + off);
-    CUDA_TRY(cudaGetLastError());
-    c->launches++;
-  }
-  return B2L_OK;
+    return elem_bytes == 4 ? launch(c, transpose_kernel<float>, grid, block, 0, (const float*)d_in + off, (int)rows,
+                                    (int)cols, (float*)d_out + off)
+                           : launch(c, transpose_kernel<float2>, grid, block, 0, (const float2*)d_in + off, (int)rows,
+                                    (int)cols, (float2*)d_out + off);
+  });
 }
 
 // ------------------------------------------------------------------ pitch tracking (pitch_kernels.cuh)
@@ -1229,11 +1121,9 @@ extern "C" int b2l_yin_cmnd(b2l_ctx* c, const b2l_yin_desc* d, const float* d_y,
   const int G = 256 / cfg.tpf;
   const size_t smem = (size_t)cfg.tw_count() * 8 + (size_t)G * cfg.xbuf_f2() * 8;
   auto fn = yin_cmnd_kernel_for(log2m);
-  int occ = 0, rc;
-  if ((rc = blocks_per_sm(c, fn, 256, smem, &occ))) return rc;
-  if (occ < 1) return fail(B2L_ERR_CUDA, "yin_cmnd_kernel does not fit on an SM (smem %zu)", smem);
-  const long long rows = n_clips * T;
-  const long long grid = std::min((rows + G - 1) / G, (long long)c->sm_count * occ);
+  long long grid = 0;
+  if (int rc = resident_grid(c, fn, 256, smem, (n_clips * T + G - 1) / G, &grid)) return rc;
+  if (!grid) return fail(B2L_ERR_CUDA, "yin_cmnd_kernel does not fit on an SM (smem %zu)", smem);
   YinCmndArgs a;
   a.y = d_y;
   a.clip_stride = y_stride;
@@ -1261,10 +1151,9 @@ extern "C" int b2l_yin_pick(b2l_ctx* c, const b2l_yin_desc* d, const float* d_cm
   DeviceGuard g(c->device);
   const int n_lags = d->max_period - d->min_period + 1;
   const size_t smem = (size_t)8 * n_lags * 4;
-  int occ = 0, rc;
-  if ((rc = blocks_per_sm(c, yin_pick_kernel, 256, smem, &occ))) return rc;
-  if (occ < 1) return fail(B2L_ERR_UNSUPPORTED, "yin: %d lags do not fit in shared memory", n_lags);
-  const long long grid = std::min<long long>((n_rows + 7) / 8, (long long)c->sm_count * occ);
+  long long grid = 0;
+  if (int rc = resident_grid(c, yin_pick_kernel, 256, smem, (n_rows + 7) / 8, &grid)) return rc;
+  if (!grid) return fail(B2L_ERR_UNSUPPORTED, "yin: %d lags do not fit in shared memory", n_lags);
   return launch(c, yin_pick_kernel, (unsigned)grid, 256, smem, d_cmnd, (long long)n_rows, n_lags, d->min_period, d->sr,
                 d->trough_threshold, d_f0);
 }
@@ -1307,11 +1196,10 @@ extern "C" int b2l_pyin_obs(b2l_ctx* c, const b2l_pyin_desc* d, const float* d_c
   a.cand_prob = d_cand_prob;
   a.voiced_prob = d_voiced_prob;
   const size_t smem = 4 * pyin_obs_slice(a.n_lags, a.max_cand, a.n_thresholds);
-  int occ = 0, rc;
   if (smem > c->smem_optin) return fail(B2L_ERR_UNSUPPORTED, "pyin: %d lags do not fit in shared memory", a.n_lags);
-  if ((rc = blocks_per_sm(c, pyin_obs_kernel, 128, smem, &occ))) return rc;
-  if (occ < 1) return fail(B2L_ERR_UNSUPPORTED, "pyin: %d lags do not fit in shared memory", a.n_lags);
-  const long long grid = std::min<long long>((n_rows + 3) / 4, (long long)c->sm_count * occ);
+  long long grid = 0;
+  if (int rc = resident_grid(c, pyin_obs_kernel, 128, smem, (n_rows + 3) / 4, &grid)) return rc;
+  if (!grid) return fail(B2L_ERR_UNSUPPORTED, "pyin: %d lags do not fit in shared memory", a.n_lags);
   return launch(c, pyin_obs_kernel, (unsigned)grid, 128, smem, a);
 }
 

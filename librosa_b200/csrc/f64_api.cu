@@ -27,7 +27,6 @@ namespace {
 
 const int kMaxFft64 = 1 << 20;   // power-of-two n_fft (work area in shared memory up to 16384, else in global memory)
 const int kMaxDft64 = 1 << 16;   // any other n_fft: direct O(n_fft^2) DFT
-const int64_t kMaxGridY = 65535; // kernels that carry the clip index in grid.y run in slices of this many clips
 
 }  // namespace
 
@@ -124,34 +123,21 @@ extern "C" int b2l_istft_f64(b2l_ctx* c, const void* d_D, int64_t n_clips, int64
   }
   int rc = blocks_per_sm(c, istft64_frames_kernel, 256, smem, nullptr);
   if (rc || (rc = launch(c, istft64_frames_kernel, (unsigned)(n_clips * n_frames_used), 256, smem, a))) return rc;
-  // the overlap-add carries the clip index in grid.y (at most 65535): larger batches go in slices
-  for (int64_t c0 = 0; c0 < n_clips; c0 += kMaxGridY) {
-    const int64_t m = std::min<int64_t>(kMaxGridY, n_clips - c0);
+  return for_clip_slices(n_clips, [&](int64_t c0, int64_t m) {
     F64InvArgs s = a;
     s.frames += c0 * n_frames_used * n_fft;
     s.y += c0 * y_stride;
-    long long bx = (out_len + 255) / 256;
-    const long long cap = (8LL * c->sm_count + m - 1) / m;
-    if (bx > cap) bx = cap;
-    if (bx < 1) bx = 1;
-    ola64_kernel<<<dim3((unsigned)bx, (unsigned)m), 256, 0, st>>>(s);
-    CUDA_TRY(cudaGetLastError());
-    c->launches++;
-  }
-  return B2L_OK;
+    const dim3 grid((unsigned)row_blocks(out_len, 256, 8LL * c->sm_count, m), (unsigned)m);
+    return launch(c, ola64_kernel, grid, 256, 0, s);
+  });
 }
 
 extern "C" int b2l_f64_abs_pow(b2l_ctx* c, const void* d_D, int64_t n, double power, double* d_S) {
   if (!c || !d_D || !d_S) return fail(B2L_ERR_INVALID, "NULL argument");
   if (n <= 0) return B2L_OK;
   DeviceGuard g(c->device);
-  long long grid = (n + 255) / 256;
-  const long long cap = 16LL * c->sm_count;
-  if (grid > cap) grid = cap;
-  abs_pow64_kernel<<<(unsigned)grid, 256, 0, c->stream>>>((const double2*)d_D, n, power, d_S);
-  CUDA_TRY(cudaGetLastError());
-  c->launches++;
-  return B2L_OK;
+  return launch(c, abs_pow64_kernel, (unsigned)grid_stride_blocks(n, 256, 16LL * c->sm_count), 256, 0,
+                (const double2*)d_D, n, power, d_S);
 }
 
 extern "C" int b2l_f64_mel(b2l_ctx* c, const double* d_S, int64_t n_clips, int64_t n_frames, int32_t n_bins,
@@ -187,10 +173,8 @@ extern "C" int b2l_f64_mel(b2l_ctx* c, const double* d_S, int64_t n_clips, int64
   const long long rows = n_clips * n_frames;
   const long long blocks = (rows * 32 + 255) / 256;
   if (blocks > 0x7fffffffLL) return fail(B2L_ERR_UNSUPPORTED, "float64 mel: too many frames in one call");
-  mel64_kernel<<<(unsigned)blocks, 256, 0, st>>>(d_S, (const float*)d_w.p, (const MelBand*)d_b.p, n_mels, n_bins, (int)n_frames, rows, d_out);
-  CUDA_TRY(cudaGetLastError());
-  c->launches++;
-  return B2L_OK;
+  return launch(c, mel64_kernel, (unsigned)blocks, 256, 0, d_S, (const float*)d_w.p, (const MelBand*)d_b.p, n_mels, n_bins,
+                (int)n_frames, rows, d_out);
 }
 
 extern "C" int b2l_f64_db(b2l_ctx* c, const double* d_in, int64_t n_clips, int64_t per_clip, double amin, double ref_value,
@@ -205,24 +189,14 @@ extern "C" int b2l_f64_db(b2l_ctx* c, const double* d_in, int64_t n_clips, int64
   CUDA_TRY(cudaMemsetAsync(d_max.p, 0, (size_t)n_clips * sizeof(unsigned long long), st));
   unsigned long long* clip_max = (unsigned long long*)d_max.p;
   const double db_sub = 10.0 * log10(fmax(amin, fabs(ref_value)));
-  // the clip index rides in grid.y (at most 65535): larger batches go in slices
-  for (int64_t c0 = 0; c0 < n_clips; c0 += kMaxGridY) {
-    const int64_t m = std::min<int64_t>(kMaxGridY, n_clips - c0);
-    long long bx = (per_clip + 255) / 256;
-    const long long cap = (8LL * c->sm_count + m - 1) / m;
-    if (bx > cap) bx = cap;
-    if (bx < 1) bx = 1;
-    const dim3 grid((unsigned)bx, (unsigned)m);
-    db64_kernel<<<grid, 256, 0, st>>>(d_in + c0 * per_clip, per_clip, amin, db_sub, d_out + c0 * per_clip, clip_max + c0);
-    CUDA_TRY(cudaGetLastError());
-    c->launches++;
-    if (top_db >= 0.0) {
-      db64_clamp_kernel<<<grid, 256, 0, st>>>(d_out + c0 * per_clip, per_clip, top_db, clip_max + c0);
-      CUDA_TRY(cudaGetLastError());
-      c->launches++;
-    }
-  }
-  return B2L_OK;
+  return for_clip_slices(n_clips, [&](int64_t c0, int64_t m) {
+    const dim3 grid((unsigned)row_blocks(per_clip, 256, 8LL * c->sm_count, m), (unsigned)m);
+    int rc = launch(c, db64_kernel, grid, 256, 0, d_in + c0 * per_clip, per_clip, amin, db_sub, d_out + c0 * per_clip,
+                    clip_max + c0);
+    if (rc == B2L_OK && top_db >= 0.0)
+      rc = launch(c, db64_clamp_kernel, grid, 256, 0, d_out + c0 * per_clip, per_clip, top_db, clip_max + c0);
+    return rc;
+  });
 }
 
 extern "C" int b2l_f64_dct(b2l_ctx* c, const double* d_L, int64_t n_clips, int32_t n_mels, int64_t n_frames,
@@ -235,15 +209,10 @@ extern "C" int b2l_f64_dct(b2l_ctx* c, const double* d_L, int64_t n_clips, int32
   if (smem > c->smem_optin) return fail(B2L_ERR_UNSUPPORTED, "float64 dct: matrix does not fit in shared memory");
   Temp d_dct(st);
   CUDA_TRY(upload(d_dct, h_dct, (size_t)n_mfcc * n_mels));
-  int rc = blocks_per_sm(c, dct64_kernel, 128, smem, nullptr);
-  if (rc) return rc;
-  long long bx = (n_frames + 127) / 128;
-  if (bx < 1) bx = 1;
-  // the clip index rides in grid.y (at most 65535): larger batches go in slices
-  for (int64_t c0 = 0; c0 < n_clips && !rc; c0 += kMaxGridY) {
-    const int64_t m = std::min<int64_t>(kMaxGridY, n_clips - c0);
-    rc = launch(c, dct64_kernel, dim3((unsigned)bx, (unsigned)m), 128, smem, d_L + c0 * n_mels * n_frames,
-                (const double*)d_dct.p, n_mels, n_mfcc, (int)n_frames, d_out + c0 * n_mfcc * n_frames);
-  }
-  return rc;
+  if (int rc = blocks_per_sm(c, dct64_kernel, 128, smem, nullptr)) return rc;
+  return for_clip_slices(n_clips, [&](int64_t c0, int64_t m) {
+    return launch(c, dct64_kernel, dim3((unsigned)((n_frames + 127) / 128), (unsigned)m), 128, smem,
+                  d_L + c0 * n_mels * n_frames, (const double*)d_dct.p, n_mels, n_mfcc, (int)n_frames,
+                  d_out + c0 * n_mfcc * n_frames);
+  });
 }

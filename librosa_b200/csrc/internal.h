@@ -4,6 +4,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <algorithm>
 #include <map>
 #include <set>
 #include <tuple>
@@ -209,12 +210,44 @@ int blocks_per_sm(b2l_ctx* c, void (*fn)(P...), int threads, size_t smem, int* o
   return blocks_per_sm(c, (const void*)fn, threads, smem, occ, smem_limit);
 }
 
-// Launches `fn` on the context's stream, checks the launch and counts it.
+// Launches `fn` on the context's stream, checks the launch and counts it: the only place that does any of the three.
 template <class... P, class... A>
-int launch(b2l_ctx* c, void (*fn)(P...), dim3 grid, int threads, size_t smem, const A&... args) {
-  fn<<<grid, threads, smem, c->stream>>>(args...);
+int launch(b2l_ctx* c, void (*fn)(P...), dim3 grid, dim3 block, size_t smem, const A&... args) {
+  fn<<<grid, block, smem, c->stream>>>(args...);
   CUDA_TRY(cudaGetLastError());
   c->launches++;
+  return B2L_OK;
+}
+
+// Grid of a kernel that keeps every block resident: sm_count * (blocks per SM with `query_smem` bytes of dynamic
+// shared memory), at most `need`; 0 when not even one block fits (each caller reports that in its own words).
+template <class... P>
+int resident_grid(b2l_ctx* c, void (*fn)(P...), int threads, size_t query_smem, long long need, long long* grid) {
+  int occ = 0;
+  if (int rc = blocks_per_sm(c, fn, threads, query_smem, &occ)) return rc;
+  *grid = occ < 1 ? 0 : std::min((long long)c->sm_count * occ, need);
+  return B2L_OK;
+}
+
+// Blocks of a grid-stride loop over `work` items, `per_block` items per block per pass, at most `cap` blocks.
+inline long long grid_stride_blocks(long long work, long long per_block, long long cap) {
+  return std::min((work + per_block - 1) / per_block, cap);
+}
+
+// x-extent of an (x, clips) grid over m clips of `per_row` items: one block per `per_block` items, but about
+// `budget` blocks in all, and at least one per clip.
+inline long long row_blocks(long long per_row, long long per_block, long long budget, long long m) {
+  return std::max(1LL, std::min((per_row + per_block - 1) / per_block, (budget + m - 1) / m));
+}
+
+// Largest grid.y / grid.z extent.  Kernels that carry the clip index there run larger batches in slices.
+constexpr int64_t kMaxGridY = 65535;
+
+// Calls body(c0, m) for consecutive slices [c0, c0 + m) of at most kMaxGridY clips; returns the first non-zero status.
+template <class F>
+int for_clip_slices(int64_t n_clips, F body) {
+  for (int64_t c0 = 0; c0 < n_clips; c0 += kMaxGridY)
+    if (int rc = body(c0, std::min(kMaxGridY, n_clips - c0))) return rc;
   return B2L_OK;
 }
 

@@ -154,9 +154,7 @@ extern "C" int b2l_nnls_mel(b2l_ctx* c, const float* d_mel, int64_t n_clips, int
   int rc = blocks_per_sm(c, nnls_fista_kernel, NNLS_WARPS * 32, smem, nullptr);
   if (rc) return rc;
   const long long cols = n_clips * n_frames;
-  long long grid = (cols + NNLS_WARPS - 1) / NNLS_WARPS;
-  const long long cap = 2LL * c->sm_count;
-  if (grid > cap) grid = cap;
+  const long long grid = grid_stride_blocks(cols, NNLS_WARPS, 2LL * c->sm_count);
   return launch(c, nnls_fista_kernel, (unsigned)grid, NNLS_WARPS * 32, smem, d_mel, cols, (int)n_frames, n_mels, n_bins,
                 (const MelBand*)d_band.p, (const float*)d_w.p, (int)w.size(), (const BinRows*)d_bins.p,
                 (const float*)d_pinv.p, (const float*)d_beta.p, n_iter, step, inv_power, d_out);

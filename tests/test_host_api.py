@@ -338,6 +338,27 @@ def test_frame_length_routing_table():
         del os.environ["B2L_MR"]
 
 
+def test_kernels_launch_only_through_launch():
+    """Every kernel of the C ABI is enqueued by b2l::launch (csrc/internal.h), the only code that counts launches:
+    a `<<<...>>>` or a `launches++` anywhere else would make Context.launch_count miss or double-count a kernel."""
+    import glob
+    import re
+
+    csrc = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "librosa_b200", "csrc")
+    with open(os.path.join(csrc, "internal.h")) as f:
+        header = f.read()
+    body = re.search(r"\nint launch\(.*?\n\}\n", header, re.S)
+    assert body and "<<<" in body.group(0) and "launches++" in body.group(0)
+    sources = {"internal.h": header.replace(body.group(0), "\n")}
+    for path in sorted(glob.glob(os.path.join(csrc, "*.cu"))):
+        with open(path) as f:
+            sources[os.path.basename(path)] = f.read()
+    assert len(sources) > 5
+    stray = [(name, i + 1, line.strip()) for name, text in sources.items() for i, line in enumerate(text.splitlines())
+             if "<<<" in line or "launches++" in line]
+    assert not stray, stray
+
+
 def test_polyphase_filter_bookkeeping_matches_scipy():
     """The host half of resample(res_type="polyphase"): the zero-padded low-pass and the crop offset handed to
     b2l_resample_poly, checked by evaluating the kernel's formula  y[j] = sum_m x[m] h[(n_pre_remove + j) down - m up]
