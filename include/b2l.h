@@ -175,6 +175,11 @@ typedef struct b2l_onset_desc {
 } b2l_onset_desc;
 int b2l_onset_from_spec(b2l_ctx* ctx, const b2l_onset_desc* desc, const float* d_S, int64_t n_clips, int64_t n_rows,
                         int64_t n_frames, float* d_out);
+/* The same envelope aggregated with np.median over each channel's rows (util.sync(..., aggregate=np.median)): the
+ * float32 mean of the two middle values for an even row count, NaN when a flux of the column is NaN.  1 to 32
+ * channels of at most 512 rows each (else B2L_ERR_UNSUPPORTED). */
+int b2l_onset_median_from_spec(b2l_ctx* ctx, const b2l_onset_desc* desc, const float* d_S, int64_t n_clips,
+                               int64_t n_rows, int64_t n_frames, float* d_out);
 /* Per-channel energy normalisation, librosa.pcen (core/spectrum.py:2396-2666), of d_S [n_clips][n_rows][n_frames]
  * along time: first-order IIR smoother with coefficient b (lfilter([b], [1, b-1])), adaptive gain and root
  * compression.  d_zi / d_zf: optional initial / final filter state, one float per (clip, row) (NULL: the
@@ -409,6 +414,52 @@ typedef struct b2l_tempo_desc {
 } b2l_tempo_desc;
 int b2l_tempo(b2l_ctx* ctx, const b2l_tempo_desc* desc, const void* d_tg, int64_t n_rows, const double* d_logprior,
               const double* d_bpms, double* d_out);
+
+/* ---- beat tracking: librosa.beat.beat_track's tracker (beat.py:510-742) and plp -----------------------------------------
+ * b2l_beat_track: onset envelopes d_env [n_clips][n] (float32, or float64 when env_f64) and frames per beat ->
+ *   d_beats [n_clips][n] (1 at a beat), one launch.  The stages restate the reference's arithmetic: normalisation
+ *   by std(ddof=1) (NumPy pairwise sums), the Gaussian local score, the DP with float32 `tightness`, the last
+ *   beat (median of the cumulative score's local maxima), the backtrack and the trim.  Frames per beat come per
+ *   clip (n_fpb == 1) or per frame (n_fpb == n) as device float64 tables [n_clips][n_fpb] built by the caller with
+ *   libm: d_fpb (integers >= 1), d_logfpb (log, or logf for the float32 DP), d_woff (index into d_wtab of the
+ *   window's centre; d_wtab[woff + d] = exp(-0.5 x x), x = d * 32.0 / fpb, for |d| <= min(fpb, n - 1)), and
+ *   d_logd [n_logd] = log(d) for 1 <= d <= min(2 max fpb, n - 1).  The DP and d_cumscore are float64 when dp_f64
+ *   (numba's choice whenever the envelope or the frames per beat are float64), else float32; d_localscore has the
+ *   envelope's type.  d_localscore, d_cumscore ([n_clips][n]) and d_backlink may be NULL (a work area is used).  With d_sparse (one clip only) the beat
+ *   frames surviving the trim are also written in ascending order, converted to `units` (int64 frames or
+ *   samples = frame * hop_length, float64 seconds = samples / sr), and their number to d_count.
+ * b2l_any_nonzero: *d_flag = 1 when an element of d_x [n] (float32, or float64 when f64) is not zero, else 0. */
+enum b2l_beat_units { B2L_BEAT_FRAMES = 0, B2L_BEAT_SAMPLES = 1, B2L_BEAT_TIME = 2 };
+typedef struct b2l_beat_desc {
+  int32_t n_fpb, env_f64, dp_f64, trim, units;
+  float tightness;
+  int32_t hop_length;
+  double sr;
+  const double* d_fpb;
+  const double* d_logfpb;
+  const double* d_woff;
+  const double* d_wtab;
+  const double* d_logd;
+} b2l_beat_desc;
+int b2l_beat_track(b2l_ctx* ctx, const b2l_beat_desc* desc, const void* d_env, int64_t n_clips, int64_t n,
+                   void* d_localscore, void* d_cumscore, int32_t* d_backlink, uint8_t* d_beats, void* d_sparse,
+                   int64_t* d_count);
+int b2l_any_nonzero(b2l_ctx* ctx, const void* d_x, int64_t n, int32_t f64, int32_t* d_flag);
+/* librosa.beat.plp (beat.py:320-507) around the stft / istft entry points:
+ * b2l_plp_select: in place on a Fourier tempogram d_ftgram [n_frames][n_bins] (complex64, or complex128 when c128;
+ *   n_frames counts every (row, frame)): zero the bins whose d_keep entry is 0 (the tempo range), zero every bin
+ *   whose log1p(1e6 |X|) (+ d_logprior[bin] in float64 when d_logprior != NULL) is below the frame's maximum, then
+ *   divide by sqrt_tiny + |max(X)| under NumPy's lexicographic complex max.  d_keep / d_logprior: float64 [n_bins].
+ * b2l_plp_finish: in place on the pulse d_pulse [n_rows][n] (float32, or float64 when f64): clip below at 0, then
+ *   divide each row by its maximum (1 when below tiny); a non-finite value sets bit 2 of the status word. */
+typedef struct b2l_plp_desc {
+  int32_t n_bins, c128;
+  double sqrt_tiny;
+  const double* d_keep;
+  const double* d_logprior;
+} b2l_plp_desc;
+int b2l_plp_select(b2l_ctx* ctx, const b2l_plp_desc* desc, void* d_ftgram, int64_t n_frames);
+int b2l_plp_finish(b2l_ctx* ctx, void* d_pulse, int64_t n_rows, int64_t n, int32_t f64);
 
 /* ---- double-precision path: float64 audio / complex128 spectra ---------------------------------
  * librosa computes a float64 signal in float64 (dtype_r2c, core/spectrum.py:341; the window product :388 and the

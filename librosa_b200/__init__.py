@@ -6,7 +6,7 @@ window_sumsquare``, ``util.frame`` (and the small helpers around them) with libr
 shapes, dtypes, warnings and exceptions.  The arithmetic runs in hand-written CUDA kernels reached
 through a C ABI (``include/b2l.h``) with ctypes — no PyTorch, no Triton, no CPU fallback.
 """
-from . import core, decompose, effects, feature, filters, onset, util
+from . import beat, core, decompose, effects, feature, filters, onset, util
 from ._native import (
     Context,
     DeviceArray,
@@ -18,8 +18,8 @@ from ._native import (
     pinned_empty,
 )
 from .core.audio import resample, stream
-from .core.convert import (fft_frequencies, fourier_tempo_frequencies, hz_to_mel, hz_to_octs, mel_frequencies, mel_to_hz,
-                           tempo_frequencies)
+from .core.convert import (fft_frequencies, fourier_tempo_frequencies, frames_to_samples, frames_to_time, hz_to_mel,
+                           hz_to_octs, mel_frequencies, mel_to_hz, samples_to_time, tempo_frequencies)
 from .core.pitch import estimate_tuning, pyin, yin
 from .core.spectrum import (_spectrogram, amplitude_to_db, db_to_amplitude, db_to_power, griffinlim, istft,
                             pcen, phase_vocoder, power_to_db, reassigned_spectrogram, stft)
@@ -46,8 +46,8 @@ def to_device(arr, device=None):
 
 
 __all__ = [
-    "stream", "resample", "stft", "istft", "griffinlim", "power_to_db", "amplitude_to_db", "pcen", "phase_vocoder", "reassigned_spectrogram", "db_to_power", "db_to_amplitude", "_spectrogram", "feature", "filters", "util", "core", "onset", "decompose", "effects",
-    "hz_to_mel", "mel_to_hz", "hz_to_octs", "estimate_tuning", "yin", "pyin", "mel_frequencies", "fft_frequencies", "tempo_frequencies", "fourier_tempo_frequencies", "ParameterError", "LibrosaError",
+    "stream", "resample", "stft", "istft", "griffinlim", "power_to_db", "amplitude_to_db", "pcen", "phase_vocoder", "reassigned_spectrogram", "db_to_power", "db_to_amplitude", "_spectrogram", "feature", "filters", "util", "core", "onset", "beat", "decompose", "effects",
+    "hz_to_mel", "mel_to_hz", "hz_to_octs", "estimate_tuning", "yin", "pyin", "mel_frequencies", "fft_frequencies", "tempo_frequencies", "fourier_tempo_frequencies", "frames_to_samples", "frames_to_time", "samples_to_time", "ParameterError", "LibrosaError",
     "Context", "DeviceArray", "default_context", "device_count", "pinned_empty", "to_device", "device_copy",
     "NativeLibraryError", "UnsupportedOnGPU", "bind_host_to_device",
 ]

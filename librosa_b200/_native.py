@@ -138,6 +138,21 @@ class TempoDesc(C.Structure):
                 ("row_stride", C.c_int64), ("lag_stride", C.c_int64), ("frame_stride", C.c_int64)]
 
 
+class BeatDesc(C.Structure):
+    """struct b2l_beat_desc (include/b2l.h); the d_* fields are device pointers."""
+    _fields_ = [("n_fpb", C.c_int32), ("env_f64", C.c_int32), ("dp_f64", C.c_int32), ("trim", C.c_int32),
+                ("units", C.c_int32),
+                ("tightness", C.c_float), ("hop_length", C.c_int32), ("sr", C.c_double), ("d_fpb", C.c_void_p),
+                ("d_logfpb", C.c_void_p), ("d_woff", C.c_void_p), ("d_wtab", C.c_void_p), ("d_logd", C.c_void_p)]
+
+
+class PlpDesc(C.Structure):
+    """struct b2l_plp_desc (include/b2l.h); the d_* fields are device pointers."""
+    _fields_ = [("n_bins", C.c_int32), ("c128", C.c_int32), ("sqrt_tiny", C.c_double), ("d_keep", C.c_void_p),
+                ("d_logprior", C.c_void_p)]
+
+
+BEAT_FRAMES, BEAT_SAMPLES, BEAT_TIME = range(3)   # enum b2l_beat_units
 TG_NORM_NONE, TG_NORM_MAX, TG_NORM_MIN, TG_NORM_COUNT, TG_NORM_P = range(5)   # enum b2l_tempogram_norm
 N_STATS = 6
 STAT_CENTROID, STAT_BANDWIDTH, STAT_ROLLOFF, STAT_FLATNESS, STAT_RMS, STAT_TOTAL = range(6)
@@ -192,6 +207,7 @@ def _declare(lib):
         "b2l_mel_project": (C.c_int, [_vp, _vp, _vp, _i64, _i64, _vp]),
         "b2l_power_to_db": (C.c_int, [_vp, _vp, _i64, _i64, C.c_float, C.c_float, C.c_float, _vp]),
         "b2l_onset_from_spec": (C.c_int, [_vp, P(OnsetDesc), _vp, _i64, _i64, _i64, _vp]),
+        "b2l_onset_median_from_spec": (C.c_int, [_vp, P(OnsetDesc), _vp, _i64, _i64, _i64, _vp]),
         "b2l_pcen": (C.c_int, [_vp, P(PcenDesc), _vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp]),
         "b2l_resample_poly": (C.c_int, [_vp, _vp, _i64, _i64, _i64, _vp, C.c_int32, C.c_int32, C.c_int32, _i64, _i64, _i64,
                                         C.c_float, _vp]),
@@ -217,6 +233,10 @@ def _declare(lib):
         "b2l_viterbi": (C.c_int, [_vp, P(PyinDesc), _vp, _vp, _vp, _vp, _i64, _i64, _vp, _vp, _vp]),
         "b2l_tempogram": (C.c_int, [_vp, P(TempogramDesc), _vp, _i64, _i64, _vp, _vp]),
         "b2l_tempo": (C.c_int, [_vp, P(TempoDesc), _vp, _i64, _vp, _vp, _vp]),
+        "b2l_beat_track": (C.c_int, [_vp, P(BeatDesc), _vp, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp]),
+        "b2l_any_nonzero": (C.c_int, [_vp, _vp, _i64, C.c_int32, _vp]),
+        "b2l_plp_select": (C.c_int, [_vp, P(PlpDesc), _vp, _i64]),
+        "b2l_plp_finish": (C.c_int, [_vp, _vp, _i64, _i64, C.c_int32]),
         "b2l_stft_f64": (C.c_int, [_vp, _vp, _i64, _i64, _i64, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                    P(C.c_double), _vp]),
         "b2l_istft_f64": (C.c_int, [_vp, _vp, _i64, _i64, _i64, C.c_int32, C.c_int32, C.c_int32, P(C.c_double),

@@ -73,3 +73,19 @@ def tempo_frequencies(n_bins: int, *, hop_length: int = 512, sr: float = 22050):
 def fourier_tempo_frequencies(*, sr: float = 22050, win_length: int = 384, hop_length: int = 512):
     """BPM of each bin of a Fourier tempogram."""
     return fft_frequencies(sr=sr * 60 / float(hop_length), n_fft=win_length)
+
+
+def frames_to_samples(frames, *, hop_length: int = 512, n_fft=None):
+    """Sample index of each frame index (plus ``n_fft // 2`` when ``n_fft`` is given), as integers."""
+    offset = 0 if n_fft is None else int(n_fft // 2)
+    return (np.asanyarray(frames) * hop_length + offset).astype(int)[()]
+
+
+def samples_to_time(samples, *, sr: float = 22050):
+    """Time in seconds of each sample index."""
+    return np.asanyarray(samples)[()] / float(sr)
+
+
+def frames_to_time(frames, *, sr: float = 22050, hop_length: int = 512, n_fft=None):
+    """Time in seconds of each frame index: ``frames_to_samples`` then ``samples_to_time``."""
+    return samples_to_time(frames_to_samples(frames, hop_length=hop_length, n_fft=n_fft), sr=sr)

@@ -822,6 +822,45 @@ extern "C" int b2l_onset_from_spec(b2l_ctx* c, const b2l_onset_desc* d, const fl
   return launch(c, detrend_kernel, (unsigned)((rows + 127) / 128), 128, 0, d_out, rows, a.T);
 }
 
+extern "C" int b2l_onset_median_from_spec(b2l_ctx* c, const b2l_onset_desc* d, const float* d_S, int64_t n_clips,
+                                          int64_t n_rows, int64_t n_frames, float* d_out) {
+  if (!c || !d || !d_S || !d_out) return fail(B2L_ERR_INVALID, "NULL argument");
+  if (d->lag < 1) return fail(B2L_ERR_INVALID, "lag=%d must be a positive integer", d->lag);
+  if (d->max_size < 1) return fail(B2L_ERR_INVALID, "max_size=%d must be a positive integer", d->max_size);
+  if (d->pad_width < 0) return fail(B2L_ERR_INVALID, "negative pad_width");
+  if (d->n_channels < 1 || d->n_channels > 32) return fail(B2L_ERR_UNSUPPORTED, "1 to 32 onset channels");
+  if (n_clips <= 0 || n_rows <= 0 || n_frames <= 0) return B2L_OK;
+  if (n_clips > kMaxGridY || n_rows > 0x7fffffffLL || n_frames > 0x7fffffffLL)
+    return fail(B2L_ERR_UNSUPPORTED, "onset: batch too large");
+  OnsetArgs a;
+  memset(&a, 0, sizeof(a));
+  int widest = 0;
+  for (int i = 0; i <= d->n_channels; ++i) {
+    a.bounds[i] = d->bounds[i];
+    if (a.bounds[i] < 0 || a.bounds[i] > n_rows || (i > 0 && a.bounds[i] < a.bounds[i - 1]))
+      return fail(B2L_ERR_INVALID, "channel boundaries must be non-decreasing row indices");
+    if (i > 0) widest = std::max(widest, a.bounds[i] - a.bounds[i - 1]);
+  }
+  if (widest > kOnsetMedMaxRows)
+    return fail(B2L_ERR_UNSUPPORTED, "onset: median aggregation over a channel of %d rows; the GPU kernel takes up to %d",
+                widest, kOnsetMedMaxRows);
+  a.n_ch = d->n_channels;
+  a.lag = d->lag;
+  a.max_size = d->max_size;
+  a.pad_width = d->pad_width;
+  a.n_rows = (int)n_rows;
+  a.T = (int)n_frames;
+  int P = 32;
+  while (P < widest) P <<= 1;
+  const size_t smem = (size_t)kOnsetMedFrames * (P + 1) * sizeof(float);
+  DeviceGuard g(c->device);
+  const dim3 grid((unsigned)((n_frames + kOnsetMedFrames - 1) / kOnsetMedFrames), (unsigned)n_clips);
+  int rc = launch(c, onset_median_kernel, grid, 256, smem, d_S, a, P, d_out);
+  if (rc || !d->detrend) return rc;
+  const long long rows = (long long)n_clips * a.n_ch;
+  return launch(c, detrend_kernel, (unsigned)((rows + 127) / 128), 128, 0, d_out, rows, a.T);
+}
+
 extern "C" int b2l_pcen(b2l_ctx* c, const b2l_pcen_desc* d, const float* d_S, int64_t n_clips, int64_t n_rows,
                         int64_t n_frames, const float* d_zi, float* d_zf, float* d_scratch, float* d_out) {
   if (!c || !d || !d_S || !d_out) return fail(B2L_ERR_INVALID, "NULL argument");

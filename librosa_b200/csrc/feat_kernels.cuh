@@ -236,6 +236,84 @@ __global__ void onset_kernel(const float* __restrict__ S, OnsetArgs a, float* __
     oc[(long long)c * a.T] = live && m1 > m0 ? acc / (float)(m1 - m0) : (live ? __int_as_float(0x7fc00000) : 0.0f);
   }
 }
+// The same flux aggregated with np.median over each channel's rows (util.sync(..., aggregate=np.median)): for an
+// even row count the float32 mean of the two middle values, NaN when any flux of the column is NaN (np.maximum
+// keeps it).  A CTA takes kOnsetMedFrames frames of one clip and one channel at a time: the flux tile is staged
+// [frame][row] in shared memory (rows read coalesced along time), then one warp per frame bitonic-sorts its
+// column of P = next power of two >= rows (padded with +inf) and reads the middle.  Channels up to
+// kOnsetMedMaxRows rows (the entry point refuses more).
+constexpr int kOnsetMedFrames = 16;
+constexpr int kOnsetMedMaxRows = 512;
+__global__ void onset_median_kernel(const float* __restrict__ S, OnsetArgs a, int P, float* __restrict__ out) {
+  extern __shared__ float s_col[];   // [kOnsetMedFrames][P + 1]
+  const int t0 = blockIdx.x * kOnsetMedFrames;
+  const long long clip = blockIdx.y;
+  const float* Sc = S + clip * (long long)a.n_rows * a.T;
+  float* oc = out + clip * (long long)a.n_ch * a.T;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, n_warps = blockDim.x >> 5;
+  const int f_ld = threadIdx.x % kOnsetMedFrames, r_ld = threadIdx.x / kOnsetMedFrames;
+  const int r_step = blockDim.x / kOnsetMedFrames;
+  for (int c = 0; c < a.n_ch; ++c) {
+    const int m0 = a.bounds[c], R = a.bounds[c + 1] - m0;
+    {
+      const int t = t0 + f_ld, tp = t - a.pad_width;
+      const bool live = t < a.T && tp >= 0 && tp + a.lag < a.T;
+      for (int r = r_ld; r < P; r += r_step) {
+        float v = INFINITY;
+        if (r < R && live) {
+          const int m = m0 + r;
+          float ref;
+          if (a.max_size == 1) {
+            ref = Sc[(long long)m * a.T + tp];
+          } else {
+            ref = -INFINITY;
+            const int lo = m - a.max_size / 2;
+            for (int j = 0; j < a.max_size; ++j) {
+              int mm = lo + j;
+              while (mm < 0 || mm >= a.n_rows) mm = mm < 0 ? -mm - 1 : 2 * a.n_rows - mm - 1;
+              ref = fmaxf(ref, Sc[(long long)mm * a.T + tp]);
+            }
+          }
+          const float d = __fsub_rn(Sc[(long long)m * a.T + tp + a.lag], ref);
+          v = d != d ? d : fmaxf(0.0f, d);
+        }
+        s_col[f_ld * (P + 1) + r] = v;
+      }
+    }
+    __syncthreads();
+    for (int f = warp; f < kOnsetMedFrames; f += n_warps) {
+      const int t = t0 + f, tp = t - a.pad_width;
+      if (t >= a.T) continue;
+      float* col = s_col + f * (P + 1);
+      bool nan = false;
+      for (int r = lane; r < R; r += 32) nan |= col[r] != col[r];
+      nan = __any_sync(0xffffffffu, nan);
+      const bool live = tp >= 0 && tp + a.lag < a.T;
+      if (live && R > 0 && !nan) {
+        for (int k = 2; k <= P; k <<= 1)
+          for (int j = k >> 1; j > 0; j >>= 1) {
+            for (int i = lane; i < P; i += 32) {
+              const int p = i ^ j;
+              if (p > i) {
+                const float x = col[i], y = col[p];
+                if (((i & k) == 0) == (x > y)) { col[i] = y; col[p] = x; }
+              }
+            }
+            __syncwarp();
+          }
+      }
+      if (lane == 0) {
+        float v = 0.0f;
+        if (live)
+          v = R == 0 || nan ? __int_as_float(0x7fc00000)
+                            : (R & 1 ? col[R >> 1] : __fmul_rn(__fadd_rn(col[(R >> 1) - 1], col[R >> 1]), 0.5f));
+        oc[(long long)c * a.T + t] = v;
+      }
+    }
+    __syncthreads();
+  }
+}
+
 // detrend: scipy.signal.lfilter([1, -1], [1, -0.99]) along time (direct form II transposed), one thread per row
 __global__ void detrend_kernel(float* __restrict__ x, long long n_rows, int T) {
   const long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x;

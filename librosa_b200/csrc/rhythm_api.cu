@@ -1,5 +1,6 @@
 // rhythm_api.cu — C ABI of the rhythm features (rhythm_kernels.cuh): librosa.feature.tempogram and the tempo
-// estimate on top of it (librosa/feature/rhythm.py:38-470).  The only unit that includes rhythm_kernels.cuh.
+// estimate on top of it (librosa/feature/rhythm.py:38-470), and librosa.beat.beat_track's tracker
+// (beat_kernels.cuh, librosa/beat.py:510-742).  The only unit that includes rhythm_kernels.cuh and beat_kernels.cuh.
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <string.h>
@@ -9,6 +10,7 @@
 
 #include "internal.h"
 #include "rhythm_kernels.cuh"
+#include "beat_kernels.cuh"
 
 using namespace b2l;
 
@@ -93,4 +95,96 @@ extern "C" int b2l_tempo(b2l_ctx* c, const b2l_tempo_desc* d, const void* d_tg, 
   if (blocks > 0x7fffffffLL) return fail(B2L_ERR_UNSUPPORTED, "tempo: too many frames in one call");
   auto fn = d->tg_f64 ? tempo_frames_kernel<double> : tempo_frames_kernel<float>;
   return launch(c, fn, (unsigned)blocks, 256, 0, a);
+}
+
+extern "C" int b2l_beat_track(b2l_ctx* c, const b2l_beat_desc* d, const void* d_env, int64_t n_clips, int64_t n,
+                              void* d_localscore, void* d_cumscore, int32_t* d_backlink, uint8_t* d_beats,
+                              void* d_sparse, int64_t* d_count) {
+  if (!c || !d) return fail(B2L_ERR_INVALID, "NULL argument");
+  if (n_clips < 0 || n < 0) return fail(B2L_ERR_INVALID, "bad envelope geometry");
+  if (d->n_fpb != 1 && d->n_fpb != n) return fail(B2L_ERR_INVALID, "n_fpb=%d must be 1 or n=%lld", d->n_fpb, (long long)n);
+  if (d->units < B2L_BEAT_FRAMES || d->units > B2L_BEAT_TIME) return fail(B2L_ERR_INVALID, "unknown units %d", d->units);
+  if (d_sparse && (n_clips != 1 || !d_count)) return fail(B2L_ERR_INVALID, "a sparse beat list needs one clip and a count");
+  if (n_clips == 0 || n == 0) {
+    if (d_count) CUDA_TRY(cudaMemsetAsync(d_count, 0, sizeof(int64_t), c->stream));
+    return B2L_OK;
+  }
+  if (n > 0x7fffffffLL) return fail(B2L_ERR_UNSUPPORTED, "beat_track: envelopes longer than 2^31-1 frames");
+  if (n_clips > 0x7fffffffLL) return fail(B2L_ERR_UNSUPPORTED, "beat_track: more than 2^31-1 clips in one call");
+  if (!d_env || !d_beats || !d->d_fpb || !d->d_logfpb || !d->d_woff || !d->d_wtab || !d->d_logd)
+    return fail(B2L_ERR_INVALID, "NULL device pointer");
+  DeviceGuard g(c->device);
+  const size_t elem = d->env_f64 ? sizeof(double) : sizeof(float);
+  const size_t row = (size_t)n_clips * (size_t)n;
+  Temp t_ls(c->stream), t_cum(c->stream), t_back(c->stream), t_scratch(c->stream);
+  if (!d_localscore) { CUDA_TRY(t_ls.alloc(row * elem)); d_localscore = t_ls.p; }
+  if (!d_cumscore) { CUDA_TRY(t_cum.alloc(row * (d->dp_f64 ? sizeof(double) : sizeof(float)))); d_cumscore = t_cum.p; }
+  if (!d_backlink) { CUDA_TRY(t_back.alloc(row * sizeof(int32_t))); d_backlink = (int32_t*)t_back.p; }
+  CUDA_TRY(t_scratch.alloc(row * sizeof(double)));
+  b2l_beat::BeatArgs a;
+  memset(&a, 0, sizeof(a));
+  a.env = d_env;
+  a.n = (int)n;
+  a.tv = d->n_fpb != 1;
+  a.fpb = d->d_fpb;
+  a.logfpb = d->d_logfpb;
+  a.woff = d->d_woff;
+  a.wtab = d->d_wtab;
+  a.logd = d->d_logd;
+  a.tightness = (double)d->tightness;
+  a.trim = d->trim;
+  a.localscore = d_localscore;
+  a.cumscore = d_cumscore;
+  a.backlink = d_backlink;
+  a.scratch = t_scratch.p;
+  a.beats = d_beats;
+  a.units = d->units;
+  a.sparse = d_sparse;
+  a.count = (long long*)d_count;
+  a.hop_length = d->hop_length;
+  a.sr = d->sr;
+  if (d->env_f64 && !d->dp_f64) return fail(B2L_ERR_INVALID, "a float64 envelope needs the float64 DP");
+  auto fn = d->env_f64 ? b2l_beat::beat_track_kernel<double, double>
+                       : d->dp_f64 ? b2l_beat::beat_track_kernel<float, double> : b2l_beat::beat_track_kernel<float, float>;
+  return launch(c, fn, (unsigned)n_clips, 256, 0, a);
+}
+
+extern "C" int b2l_any_nonzero(b2l_ctx* c, const void* d_x, int64_t n, int32_t f64, int32_t* d_flag) {
+  if (!c || !d_flag) return fail(B2L_ERR_INVALID, "NULL argument");
+  if (n < 0) return fail(B2L_ERR_INVALID, "negative length");
+  DeviceGuard g(c->device);
+  CUDA_TRY(cudaMemsetAsync(d_flag, 0, sizeof(int32_t), c->stream));
+  if (n == 0) return B2L_OK;
+  if (!d_x) return fail(B2L_ERR_INVALID, "NULL device pointer");
+  const unsigned blocks = (unsigned)grid_stride_blocks(n, 256, 4LL * c->sm_count);
+  if (f64) return launch(c, b2l_beat::any_nonzero_kernel<double>, blocks, 256, 0, (const double*)d_x, (long long)n, d_flag);
+  return launch(c, b2l_beat::any_nonzero_kernel<float>, blocks, 256, 0, (const float*)d_x, (long long)n, d_flag);
+}
+
+extern "C" int b2l_plp_select(b2l_ctx* c, const b2l_plp_desc* d, void* d_ftgram, int64_t n_frames) {
+  if (!c || !d) return fail(B2L_ERR_INVALID, "NULL argument");
+  if (d->n_bins < 1 || n_frames < 0) return fail(B2L_ERR_INVALID, "bad Fourier tempogram geometry");
+  if (n_frames == 0) return B2L_OK;
+  if (!d_ftgram || !d->d_keep) return fail(B2L_ERR_INVALID, "NULL device pointer");
+  const long long blocks = (n_frames + 7) / 8;   // 8 warps per CTA, one per frame
+  if (blocks > 0x7fffffffLL) return fail(B2L_ERR_UNSUPPORTED, "plp: too many frames in one call");
+  DeviceGuard g(c->device);
+  if (d->c128)
+    return launch(c, b2l_beat::plp_select_kernel<double2>, (unsigned)blocks, 256, 0, (double2*)d_ftgram,
+                  (long long)n_frames, d->n_bins, d->d_keep, d->d_logprior, d->sqrt_tiny);
+  return launch(c, b2l_beat::plp_select_kernel<float2>, (unsigned)blocks, 256, 0, (float2*)d_ftgram,
+                (long long)n_frames, d->n_bins, d->d_keep, d->d_logprior, d->sqrt_tiny);
+}
+
+extern "C" int b2l_plp_finish(b2l_ctx* c, void* d_pulse, int64_t n_rows, int64_t n, int32_t f64) {
+  if (!c) return fail(B2L_ERR_INVALID, "NULL argument");
+  if (n_rows < 0 || n < 0) return fail(B2L_ERR_INVALID, "bad pulse geometry");
+  if (n_rows == 0 || n == 0) return B2L_OK;
+  if (n_rows > 0x7fffffffLL || n > 0x7fffffffLL) return fail(B2L_ERR_UNSUPPORTED, "plp: batch too large");
+  if (!d_pulse) return fail(B2L_ERR_INVALID, "NULL device pointer");
+  DeviceGuard g(c->device);
+  if (f64) return launch(c, b2l_beat::plp_finish_kernel<double>, (unsigned)n_rows, 256, 0, (double*)d_pulse, (int)n,
+                         c->d_status);
+  return launch(c, b2l_beat::plp_finish_kernel<float>, (unsigned)n_rows, 256, 0, (float*)d_pulse, (int)n,
+                c->d_status);
 }

@@ -76,15 +76,16 @@ class _Envelope:
 
     ``y`` runs onset_strength on the device: a host signal is uploaded once and checked like util.valid_audio,
     the envelope never leaves the GPU.  A host envelope is uploaded as it is.  The status word is cleared for this
-    call's verdict (``verdict``); ``on_device``: the caller passed device data and gets a DeviceArray back."""
+    call's verdict (``verdict``); ``on_device``: the caller passed device data and gets a DeviceArray back.
+    ``aggregate`` is onset_strength's (beat tracking uses np.median)."""
 
-    def __init__(self, y, sr, onset_envelope, hop_length):
+    def __init__(self, y, sr, onset_envelope, hop_length, aggregate=None):
         from ..onset import onset_strength
 
         self.audio = None
         if onset_envelope is None:
             self.audio = pl.StagedInput(y)
-            self.dev = onset_strength(y=self.audio.dev, sr=sr, hop_length=hop_length)
+            self.dev = onset_strength(y=self.audio.dev, sr=sr, hop_length=hop_length, aggregate=aggregate)
             self.audio.scan_all()
             self.staged = self.audio
         else:

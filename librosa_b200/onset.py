@@ -17,6 +17,8 @@ _vp = C.c_void_p
 
 __all__ = ["onset_strength", "onset_strength_multi"]
 
+MAX_MEDIAN_ROWS = 512   # csrc/feat_kernels.cuh kOnsetMedMaxRows: rows of one channel under np.median
+
 
 def _edges(channels, n_rows: int, pad: bool):
     """Row boundaries of the aggregation channels (util.sync -> index_to_slice -> fix_frames)."""
@@ -40,8 +42,9 @@ def onset_strength_multi(*, y=None, sr: float = 22050, S=None, n_fft: int = 2048
                          max_size: int = 1, ref=None, detrend: bool = False, center: bool = True, feature=None,
                          aggregate=None, channels=None, **kwargs):
     """Spectral-flux onset strength over sub-bands, shape ``(..., n_channels, frames)``; same contract as
-    ``librosa.onset.onset_strength_multi`` for the default ``feature`` (mel) and mean aggregation (or
-    ``aggregate=False`` for the per-bin flux)."""
+    ``librosa.onset.onset_strength_multi`` for the default ``feature`` (mel) and mean or median aggregation
+    (``np.mean`` / ``np.median``; channels of up to 512 rows under the median), or ``aggregate=False`` for the
+    per-bin flux."""
     from .feature.spectral import melspectrogram
 
     if feature is not None and feature is not melspectrogram:
@@ -50,14 +53,21 @@ def onset_strength_multi(*, y=None, sr: float = 22050, S=None, n_fft: int = 2048
         kwargs.setdefault("fmax", 0.5 * sr)
     if aggregate is None:
         aggregate = np.mean
-    if callable(aggregate) and aggregate is not np.mean:
-        raise nat.UnsupportedOnGPU("only mean aggregation (or aggregate=False) is computed on the GPU")
+    if callable(aggregate) and aggregate is not np.mean and aggregate is not np.median:
+        raise nat.UnsupportedOnGPU("only mean or median aggregation (or aggregate=False) is computed on the GPU")
     if not is_positive_int(lag):
         raise ParameterError(f"lag={lag} must be a positive integer")
     if not is_positive_int(max_size):
         raise ParameterError(f"max_size={max_size} must be a positive integer")
     if ref is not None:
         raise nat.UnsupportedOnGPU("a caller-supplied reference spectrum is not supported on the GPU")
+    if aggregate is np.median:   # the kernel's channel limit, known from the shapes before any device work
+        n_rows = kwargs.get("n_mels", 128) if S is None else (S.shape[-2] if np.ndim(S) >= 2 else 1)
+        edges = _edges([slice(None)] if channels is None else list(channels), n_rows, channels is None)
+        widest = max((b - a for a, b in zip(edges[:-1], edges[1:])), default=0)
+        if widest > MAX_MEDIAN_ROWS:
+            raise nat.UnsupportedOnGPU(f"median onset aggregation over a channel of {widest} rows: the GPU kernel takes "
+                                       f"up to {MAX_MEDIAN_ROWS} (no CPU fallback)")
 
     staged = None
     if S is None:
@@ -99,8 +109,8 @@ def onset_strength_multi(*, y=None, sr: float = 22050, S=None, n_fft: int = 2048
         desc.n_channels = 0
         n_out = rows
     out = nat.DeviceArray.empty(ctx, tuple(lead) + (n_out, T), np.float32)
-    nat.check(nat.lib().b2l_onset_from_spec(ctx.handle, C.byref(desc), _vp(Sd.ptr), pl.clip_count(lead), rows, T,
-                                            _vp(out.ptr)))
+    entry = nat.lib().b2l_onset_median_from_spec if aggregate is np.median else nat.lib().b2l_onset_from_spec
+    nat.check(entry(ctx.handle, C.byref(desc), _vp(Sd.ptr), pl.clip_count(lead), rows, T, _vp(out.ptr)))
     if staged is not None or not on_device:
         Sd.free()
     if detrend:   # scipy.signal.lfilter with float64 coefficients returns float64

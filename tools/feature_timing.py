@@ -1,7 +1,8 @@
 """Device-resident timings of the frame-wise features (SURVEY 8f rank 2) on a cfg-2 shaped batch, next to the
 oracle (CPU, one process) on a small sample.  CUDA events around `reps` calls after warm-up.  The pitch trackers
 run with fmin C2, fmax C7 and their other defaults (frame_length 2048, hop 512); their oracle sample is one clip.
-The rhythm features take the device onset envelope of the batch (431 frames per 10 s clip) and their defaults;
+The rhythm features and beat_track (dense output) take the device onset envelope of the batch (431 frames per 10 s
+clip) and their defaults;
 ``rhythm_bounds`` holds the tempogram kernel's least time on the card (output bytes at 3.35 TB/s, two packed FP64
 transforms per frame at 34 TFLOP/s), and ``card`` the GPU's name and power limit read in the same run.
 
@@ -74,6 +75,11 @@ FEATURES = {
     "tempo(onset_envelope)": (lambda: lb.feature.tempo(onset_envelope=oenv),
                               lambda y: RO.tempo(onset_envelope=oenv_host[:len(y)])),
     "tempo(tg, aggregate=None)": (lambda: lb.feature.tempo(tg=tg_dev, aggregate=None), None),
+    "onset_strength(aggregate=np.median)": (lambda: lb.onset.onset_strength(y=dev, sr=sr, aggregate=np.median), None),
+    "beat_track(onset_envelope)": (lambda: lb.beat.beat_track(onset_envelope=oenv, sparse=False), None),
+    "beat_track(onset_envelope, bpm=120)": (lambda: lb.beat.beat_track(onset_envelope=oenv, bpm=120.0, sparse=False),
+                                            None),
+    "plp(onset_envelope)": (lambda: lb.beat.plp(onset_envelope=oenv), None),
 }
 CPU_SAMPLE = {"yin(C2-C7)": 1, "pyin(C2-C7)": 1}   # clips in the oracle sample (default 8)
 

@@ -2,7 +2,7 @@
 (tests/feature_cases.py) and tests/golden/reference_pins_v1.npz (tests/reference_pins.py) by running the
 cases through the UNMODIFIED reference; ``--pitch`` writes only tests/golden/pitch_v1.npz (tests/pitch_cases.py)
 and leaves the other fixtures as they are; ``--rhythm`` likewise writes only tests/golden/rhythm_v1.npz
-(tests/rhythm_cases.py).
+(tests/rhythm_cases.py), and ``--beat`` only tests/golden/beat_v1.npz (tests/beat_cases.py).
 
 Needs a checkout of the reference (see tools/ref_shim.py); the tests only read the stored fixtures.  Also
 stores a handful of constant tables (mel bases, window sum-square, mel-scale known answers) produced by the
@@ -11,6 +11,7 @@ reference.
     python tools/make_golden.py
     python tools/make_golden.py --pitch
     python tools/make_golden.py --rhythm
+    python tools/make_golden.py --beat
 """
 from __future__ import annotations
 
@@ -139,10 +140,66 @@ def write_rhythm():
     print("wrote", path, os.path.getsize(path), "bytes")
 
 
+def write_beat():
+    """tests/golden/beat_v1.npz: per case of tests/beat_cases.py, beat_track's ``bpm`` and ``beats``, plp's ``pulse``,
+    beat_track(y=) on click trains, and the tracker stages (the reference module's own private functions) for that bpm: ``localscore``, ``cumscore``, ``backlink``
+    and ``tail``.  The batch with an all-zero clip has no ``beats``: the reference's trim loop runs past the end of
+    that clip's array."""
+    import beat_cases as BC
+
+    ref = ref_shim.load_reference()
+    rb = ref.beat
+    stage = {name: getattr(rb, "__" + name) for name in ("normalize_onsets", "beat_local_score", "beat_track_dp",
+                                                           "last_beat")}
+    store = {}
+    for case in BC.BEAT_CASES:
+        name, kw = case["name"], BC.kwargs(case)
+        x = BC.make_input(case)
+        with warnings.catch_warnings():
+            warnings.simplefilter("ignore")
+            bpm = kw["bpm"]
+            if bpm is None and BC.has_stages(case):
+                bpm = ref.feature.tempo(onset_envelope=x, sr=kw["sr"], hop_length=kw["hop_length"],
+                                        prior=kw.get("prior"))
+            if case["env"][0] != "zero_clip":
+                got_bpm, beats = BC.run(ref, case)
+                store[name + "/beats"] = np.asarray(beats)
+                store[name + "/bpm"] = np.asarray(got_bpm, dtype=np.float64)
+            else:
+                store[name + "/bpm"] = np.asarray(bpm, dtype=np.float64)
+            if BC.has_stages(case):
+                _bpm = np.atleast_1d(bpm)
+                bpm_exp = ref.util.expand_to(_bpm, ndim=x.ndim, axes=range(_bpm.ndim))
+                fpb = np.round(float(kw["sr"]) / kw["hop_length"] * 60.0 / bpm_exp)
+                ls = np.empty_like(x)
+                stage["beat_local_score"](stage["normalize_onsets"](x), fpb, ls)
+                back, cum = stage["beat_track_dp"](ls, fpb, BC.stage_kwargs(case)["tightness"])
+                store[name + "/localscore"] = ls
+                store[name + "/cumscore"] = cum
+                store[name + "/backlink"] = back
+                store[name + "/tail"] = np.asarray(stage["last_beat"](cum), dtype=np.int64)
+        for key in [k for k in store if k.startswith(name + "/")]:
+            print(f"{key:48s} {store[key].shape} {store[key].dtype}")
+    for case in BC.PLP_CASES:
+        with warnings.catch_warnings():
+            warnings.simplefilter("ignore")
+            store[case["name"] + "/pulse"] = np.ascontiguousarray(BC.run_plp(ref, case))
+    for name, bpm in BC.Y_CASES.items():
+        got_bpm, beats = ref.beat.beat_track(y=BC.clicks_audio(bpm), sr=BC.SR, hop_length=BC.HOP)
+        store[name + "/bpm"] = np.asarray(got_bpm, dtype=np.float64)
+        store[name + "/beats"] = np.asarray(beats)
+        print(name, got_bpm, beats)
+    path = os.path.join(ROOT, "tests", "golden", "beat_v1.npz")
+    np.savez_compressed(path, **store)
+    print("wrote", path, os.path.getsize(path), "bytes")
+
+
 if __name__ == "__main__":
     if "--pitch" in sys.argv[1:]:
         write_pitch()
     elif "--rhythm" in sys.argv[1:]:
         write_rhythm()
+    elif "--beat" in sys.argv[1:]:
+        write_beat()
     else:
         main()
