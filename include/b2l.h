@@ -461,6 +461,39 @@ typedef struct b2l_plp_desc {
 int b2l_plp_select(b2l_ctx* ctx, const b2l_plp_desc* desc, void* d_ftgram, int64_t n_frames);
 int b2l_plp_finish(b2l_ctx* ctx, void* d_pulse, int64_t n_rows, int64_t n, int32_t f64);
 
+/* ---- onset detection: librosa.onset.onset_detect, util.peak_pick and onset.onset_backtrack (onset.py:31-214,
+ *      :370-441, util/utils.py:1188-1496) ----------------------------------------------------------------------------
+ * b2l_onset_normalize: one launch over d_x [n_rows][n] (float32, or float64 when f64).  With d_out != NULL each row
+ *   is written there as (x - min x) / (max(x - min x) + tiny), NaN propagating, every step in the envelope's type.
+ *   d_flags [2] is cleared first; bit 0 of d_flags[0] is set when an element of the (normalised) batch is not zero,
+ *   bit 1 when one is not finite — onset_detect's verdict over the whole call.
+ * b2l_peak_pick: one launch, one CTA per row of d_x.  The picks of util.peak_pick(method) with integer windows
+ *   (pre_* >= 0, post_* >= 1, wait >= 0) and float64 delta: the greedy picker takes a frame when it equals the
+ *   maximum of its window (NaN: never) and is >= the window mean + delta (a left-to-right sum in the data's type,
+ *   divided by the count in float64), then skips `wait` frames; the dynamic-programming pickers run numba's
+ *   sequential cumsum and backward DP (dp_count maximises the number of picks, dp_value their sum).  With d_flags
+ *   (from b2l_onset_normalize) every row is all-False unless the verdict is "nonzero and finite".  Writes d_dense
+ *   [n_rows][n] (1 at a pick) when not NULL and, with d_sparse (one row only), the picks in ascending order
+ *   converted to `units` (as b2l_beat_track) and their number to d_count.
+ * b2l_onset_backtrack: one launch.  Each of the first *d_count (NULL: n_events) int64 frames of d_events is replaced
+ *   by the last local minimum of d_energy [n] at or before it (e[i] <= e[i-1] and e[i] < e[i+1]; frame 0 always
+ *   counts; frames past n - 1 take the last), converted to `units`, in d_out.  A negative event sets bit 3 of the
+ *   status word and writes nothing. */
+enum b2l_peak_method { B2L_PEAK_GREEDY = 0, B2L_PEAK_DP_COUNT = 1, B2L_PEAK_DP_VALUE = 2 };
+typedef struct b2l_peak_desc {
+  int64_t pre_max, post_max, pre_avg, post_avg, wait;
+  double delta;
+  int32_t method, f64, units, hop_length;
+  double sr;
+} b2l_peak_desc;
+int b2l_onset_normalize(b2l_ctx* ctx, const void* d_x, int64_t n_rows, int64_t n, int32_t f64, double tiny,
+                        void* d_out, int64_t* d_flags);
+int b2l_peak_pick(b2l_ctx* ctx, const b2l_peak_desc* desc, const void* d_x, int64_t n_rows, int64_t n,
+                  const int64_t* d_flags, uint8_t* d_dense, void* d_sparse, int64_t* d_count);
+int b2l_onset_backtrack(b2l_ctx* ctx, const void* d_energy, int64_t n, int32_t f64, const int64_t* d_events,
+                        int64_t n_events, const int64_t* d_count, int32_t units, int32_t hop_length, double sr,
+                        void* d_out);
+
 /* ---- double-precision path: float64 audio / complex128 spectra ---------------------------------
  * librosa computes a float64 signal in float64 (dtype_r2c, core/spectrum.py:341; the window product :388 and the
  * irfft :598 follow the input's precision; the mel einsum feature/spectral.py:2160 and scipy.fft.dct :2005

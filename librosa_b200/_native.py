@@ -152,7 +152,15 @@ class PlpDesc(C.Structure):
                 ("d_logprior", C.c_void_p)]
 
 
+class PeakDesc(C.Structure):
+    """struct b2l_peak_desc (include/b2l.h)."""
+    _fields_ = [("pre_max", C.c_int64), ("post_max", C.c_int64), ("pre_avg", C.c_int64), ("post_avg", C.c_int64),
+                ("wait", C.c_int64), ("delta", C.c_double), ("method", C.c_int32), ("f64", C.c_int32),
+                ("units", C.c_int32), ("hop_length", C.c_int32), ("sr", C.c_double)]
+
+
 BEAT_FRAMES, BEAT_SAMPLES, BEAT_TIME = range(3)   # enum b2l_beat_units
+PEAK_GREEDY, PEAK_DP_COUNT, PEAK_DP_VALUE = range(3)   # enum b2l_peak_method
 TG_NORM_NONE, TG_NORM_MAX, TG_NORM_MIN, TG_NORM_COUNT, TG_NORM_P = range(5)   # enum b2l_tempogram_norm
 N_STATS = 6
 STAT_CENTROID, STAT_BANDWIDTH, STAT_ROLLOFF, STAT_FLATNESS, STAT_RMS, STAT_TOTAL = range(6)
@@ -237,6 +245,10 @@ def _declare(lib):
         "b2l_any_nonzero": (C.c_int, [_vp, _vp, _i64, C.c_int32, _vp]),
         "b2l_plp_select": (C.c_int, [_vp, P(PlpDesc), _vp, _i64]),
         "b2l_plp_finish": (C.c_int, [_vp, _vp, _i64, _i64, C.c_int32]),
+        "b2l_onset_normalize": (C.c_int, [_vp, _vp, _i64, _i64, C.c_int32, C.c_double, _vp, _vp]),
+        "b2l_peak_pick": (C.c_int, [_vp, P(PeakDesc), _vp, _i64, _i64, _vp, _vp, _vp, _vp]),
+        "b2l_onset_backtrack": (C.c_int, [_vp, _vp, _i64, C.c_int32, _vp, _i64, _vp, C.c_int32, C.c_int32, C.c_double,
+                                          _vp]),
         "b2l_stft_f64": (C.c_int, [_vp, _vp, _i64, _i64, _i64, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                    P(C.c_double), _vp]),
         "b2l_istft_f64": (C.c_int, [_vp, _vp, _i64, _i64, _i64, C.c_int32, C.c_int32, C.c_int32, P(C.c_double),

@@ -1,6 +1,7 @@
 // rhythm_api.cu — C ABI of the rhythm features (rhythm_kernels.cuh): librosa.feature.tempogram and the tempo
 // estimate on top of it (librosa/feature/rhythm.py:38-470), and librosa.beat.beat_track's tracker
-// (beat_kernels.cuh, librosa/beat.py:510-742).  The only unit that includes rhythm_kernels.cuh and beat_kernels.cuh.
+// (beat_kernels.cuh, librosa/beat.py:510-742), and librosa.onset.onset_detect's normaliser, peak picker and backtracker
+// (onset_kernels.cuh).  The only unit that includes rhythm_kernels.cuh, beat_kernels.cuh and onset_kernels.cuh.
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <string.h>
@@ -11,6 +12,7 @@
 #include "internal.h"
 #include "rhythm_kernels.cuh"
 #include "beat_kernels.cuh"
+#include "onset_kernels.cuh"
 
 using namespace b2l;
 
@@ -187,4 +189,93 @@ extern "C" int b2l_plp_finish(b2l_ctx* c, void* d_pulse, int64_t n_rows, int64_t
                          c->d_status);
   return launch(c, b2l_beat::plp_finish_kernel<float>, (unsigned)n_rows, 256, 0, (float*)d_pulse, (int)n,
                 c->d_status);
+}
+
+extern "C" int b2l_onset_normalize(b2l_ctx* c, const void* d_x, int64_t n_rows, int64_t n, int32_t f64, double tiny,
+                                   void* d_out, int64_t* d_flags) {
+  if (!c || !d_flags) return fail(B2L_ERR_INVALID, "NULL argument");
+  if (n_rows < 0 || n < 0) return fail(B2L_ERR_INVALID, "bad envelope geometry");
+  if (n > 0x7fffffffLL) return fail(B2L_ERR_UNSUPPORTED, "onset_detect: envelopes of 2^31 frames or more");
+  if (n_rows > 0x7fffffffLL) return fail(B2L_ERR_UNSUPPORTED, "onset_detect: more than 2^31-1 rows in one call");
+  DeviceGuard g(c->device);
+  CUDA_TRY(cudaMemsetAsync(d_flags, 0, 2 * sizeof(int64_t), c->stream));
+  if (n_rows == 0 || n == 0) return B2L_OK;
+  if (!d_x) return fail(B2L_ERR_INVALID, "NULL device pointer");
+  long long* flags = (long long*)d_flags;
+  if (f64)
+    return launch(c, b2l_onset::onset_normalize_kernel<double>, (unsigned)n_rows, 256, 0, (const double*)d_x, (int)n,
+                  tiny, (double*)d_out, flags);
+  return launch(c, b2l_onset::onset_normalize_kernel<float>, (unsigned)n_rows, 256, 0, (const float*)d_x, (int)n,
+                (float)tiny, (float*)d_out, flags);
+}
+
+extern "C" int b2l_peak_pick(b2l_ctx* c, const b2l_peak_desc* d, const void* d_x, int64_t n_rows, int64_t n,
+                             const int64_t* d_flags, uint8_t* d_dense, void* d_sparse, int64_t* d_count) {
+  if (!c || !d) return fail(B2L_ERR_INVALID, "NULL argument");
+  if (n_rows < 0 || n < 0) return fail(B2L_ERR_INVALID, "bad envelope geometry");
+  if (d->pre_max < 0 || d->pre_avg < 0 || d->wait < 0 || d->post_max < 1 || d->post_avg < 1)
+    return fail(B2L_ERR_INVALID, "peak_pick: window lengths out of range");
+  if (d->method < B2L_PEAK_GREEDY || d->method > B2L_PEAK_DP_VALUE) return fail(B2L_ERR_INVALID, "unknown method %d", d->method);
+  if (d->units < B2L_BEAT_FRAMES || d->units > B2L_BEAT_TIME) return fail(B2L_ERR_INVALID, "unknown units %d", d->units);
+  if (d_sparse && (n_rows != 1 || !d_count)) return fail(B2L_ERR_INVALID, "a sparse peak list needs one row and a count");
+  if (n > 0x7fffffffLL) return fail(B2L_ERR_UNSUPPORTED, "peak_pick: rows of 2^31 frames or more");
+  if (n_rows > 0x7fffffffLL) return fail(B2L_ERR_UNSUPPORTED, "peak_pick: more than 2^31-1 rows in one call");
+  DeviceGuard g(c->device);
+  if (n_rows == 0 || n == 0) {
+    if (d_count) CUDA_TRY(cudaMemsetAsync(d_count, 0, sizeof(int64_t), c->stream));
+    return B2L_OK;
+  }
+  if (!d_x) return fail(B2L_ERR_INVALID, "NULL device pointer");
+  b2l_onset::PeakArgs a;
+  memset(&a, 0, sizeof(a));
+  auto clamp = [n](int64_t v) { return (long long)std::min<int64_t>(v, n); };   // longer windows clip the same way
+  a.x = d_x;
+  a.n = (int)n;
+  a.pre_max = clamp(d->pre_max);
+  a.post_max = clamp(d->post_max);
+  a.pre_avg = clamp(d->pre_avg);
+  a.post_avg = clamp(d->post_avg);
+  a.wait = clamp(d->wait);
+  a.delta = d->delta;
+  a.flags = (const long long*)d_flags;
+  a.dense = d_dense;
+  a.sparse = d_sparse;
+  a.count = (long long*)d_count;
+  a.units = d->units;
+  a.hop_length = d->hop_length;
+  a.sr = d->sr;
+  Temp t_scratch(c->stream), t_marks(c->stream);
+  if (d->method != B2L_PEAK_GREEDY) {
+    CUDA_TRY(t_scratch.alloc((size_t)n_rows * 2 * (size_t)(n + 1) * sizeof(double)));
+    CUDA_TRY(t_marks.alloc((size_t)n_rows * (size_t)n));
+    a.scratch = (double*)t_scratch.p;
+    a.marks = (uint8_t*)t_marks.p;
+  }
+  using namespace b2l_onset;
+  void (*fn)(PeakArgs);
+  if (d->method == B2L_PEAK_GREEDY) fn = d->f64 ? peak_pick_kernel<double, kGreedy> : peak_pick_kernel<float, kGreedy>;
+  else if (d->method == B2L_PEAK_DP_COUNT) fn = d->f64 ? peak_pick_kernel<double, kDpCount> : peak_pick_kernel<float, kDpCount>;
+  else fn = d->f64 ? peak_pick_kernel<double, kDpValue> : peak_pick_kernel<float, kDpValue>;
+  return launch(c, fn, (unsigned)n_rows, 256, 0, a);
+}
+
+extern "C" int b2l_onset_backtrack(b2l_ctx* c, const void* d_energy, int64_t n, int32_t f64, const int64_t* d_events,
+                                   int64_t n_events, const int64_t* d_count, int32_t units, int32_t hop_length,
+                                   double sr, void* d_out) {
+  if (!c) return fail(B2L_ERR_INVALID, "NULL argument");
+  if (n < 0 || n_events < 0) return fail(B2L_ERR_INVALID, "bad geometry");
+  if (units < B2L_BEAT_FRAMES || units > B2L_BEAT_TIME) return fail(B2L_ERR_INVALID, "unknown units %d", units);
+  if (n > 0x7fffffffLL) return fail(B2L_ERR_UNSUPPORTED, "onset_backtrack: energy of 2^31 frames or more");
+  if (n_events == 0) return B2L_OK;
+  if ((n && !d_energy) || !d_events || !d_out) return fail(B2L_ERR_INVALID, "NULL device pointer");
+  DeviceGuard g(c->device);
+  Temp t_last(c->stream);
+  CUDA_TRY(t_last.alloc((size_t)n * sizeof(int)));
+  const long long* ev = (const long long*)d_events;
+  const long long* cnt = (const long long*)d_count;
+  if (f64)
+    return launch(c, b2l_onset::onset_backtrack_kernel<double>, 1u, 1024, 0, (const double*)d_energy, (int)n, ev,
+                  (long long)n_events, cnt, (int*)t_last.p, (int)units, (int)hop_length, sr, d_out, c->d_status);
+  return launch(c, b2l_onset::onset_backtrack_kernel<float>, 1u, 1024, 0, (const float*)d_energy, (int)n, ev,
+                (long long)n_events, cnt, (int*)t_last.p, (int)units, (int)hop_length, sr, d_out, c->d_status);
 }

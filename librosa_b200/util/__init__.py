@@ -1,5 +1,6 @@
-"""``librosa.util`` names used on the FFT time-frequency path."""
+"""``librosa.util`` names used on the FFT time-frequency path, and ``peak_pick``."""
 from .exceptions import LibrosaError, ParameterError
+from .peak import peak_pick
 from .utils import (
     MAX_MEM_BLOCK,
     abs2,
@@ -17,5 +18,5 @@ from .utils import (
 
 __all__ = [
     "LibrosaError", "ParameterError", "MAX_MEM_BLOCK", "abs2", "dtype_c2r", "dtype_r2c", "expand_to",
-    "fix_length", "frame", "is_positive_int", "normalize", "pad_center", "tiny", "valid_audio",
+    "fix_length", "frame", "is_positive_int", "normalize", "pad_center", "peak_pick", "tiny", "valid_audio",
 ]

@@ -1,7 +1,7 @@
 """Device-resident timings of the frame-wise features (SURVEY 8f rank 2) on a cfg-2 shaped batch, next to the
 oracle (CPU, one process) on a small sample.  CUDA events around `reps` calls after warm-up.  The pitch trackers
 run with fmin C2, fmax C7 and their other defaults (frame_length 2048, hop 512); their oracle sample is one clip.
-The rhythm features and beat_track (dense output) take the device onset envelope of the batch (431 frames per 10 s
+The rhythm features, beat_track and onset detection (dense output) take the device onset envelope of the batch (431 frames per 10 s
 clip) and their defaults;
 ``rhythm_bounds`` holds the tempogram kernel's least time on the card (output bytes at 3.35 TB/s, two packed FP64
 transforms per frame at 34 TFLOP/s), and ``card`` the GPU's name and power limit read in the same run.
@@ -22,6 +22,7 @@ import numpy as np
 
 import bench
 import librosa_b200 as lb
+import onset_oracle as OD
 import pitch_oracle as PO
 import rhythm_oracle as RO
 from oracle import ref_np as O
@@ -44,6 +45,7 @@ tg_dev = lb.feature.tempogram(onset_envelope=oenv)
 
 
 C2, C7 = 65.40639132514966, 2093.004522404789
+PEAK_KW = dict(pre_max=1, post_max=1, pre_avg=4, post_avg=5, delta=0.07, wait=1)   # onset_detect's at 22050 / 512
 
 
 def free(x):
@@ -80,6 +82,11 @@ FEATURES = {
     "beat_track(onset_envelope, bpm=120)": (lambda: lb.beat.beat_track(onset_envelope=oenv, bpm=120.0, sparse=False),
                                             None),
     "plp(onset_envelope)": (lambda: lb.beat.plp(onset_envelope=oenv), None),
+    "onset_detect(onset_envelope)": (lambda: lb.onset.onset_detect(onset_envelope=oenv, sparse=False),
+                                     lambda y: OD.onset_detect(onset_envelope=oenv_host[:len(y)], sparse=False)),
+    "onset_detect(y)": (lambda: lb.onset.onset_detect(y=dev, sr=sr, sparse=False), None),
+    "peak_pick(dp_value)": (lambda: lb.util.peak_pick(oenv, sparse=False, method="dp_value", **PEAK_KW),
+                            lambda y: OD.peak_pick(oenv_host[:len(y)], sparse=False, method="dp_value", **PEAK_KW)),
 }
 CPU_SAMPLE = {"yin(C2-C7)": 1, "pyin(C2-C7)": 1}   # clips in the oracle sample (default 8)
 

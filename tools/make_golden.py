@@ -2,7 +2,8 @@
 (tests/feature_cases.py) and tests/golden/reference_pins_v1.npz (tests/reference_pins.py) by running the
 cases through the UNMODIFIED reference; ``--pitch`` writes only tests/golden/pitch_v1.npz (tests/pitch_cases.py)
 and leaves the other fixtures as they are; ``--rhythm`` likewise writes only tests/golden/rhythm_v1.npz
-(tests/rhythm_cases.py), and ``--beat`` only tests/golden/beat_v1.npz (tests/beat_cases.py).
+(tests/rhythm_cases.py), ``--beat`` only tests/golden/beat_v1.npz (tests/beat_cases.py), and ``--onset`` only
+tests/golden/onset_v1.npz (tests/onset_cases.py).
 
 Needs a checkout of the reference (see tools/ref_shim.py); the tests only read the stored fixtures.  Also
 stores a handful of constant tables (mel bases, window sum-square, mel-scale known answers) produced by the
@@ -12,6 +13,7 @@ reference.
     python tools/make_golden.py --pitch
     python tools/make_golden.py --rhythm
     python tools/make_golden.py --beat
+    python tools/make_golden.py --onset
 """
 from __future__ import annotations
 
@@ -194,6 +196,37 @@ def write_beat():
     print("wrote", path, os.path.getsize(path), "bytes")
 
 
+def write_onset():
+    """tests/golden/onset_v1.npz: per case of tests/onset_cases.py, ``<name>/out`` (the reference's result) or
+    ``<name>/error`` ("Class: message"); ``<name>/norm``, onset_detect's normalised envelope, for the detection
+    cases that normalise; and ``onset_detect(y=)`` on click trains."""
+    import onset_cases as OC
+
+    ref = ref_shim.load_reference()
+    store = {}
+    for case in OC.CASES:
+        name = case["name"]
+        with warnings.catch_warnings():
+            warnings.simplefilter("ignore")
+            got = OC.outcome(ref, case)
+        if "out" in got:
+            store[name + "/out"] = np.ascontiguousarray(got["out"])
+        else:
+            store[name + "/error"] = np.array(got["error"])
+        if (case["op"] == "onset_detect" and case["env"] is not None and case["kw"].get("normalize", True)
+                and case["env"][2] > 0):   # zero frames: the reference's np.min raises
+            with warnings.catch_warnings():
+                warnings.simplefilter("ignore")
+                store[name + "/norm"] = OC.normalized(OC.envelope(case["env"]))
+        print(f"{name:48s} {got.get('error') or (got['out'].shape, got['out'].dtype)}")
+    for name, bpm in OC.Y_CASES.items():
+        store[name + "/out"] = np.asarray(ref.onset.onset_detect(y=OC.clicks_audio(bpm), sr=OC.SR, hop_length=OC.HOP))
+        print(name, store[name + "/out"])
+    path = os.path.join(ROOT, "tests", "golden", "onset_v1.npz")
+    np.savez_compressed(path, **store)
+    print("wrote", path, os.path.getsize(path), "bytes")
+
+
 if __name__ == "__main__":
     if "--pitch" in sys.argv[1:]:
         write_pitch()
@@ -201,5 +234,7 @@ if __name__ == "__main__":
         write_rhythm()
     elif "--beat" in sys.argv[1:]:
         write_beat()
+    elif "--onset" in sys.argv[1:]:
+        write_onset()
     else:
         main()
