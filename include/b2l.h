@@ -494,6 +494,47 @@ int b2l_onset_backtrack(b2l_ctx* ctx, const void* d_energy, int64_t n, int32_t f
                         int64_t n_events, const int64_t* d_count, int32_t units, int32_t hop_length, double sr,
                         void* d_out);
 
+/* ---- HMM decoding: librosa.sequence.viterbi, viterbi_discriminative, viterbi_binary (sequence.py:1175-1876) -------
+ * b2l_seq_logobs: one launch over d_prob [n_clips][n_states][n_steps] (float32, or float64 when f64), one thread
+ *   per (clip, frame).  With d_out != NULL writes the float64 log-likelihoods the decoder reads:
+ *     B2L_SEQ_PLAIN   log(p + eps) in prob's dtype                                   -> [clip][state][frame]
+ *     B2L_SEQ_DISC    log(p + eps) in prob's dtype, minus d_log_marginal[state]      -> [clip][state][frame]
+ *     B2L_SEQ_BINARY  rows (1 - p) (prob's dtype) and p as float64, log(. + eps) minus d_log_marginal[label][2]
+ *                                                                                    -> [clip][label][2][frame]
+ *   and ORs the verdict into d_flags (never cleared here): d_flags[0] bit 0 when a p is outside [0, 1] (PLAIN,
+ *   BINARY; NaN passes) or, for DISC, negative or in a column whose sum over the states (in order, in prob's dtype)
+ *   fails np.allclose(., 1); BINARY sets d_flags[1 + label] when (1 - p) + p fails np.allclose(., 1) in float64.
+ * b2l_seq_decode: one launch.  Decodes n_problems problems of d_lp [problem][n_states][n_steps] (n_steps >= 1)
+ *   with model problem % n_models: value[0] = lp[0] + log_p_init; value[t, j] = lp[t, j] + max over the
+ *   predecessors k of j (ascending, first maximum, a NaN cost never taken, pointer 0 when none beats -inf) of
+ *   value[t-1, k] + log_trans[k, j]; the last state is np.argmax(value[-1]) (the first NaN, else the first maximum).
+ *   Writes d_states [problem][n_steps] and d_logp [problem] = value[-1, state[-1]].  Back-pointers take
+ *   2 n_states n_steps bytes per problem of stream-ordered scratch.  Size classes (B2L_SEQ_*): up to 32 states W
+ *   lanes per problem; otherwise one CTA per problem with the two value rows in shared memory and
+ *   the model tables there too when they fit (MEDIUM) or read through L2 (LARGE); more states than two float64 rows
+ *   of the shared memory hold -> B2L_ERR_UNSUPPORTED.  Several models need at most 32 states.
+ * b2l_seq_route: the class (out[0]) and lanes per problem (out[1], small class) b2l_seq_decode would use. */
+enum b2l_seq_mode { B2L_SEQ_PLAIN = 0, B2L_SEQ_DISC = 1, B2L_SEQ_BINARY = 2 };
+enum b2l_seq_class { B2L_SEQ_SMALL = 0, B2L_SEQ_MEDIUM = 1, B2L_SEQ_LARGE = 2 };
+typedef struct b2l_seq_logobs_desc {
+  int32_t mode, f64;
+  int64_t n_clips, n_states, n_steps;
+  double eps;                        /* tiny(prob) for PLAIN / DISC, tiny(float64) for BINARY */
+  const double* d_log_marginal;      /* DISC: [n_states]; BINARY: [n_states][2]; device */
+} b2l_seq_logobs_desc;
+typedef struct b2l_seq_model {
+  int32_t n_states, n_models;
+  int32_t deg, dense;                /* predecessor entries per state; dense: deg = n_states, entry m is state m */
+  const double* d_lt;                /* [model][deg][n_states] log_trans[pred, j], padded with -inf */
+  const uint16_t* d_idx;             /* [model][deg][n_states] pred, ascending, padded with 0 (NULL when dense) */
+  const double* d_log_p_init;        /* [model][n_states] */
+} b2l_seq_model;
+int b2l_seq_logobs(b2l_ctx* ctx, const b2l_seq_logobs_desc* desc, const void* d_prob, double* d_out,
+                   int32_t* d_flags);
+int b2l_seq_decode(b2l_ctx* ctx, const b2l_seq_model* model, const double* d_lp, int64_t n_problems,
+                   int64_t n_steps, uint16_t* d_states, double* d_logp);
+int b2l_seq_route(b2l_ctx* ctx, const b2l_seq_model* model, int64_t n_problems, int32_t* out);
+
 /* ---- double-precision path: float64 audio / complex128 spectra ---------------------------------
  * librosa computes a float64 signal in float64 (dtype_r2c, core/spectrum.py:341; the window product :388 and the
  * irfft :598 follow the input's precision; the mel einsum feature/spectral.py:2160 and scipy.fft.dct :2005

@@ -159,7 +159,21 @@ class PeakDesc(C.Structure):
                 ("units", C.c_int32), ("hop_length", C.c_int32), ("sr", C.c_double)]
 
 
+class SeqLogObsDesc(C.Structure):
+    """struct b2l_seq_logobs_desc (include/b2l.h); d_log_marginal is a device pointer."""
+    _fields_ = [("mode", C.c_int32), ("f64", C.c_int32), ("n_clips", C.c_int64), ("n_states", C.c_int64),
+                ("n_steps", C.c_int64), ("eps", C.c_double), ("d_log_marginal", C.c_void_p)]
+
+
+class SeqModel(C.Structure):
+    """struct b2l_seq_model (include/b2l.h); the d_* fields are device pointers."""
+    _fields_ = [("n_states", C.c_int32), ("n_models", C.c_int32), ("deg", C.c_int32), ("dense", C.c_int32),
+                ("d_lt", C.c_void_p), ("d_idx", C.c_void_p), ("d_log_p_init", C.c_void_p)]
+
+
 BEAT_FRAMES, BEAT_SAMPLES, BEAT_TIME = range(3)   # enum b2l_beat_units
+SEQ_PLAIN, SEQ_DISC, SEQ_BINARY = range(3)        # enum b2l_seq_mode
+SEQ_SMALL, SEQ_MEDIUM, SEQ_LARGE = range(3)       # enum b2l_seq_class
 PEAK_GREEDY, PEAK_DP_COUNT, PEAK_DP_VALUE = range(3)   # enum b2l_peak_method
 TG_NORM_NONE, TG_NORM_MAX, TG_NORM_MIN, TG_NORM_COUNT, TG_NORM_P = range(5)   # enum b2l_tempogram_norm
 N_STATS = 6
@@ -249,6 +263,9 @@ def _declare(lib):
         "b2l_peak_pick": (C.c_int, [_vp, P(PeakDesc), _vp, _i64, _i64, _vp, _vp, _vp, _vp]),
         "b2l_onset_backtrack": (C.c_int, [_vp, _vp, _i64, C.c_int32, _vp, _i64, _vp, C.c_int32, C.c_int32, C.c_double,
                                           _vp]),
+        "b2l_seq_logobs": (C.c_int, [_vp, P(SeqLogObsDesc), _vp, _vp, _vp]),
+        "b2l_seq_decode": (C.c_int, [_vp, P(SeqModel), _vp, _i64, _i64, _vp, _vp]),
+        "b2l_seq_route": (C.c_int, [_vp, P(SeqModel), _i64, P(C.c_int32)]),
         "b2l_stft_f64": (C.c_int, [_vp, _vp, _i64, _i64, _i64, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                    P(C.c_double), _vp]),
         "b2l_istft_f64": (C.c_int, [_vp, _vp, _i64, _i64, _i64, C.c_int32, C.c_int32, C.c_int32, P(C.c_double),

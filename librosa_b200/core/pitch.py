@@ -233,39 +233,6 @@ def yin(y: np.ndarray, *, fmin: float, fmax: float, sr: float = 22050, frame_len
     return staged.result(f0)
 
 
-def _transition_loop(n_states, prob):
-    """librosa/sequence.py:1905-1967 for a scalar probability."""
-    prob = np.asarray(prob, dtype=np.float64)
-    if np.any(prob < 0) or np.any(prob > 1):
-        raise ParameterError(f"prob={np.tile(prob, n_states)} must have values in the range [0, 1]")
-    transition = np.empty((n_states, n_states), dtype=np.float64)
-    for i in range(n_states):
-        transition[i] = (1.0 - prob) / (n_states - 1)
-        transition[i, i] = prob
-    return transition
-
-
-def _transition_local(n_states, width):
-    """librosa/sequence.py:2034-2146 for a scalar width, triangle window, no wrap: (the window padded to n_states,
-    the row sums before normalisation, the normalised matrix)."""
-    import scipy.signal
-
-    if not (n_states > 1):
-        raise ParameterError(f"n_states={n_states} must be a positive integer > 1")
-    if width < 1:
-        raise ParameterError(f"width={np.tile(width, n_states)} must be at least 1")
-    transition = np.zeros((n_states, n_states), dtype=np.float64)
-    row = pad_center(scipy.signal.get_window("triangle", width, fftbins=False), size=n_states)
-    for i in range(n_states):
-        trans_row = np.roll(row, n_states // 2 + i + 1)
-        trans_row[min(n_states, i + width // 2 + 1):] = 0
-        trans_row[: max(0, i - width // 2)] = 0
-        transition[i] = trans_row
-    sums = transition.sum(axis=1, keepdims=True)
-    transition /= sums
-    return row, sums[:, 0], transition
-
-
 @lru_cache(maxsize=8)
 def _viterbi_tables(n_pitch_bins, width, switch_prob, transition_min_prob):
     """log(T + tiny) of pyin's transition matrix T = kron(transition_loop(2, 1 - switch_prob), transition_local(...))
@@ -276,9 +243,15 @@ def _viterbi_tables(n_pitch_bins, width, switch_prob, transition_min_prob):
     values.  Each is formed with the reference's own operations and the whole form is compared with the dense
     matrix, so the kernel sees exactly the reference's log_trans and predecessor sets (flatnonzero(log_trans[:, j] >=
     log_thr), librosa/sequence.py:1215-1224)."""
+    from ..filters import get_window
+    from ..sequence import _transition_local_rows, transition_loop
+
     eps = np.finfo(np.float64).tiny
-    row, sums, local = _transition_local(n_pitch_bins, width)
-    t_switch = _transition_loop(2, 1 - switch_prob)
+    local, sums = _transition_local_rows(n_pitch_bins, width)
+    local /= sums
+    sums = sums[:, 0]
+    row = pad_center(get_window("triangle", width, fftbins=False), size=n_pitch_bins)   # the window, centred
+    t_switch = transition_loop(2, 1 - switch_prob)
     log_trans = np.log(np.kron(t_switch, local) + eps)
     if transition_min_prob is not None and transition_min_prob > 0:
         log_thr = np.log(transition_min_prob + eps)

@@ -9,6 +9,7 @@
 #pragma once
 #include <float.h>
 
+#include "argmax.cuh"
 #include "common.cuh"
 #include "fft_engine.cuh"
 #include "fwd_kernel.cuh"   // load_padded
@@ -461,26 +462,10 @@ __global__ void __launch_bounds__(256) viterbi_kernel(const ViterbiArgs a) {
   __syncthreads();
   // ---- first argmax of the last row (np.argmax: the first NaN, else the first maximum)
   double bv = -INFINITY;
-  int bi = 0x7fffffff;
-  auto better = [](double va, int ia, double vb, int ib) {
-    const bool na = isnan(va), nb = isnan(vb);
-    if (na != nb) return na;
-    if (na) return ia < ib;
-    return va > vb || (va == vb && ia < ib);
-  };
-  for (int j = tid; j < S; j += nt)
-    if (bi == 0x7fffffff || better(prev[j], j, bv, bi)) { bv = prev[j]; bi = j; }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    const double ov = __shfl_xor_sync(0xffffffffu, bv, o);
-    const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-    if (oi != 0x7fffffff && (bi == 0x7fffffff || better(ov, oi, bv, bi))) { bv = ov; bi = oi; }
-  }
-  if ((tid & 31) == 0) { s_red_v[tid >> 5] = bv; s_red_i[tid >> 5] = bi; }
-  __syncthreads();
+  int bi = kArgNone;
+  for (int j = tid; j < S; j += nt) argmax_merge(bv, bi, prev[j], j);
+  block_argmax(bv, bi, s_red_v, s_red_i);
   if (tid == 0) {
-    for (int w = 1; w < (nt + 31) / 32; ++w)
-      if (s_red_i[w] != 0x7fffffff && better(s_red_v[w], s_red_i[w], bv, bi)) { bv = s_red_v[w]; bi = s_red_i[w]; }
     // ---- backtrace and the state -> (f0, voiced) map (:844-850)
     int s = bi;
     for (int t = a.n_frames - 1; t >= 0; --t) {

@@ -4,7 +4,10 @@ run with fmin C2, fmax C7 and their other defaults (frame_length 2048, hop 512);
 The rhythm features, beat_track and onset detection (dense output) take the device onset envelope of the batch (431 frames per 10 s
 clip) and their defaults;
 ``rhythm_bounds`` holds the tempogram kernel's least time on the card (output bytes at 3.35 TB/s, two packed FP64
-transforms per frame at 34 TFLOP/s), and ``card`` the GPU's name and power limit read in the same run.
+transforms per frame at 34 TFLOP/s), and ``card`` the GPU's name and power limit read in the same run.  ``sequence``
+times the HMM decoders on their own device-resident float32 shapes (independent of ``clips``), each with its least
+time from the shapes (predecessor visits x frames as FP64 add-compares at 34 TFLOP/s; bytes of prob, back-pointers
+and states at 3.35 TB/s) and the oracle's CPU time per clip.
 
     python tools/feature_timing.py [clips=1024] [reps=10] > gpurun_out/feature_timing.json
 """
@@ -25,6 +28,7 @@ import librosa_b200 as lb
 import onset_oracle as OD
 import pitch_oracle as PO
 import rhythm_oracle as RO
+import sequence_oracle as SQ
 from oracle import ref_np as O
 
 clips = int(sys.argv[1]) if len(sys.argv) > 1 else 1024
@@ -137,4 +141,57 @@ with warnings.catch_warnings():
             row["cpu_oracle_s_per_clip"] = round(dt / sample.shape[0], 4)
         out["features"][name] = row
         print(name, row, file=sys.stderr)
+
+
+def sequence_timings():
+    rng = np.random.default_rng(0)
+    loop25, local720 = lb.sequence.transition_loop(25, 0.9), lb.sequence.transition_local(720, 31)
+    dense = rng.random((1024, 1024))
+    dense /= dense.sum(axis=1, keepdims=True)
+    binary = np.array([[0.9, 0.1], [0.2, 0.8]])
+    p25 = rng.random((1024, 25, 431)).astype(np.float32)
+    p25 /= p25.sum(axis=-2, keepdims=True)
+    # name: (prob shape, call on a device prob, problems, states per problem, predecessor visits per frame, oracle)
+    cases = {
+        "viterbi_discriminative(25 states, loop)": (p25, lambda x: lb.sequence.viterbi_discriminative(x, loop25),
+                                                    1024, 25, 25 * 25, "disc", loop25, {}),
+        "viterbi(1024 states, dense)": ((64, 1024, 1000), lambda x: lb.sequence.viterbi(x, dense), 64, 1024,
+                                        1024 * 1024, "viterbi", dense, {}),
+        "viterbi(transition_local(720, 31), min_prob=1e-4)": (
+            (1024, 720, 431), lambda x: lb.sequence.viterbi(x, local720, transition_min_prob=1e-4), 1024, 720,
+            int((np.log(local720 + np.finfo(np.float32).tiny) >= np.log(1e-4 + np.finfo(np.float32).tiny)).sum()),
+            "viterbi", local720, dict(transition_min_prob=1e-4)),
+        "viterbi_binary(88 labels)": ((1024, 88, 431), lambda x: lb.sequence.viterbi_binary(x, binary), 1024 * 88, 2,
+                                      4, "binary", binary, {}),
+    }
+    res = {}
+    for name, (shape, call, problems, S, visits, op, trans, kw) in cases.items():
+        host_p = shape if isinstance(shape, np.ndarray) else rng.random(shape).astype(np.float32)
+        x = ctx.to_device(host_p)
+        call(x)
+        ctx.synchronize()
+        e0, e1 = ctx.event(), ctx.event()
+        l0 = ctx.launch_count
+        e0.record()
+        n = max(1, reps // 5) if S >= 720 else reps
+        for _ in range(n):
+            call(x)
+        e1.record()
+        ctx.synchronize()
+        ms = e0.elapsed_ms(e1) / n
+        T_ = host_p.shape[-1]
+        ops = 2.0 * visits * T_ * (problems // (88 if op == "binary" else 1)) * (88 if op == "binary" else 1)
+        nbytes = host_p.nbytes + problems * (2 * S * T_ + 2 * T_)
+        t0 = time.perf_counter()
+        SQ.run(op, host_p[0], trans, **kw)
+        cpu = time.perf_counter() - t0
+        res[name] = {"gpu_ms": round(ms, 3), "launches_per_call": (ctx.launch_count - l0) / n,
+                     "least_ms_fp64": round(ops / 34e12 * 1e3, 3), "least_ms_bytes": round(nbytes / 3.35e12 * 1e3, 3),
+                     "cpu_oracle_s_per_clip": round(cpu, 4)}
+        print(name, res[name], file=sys.stderr)
+        x.free()
+    return res
+
+
+out["sequence"] = sequence_timings()
 print(json.dumps(out, indent=1))

@@ -2,8 +2,9 @@
 (tests/feature_cases.py) and tests/golden/reference_pins_v1.npz (tests/reference_pins.py) by running the
 cases through the UNMODIFIED reference; ``--pitch`` writes only tests/golden/pitch_v1.npz (tests/pitch_cases.py)
 and leaves the other fixtures as they are; ``--rhythm`` likewise writes only tests/golden/rhythm_v1.npz
-(tests/rhythm_cases.py), ``--beat`` only tests/golden/beat_v1.npz (tests/beat_cases.py), and ``--onset`` only
-tests/golden/onset_v1.npz (tests/onset_cases.py).
+(tests/rhythm_cases.py), ``--beat`` only tests/golden/beat_v1.npz (tests/beat_cases.py), ``--onset`` only
+tests/golden/onset_v1.npz (tests/onset_cases.py), and ``--sequence`` only tests/golden/sequence_v1.npz
+(tests/sequence_cases.py).
 
 Needs a checkout of the reference (see tools/ref_shim.py); the tests only read the stored fixtures.  Also
 stores a handful of constant tables (mel bases, window sum-square, mel-scale known answers) produced by the
@@ -14,6 +15,7 @@ reference.
     python tools/make_golden.py --rhythm
     python tools/make_golden.py --beat
     python tools/make_golden.py --onset
+    python tools/make_golden.py --sequence
 """
 from __future__ import annotations
 
@@ -227,6 +229,73 @@ def write_onset():
     print("wrote", path, os.path.getsize(path), "bytes")
 
 
+def _zero_frames_outcome(ref, case):
+    """The reference's outcome for a zero-frame case, run in a forked child.  Its numba decoder writes value[0] of a
+    zero-row array (no bounds checks), so the process may die there; a dead child is reported, not recorded."""
+    import multiprocessing as mp
+    import sequence_cases as SC
+
+    def child(conn):
+        with warnings.catch_warnings():
+            warnings.simplefilter("ignore")
+            conn.send(SC.call(ref, case))
+
+    parent, conn = mp.get_context("fork").Pipe(duplex=False)
+    proc = mp.get_context("fork").Process(target=child, args=(conn,))
+    proc.start()
+    got = parent.recv() if parent.poll(60) else None
+    proc.join()
+    if got is None:
+        raise RuntimeError(f"{case['name']}: the reference's process died (exit code {proc.exitcode})")
+    return got
+
+
+def write_sequence():
+    """tests/golden/sequence_v1.npz: per case of tests/sequence_cases.py, the reference's ``<name>/states`` and
+    ``<name>/logp`` or ``<name>/error``; ``<name>/lp_sha256``, the SHA-256 of the float64 log-likelihoods its decoder
+    reads (formed with the reference's own expressions, tests/sequence_oracle.py; the arrays themselves are megabytes
+    of incompressible float64, rebuilt from the seeded inputs by the tests); and ``builder/<name>``, each ``transition_*`` output or
+    ``builder/<name>/error``."""
+    import sequence_cases as SC
+    import sequence_oracle as SO
+
+    ref = ref_shim.load_reference()
+    store = {}
+    for case in SC.CASES:
+        name = case["name"]
+        if case["obs"][3] == 0:
+            got = _zero_frames_outcome(ref, case)
+        else:
+            with warnings.catch_warnings():
+                warnings.simplefilter("ignore")
+                got = SC.call(ref, case)
+        if "error" in got:
+            store[name + "/error"] = np.array(got["error"])
+        else:
+            store[name + "/states"] = np.asarray(got["states"])
+            if "logp" in got:
+                store[name + "/logp"] = np.asarray(got["logp"])
+            prob, transition, kw = SC.make(case, ref)
+            kw.pop("return_logp", None)
+            if prob.shape[-1] == 0:
+                continue
+            with warnings.catch_warnings():
+                warnings.simplefilter("ignore")
+                store[name + "/lp_sha256"] = np.array(SO.digest(SO.run(case["op"], prob, transition, **kw)["lp"]))
+        print(f"{name:44s} {got.get('error') or (got['states'].shape, got['states'].dtype)}")
+    for key, spec in SC.BUILDERS.items():
+        store["builder/" + key] = SC.builder(ref, spec)
+    for key, spec in SC.BUILDER_ERRORS.items():
+        try:
+            SC.builder(ref, spec)
+            raise RuntimeError(key)
+        except ref.util.exceptions.ParameterError as exc:
+            store["builder/" + key + "/error"] = np.array(f"{type(exc).__name__}: {exc}")
+    path = os.path.join(ROOT, "tests", "golden", "sequence_v1.npz")
+    np.savez_compressed(path, **store)
+    print("wrote", path, os.path.getsize(path), "bytes")
+
+
 if __name__ == "__main__":
     if "--pitch" in sys.argv[1:]:
         write_pitch()
@@ -236,5 +305,7 @@ if __name__ == "__main__":
         write_beat()
     elif "--onset" in sys.argv[1:]:
         write_onset()
+    elif "--sequence" in sys.argv[1:]:
+        write_sequence()
     else:
         main()
