@@ -535,6 +535,55 @@ int b2l_seq_decode(b2l_ctx* ctx, const b2l_seq_model* model, const double* d_lp,
                    int64_t n_steps, uint16_t* d_states, double* d_logp);
 int b2l_seq_route(b2l_ctx* ctx, const b2l_seq_model* model, int64_t n_problems, int32_t* out);
 
+/* ---- alignment: librosa.sequence.dtw, dtw_backtracking, rqa (sequence.py:185-1075) ------------------------------
+ * b2l_dtw_cost: one launch, one thread per cell.  C = scipy's cdist(X, Y, metric) in float64 (float32 features are
+ *   widened), written [N][M], or [M][N] (C.T) with transpose.  Feature f of frame n of X is d_x[h_x_off[f] + n]
+ *   (float32, or float64 when f64), likewise Y; the K features are summed in table order, unfused.  Sets bit 0 of
+ *   d_flags[0] when a cost is NaN.
+ * b2l_nan_flag: one launch; sets bit 0 of d_flags[0] when one of the n elements of d_x is NaN.
+ * b2l_dtw_accumulate: one launch per anti-diagonal of 32 x 32 tiles.  D [n][m] float64 and steps [n][m] int32 of
+ *   C [n][m] (float32, or float64 when c_f64): D = min over the steps k in table order (strictly better only) of
+ *   D[i - a_k][j - b_k] + (w_mul[k] C[i][j] + w_add[k]), predecessors outside the matrix +inf; D[0][0] = C[0][0]
+ *   (subseq: D[0][j] = C[0][j]) and +inf elsewhere before the scan.  With band, C counts as +inf unless
+ *   band_lo < j - i < band_hi.
+ * b2l_dtw_backtrack: one launch.  Walks d_steps from row n - 1 at column `start` (< 0: the last column, or with d_D
+ *   and subseq the first argmin of D's last row) until row 0 (subseq) or (0, 0), or an index below 0, writing
+ *   (row, column) pairs (flip: (column, row)) to d_wp [n + m][2] int64 in walk order and the count to *d_len.  A
+ *   failure writes -status instead: 1 an all-inf last row and 2 an inf end cell (both with check_end and d_D), 3 a
+ *   path that misses (0, 0) (check_end, not subseq), 4 a (0, 0) step, 5 a step index outside the table, 6 bit 0 of
+ *   d_flags[0] (d_flags may be NULL).
+ * b2l_rqa: one launch per anti-diagonal of 32 x 32 tiles.  librosa's RQA score (sim's dtype: float32, or float64
+ *   when f64) and int8 pointers of sim [n][m].
+ * b2l_rqa_path: two launches.  The path from the first np.argmax of score (64-bit index) along the pointers, start
+ *   to end, as uint64 pairs in d_path [n][2], and its length in *d_len (-1: a column index below -m). */
+enum b2l_dtw_metric { B2L_DTW_EUCLIDEAN = 0, B2L_DTW_SQEUCLIDEAN = 1, B2L_DTW_CITYBLOCK = 2, B2L_DTW_CHEBYSHEV = 3,
+                      B2L_DTW_COSINE = 4 };
+typedef struct b2l_dtw_cost_desc {
+  int32_t f64, metric, transpose;
+  int64_t K, N, M;
+  const int64_t* h_x_off;            /* [K] host */
+  const int64_t* h_y_off;            /* [K] host */
+} b2l_dtw_cost_desc;
+typedef struct b2l_dtw_desc {
+  int64_t n, m;
+  int32_t c_f64, n_steps, subseq, band;
+  int64_t band_lo, band_hi;
+  const int64_t* h_steps;            /* [n_steps][2] host */
+  const double* h_w_add;             /* [n_steps] host */
+  const double* h_w_mul;             /* [n_steps] host */
+} b2l_dtw_desc;
+int b2l_dtw_cost(b2l_ctx* ctx, const b2l_dtw_cost_desc* desc, const void* d_x, const void* d_y, double* d_C,
+                 int32_t* d_flags);
+int b2l_nan_flag(b2l_ctx* ctx, const void* d_x, int64_t n, int32_t f64, int32_t* d_flags);
+int b2l_dtw_accumulate(b2l_ctx* ctx, const b2l_dtw_desc* desc, const void* d_C, double* d_D, int32_t* d_steps);
+int b2l_dtw_backtrack(b2l_ctx* ctx, const b2l_dtw_desc* desc, const int32_t* d_steps, const double* d_D,
+                      int64_t start, int32_t check_end, int32_t flip, const int32_t* d_flags, int64_t* d_wp,
+                      int64_t* d_len);
+int b2l_rqa(b2l_ctx* ctx, const void* d_sim, int64_t n, int64_t m, int32_t f64, double gap_onset, double gap_extend,
+            int32_t knight, void* d_score, int8_t* d_ptr);
+int b2l_rqa_path(b2l_ctx* ctx, const void* d_score, const int8_t* d_ptr, int64_t n, int64_t m, int32_t f64,
+                 uint64_t* d_path, int64_t* d_len);
+
 /* ---- double-precision path: float64 audio / complex128 spectra ---------------------------------
  * librosa computes a float64 signal in float64 (dtype_r2c, core/spectrum.py:341; the window product :388 and the
  * irfft :598 follow the input's precision; the mel einsum feature/spectral.py:2160 and scipy.fft.dct :2005

@@ -171,6 +171,20 @@ class SeqModel(C.Structure):
                 ("d_lt", C.c_void_p), ("d_idx", C.c_void_p), ("d_log_p_init", C.c_void_p)]
 
 
+class DtwCostDesc(C.Structure):
+    """struct b2l_dtw_cost_desc (include/b2l.h); the h_* fields are host pointers."""
+    _fields_ = [("f64", C.c_int32), ("metric", C.c_int32), ("transpose", C.c_int32), ("K", C.c_int64),
+                ("N", C.c_int64), ("M", C.c_int64), ("h_x_off", C.c_void_p), ("h_y_off", C.c_void_p)]
+
+
+class DtwDesc(C.Structure):
+    """struct b2l_dtw_desc (include/b2l.h); the h_* fields are host pointers."""
+    _fields_ = [("n", C.c_int64), ("m", C.c_int64), ("c_f64", C.c_int32), ("n_steps", C.c_int32),
+                ("subseq", C.c_int32), ("band", C.c_int32), ("band_lo", C.c_int64), ("band_hi", C.c_int64),
+                ("h_steps", C.c_void_p), ("h_w_add", C.c_void_p), ("h_w_mul", C.c_void_p)]
+
+
+DTW_METRICS = {"euclidean": 0, "sqeuclidean": 1, "cityblock": 2, "chebyshev": 3, "cosine": 4}   # enum b2l_dtw_metric
 BEAT_FRAMES, BEAT_SAMPLES, BEAT_TIME = range(3)   # enum b2l_beat_units
 SEQ_PLAIN, SEQ_DISC, SEQ_BINARY = range(3)        # enum b2l_seq_mode
 SEQ_SMALL, SEQ_MEDIUM, SEQ_LARGE = range(3)       # enum b2l_seq_class
@@ -266,6 +280,12 @@ def _declare(lib):
         "b2l_seq_logobs": (C.c_int, [_vp, P(SeqLogObsDesc), _vp, _vp, _vp]),
         "b2l_seq_decode": (C.c_int, [_vp, P(SeqModel), _vp, _i64, _i64, _vp, _vp]),
         "b2l_seq_route": (C.c_int, [_vp, P(SeqModel), _i64, P(C.c_int32)]),
+        "b2l_dtw_cost": (C.c_int, [_vp, P(DtwCostDesc), _vp, _vp, _vp, _vp]),
+        "b2l_nan_flag": (C.c_int, [_vp, _vp, _i64, C.c_int32, _vp]),
+        "b2l_dtw_accumulate": (C.c_int, [_vp, P(DtwDesc), _vp, _vp, _vp]),
+        "b2l_dtw_backtrack": (C.c_int, [_vp, P(DtwDesc), _vp, _vp, _i64, C.c_int32, C.c_int32, _vp, _vp, _vp]),
+        "b2l_rqa": (C.c_int, [_vp, _vp, _i64, _i64, C.c_int32, C.c_double, C.c_double, C.c_int32, _vp, _vp]),
+        "b2l_rqa_path": (C.c_int, [_vp, _vp, _vp, _i64, _i64, C.c_int32, _vp, _vp]),
         "b2l_stft_f64": (C.c_int, [_vp, _vp, _i64, _i64, _i64, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                    P(C.c_double), _vp]),
         "b2l_istft_f64": (C.c_int, [_vp, _vp, _i64, _i64, _i64, C.c_int32, C.c_int32, C.c_int32, P(C.c_double),

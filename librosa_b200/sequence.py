@@ -1,5 +1,6 @@
-"""``librosa.sequence`` HMM decoding (reference: librosa/sequence.py:1175-2146): ``viterbi``,
-``viterbi_discriminative``, ``viterbi_binary`` and the ``transition_*`` builders.
+"""``librosa.sequence`` (reference: librosa/sequence.py): alignment — ``dtw``, ``dtw_backtracking``, ``rqa`` and
+``path_to_steps`` — and HMM decoding — ``viterbi``, ``viterbi_discriminative``, ``viterbi_binary`` and the
+``transition_*`` builders.
 
 The builders run on the host in NumPy.  The decoders build every model constant on the host with NumPy's own
 operations — ``log(transition + eps)``, ``log(p_init + eps)``, ``log(p_state + eps)``, the threshold and the
@@ -19,7 +20,7 @@ from .util.utils import is_positive_int, pad_center
 
 _vp = C.c_void_p
 
-__all__ = ["viterbi", "viterbi_discriminative", "viterbi_binary", "transition_uniform", "transition_loop",
+__all__ = ["dtw", "dtw_backtracking", "rqa", "path_to_steps", "viterbi", "viterbi_discriminative", "viterbi_binary", "transition_uniform", "transition_loop",
            "transition_cycle", "transition_local"]
 
 # Two float64 value rows per state in the 227 KiB of shared memory an H100 CTA may opt into, less 1 KiB of static
@@ -494,3 +495,371 @@ def viterbi_binary(prob, transition, *, p_state=None, p_init=None, return_logp: 
     if return_logp:
         return states, logp
     return states
+
+
+# --------------------------------------------------------------------------------------------- alignment
+# librosa.sequence.dtw, dtw_backtracking, rqa and path_to_steps (reference: librosa/sequence.py:185-1172).  Argument
+# checks and the step tables are the reference's, on the host; the cost matrix, the accumulation, the argmin / argmax
+# and the path walks run on the device (csrc/align_kernels.cuh).  Host arrays in give host arrays out; a DeviceArray
+# in gives DeviceArrays out.
+_byref = C.byref     # dtw's argument C hides the ctypes module inside it
+_DEFAULT_STEPS = np.array([[1, 1], [0, 1], [1, 0]], dtype=np.uint32)
+# Status words of b2l_dtw_backtrack (include/b2l.h): the negated length word
+_WALK_ALL_INF, _WALK_INF_END, _WALK_NOT_ORIGIN, _WALK_ZERO_STEP, _WALK_BAD_STEP, _WALK_NAN = range(1, 7)
+_NO_PATH = "No valid sub-sequence warping path could be constructed with the given step sizes."
+_CDIST_ERROR = ("scipy.spatial.distance.cdist returned an error.\nPlease provide your input in the form X.shape=(K, N) "
+                "and Y.shape=(K, M).\n 1-dimensional sequences should be reshaped to X.shape=(1, N) and Y.shape=(1, M).")
+
+
+def _feature_offsets(shape):
+    """Element offset, in the C-ordered array of ``shape`` (..., K, N), of each feature of frame 0 in the order of the
+    reference's ``swapaxes(X, -1, 0).reshape(N, -1, order="F")``; feature f of frame n is at offset[f] + n."""
+    n = shape[-1]
+    base = (np.arange(int(np.prod(shape[:-1], dtype=np.int64)), dtype=np.int64) * n).reshape(shape[:-1] + (1,))
+    return np.ascontiguousarray(np.swapaxes(base, -1, 0).reshape((1, -1), order="F")[0])
+
+
+def _band(shape, band_rad):
+    """fill_off_diagonal's band as (lo, hi): cell (n, m) keeps its cost iff lo < m - n < hi."""
+    radius = int(np.round(band_rad * np.min(shape)))
+    offset = abs(shape[0] - shape[1])
+    if shape[0] < shape[1]:
+        return -radius, radius + offset
+    return -radius - offset, radius
+
+
+def _metric_code(metric):
+    """The device metric of a cdist metric name; UnsupportedOnGPU for a callable or another metric scipy knows,
+    the reference's ParameterError for a name scipy rejects."""
+    from scipy.spatial import distance
+
+    if callable(metric):
+        raise nat.UnsupportedOnGPU("dtw: a callable metric is not supported on the GPU (euclidean, sqeuclidean, "
+                                   "cityblock, chebyshev and cosine are)")
+    if not isinstance(metric, str):
+        raise TypeError("2nd argument metric must be a string identifier or a function.")
+    name = metric.lower()
+    info = distance._METRIC_ALIAS.get(name)
+    if info is None and not name.startswith("test_"):
+        raise ParameterError(_CDIST_ERROR)
+    code = nat.DTW_METRICS.get(info.canonical_name) if info is not None else None
+    if code is None:
+        raise nat.UnsupportedOnGPU(f"dtw: metric {metric!r} is not supported on the GPU (euclidean, sqeuclidean, "
+                                   "cityblock, chebyshev and cosine are)")
+    return code
+
+
+def _features(x, what):
+    """(array to upload or DeviceArray, shape, f64) of dtw's X or Y, at least 2-D."""
+    if isinstance(x, nat.DeviceArray):
+        if x.layout != "c" or x.dtype not in (np.float32, np.float64):
+            raise nat.UnsupportedOnGPU(f"dtw: {what} must be a C-ordered float32 or float64 DeviceArray")
+        if x.ndim < 2:
+            x = _view(x, (1,) * (2 - x.ndim) + x.shape)
+        return x, x.shape, x.dtype == np.float64
+    x = np.atleast_2d(np.asarray(x))
+    if np.iscomplexobj(x):
+        raise nat.UnsupportedOnGPU(f"dtw: complex {what} is not supported on the GPU")
+    if x.dtype != np.float32:
+        x = x.astype(np.float64)      # what cdist computes in
+    return np.ascontiguousarray(x), x.shape, x.dtype == np.float64
+
+
+class _Align:
+    """Device buffers of one alignment call: what it allocates, freed by release() unless handed to the caller."""
+
+    def __init__(self, ctx=None):
+        self._ctx, self.owned = ctx, []
+
+    @property
+    def ctx(self):
+        """The device context; a host call creates it only when it reaches device work."""
+        if self._ctx is None:
+            self._ctx = nat.default_context()
+        return self._ctx
+
+    def empty(self, shape, dtype):
+        d = nat.DeviceArray.empty(self.ctx, shape, dtype)
+        self.owned.append(d)
+        return d
+
+    def stage(self, x):
+        if isinstance(x, nat.DeviceArray):
+            return x
+        d = self.ctx.to_device(x)
+        self.owned.append(d)
+        return d
+
+    def flags(self):
+        f = self.empty((1,), np.int32)
+        nat.check(nat.lib().b2l_memset(self.ctx.handle, _vp(f.ptr), 0, 4))
+        return f
+
+    def keep(self, d):
+        self.owned.remove(d)
+        return d
+
+    def release(self):
+        for d in self.owned:
+            d.free()
+        self.owned = []
+
+
+def _dtw_desc(shape, steps, w_add, w_mul, *, c_f64=True, subseq=False, band=None):
+    lo, hi = band if band is not None else (0, 0)
+    desc = nat.DtwDesc(n=shape[0], m=shape[1], c_f64=int(c_f64), n_steps=len(steps), subseq=int(bool(subseq)),
+                       band=int(band is not None), band_lo=lo, band_hi=hi, h_steps=steps.ctypes.data,
+                       h_w_add=w_add.ctypes.data, h_w_mul=w_mul.ctypes.data)
+    return desc
+
+
+def _walk(run, desc, d_steps, d_D, start, check_end, flip, flags):
+    """b2l_dtw_backtrack and one 8-byte read-back of the length word: (wp buffer, length or -status)."""
+    n, m = desc.n, desc.m
+    wp = run.empty((n + m, 2), np.int64)
+    length = run.empty((1,), np.int64)
+    nat.check(nat.lib().b2l_dtw_backtrack(run.ctx.handle, C.byref(desc), _vp(d_steps.ptr),
+                                          _vp(d_D.ptr) if d_D is not None else None, start, check_end, flip,
+                                          _vp(flags.ptr) if flags is not None else None, _vp(wp.ptr),
+                                          _vp(length.ptr)))
+    return wp, int(length.get()[0])
+
+
+def _walk_refusal(status):
+    if status == -_WALK_ZERO_STEP:
+        raise nat.UnsupportedOnGPU("dtw: the warping path takes a (0, 0) step, where the reference's backtracking "
+                                   "never ends")
+    if status == -_WALK_BAD_STEP:
+        raise nat.UnsupportedOnGPU("dtw: steps holds an index outside the step table")
+
+
+def _path_out(run, buf, length, on_device):
+    if on_device:
+        return _view(run.keep(buf), (length, 2))
+    return buf.get()[:length].copy()
+
+
+def dtw(X=None, Y=None, *, C=None, metric: str = "euclidean", step_sizes_sigma=None, weights_add=None,
+        weights_mul=None, subseq: bool = False, backtrack: bool = True, global_constraints: bool = False,
+        band_rad: float = 0.25, return_steps: bool = False):
+    """Dynamic time warping; same contract as ``librosa.sequence.dtw``.
+
+    ``X`` (..., K, N) / ``Y`` (..., K, M) features, or a cost matrix ``C`` (N, M), float32 or float64, host or
+    DeviceArray.  Returns float64 ``D``, with ``backtrack`` the int64 warping path ``wp`` (end to start) and with
+    ``return_steps`` the int32 step matrix.  The metrics euclidean, sqeuclidean, cityblock, chebyshev and cosine
+    give scipy's cdist bit for bit; another metric, or a callable, raises UnsupportedOnGPU."""
+    default_weights_add = np.zeros(3, dtype=np.float64)
+    default_weights_mul = np.ones(3, dtype=np.float64)
+    if step_sizes_sigma is None:
+        step_sizes_sigma = _DEFAULT_STEPS
+        if weights_add is None:
+            weights_add = default_weights_add
+        if weights_mul is None:
+            weights_mul = default_weights_mul
+    else:
+        if weights_add is None:
+            weights_add = np.zeros(len(step_sizes_sigma), dtype=np.float64)
+        if weights_mul is None:
+            weights_mul = np.ones(len(step_sizes_sigma), dtype=np.float64)
+        default_weights_add.fill(np.inf)
+        default_weights_mul.fill(np.inf)
+        step_sizes_sigma = np.concatenate((_DEFAULT_STEPS, step_sizes_sigma))
+        weights_add = np.concatenate((default_weights_add, weights_add))
+        weights_mul = np.concatenate((default_weights_mul, weights_mul))
+    if np.any(step_sizes_sigma < 0):
+        raise ParameterError("step_sizes_sigma cannot contain negative values")
+    if len(step_sizes_sigma) != len(weights_add):
+        raise ParameterError("len(weights_add) must be equal to len(step_sizes_sigma)")
+    if len(step_sizes_sigma) != len(weights_mul):
+        raise ParameterError("len(weights_mul) must be equal to len(step_sizes_sigma)")
+    if C is None and (X is None or Y is None):
+        raise ParameterError("If C is not supplied, both X and Y must be supplied")
+    if C is not None and (X is not None or Y is not None):
+        raise ParameterError("If C is supplied, both X and Y must not be supplied")
+
+    on_device = any(isinstance(a, nat.DeviceArray) for a in (X, Y, C))
+    run = _Align(next((a.ctx for a in (X, Y, C) if isinstance(a, nat.DeviceArray)), None))
+    try:
+        transposed = False
+        flags = None
+        if C is None:
+            X, x_shape, x_f64 = _features(X, "X")
+            Y, y_shape, y_f64 = _features(Y, "Y")
+            N, M = x_shape[-1], y_shape[-1]
+            K = int(np.prod(x_shape[:-1], dtype=np.int64))
+            if K != int(np.prod(y_shape[:-1], dtype=np.int64)):
+                raise ParameterError(_CDIST_ERROR)
+            code = _metric_code(metric)
+            if x_f64 != y_f64:        # the kernel reads both in one dtype; widening is exact
+                if on_device:
+                    raise nat.UnsupportedOnGPU("dtw: X and Y must share a dtype when one is a DeviceArray")
+                X, Y, x_f64 = X.astype(np.float64), Y.astype(np.float64), True
+            if N == 0 or M == 0 or K == 0:
+                raise nat.UnsupportedOnGPU("dtw: empty features (the reference indexes past its arrays)")
+            transposed = bool(subseq and N > M)
+            shape = (M, N) if transposed else (N, M)
+            dX, dY = run.stage(X), run.stage(Y)
+            d_C = run.empty(shape, np.float64)
+            flags = run.flags()
+            x_off, y_off = _feature_offsets(x_shape), _feature_offsets(y_shape)
+            cdesc = nat.DtwCostDesc(f64=int(x_f64), metric=code, transpose=int(transposed), K=K, N=N, M=M,
+                                    h_x_off=x_off.ctypes.data, h_y_off=y_off.ctypes.data)
+            nat.check(nat.lib().b2l_dtw_cost(run.ctx.handle, _byref(cdesc), _vp(dX.ptr), _vp(dY.ptr), _vp(d_C.ptr),
+                                             _vp(flags.ptr)))
+            c_f64 = True
+        else:
+            if isinstance(C, nat.DeviceArray):
+                if C.layout != "c" or C.dtype not in (np.float32, np.float64):
+                    raise nat.UnsupportedOnGPU("dtw: C must be a C-ordered float32 or float64 DeviceArray")
+                d_C = C if C.ndim == 2 else _view(C, (1,) * (2 - C.ndim) + C.shape)
+                if C.ndim > 2:
+                    raise nat.UnsupportedOnGPU("dtw: C must be 2-D")
+            else:
+                C = np.atleast_2d(np.asarray(C))
+                if C.ndim != 2 or np.iscomplexobj(C):
+                    raise nat.UnsupportedOnGPU("dtw: C must be a real 2-D matrix")
+                if C.dtype != np.float32:
+                    C = C.astype(np.float64)
+                d_C = None
+            shape = (C.shape[-2], C.shape[-1]) if not isinstance(C, nat.DeviceArray) else d_C.shape
+            c_f64 = C.dtype == np.float64
+            if 0 in shape:
+                raise nat.UnsupportedOnGPU("dtw: an empty cost matrix (the reference indexes past its arrays)")
+        if np.array_equal(step_sizes_sigma, np.array([[1, 1]])) and shape[0] > shape[1]:
+            raise ParameterError("For diagonal matching: Y.shape[-1] >= X.shape[-11] (C.shape[1] >= C.shape[0])")
+        nan_error = ParameterError("DTW cost matrix C has NaN values. ")
+        if C is not None:
+            if isinstance(C, nat.DeviceArray):
+                flags = run.flags()
+                nat.check(nat.lib().b2l_nan_flag(run.ctx.handle, _vp(d_C.ptr), d_C.size, int(c_f64), _vp(flags.ptr)))
+            else:
+                if np.any(np.isnan(C)):
+                    raise nan_error
+                d_C = run.stage(np.ascontiguousarray(C))
+        steps_tab = np.ascontiguousarray(step_sizes_sigma, dtype=np.int64).reshape(-1, 2)
+        w_add = np.ascontiguousarray(weights_add, dtype=np.float64)
+        w_mul = np.ascontiguousarray(weights_mul, dtype=np.float64)
+        desc = _dtw_desc(shape, steps_tab, w_add, w_mul, c_f64=c_f64, subseq=subseq,
+                         band=_band(shape, band_rad) if global_constraints else None)
+        D = run.empty(shape, np.float64)
+        steps = run.empty(shape, np.int32)
+        nat.check(nat.lib().b2l_dtw_accumulate(run.ctx.handle, _byref(desc), _vp(d_C.ptr), _vp(D.ptr), _vp(steps.ptr)))
+        out = []
+        if backtrack:
+            flip = int(bool(subseq) and (transposed or shape[0] > shape[1]))
+            wp, length = _walk(run, desc, steps, D, -1, 1, flip, flags)
+            if length == -_WALK_NAN:
+                raise nan_error
+            if length in (-_WALK_ALL_INF, -_WALK_INF_END):
+                raise ParameterError(_NO_PATH)
+            if length == -_WALK_NOT_ORIGIN:
+                raise ParameterError("Unable to compute a full DTW warping path. "
+                                     "You may want to try again with subseq=True.")
+            _walk_refusal(length)
+            out.append(_path_out(run, wp, length, on_device))
+        elif flags is not None and flags.get()[0]:
+            raise nan_error
+        D_out = run.keep(D) if on_device else D.get()
+        steps_out = (run.keep(steps) if on_device else steps.get()) if return_steps else None
+    finally:
+        run.release()
+    ret = [D_out] + out + ([steps_out] if return_steps else [])
+    return tuple(ret) if len(ret) > 1 else ret[0]
+
+
+def dtw_backtracking(steps, *, step_sizes_sigma=None, subseq: bool = False, start=None):
+    """Backtrack a warping path from a step matrix; same contract as ``librosa.sequence.dtw_backtracking``.
+    ``steps`` (N, M) host integer array or int32 DeviceArray; returns the int64 path (L, 2), end to start."""
+    if subseq is False and start is not None:
+        raise ParameterError(f"start is only allowed to be set if subseq is True (start={start}, subseq={subseq})")
+    if step_sizes_sigma is None:
+        step_sizes_sigma = _DEFAULT_STEPS
+    else:
+        step_sizes_sigma = np.concatenate((_DEFAULT_STEPS, step_sizes_sigma))
+    table = np.ascontiguousarray(step_sizes_sigma, dtype=np.int64).reshape(-1, 2)
+    if np.any(table < 0):
+        raise nat.UnsupportedOnGPU("dtw_backtracking: negative step sizes")
+    on_device = isinstance(steps, nat.DeviceArray)
+    if on_device:
+        if steps.layout != "c" or steps.dtype != np.int32 or steps.ndim != 2:
+            raise nat.UnsupportedOnGPU("dtw_backtracking: steps must be a C-ordered 2-D int32 DeviceArray")
+    else:
+        steps = np.asarray(steps)
+        if steps.ndim != 2 or steps.dtype.kind not in "iu" or np.any(steps.astype(np.int32) != steps):
+            raise nat.UnsupportedOnGPU("dtw_backtracking: steps must be a 2-D integer array of step indices")
+        steps = np.ascontiguousarray(steps, dtype=np.int32)
+    n, m = steps.shape
+    if 0 in (n, m):
+        raise nat.UnsupportedOnGPU("dtw_backtracking: an empty step matrix")
+    if start is not None and not 0 <= int(start) < m:
+        raise nat.UnsupportedOnGPU(f"dtw_backtracking: start={start} outside the {m} columns (the reference reads "
+                                   "outside its array)")
+    run = _Align(steps.ctx if on_device else None)
+    zeros = np.zeros(len(table))
+    try:
+        desc = _dtw_desc((n, m), table, zeros, zeros, subseq=subseq)
+        wp, length = _walk(run, desc, run.stage(steps), None, -1 if start is None else int(start), 0, 0, None)
+        _walk_refusal(length)
+        return _path_out(run, wp, length, on_device)
+    finally:
+        run.release()
+
+
+def rqa(sim, *, gap_onset: float = 1, gap_extend: float = 1, knight_moves: bool = True, backtrack: bool = True):
+    """Recurrence quantification analysis; same contract as ``librosa.sequence.rqa``.
+
+    ``sim`` (N, M) float32 or float64, host or DeviceArray.  Returns ``score`` in sim's dtype and, with ``backtrack``,
+    the uint64 ``path`` (k, 2) start to end — (0, 2) when there is none."""
+    if gap_onset < 0:
+        raise ParameterError("gap_onset={} must be strictly positive")
+    if gap_extend < 0:
+        raise ParameterError("gap_extend={} must be strictly positive")
+    on_device = isinstance(sim, nat.DeviceArray)
+    if not on_device:
+        sim = np.asarray(sim)
+    if np.dtype(sim.dtype) not in (np.float32, np.float64):
+        raise nat.UnsupportedOnGPU(f"rqa of a {np.dtype(sim.dtype)} similarity matrix is not supported on the GPU "
+                                   "(float32 and float64 only)")
+    if sim.ndim != 2 or 0 in sim.shape:
+        raise nat.UnsupportedOnGPU("rqa needs a non-empty 2-D similarity matrix")
+    if on_device and sim.layout != "c":
+        raise nat.UnsupportedOnGPU("rqa needs a C-ordered DeviceArray")
+    n, m = sim.shape
+    f64 = int(sim.dtype == np.float64)
+    run = _Align(sim.ctx if on_device else None)
+    try:
+        d_sim = run.stage(np.ascontiguousarray(sim) if not on_device else sim)
+        score = run.empty((n, m), sim.dtype)
+        ptr = run.empty((n, m), np.int8)
+        L = nat.lib()
+        nat.check(L.b2l_rqa(run.ctx.handle, _vp(d_sim.ptr), n, m, f64, float(gap_onset), float(gap_extend),
+                            int(bool(knight_moves)), _vp(score.ptr), _vp(ptr.ptr)))
+        if not backtrack:
+            return run.keep(score) if on_device else score.get()
+        path = run.empty((n, 2), np.uint64)
+        length = run.empty((1,), np.int64)
+        nat.check(L.b2l_rqa_path(run.ctx.handle, _vp(score.ptr), _vp(ptr.ptr), n, m, f64, _vp(path.ptr),
+                                 _vp(length.ptr)))
+        k = int(length.get()[0])
+        if k < 0:
+            raise nat.UnsupportedOnGPU("rqa: the path's column index passes -M (the reference raises IndexError)")
+        score_out = run.keep(score) if on_device else score.get()
+        return score_out, _path_out(run, path, k, on_device)
+    finally:
+        run.release()
+
+
+def path_to_steps(path, *, inverse: bool = False):
+    """Fractional steps from a warping path by linear interpolation; same contract as
+    ``librosa.sequence.path_to_steps``.  Runs on the host (a DeviceArray path is read back first)."""
+    import scipy.interpolate
+
+    if isinstance(path, nat.DeviceArray):
+        path = path.get()
+    if inverse:
+        idx_from, idx_to = 1, 0
+    else:
+        idx_from, idx_to = 0, 1
+    step_interp = scipy.interpolate.interp1d(path[:, idx_to], path[:, idx_from], kind="linear")
+    frames_in = np.arange(path[:, idx_to].min(), path[:, idx_to].max() + 1)
+    return step_interp(frames_in)

@@ -1,4 +1,4 @@
-"""``librosa.util`` names used on the FFT time-frequency path, and ``peak_pick``."""
+"""``librosa.util`` names used on the FFT time-frequency path, ``peak_pick`` and ``fill_off_diagonal``."""
 from .exceptions import LibrosaError, ParameterError
 from .peak import peak_pick
 from .utils import (
@@ -7,6 +7,7 @@ from .utils import (
     dtype_c2r,
     dtype_r2c,
     expand_to,
+    fill_off_diagonal,
     fix_length,
     frame,
     is_positive_int,
@@ -18,5 +19,5 @@ from .utils import (
 
 __all__ = [
     "LibrosaError", "ParameterError", "MAX_MEM_BLOCK", "abs2", "dtype_c2r", "dtype_r2c", "expand_to",
-    "fix_length", "frame", "is_positive_int", "normalize", "pad_center", "peak_pick", "tiny", "valid_audio",
+    "fill_off_diagonal", "fix_length", "frame", "is_positive_int", "normalize", "pad_center", "peak_pick", "tiny", "valid_audio",
 ]

@@ -196,3 +196,25 @@ def cyclic_gradient(data: np.ndarray, *, edge_order: int = 1, axis: int = -1) ->
     keep = [slice(None)] * data.ndim
     keep[axis] = slice(edge_order, -edge_order)
     return grad[tuple(keep)]
+
+
+def fill_off_diagonal(x: np.ndarray, *, radius: float, value: float = 0) -> None:
+    """Set every entry of ``x`` outside the Sakoe-Chiba band to ``value``, in place; same contract as
+    ``librosa.util.fill_off_diagonal``.  The band's half-width is ``int(np.round(radius * min(x.shape)))``, widened
+    by ``|N - M|`` on the long side so that ``x[-1, -1]`` stays inside.  dtw's ``global_constraints`` applies the
+    same band on the device (sequence._band)."""
+    from .._native import DeviceArray, UnsupportedOnGPU
+
+    if isinstance(x, DeviceArray):
+        raise UnsupportedOnGPU("fill_off_diagonal works in place on a host ndarray")
+    nx, ny = x.shape
+    radius = int(np.round(radius * np.min(x.shape)))
+    offset = np.abs(x.shape[0] - x.shape[1])
+    if nx < ny:
+        idx_u = np.triu_indices_from(x, k=radius + offset)
+        idx_l = np.tril_indices_from(x, k=-radius)
+    else:
+        idx_u = np.triu_indices_from(x, k=radius)
+        idx_l = np.tril_indices_from(x, k=-radius - offset)
+    x[idx_u] = value
+    x[idx_l] = value

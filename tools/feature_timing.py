@@ -7,7 +7,10 @@ clip) and their defaults;
 transforms per frame at 34 TFLOP/s), and ``card`` the GPU's name and power limit read in the same run.  ``sequence``
 times the HMM decoders on their own device-resident float32 shapes (independent of ``clips``), each with its least
 time from the shapes (predecessor visits x frames as FP64 add-compares at 34 TFLOP/s; bytes of prob, back-pointers
-and states at 3.35 TB/s) and the oracle's CPU time per clip.
+and states at 3.35 TB/s) and the oracle's CPU time per clip.  ``alignment`` times dtw (device float32 features,
+cost matrix, accumulation and path) and rqa (device float32 similarity, score and path), each with its least time from
+the shapes: about 20 bytes per cell (C, D, steps) for dtw and 1 + 2 * 4 per cell for rqa at 3.35 TB/s, and the
+number of anti-diagonals the cells' dependency chain must pass through one after another.
 
     python tools/feature_timing.py [clips=1024] [reps=10] > gpurun_out/feature_timing.json
 """
@@ -193,5 +196,37 @@ def sequence_timings():
     return res
 
 
+def alignment_timings():
+    rng = np.random.default_rng(0)
+    cases = {}
+    for N, M in ((4000, 4500), (20000, 20000)):
+        X = ctx.to_device(rng.random((12, N)).astype(np.float32))
+        Y = ctx.to_device(rng.random((12, M)).astype(np.float32))
+        cases[f"dtw(12 x {N}, 12 x {M})"] = (lambda X=X, Y=Y: lb.sequence.dtw(X, Y), N, M, 20, (X, Y))
+    sim = ctx.to_device((rng.random((4000, 4000)) > 0.7).astype(np.float32))
+    cases["rqa(4000 x 4000, float32)"] = (lambda: lb.sequence.rqa(sim), 4000, 4000, 9, (sim,))
+    res = {}
+    for name, (call, N, M, per_cell, keep) in cases.items():
+        free(call())
+        ctx.synchronize()
+        n = 3 if N * M > 1e8 else 10
+        e0, e1 = ctx.event(), ctx.event()
+        l0 = ctx.launch_count
+        e0.record()
+        for _ in range(n):
+            free(call())
+        e1.record()
+        ctx.synchronize()
+        ms = e0.elapsed_ms(e1) / n
+        res[name] = {"gpu_ms": round(ms, 3), "launches_per_call": (ctx.launch_count - l0) / n,
+                     "gcells_per_s": round(N * M / ms / 1e6, 2),
+                     "least_ms_bytes": round(N * M * per_cell / 3.35e12 * 1e3, 3), "anti_diagonals": N + M - 1}
+        print(name, res[name], file=sys.stderr)
+        for a in keep:
+            a.free()
+    return res
+
+
 out["sequence"] = sequence_timings()
+out["alignment"] = alignment_timings()
 print(json.dumps(out, indent=1))

@@ -3,8 +3,8 @@
 cases through the UNMODIFIED reference; ``--pitch`` writes only tests/golden/pitch_v1.npz (tests/pitch_cases.py)
 and leaves the other fixtures as they are; ``--rhythm`` likewise writes only tests/golden/rhythm_v1.npz
 (tests/rhythm_cases.py), ``--beat`` only tests/golden/beat_v1.npz (tests/beat_cases.py), ``--onset`` only
-tests/golden/onset_v1.npz (tests/onset_cases.py), and ``--sequence`` only tests/golden/sequence_v1.npz
-(tests/sequence_cases.py).
+tests/golden/onset_v1.npz (tests/onset_cases.py), ``--sequence`` only tests/golden/sequence_v1.npz
+(tests/sequence_cases.py), and ``--alignment`` only tests/golden/alignment_v1.npz (tests/alignment_cases.py).
 
 Needs a checkout of the reference (see tools/ref_shim.py); the tests only read the stored fixtures.  Also
 stores a handful of constant tables (mel bases, window sum-square, mel-scale known answers) produced by the
@@ -16,6 +16,7 @@ reference.
     python tools/make_golden.py --beat
     python tools/make_golden.py --onset
     python tools/make_golden.py --sequence
+    python tools/make_golden.py --alignment
 """
 from __future__ import annotations
 
@@ -296,6 +297,25 @@ def write_sequence():
     print("wrote", path, os.path.getsize(path), "bytes")
 
 
+def write_alignment():
+    """tests/golden/alignment_v1.npz: per case of tests/alignment_cases.py, the reference's outputs (large ones as
+    SHA-256) or ``<name>/error``.  A dtw whose path takes a (0, 0) step is never run: the reference's walk does not
+    end there."""
+    import alignment_cases as AC
+
+    ref = ref_shim.load_reference()
+    store = {}
+    for case in AC.CASES:
+        with warnings.catch_warnings():
+            warnings.simplefilter("ignore")
+            got = AC.call(ref, case)
+        store.update(AC.pack(case["name"], got))
+        print(f"{case['name']:44s} {got.get('error') or {k: np.shape(v) for k, v in got.items()}}")
+    path = os.path.join(ROOT, "tests", "golden", "alignment_v1.npz")
+    np.savez_compressed(path, **store)
+    print("wrote", path, os.path.getsize(path), "bytes")
+
+
 if __name__ == "__main__":
     if "--pitch" in sys.argv[1:]:
         write_pitch()
@@ -307,5 +327,7 @@ if __name__ == "__main__":
         write_onset()
     elif "--sequence" in sys.argv[1:]:
         write_sequence()
+    elif "--alignment" in sys.argv[1:]:
+        write_alignment()
     else:
         main()
