@@ -81,13 +81,25 @@ int b2l_ctx_sm_count(const b2l_ctx* ctx, int* sms);
 int b2l_ctx_launch_count(const b2l_ctx* ctx, uint64_t* launches);
 
 /* ---- util.valid_audio on the device (librosa/util/utils.py:246-308) ----------------------------
- * The forward kernels set bit 0 of a per-context status word when a non-finite sample reaches a frame;
+ * The forward kernels set B2L_STATUS_NOT_FINITE_SAMPLE in a per-context status word when a non-finite sample
+ * reaches a frame;
  * b2l_scan_finite covers samples [begin, n) that no frame reads (tail / hop > n_fft gaps);
  * b2l_scan_finite_f64 does the same for the float64 signals of the FP64 path and flags exactly the samples
  * np.isfinite rejects.  The Python layer resets the word before a call on host data, reads it with the
  * results and raises ParameterError("Audio buffer is not finite everywhere") exactly as the reference does. */
 int b2l_status_reset(b2l_ctx* ctx);
 int b2l_status_read(b2l_ctx* ctx, int* status); /* synchronises the ctx stream */
+
+/* Bits of the status word.  The forward transforms and b2l_scan_finite* set B2L_STATUS_NOT_FINITE_SAMPLE with a
+ * plain store of that bit, which clears any other bit already set; every other setter uses atomicOr.  So within one
+ * reset epoch nothing may set bits 1-3 before a forward kernel or a finite scan runs: each caller that reads bits
+ * 1-3 either resets the word right before the kernels that set them, or runs them after its last forward kernel. */
+enum b2l_status_bit {
+  B2L_STATUS_NOT_FINITE_SAMPLE = 1, /* a kernel read a non-finite input sample (util.valid_audio)      */
+  B2L_STATUS_NEGATIVE_ENTRY = 2,    /* b2l_spectral_stats_from_spec read a negative spectrogram entry */
+  B2L_STATUS_NOT_FINITE_VALUE = 4,  /* b2l_tempogram or b2l_plp_finish met a non-finite value         */
+  B2L_STATUS_NEGATIVE_EVENT = 8     /* b2l_onset_backtrack was given a negative event frame          */
+};
 int b2l_scan_finite(b2l_ctx* ctx, const float* d_y, int64_t n_clips, int64_t n, int64_t y_stride,
                     int64_t begin);
 int b2l_scan_finite_f64(b2l_ctx* ctx, const double* d_y, int64_t n_clips, int64_t n, int64_t y_stride,
@@ -317,8 +329,8 @@ typedef struct b2l_stats_desc {
 /* y= form: fused with the stft (no spectrogram is written); power-of-two n_fft plans. */
 int b2l_spectral_stats(b2l_ctx* ctx, const b2l_plan* plan, const b2l_stats_desc* desc, const float* d_y,
                        int64_t n_clips, int64_t n, int64_t y_stride, const float* d_freq, float* d_out);
-/* S= form: d_S [n_clips][n_frames][n_bins] magnitudes.  Bit 1 of the status word (b2l_status_read) is set
- * when S holds a negative entry (the reference raises ParameterError). */
+/* S= form: d_S [n_clips][n_frames][n_bins] magnitudes.  B2L_STATUS_NEGATIVE_ENTRY is set in the status word
+ * (b2l_status_read) when S holds a negative entry (the reference raises ParameterError). */
 int b2l_spectral_stats_from_spec(b2l_ctx* ctx, const b2l_stats_desc* desc, const float* d_S, int64_t n_clips,
                                  int64_t n_frames, int32_t n_bins, const float* d_freq, float* d_out);
 /* Time-domain framings, out [n_clips][n_frames] with n_frames = 1 + (n + 2*pad - frame_length) / hop:
@@ -337,7 +349,7 @@ int b2l_frame_feature(b2l_ctx* ctx, int32_t what, const float* d_y, int64_t n_cl
  * b2l_yin_cmnd: frames (frame_length, hop_length, center / pad_mode as librosa.util.frame after np.pad) -> the
  *   cumulative mean normalised difference, float32 d_cmnd [n_clips][n_frames][n_lags]; the autocorrelation comes
  *   from the register FFT at N = the smallest power of two >= frame_length + max_period + 1 (up to 8192, else
- *   B2L_ERR_UNSUPPORTED).  Sets bit 0 of the status word when a frame reads a non-finite sample.
+ *   B2L_ERR_UNSUPPORTED).  Sets B2L_STATUS_NOT_FINITE_SAMPLE when a frame reads a non-finite sample.
  * b2l_yin_pick: CMND rows -> f0 of yin, float64 [n_rows]. */
 typedef struct b2l_yin_desc {
   int32_t frame_length, hop_length, center, pad_mode;
@@ -389,7 +401,7 @@ int b2l_viterbi(b2l_ctx* ctx, const b2l_pyin_desc* desc, const int32_t* d_count,
  *   (np.pad mode "linear_ramp", then the first n frames), n - win_length + 1 otherwise.  d_window [win_length] is
  *   the float64 window.  The arithmetic is FP64 for both envelope types.  win_length up to 4096
  *   (else B2L_ERR_UNSUPPORTED).  util.normalize along the lags with `norm` (B2L_TG_NORM_*; norm_p the exponent of
- *   B2L_TG_NORM_P) and threshold tiny(float64); sets bit 2 of the status word when an autocorrelation value is not
+ *   B2L_TG_NORM_P) and threshold tiny(float64); sets B2L_STATUS_NOT_FINITE_VALUE when an autocorrelation value is not
  *   finite (normalize's "Input must be finite").
  * b2l_tempo: tempograms -> the BPM d_bpms[k] of the first lag k maximising log1p(1e6 tg) + d_logprior[k]
  *   (NaN counts as the maximum), float64.  Element (row, lag, frame) of d_tg (float32, or float64 when tg_f64)
@@ -451,7 +463,7 @@ int b2l_any_nonzero(b2l_ctx* ctx, const void* d_x, int64_t n, int32_t f64, int32
  *   whose log1p(1e6 |X|) (+ d_logprior[bin] in float64 when d_logprior != NULL) is below the frame's maximum, then
  *   divide by sqrt_tiny + |max(X)| under NumPy's lexicographic complex max.  d_keep / d_logprior: float64 [n_bins].
  * b2l_plp_finish: in place on the pulse d_pulse [n_rows][n] (float32, or float64 when f64): clip below at 0, then
- *   divide each row by its maximum (1 when below tiny); a non-finite value sets bit 2 of the status word. */
+ *   divide each row by its maximum (1 when below tiny); a non-finite value sets B2L_STATUS_NOT_FINITE_VALUE. */
 typedef struct b2l_plp_desc {
   int32_t n_bins, c128;
   double sqrt_tiny;
@@ -477,8 +489,8 @@ int b2l_plp_finish(b2l_ctx* ctx, void* d_pulse, int64_t n_rows, int64_t n, int32
  *   converted to `units` (as b2l_beat_track) and their number to d_count.
  * b2l_onset_backtrack: one launch.  Each of the first *d_count (NULL: n_events) int64 frames of d_events is replaced
  *   by the last local minimum of d_energy [n] at or before it (e[i] <= e[i-1] and e[i] < e[i+1]; frame 0 always
- *   counts; frames past n - 1 take the last), converted to `units`, in d_out.  A negative event sets bit 3 of the
- *   status word and writes nothing. */
+ *   counts; frames past n - 1 take the last), converted to `units`, in d_out.  A negative event sets
+ *   B2L_STATUS_NEGATIVE_EVENT and writes nothing. */
 enum b2l_peak_method { B2L_PEAK_GREEDY = 0, B2L_PEAK_DP_COUNT = 1, B2L_PEAK_DP_VALUE = 2 };
 typedef struct b2l_peak_desc {
   int64_t pre_max, post_max, pre_avg, post_avg, wait;

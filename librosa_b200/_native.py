@@ -6,6 +6,7 @@ CPU fallback — if the shared library is missing or no sm_90 GPU is present, ev
 from __future__ import annotations
 
 import ctypes as C
+import math
 import os
 import threading
 import weakref
@@ -37,6 +38,7 @@ class UnsupportedOnGPU(NotImplementedError):
 
 
 class PlanDesc(C.Structure):
+    """struct b2l_plan_desc (include/b2l.h)."""
     _fields_ = [
         ("n_fft", C.c_int32),
         ("hop_length", C.c_int32),
@@ -194,6 +196,7 @@ N_STATS = 6
 STAT_CENTROID, STAT_BANDWIDTH, STAT_ROLLOFF, STAT_FLATNESS, STAT_RMS, STAT_TOTAL = range(6)
 FRAME_RMS, FRAME_ZERO_CROSSINGS = 0, 1
 UNARY_SQUARE, UNARY_DB_TO_POWER, UNARY_DB_TO_AMPLITUDE = 0, 1, 2
+STATUS_NOT_FINITE_SAMPLE, STATUS_NEGATIVE_ENTRY, STATUS_NOT_FINITE_VALUE, STATUS_NEGATIVE_EVENT = 1, 2, 4, 8   # enum b2l_status_bit
 
 _lib = None
 _lib_lock = threading.Lock()
@@ -469,6 +472,13 @@ class Context:
     def empty(self, shape, dtype, layout: str = "c") -> "DeviceArray":
         return DeviceArray.empty(self, shape, dtype, layout=layout)
 
+    def zeros(self, shape, dtype) -> "DeviceArray":
+        """A C-ordered buffer cleared on the stream."""
+        out = DeviceArray.empty(self, shape, dtype)
+        if out.nbytes:
+            check(lib().b2l_memset(self._h, _vp(out.ptr), 0, out.nbytes))
+        return out
+
     def to_device(self, arr: np.ndarray) -> "DeviceArray":
         arr = np.ascontiguousarray(arr)
         out = DeviceArray.empty(self, arr.shape, arr.dtype)
@@ -574,6 +584,7 @@ class DeviceArray:
         self.shape = tuple(int(s) for s in shape)
         self.dtype = np.dtype(dtype)
         self.layout = layout
+        self.base: Optional[DeviceArray] = None   # the buffer a view reads; kept alive with the view
         self._finalizer = weakref.finalize(self, DeviceArray._release, ctx, ptr) if owner and ptr else None
 
     @staticmethod
@@ -600,6 +611,17 @@ class DeviceArray:
     @property
     def nbytes(self):
         return self.size * self.dtype.itemsize
+
+    def view(self, shape, offset: int = 0) -> "DeviceArray":
+        """A non-owning C-ordered array of ``shape`` over this buffer's memory, starting ``offset`` elements in."""
+        shape = tuple(int(s) for s in shape)
+        start = int(offset)
+        # math.prod, not np.prod: the small device calls that return views would notice the microseconds
+        if start < 0 or start + math.prod(shape) > math.prod(self.shape):
+            raise ValueError(f"a view of {shape} at offset {offset} reaches past a buffer of {self.shape}")
+        out = DeviceArray(self.ctx, self.ptr + start * self.dtype.itemsize, shape, self.dtype, layout="c", owner=False)
+        out.base = self
+        return out
 
     def free(self):
         if self._finalizer is not None and self._finalizer.alive:

@@ -277,8 +277,7 @@ def forward_front(y, n_fft, hop_length, win_length, window, center, pad_mode, na
 
 # --------------------------------------------------------------------------------------------- status word
 def status_word(ctx) -> int:
-    """The context's status word once its stream has drained: bit 0 — a kernel saw a non-finite input sample
-    (the device half of util.valid_audio), bit 1 — a negative spectrogram entry."""
+    """The context's status word once its stream has drained: the ``nat.STATUS_*`` bits (enum b2l_status_bit)."""
     flag = C.c_int(0)
     nat.check(nat.lib().b2l_status_read(ctx.handle, C.byref(flag)))
     return flag.value
@@ -292,7 +291,7 @@ def finish(dev: nat.DeviceArray, dtype=None, validate: bool = False) -> np.ndarr
     to ``dtype``; ``validate``: raise like util.valid_audio when a kernel flagged a non-finite sample."""
     arr = dev.get()
     dev.free()
-    if validate and status_word(dev.ctx) & 1:
+    if validate and status_word(dev.ctx) & nat.STATUS_NOT_FINITE_SAMPLE:
         raise ParameterError(_NOT_FINITE)
     if dtype is not None and arr.dtype != dtype:
         arr = arr.astype(dtype)
@@ -349,13 +348,121 @@ class StagedInput:
             self.dev.free()
 
     def check_finite(self):
-        if not self.on_device and status_word(self.ctx) & 1:
+        if not self.on_device and status_word(self.ctx) & nat.STATUS_NOT_FINITE_SAMPLE:
             raise ParameterError(_NOT_FINITE)
 
     def result(self, dev: nat.DeviceArray, dtype=None):
         """The caller's return value: ``dev`` itself for a device signal, else a NumPy array of ``dtype``,
         validated with the status verdict."""
         return dev if self.on_device else finish(dev, dtype, validate=True)
+
+
+class Scope:
+    """The device buffers of one call, as a context manager: whatever it still owns is freed on exit, on the normal
+    and the exception path alike.  ``args`` are the call's array arguments: the first DeviceArray among them gives
+    the context (else the default context, created only when device work begins) and makes the call ``on_device``.
+    Those arrays belong to the caller and are never owned."""
+
+    def __init__(self, *args):
+        self._args = [a for a in args if isinstance(a, nat.DeviceArray)]
+        self.on_device = bool(self._args)
+        self._ctx = self._args[0].ctx if self._args else None
+        self._owned = []
+
+    @property
+    def ctx(self):
+        if self._ctx is None:
+            self._ctx = nat.default_context()
+        return self._ctx
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        for d in self._owned:
+            d.free()
+        self._owned = []
+
+    def own(self, d: nat.DeviceArray) -> nat.DeviceArray:
+        """Free ``d`` on exit (unless it is one of the caller's arrays)."""
+        if not any(d is a for a in self._args):
+            self._owned.append(d)
+        return d
+
+    def stage(self, x, dtype=None) -> nat.DeviceArray:
+        """A DeviceArray as it is; a host array uploaded C-ordered as ``dtype`` (default: its own)."""
+        if isinstance(x, nat.DeviceArray):
+            return x
+        return self.own(self.ctx.to_device(np.ascontiguousarray(x, dtype=dtype)))
+
+    def empty(self, shape, dtype, layout: str = "c") -> nat.DeviceArray:
+        return self.own(self.ctx.empty(shape, dtype, layout))
+
+    def zeros(self, shape, dtype) -> nat.DeviceArray:
+        return self.own(self.ctx.zeros(shape, dtype))
+
+    def keep(self, d: nat.DeviceArray) -> nat.DeviceArray:
+        """Hand ``d`` to the caller: it is no longer freed on exit."""
+        self._owned = [o for o in self._owned if o is not d]
+        return d
+
+    def result(self, d: nat.DeviceArray, dtype=None, validate: bool = False):
+        """The caller's return value: ``d`` itself for a device call, else ``finish(d, dtype, validate)``."""
+        return self.keep(d) if self.on_device else finish(self.keep(d), dtype, validate)
+
+
+def check_envelope(y, onset_envelope, missing: str = "Either y or onset_envelope must be provided"):
+    """The host checks of an onset-envelope argument (``missing``: the caller's message when neither is given)."""
+    if onset_envelope is None:
+        if y is None:
+            raise ParameterError(missing)
+        precheck_signal(y)
+    elif isinstance(onset_envelope, nat.DeviceArray):
+        if onset_envelope.dtype not in (np.float32, np.float64) or onset_envelope.layout != "c":
+            raise ParameterError("device onset envelope must be a C-ordered float32 or float64 DeviceArray")
+    elif np.asarray(onset_envelope).dtype not in (np.float32, np.float64):
+        raise nat.UnsupportedOnGPU("onset_envelope must be float32 or float64 on the GPU")
+
+
+class Envelope:
+    """The onset envelope of a call on the device, C-ordered (..., n).
+
+    ``y`` runs onset_strength on the device: a host signal is uploaded once and checked like util.valid_audio,
+    the envelope never leaves the GPU.  A host envelope is uploaded as it is.  The status word is cleared for this
+    call's verdict (``verdict``); ``on_device``: the caller passed device data and gets a DeviceArray back.
+    ``aggregate`` is onset_strength's (beat tracking uses np.median)."""
+
+    def __init__(self, y, sr, onset_envelope, hop_length, aggregate=None):
+        from .onset import onset_strength
+
+        self.audio = None
+        if onset_envelope is None:
+            self.audio = StagedInput(y)
+            self.dev = onset_strength(y=self.audio.dev, sr=sr, hop_length=hop_length, aggregate=aggregate)
+            self.audio.scan_all()
+            self.staged = self.audio
+        else:
+            x = onset_envelope if isinstance(onset_envelope, nat.DeviceArray) else np.asarray(onset_envelope)
+            self.staged = StagedInput(x, dtype=x.dtype)
+            self.dev = self.staged.dev
+        self.on_device = self.staged.on_device
+        self.ctx = self.staged.ctx
+        if self.dev.ndim < 1:
+            raise ParameterError("onset envelope must be at least one-dimensional")
+        if self.on_device:   # a host input was staged after a reset of the status word
+            nat.check(nat.lib().b2l_status_reset(self.ctx.handle))
+
+    def release(self):
+        self.staged.release()
+        self.dev = None   # the envelope onset_strength made goes with its last reference (stream-ordered free)
+
+    def verdict(self):
+        """Raise like the reference when a kernel of this call flagged non-finite data (synchronises)."""
+        flags = status_word(self.ctx)
+        if self.audio is not None and not self.on_device and flags & nat.STATUS_NOT_FINITE_SAMPLE:
+            self.audio.check_finite()
+        if flags & nat.STATUS_NOT_FINITE_VALUE:
+            raise ParameterError("Input must be finite")
 
 
 # --------------------------------------------------------------------------------------------- spectrogram inputs
@@ -494,7 +601,7 @@ def run_forward(y, *, plan_key, plan_kw, n_frames: int, out_tail, dtype, launch,
             ctx.free(d_in)
             ctx.free(d_out)
             ctx.free(d_scr)
-    if any(f & 1 for f in flags):
+    if any(f & nat.STATUS_NOT_FINITE_SAMPLE for f in flags):
         raise ParameterError(_NOT_FINITE)
     res = out.reshape(lead + mem_tail)
     return np.swapaxes(res, -1, -2) if layout == "ft" else res

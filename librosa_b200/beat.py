@@ -112,14 +112,15 @@ def host_tables(fpb: np.ndarray, n: int, f64: bool):
     return per_clip, np.concatenate(pieces), log_table(max(1, min(2 * int(uniq.max()), n - 1)))
 
 
-def _launch(ctx, x, fpb, fpb_f64, *, tightness, trim, units=None, hop_length=512, sr=22050.0, stages=None):
-    """One launch of the tracker on the device envelope ``x`` (..., n).  Returns the dense beats (DeviceArray of
-    bool) and, with ``units``, the compacted list and its count.  ``stages``: a dict that receives the
-    localscore / cumscore / backlink DeviceArrays."""
+def _launch(sc, x, fpb, fpb_f64, *, tightness, trim, units=None, hop_length=512, sr=22050.0, stages=None):
+    """One launch of the tracker on the device envelope ``x`` (..., n), its buffers owned by the scope ``sc``.
+    Returns the dense beats (DeviceArray of bool) and, with ``units``, the compacted list and its count.
+    ``stages``: a dict that receives the localscore / cumscore / backlink DeviceArrays."""
+    ctx = sc.ctx
     n, f64 = x.shape[-1], x.dtype == np.float64
     dp64 = f64 or fpb_f64
     per_clip, wtab, logd = host_tables(fpb, n, dp64)
-    d_clip = ctx.to_device(per_clip)
+    d_clip = sc.stage(per_clip)
     m = per_clip.size // 3
     d_wtab = pl.f64_constant(ctx, ("beat_window", pl.digest(wtab)), wtab)
     d_logd = pl.f64_constant(ctx, ("beat_log", logd.size), logd)
@@ -127,21 +128,20 @@ def _launch(ctx, x, fpb, fpb_f64, *, tightness, trim, units=None, hop_length=512
                         units=_UNITS.get(units, 0), tightness=float(np.float32(tightness)),
                         hop_length=int(hop_length), sr=float(sr), d_fpb=d_clip.ptr, d_logfpb=d_clip.ptr + 8 * m,
                         d_woff=d_clip.ptr + 16 * m, d_wtab=d_wtab, d_logd=d_logd)
-    beats = nat.DeviceArray.empty(ctx, x.shape, np.bool_)
+    beats = sc.empty(x.shape, np.bool_)
     ptrs = [None, None, None]
     if stages is not None:
-        stages["localscore"] = nat.DeviceArray.empty(ctx, x.shape, x.dtype)
-        stages["cumscore"] = nat.DeviceArray.empty(ctx, x.shape, np.float64 if dp64 else np.float32)
-        stages["backlink"] = nat.DeviceArray.empty(ctx, x.shape, np.int32)
+        stages["localscore"] = sc.empty(x.shape, x.dtype)
+        stages["cumscore"] = sc.empty(x.shape, np.float64 if dp64 else np.float32)
+        stages["backlink"] = sc.empty(x.shape, np.int32)
         ptrs = [_vp(stages[k].ptr) for k in ("localscore", "cumscore", "backlink")]
     lst = count = None
     if units is not None:
-        lst = nat.DeviceArray.empty(ctx, (n,), np.float64 if units == "time" else np.int64)
-        count = nat.DeviceArray.empty(ctx, (1,), np.int64)
+        lst = sc.empty((n,), np.float64 if units == "time" else np.int64)
+        count = sc.empty((1,), np.int64)
     nat.check(nat.lib().b2l_beat_track(ctx.handle, C.byref(desc), _vp(x.ptr), pl.clip_count(x.shape[:-1]), n, *ptrs,
                                        _vp(beats.ptr), _vp(lst.ptr) if lst else None,
                                        _vp(count.ptr) if count else None))
-    d_clip.free()
     return beats, lst, count
 
 
@@ -149,13 +149,6 @@ def _any_nonzero(x: nat.DeviceArray) -> bool:
     flag = nat.DeviceArray.empty(x.ctx, (1,), np.int32)
     nat.check(nat.lib().b2l_any_nonzero(x.ctx.handle, _vp(x.ptr), x.size, int(x.dtype == np.float64), _vp(flag.ptr)))
     return bool(flag.get()[0])
-
-
-def _zeros(ctx, shape, dtype):
-    out = nat.DeviceArray.empty(ctx, shape, dtype)
-    if out.nbytes:
-        nat.check(nat.lib().b2l_memset(ctx.handle, _vp(out.ptr), 0, out.nbytes))
-    return out
 
 
 def beat_track(*, y=None, sr: float = 22050, onset_envelope=None, hop_length: int = 512, start_bpm: float = 120.0,
@@ -169,73 +162,62 @@ def beat_track(*, y=None, sr: float = 22050, onset_envelope=None, hop_length: in
     reference's float32 and float64 tracker arithmetic; a ``y=`` envelope is float32."""
     from .feature.rhythm import _Envelope, tempo
 
-    if onset_envelope is None:
-        if y is None:
-            raise ParameterError("y or onset_envelope must be provided")
-        pl.precheck_signal(y)
-    elif isinstance(onset_envelope, nat.DeviceArray):
-        if onset_envelope.dtype not in (np.float32, np.float64) or onset_envelope.layout != "c":
-            raise ParameterError("device onset envelope must be a C-ordered float32 or float64 DeviceArray")
-    elif np.asarray(onset_envelope).dtype not in (np.float32, np.float64):
-        raise nat.UnsupportedOnGPU("onset_envelope must be float32 or float64 on the GPU")
-    env = _Envelope(y, sr, onset_envelope, hop_length, aggregate=np.median)
-    try:
-        env.verdict()
-        x, ctx, on_device = env.dev, env.ctx, env.on_device
-        if sparse and x.ndim != 1:
-            raise ParameterError(f"sparse=True (default) does not support "
-                                 f"{x.ndim}-dimensional inputs. "
-                                 f"Either set sparse=False or convert the signal to mono.")
-        if onset_envelope is not None and not on_device:
-            nonzero = bool(np.asarray(onset_envelope).any())
-        else:
-            nonzero = _any_nonzero(x)
-        if not nonzero:
-            if sparse:
-                return 0.0, (nat.DeviceArray.empty(ctx, (0,), np.int64) if on_device else np.array([], dtype=int))
-            if on_device:
-                return _zeros(ctx, x.shape[:-1], np.float64), _zeros(ctx, x.shape, np.bool_)
-            return np.zeros(shape=x.shape[:-1], dtype=float), np.zeros(x.shape, dtype=bool)
-        if bpm is None:
-            bpm = tempo(onset_envelope=x, sr=sr, hop_length=hop_length, start_bpm=start_bpm, prior=prior)
-            bpm_host = bpm.get()   # 8 bytes per clip: the host builds the tracker's tables
-            if not on_device:
-                bpm = bpm_host
-        else:
-            bpm_host = bpm.get() if isinstance(bpm, nat.DeviceArray) else bpm
-        bpm_expanded, frame_rate = frames_per_beat(bpm_host, sr, hop_length, x.shape)
-        fpb, fpb_f64 = _check_tracker_args(bpm_expanded, frame_rate, tightness, x.shape)
-        if sparse and units not in _UNITS:
-            raise ParameterError(f"Invalid unit type: {units}")
-        dense, lst, count = _launch(ctx, x, fpb, fpb_f64, tightness=tightness, trim=trim, units=units if sparse else None,
-                                    hop_length=hop_length, sr=sr)
-    finally:
-        env.release()
-    if not sparse:
-        return bpm, (dense if on_device else dense.get())
-    dense.free()
-    k = int(count.get()[0])
-    if on_device:
-        view = nat.DeviceArray(ctx, lst.ptr, (k,), lst.dtype, layout="c", owner=False)
-        view._base = lst
-        return bpm, view
-    return bpm, lst.get()[:k].copy()
+    pl.check_envelope(y, onset_envelope, "y or onset_envelope must be provided")
+    with pl.Scope(y if onset_envelope is None else onset_envelope) as sc:
+        env = _Envelope(y, sr, onset_envelope, hop_length, aggregate=np.median)
+        try:
+            env.verdict()
+            x, ctx, on_device = env.dev, env.ctx, env.on_device
+            if sparse and x.ndim != 1:
+                raise ParameterError(f"sparse=True (default) does not support "
+                                     f"{x.ndim}-dimensional inputs. "
+                                     f"Either set sparse=False or convert the signal to mono.")
+            if onset_envelope is not None and not on_device:
+                nonzero = bool(np.asarray(onset_envelope).any())
+            else:
+                nonzero = _any_nonzero(x)
+            if not nonzero:
+                if sparse:
+                    return 0.0, (ctx.empty((0,), np.int64) if on_device else np.array([], dtype=int))
+                if on_device:
+                    return ctx.zeros(x.shape[:-1], np.float64), ctx.zeros(x.shape, np.bool_)
+                return np.zeros(shape=x.shape[:-1], dtype=float), np.zeros(x.shape, dtype=bool)
+            if bpm is None:
+                bpm = tempo(onset_envelope=x, sr=sr, hop_length=hop_length, start_bpm=start_bpm, prior=prior)
+                bpm_host = bpm.get()   # 8 bytes per clip: the host builds the tracker's tables
+                if not on_device:
+                    bpm = bpm_host
+            else:
+                bpm_host = bpm.get() if isinstance(bpm, nat.DeviceArray) else bpm
+            bpm_expanded, frame_rate = frames_per_beat(bpm_host, sr, hop_length, x.shape)
+            fpb, fpb_f64 = _check_tracker_args(bpm_expanded, frame_rate, tightness, x.shape)
+            if sparse and units not in _UNITS:
+                raise ParameterError(f"Invalid unit type: {units}")
+            dense, lst, count = _launch(sc, x, fpb, fpb_f64, tightness=tightness, trim=trim,
+                                        units=units if sparse else None, hop_length=hop_length, sr=sr)
+        finally:
+            env.release()
+        if not sparse:
+            return bpm, sc.result(dense)
+        k = int(count.get()[0])
+        if on_device:
+            return bpm, sc.keep(lst).view((k,))
+        return bpm, lst.get()[:k].copy()
 
 
 def track_stages(onset_envelope, *, bpm, sr: float = 22050, hop_length: int = 512, tightness: float = 100,
                  trim: bool = True):
     """The tracker's intermediates for a host envelope and tempo (testing aid): a dict of NumPy arrays
     ``localscore``, ``cumscore``, ``backlink`` and the dense ``beats``."""
-    x_host = np.ascontiguousarray(onset_envelope)
-    ctx = nat.default_context()
-    x = ctx.to_device(x_host)
-    bpm_expanded, frame_rate = frames_per_beat(bpm, sr, hop_length, x.shape)
-    fpb, fpb_f64 = _check_tracker_args(bpm_expanded, frame_rate, tightness, x.shape)
-    stages = {}
-    dense, _, _ = _launch(ctx, x, fpb, fpb_f64, tightness=tightness, trim=trim, stages=stages)
-    out = {k: v.get() for k, v in stages.items()}
-    out["beats"] = dense.get()
-    return out
+    with pl.Scope() as sc:
+        x = sc.stage(onset_envelope)
+        bpm_expanded, frame_rate = frames_per_beat(bpm, sr, hop_length, x.shape)
+        fpb, fpb_f64 = _check_tracker_args(bpm_expanded, frame_rate, tightness, x.shape)
+        stages = {}
+        dense, _, _ = _launch(sc, x, fpb, fpb_f64, tightness=tightness, trim=trim, stages=stages)
+        out = {k: v.get() for k, v in stages.items()}
+        out["beats"] = dense.get()
+        return out
 
 
 
@@ -266,15 +248,7 @@ def plp(*, y=None, sr: float = 22050, onset_envelope=None, hop_length: int = 512
     from .core.spectrum import istft
     from .feature.rhythm import _Envelope, fourier_tempogram
 
-    if onset_envelope is None:
-        if y is None:
-            raise ParameterError("Input signal must be provided to compute a spectrogram")
-        pl.precheck_signal(y)
-    elif isinstance(onset_envelope, nat.DeviceArray):
-        if onset_envelope.dtype not in (np.float32, np.float64) or onset_envelope.layout != "c":
-            raise ParameterError("device onset envelope must be a C-ordered float32 or float64 DeviceArray")
-    elif np.asarray(onset_envelope).dtype not in (np.float32, np.float64):
-        raise nat.UnsupportedOnGPU("onset_envelope must be float32 or float64 on the GPU")
+    pl.check_envelope(y, onset_envelope, "Input signal must be provided to compute a spectrogram")
     if tempo_min is not None and tempo_max is not None and tempo_max <= tempo_min:
         raise ParameterError(f"tempo_max={tempo_max} must be larger than tempo_min={tempo_min}")
     freqs = fourier_tempo_frequencies(sr=sr, hop_length=hop_length, win_length=win_length)
@@ -284,20 +258,19 @@ def plp(*, y=None, sr: float = 22050, onset_envelope=None, hop_length: int = 512
     if tempo_max is not None:
         keep &= ~(freqs > tempo_max)
     logprior = None if prior is None else np.ascontiguousarray(prior.logpdf(freqs), dtype=np.float64)
-    env = _Envelope(y, sr, onset_envelope, hop_length, aggregate=np.median)
-    try:
-        env.verdict()
-        x, ctx = env.dev, env.ctx
-        ft = fourier_tempogram(onset_envelope=x, sr=sr, hop_length=hop_length, win_length=win_length)
-    finally:
-        env.release()
-    select_peaks(ft, keep, logprior)
-    n = x.shape[-1]
-    pulse = istft(ft, hop_length=1, n_fft=win_length, length=n)
-    ft.free()
-    nat.check(nat.lib().b2l_plp_finish(ctx.handle, _vp(pulse.ptr), pl.clip_count(pulse.shape[:-1]), n,
-                                       int(pulse.dtype == np.float64)))
-    if pl.status_word(ctx) & 4:
-        pulse.free()
-        raise ParameterError("Input must be finite")
-    return pulse if env.on_device else pl.finish(pulse)
+    with pl.Scope(y if onset_envelope is None else onset_envelope) as sc:
+        env = _Envelope(y, sr, onset_envelope, hop_length, aggregate=np.median)
+        try:
+            env.verdict()
+            x, ctx = env.dev, env.ctx
+            ft = sc.own(fourier_tempogram(onset_envelope=x, sr=sr, hop_length=hop_length, win_length=win_length))
+        finally:
+            env.release()
+        select_peaks(ft, keep, logprior)
+        n = x.shape[-1]
+        pulse = sc.own(istft(ft, hop_length=1, n_fft=win_length, length=n))
+        nat.check(nat.lib().b2l_plp_finish(ctx.handle, _vp(pulse.ptr), pl.clip_count(pulse.shape[:-1]), n,
+                                           int(pulse.dtype == np.float64)))
+        if pl.status_word(ctx) & nat.STATUS_NOT_FINITE_VALUE:
+            raise ParameterError("Input must be finite")
+        return sc.result(pulse)

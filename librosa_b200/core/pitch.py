@@ -196,20 +196,15 @@ class _Frames:
                                 min_period=self.min_period, max_period=self.max_period, sr=float(sr))
         self.y = y
 
-    def cmnd(self):
-        """Stage the signal and run the CMND kernel: (staged input, device pointer of [rows][n_lags] float32)."""
+    def cmnd(self, sc):
+        """Stage the signal and run the CMND kernel: (staged input, [rows][n_lags] float32 owned by ``sc``)."""
         staged = pl.StagedInput(self.y)
-        ctx = staged.ctx
         self.rows = staged.n_clips * self.n_frames
-        d_cmnd = ctx.alloc(self.rows * self.n_lags * 4)
-        try:
-            nat.check(nat.lib().b2l_yin_cmnd(ctx.handle, C.byref(self.desc), _vp(staged.dev.ptr), staged.n_clips,
-                                             staged.n, staged.n, _vp(d_cmnd)))
-            staged.scan_uncovered(self.frame_length, self.hop, self.frame_length, self.center, self.n_frames)
-        except Exception:
-            ctx.free(d_cmnd)
-            raise
-        return staged, d_cmnd
+        cmnd = sc.empty((self.rows, self.n_lags), np.float32)
+        nat.check(nat.lib().b2l_yin_cmnd(sc.ctx.handle, C.byref(self.desc), _vp(staged.dev.ptr), staged.n_clips,
+                                         staged.n, staged.n, _vp(cmnd.ptr)))
+        staged.scan_uncovered(self.frame_length, self.hop, self.frame_length, self.center, self.n_frames)
+        return staged, cmnd
 
 
 def yin(y: np.ndarray, *, fmin: float, fmax: float, sr: float = 22050, frame_length: int = 2048,
@@ -221,16 +216,13 @@ def yin(y: np.ndarray, *, fmin: float, fmax: float, sr: float = 22050, frame_len
     ``f0`` (..., n_frames): a NumPy array for host input, a DeviceArray for device input."""
     fr = _Frames(y, fmin=fmin, fmax=fmax, sr=sr, frame_length=frame_length, hop_length=hop_length, center=center,
                  pad_mode=pad_mode)
-    staged, d_cmnd = fr.cmnd()
-    ctx = staged.ctx
-    try:
-        f0 = nat.DeviceArray.empty(ctx, staged.lead + (fr.n_frames,), np.float64)
+    with pl.Scope(y) as sc:
+        staged, cmnd = fr.cmnd(sc)
+        f0 = sc.empty(staged.lead + (fr.n_frames,), np.float64)
         fr.desc.trough_threshold = float(trough_threshold)
-        nat.check(nat.lib().b2l_yin_pick(ctx.handle, C.byref(fr.desc), _vp(d_cmnd), fr.rows, _vp(f0.ptr)))
-    finally:
-        ctx.free(d_cmnd)
-    staged.release()
-    return staged.result(f0)
+        nat.check(nat.lib().b2l_yin_pick(sc.ctx.handle, C.byref(fr.desc), _vp(cmnd.ptr), fr.rows, _vp(f0.ptr)))
+        staged.release()
+        return sc.result(f0, validate=True)
 
 
 @lru_cache(maxsize=8)
@@ -362,26 +354,20 @@ def pyin(y: np.ndarray, *, fmin: float, fmax: float, sr: float = 22050, frame_le
                                       resolution=resolution, max_transition_rate=max_transition_rate,
                                       switch_prob=switch_prob, no_trough_prob=no_trough_prob, fill_na=fill_na,
                                       transition_min_prob=transition_min_prob)
-    staged, d_cmnd = fr.cmnd()
-    lead, rows = staged.lead, fr.rows
-    L = nat.lib()
-    d_count = ctx.alloc(rows * 4)
-    d_bin = ctx.alloc(rows * max_cand * 4)
-    d_prob = ctx.alloc(rows * max_cand * 8)
-    d_states = ctx.alloc(rows * 2)
-    try:
-        vp = nat.DeviceArray.empty(ctx, lead + (fr.n_frames,), np.float64)
-        f0 = nat.DeviceArray.empty(ctx, lead + (fr.n_frames,), np.float64)
-        vf = nat.DeviceArray.empty(ctx, lead + (fr.n_frames,), np.bool_)
-        nat.check(L.b2l_pyin_obs(ctx.handle, C.byref(desc), _vp(d_cmnd), rows, _vp(d_count), _vp(d_bin), _vp(d_prob),
-                                 _vp(vp.ptr)))
-        nat.check(L.b2l_viterbi(ctx.handle, C.byref(desc), _vp(d_count), _vp(d_bin), _vp(d_prob), _vp(vp.ptr),
-                                staged.n_clips, fr.n_frames, _vp(d_states), _vp(f0.ptr), _vp(vf.ptr)))
-    finally:
-        for p in (d_cmnd, d_count, d_bin, d_prob, d_states):
-            ctx.free(p)
-    staged.release()
-    if staged.on_device:
-        return f0, vf, vp
-    out_f0 = pl.finish(f0, validate=True)
-    return out_f0, pl.finish(vf), pl.finish(vp)
+    with pl.Scope(y) as sc:
+        staged, cmnd = fr.cmnd(sc)
+        lead, rows = staged.lead, fr.rows
+        L = nat.lib()
+        count = sc.empty((rows,), np.int32)
+        bins = sc.empty((rows, max_cand), np.int32)
+        prob = sc.empty((rows, max_cand), np.float64)
+        states = sc.empty((rows,), np.uint16)
+        vp = sc.empty(lead + (fr.n_frames,), np.float64)
+        f0 = sc.empty(lead + (fr.n_frames,), np.float64)
+        vf = sc.empty(lead + (fr.n_frames,), np.bool_)
+        nat.check(L.b2l_pyin_obs(ctx.handle, C.byref(desc), _vp(cmnd.ptr), rows, _vp(count.ptr), _vp(bins.ptr),
+                                 _vp(prob.ptr), _vp(vp.ptr)))
+        nat.check(L.b2l_viterbi(ctx.handle, C.byref(desc), _vp(count.ptr), _vp(bins.ptr), _vp(prob.ptr), _vp(vp.ptr),
+                                staged.n_clips, fr.n_frames, _vp(states.ptr), _vp(f0.ptr), _vp(vf.ptr)))
+        staged.release()
+        return sc.result(f0, validate=True), sc.result(vf), sc.result(vp)

@@ -374,8 +374,7 @@ def _to_db_f64(ctx, S, ref, amin, top_db, amplitude):
     if ref_value.size > 1:
         parts = []
         for i in range(n_lead):                     # one reference level per leading index
-            one = nat.DeviceArray(ctx, dev.ptr + 8 * i * work.shape[-2] * work.shape[-1], (1,) + work.shape[-2:], np.float64,
-                                  owner=False)
+            one = dev.view((1,) + work.shape[-2:], offset=i * work.shape[-2] * work.shape[-1])
             parts.append(f64.power_to_db(ctx, one, ref_value=float(ref_value[i]), amin=amin, top_db=top_db))
         res = np.concatenate([pl.finish(p) for p in parts], axis=0)
     else:

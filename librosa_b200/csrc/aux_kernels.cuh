@@ -327,7 +327,7 @@ __global__ void finite_scan_kernel(const float* __restrict__ y, long long stride
          i += (long long)gridDim.x * blockDim.x)
       bad |= !(fabsf(yc[i]) <= 3.0e38f);
   }
-  if (bad) *status = 1;
+  if (bad) *status = B2L_STATUS_NOT_FINITE_SAMPLE;
 }
 // The same scan over float64 signals (the FP64 path): flags exactly what np.isfinite rejects.
 __global__ void finite_scan64_kernel(const double* __restrict__ y, long long stride, int n, int begin,
@@ -339,7 +339,7 @@ __global__ void finite_scan64_kernel(const double* __restrict__ y, long long str
          i += (long long)gridDim.x * blockDim.x)
       bad |= !isfinite(yc[i]);
   }
-  if (bad) *status = 1;
+  if (bad) *status = B2L_STATUS_NOT_FINITE_SAMPLE;
 }
 
 // ------------------------------------------------------------------ Griffin-Lim phase update

@@ -16,6 +16,8 @@
 #include <math.h>
 #include <stdint.h>
 
+#include "../../include/b2l.h"
+
 namespace b2l_beat {
 
 struct BeatArgs {
@@ -397,8 +399,8 @@ __global__ void plp_select_kernel(C* __restrict__ X, long long n_frames, int n_b
 }
 
 // One CTA per row of the pulse x [rows][n]: x = max(x, 0) (NaN stays), then x / max|x| (1 when below tiny), as
-// util.normalize(norm=inf, axis=-1).  A non-finite value sets bit 2 of the status word (normalize's "Input must be
-// finite").
+// util.normalize(norm=inf, axis=-1).  A non-finite value sets B2L_STATUS_NOT_FINITE_VALUE (normalize's "Input must
+// be finite").
 template <class T>
 __global__ void plp_finish_kernel(T* __restrict__ x, int n, int* __restrict__ status) {
   __shared__ T s_max[32];
@@ -427,7 +429,7 @@ __global__ void plp_finish_kernel(T* __restrict__ x, int n, int* __restrict__ st
     for (int w = 0; w < (int)(blockDim.x >> 5); ++w) r = s_max[w] > r ? s_max[w] : r;
     const T tiny = sizeof(T) == 4 ? (T)1.17549435e-38f : (T)2.2250738585072014e-308;
     s_max[0] = r < tiny ? T(1) : r;
-    if (s_bad) atomicOr(status, 4);
+    if (s_bad) atomicOr(status, B2L_STATUS_NOT_FINITE_VALUE);
   }
   __syncthreads();
   const T len = s_max[0];

@@ -3,6 +3,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "../../include/b2l.h"   // enum b2l_status_bit
+
 namespace b2l {
 
 enum PadMode : int {   // librosa/_typing.py:60-71 (_PadModeSTFT); callables are rejected on the host
@@ -98,7 +100,7 @@ struct FwdArgs {
   int out_tiled;             // MODE_MEL: out_r is the mfcc scratch [clip][tile of 64 frames][mel][64] (dct_clamp4_kernel)
   float amin, db_sub;
   unsigned int* clip_max;    // order-preserving uint keys of the per-clip max (log_mode)
-  int* status;               // bit 0 is set when a non-finite sample reached a frame (util.valid_audio)
+  int* status;               // B2L_STATUS_NOT_FINITE_SAMPLE: a non-finite sample reached a frame (util.valid_audio)
   StatsParams stats;         // MODE_STATS (the frequency table travels in mel_w / mel_w_count)
   // dynamic shared-memory layout (byte offsets)
   int off_win, off_tw, off_in, off_xbuf, off_melw, off_melband, off_bar;

@@ -88,7 +88,7 @@ __global__ void __launch_bounds__(NW * 32, 1) czt_kernel(const CztArgs a) {
       return make_float2(fmaf(xa, w.x, -xb * w.y), fmaf(xa, w.y, xb * w.x));      // (xa + i xb) * w
     });
     fft_forward<Cfg>(v, t, gbar, xbuf, s_tw);
-    if (live_a && !(fabsf(v[0].x) + fabsf(v[0].y) <= 3.0e38f)) *a.status = 1;   // util.valid_audio
+    if (live_a && !(fabsf(v[0].x) + fabsf(v[0].y) <= 3.0e38f)) *a.status = B2L_STATUS_NOT_FINITE_SAMPLE;   // util.valid_audio
     // C = A . FFT(h)/P in registers, published (re/im swapped) for the inverse transform's first pass
     if constexpr (Cfg::NPASS > 1) group_sync<TPF>(gbar);
     static_for<0, PPT>([&](auto S) {

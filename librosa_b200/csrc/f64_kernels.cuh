@@ -111,7 +111,7 @@ __global__ void stft64_kernel(const F64FwdArgs a) {
       orow[k] = make_double2(re, im);
     }
   }
-  if (bad) *a.status = 1;
+  if (bad) *a.status = B2L_STATUS_NOT_FINITE_SAMPLE;
 }
 
 struct F64InvArgs {

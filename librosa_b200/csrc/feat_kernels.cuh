@@ -10,7 +10,7 @@
 namespace b2l {
 
 // S [n_rows][F] (one row per (clip, frame), bins contiguous) -> out [clip][N_STATS][n_frames].
-// One warp per row: coalesced copy into shared memory, then frame_stats.  Sets bit 1 of *status when a
+// One warp per row: coalesced copy into shared memory, then frame_stats.  Sets B2L_STATUS_NEGATIVE_ENTRY when a
 // negative entry is seen (the reference raises "only defined with non-negative energies").
 __global__ void stats_kernel(const float* __restrict__ S, long long n_rows, int n_frames, int F,
                              const float* __restrict__ freq, StatsParams sp, float* __restrict__ out, int* status) {
@@ -27,7 +27,7 @@ __global__ void stats_kernel(const float* __restrict__ S, long long n_rows, int 
     __syncwarp();
     bool negative;
     const float v = frame_stats(s_row, s_freq, F, lane, sp, &negative);
-    if (negative && lane == 0) atomicOr(status, 2);
+    if (negative && lane == 0) atomicOr(status, B2L_STATUS_NEGATIVE_ENTRY);
     const long long clip = r / n_frames, frame = r % n_frames;
     if (lane < N_STATS) out[(clip * N_STATS + lane) * n_frames + frame] = v;
     __syncwarp();
@@ -77,7 +77,7 @@ __global__ void frame_td_kernel(const float* __restrict__ y, long long clip_stri
         const bool cross = i < L && (i == 0 ? pad_first != 0 : c != prev);
         count += __popc(__ballot_sync(0xffffffffu, cross));
       }
-      if (__any_sync(0xffffffffu, bad) && lane == 0) atomicOr(status, 1);
+      if (__any_sync(0xffffffffu, bad) && lane == 0) atomicOr(status, B2L_STATUS_NOT_FINITE_SAMPLE);
       if (lane == 0) out[r] = (float)count * out_scale;
     }
   }
@@ -178,7 +178,7 @@ __global__ void __launch_bounds__(256) frame_td_block_kernel(const float* __rest
       }
     }
   }
-  if (what != 0 && __any_sync(0xffffffffu, bad) && lane == 0) atomicOr(status, 1);
+  if (what != 0 && __any_sync(0xffffffffu, bad) && lane == 0) atomicOr(status, B2L_STATUS_NOT_FINITE_SAMPLE);
   __syncthreads();
   for (int f = threadIdx.x; f < TD_FRAMES; f += blockDim.x) {
     const int t = t0 + f;

@@ -355,7 +355,7 @@ __global__ void __launch_bounds__(NW * 32, 1) fwd_kernel(const FwdArgs a) {
     // util.valid_audio (librosa/util/utils.py:303-306) on the device: one NaN / Inf sample makes every
     // bin of every frame that reads it non-finite, so testing one spectrum value per thread and frame
     // catches it without a separate pass over the input.
-    if (frame_ok && !(fabsf(v[0].x) + fabsf(v[0].y) <= 3.0e38f)) *a.status = 1;
+    if (frame_ok && !(fabsf(v[0].x) + fabsf(v[0].y) <= 3.0e38f)) *a.status = B2L_STATUS_NOT_FINITE_SAMPLE;
 
     if constexpr (MODE == MODE_STFT) {
       float2* orow = a.out_c + ((long long)clip * a.n_frames + frame) * (M + 1);

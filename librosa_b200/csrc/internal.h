@@ -97,7 +97,7 @@ struct b2l_ctx {
   struct ncclComm* comm = nullptr;
   int rank = 0, world = 1;
   unsigned int* d_clip_max = nullptr;   // scratch for per-clip maxima
-  int* d_status = nullptr;              // bit 0: a non-finite input sample was seen since the last reset
+  int* d_status = nullptr;              // enum b2l_status_bit flags set since the last reset
   float* d_scratch = nullptr;           // grow-only scratch (istft frames, pip_pass histograms)
   size_t scratch_bytes = 0;
   size_t clip_max_cap = 0;

@@ -255,7 +255,7 @@ __global__ void __launch_bounds__(512, 2) mr_kernel(const MrArgs a) {
     if (MODE == 0 || a.power_mode == 2) unmix([](float p2) { return p2; });
     else if (a.power_mode == 1) unmix([](float p2) { return sqrt_approx(p2); });
     else unmix([&](float p2) { return power_from_sq(p2, a.power_mode, a.power); });
-    if (bad) *a.status = 1;   // util.valid_audio (librosa/util/utils.py:303-306): a non-finite sample poisons every bin
+    if (bad) *a.status = B2L_STATUS_NOT_FINITE_SAMPLE;   // util.valid_audio (librosa/util/utils.py:303-306): a non-finite sample poisons every bin
     if constexpr (MODE == 2) {
       __syncwarp();
       if (a.log_mode && clip != wmax_clip) {

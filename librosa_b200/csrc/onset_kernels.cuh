@@ -17,6 +17,8 @@
 #include <math.h>
 #include <stdint.h>
 
+#include "../../include/b2l.h"
+
 namespace b2l_onset {
 
 // verdict flags (word 0 of the flags pair; word 1 is the pick count)
@@ -24,7 +26,6 @@ constexpr int kNonzero = 1, kNonfinite = 2;
 constexpr int kGreedy = 0, kDpCount = 1, kDpValue = 2;
 constexpr int kChunk = 8192;              // frames per candidate bitmask in shared memory
 constexpr int kWords = kChunk / 32;
-constexpr int kStatusNegativeEvent = 8;   // bit 3 of the status word: a device event list holds a negative frame
 
 __device__ __forceinline__ float sub_rn(float a, float b) { return __fsub_rn(a, b); }
 __device__ __forceinline__ double sub_rn(double a, double b) { return __dsub_rn(a, b); }
@@ -259,7 +260,7 @@ __global__ void __launch_bounds__(256) peak_pick_kernel(PeakArgs a) {
 // One CTA.  energy [n] (T): a minimum is a frame 1 <= i <= n - 2 with e[i] <= e[i-1] and e[i] < e[i+1]; frame 0
 // always counts.  last[i] = the last minimum at or before i (block max-scan in chunks with a carry), then
 // out[k] = last[min(events[k], n - 1)] in the requested units.  events [n_events] int64, of which *count are used
-// when count != NULL; a negative event sets kStatusNegativeEvent in *status and writes nothing.
+// when count != NULL; a negative event sets B2L_STATUS_NEGATIVE_EVENT in *status and writes nothing.
 template <class T>
 __global__ void __launch_bounds__(1024) onset_backtrack_kernel(const T* __restrict__ e, int n,
                                                                const long long* __restrict__ events,
@@ -273,7 +274,7 @@ __global__ void __launch_bounds__(1024) onset_backtrack_kernel(const T* __restri
   bool neg = false;
   for (long long k = threadIdx.x; k < m; k += blockDim.x) neg |= events[k] < 0;
   if (__syncthreads_or(neg)) {
-    if (threadIdx.x == 0) atomicOr(status, kStatusNegativeEvent);
+    if (threadIdx.x == 0) atomicOr(status, B2L_STATUS_NEGATIVE_EVENT);
     return;
   }
   if (threadIdx.x == 0) s_carry = 0;

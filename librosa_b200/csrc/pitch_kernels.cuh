@@ -146,7 +146,7 @@ __global__ void __launch_bounds__(256) yin_cmnd_kernel(const YinCmndArgs a) {
         dsum = __shfl_sync(0xffffffffu, ds, GS - 1, GS);
       }
     }
-    if (store && bad && a.status) atomicOr(a.status, 1);
+    if (store && bad && a.status) atomicOr(a.status, B2L_STATUS_NOT_FINITE_SAMPLE);
     group_sync<TPF>(gbar);    // r[] is read before the next round overwrites the exchange area
   }
 }

@@ -24,7 +24,7 @@ struct TempogramArgs {
   int norm;               // B2L_TG_NORM_*
   double norm_p;          // the exponent of B2L_TG_NORM_P
   double* out;            // [rows][n_frames][win]
-  int* status;            // bit 2: a value of the autocorrelation is not finite
+  int* status;            // B2L_STATUS_NOT_FINITE_VALUE: a value of the autocorrelation is not finite
 };
 
 // Dynamic shared memory of tempogram_kernel in doubles: z [M] double2, p [M + 1], window [win], reduction [32].
@@ -126,7 +126,7 @@ __global__ void tempogram_kernel(const TempogramArgs a) {
   if (length < DBL_MIN) length = 1.0;      // below tiny(float64): left as it is
   double* o = a.out + item * W;
   for (int k = threadIdx.x; k < W; k += blockDim.x) o[k] = p[k] / length;
-  if (bad && a.status) atomicOr(a.status, 4);
+  if (bad && a.status) atomicOr(a.status, B2L_STATUS_NOT_FINITE_VALUE);
 }
 
 struct TempoArgs {

@@ -110,13 +110,10 @@ def pitch_shift(y, *, sr: float, n_steps: float, bins_per_octave: int = 12, res_
         ctx = shifted.ctx
         lead = shifted.shape[:-1]
         rows = pl.clip_count(lead)
-        out = nat.DeviceArray.empty(ctx, tuple(lead) + (n,), np.float32)
-        L = nat.lib()
-        if m < n:
-            nat.check(L.b2l_memset(ctx.handle, C.c_void_p(out.ptr), 0, out.nbytes))
+        out = (ctx.zeros if m < n else ctx.empty)(tuple(lead) + (n,), np.float32)
         if rows and min(m, n):
-            nat.check(L.b2l_copy2d(ctx.handle, C.c_void_p(out.ptr), n * 4, C.c_void_p(shifted.ptr), m * 4,
-                                   min(m, n) * 4, rows))
+            nat.check(nat.lib().b2l_copy2d(ctx.handle, C.c_void_p(out.ptr), n * 4, C.c_void_p(shifted.ptr), m * 4,
+                                           min(m, n) * 4, rows))
         shifted.free()
     staged.release()
     return staged.result(out, req)

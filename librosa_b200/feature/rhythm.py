@@ -15,6 +15,7 @@ import numpy as np
 from .. import _native as nat
 from .. import _pipeline as pl
 from .. import filters
+from .._pipeline import Envelope as _Envelope
 from ..core.convert import tempo_frequencies
 from ..util.exceptions import ParameterError
 
@@ -23,7 +24,6 @@ _vp = C.c_void_p
 __all__ = ["tempogram", "fourier_tempogram", "tempo"]
 
 MAX_WIN_LENGTH = 4096   # csrc/rhythm_api.cu: the packed FP64 transform of 8192 points fills 64 KB of shared memory
-_STATUS_NOT_FINITE = 4  # bit 2 of the status word: a tempogram value is not finite (b2l_tempogram)
 
 
 def _norm_mode(norm):
@@ -55,15 +55,7 @@ class _Front:
         if win_length < 1:
             raise ParameterError("win_length must be a positive integer")
         self.window = np.ascontiguousarray(filters.get_window(window, win_length, fftbins=True), dtype=np.float64)
-        if onset_envelope is None:
-            if y is None:
-                raise ParameterError("Either y or onset_envelope must be provided")
-            pl.precheck_signal(y)
-        elif isinstance(onset_envelope, nat.DeviceArray):
-            if onset_envelope.dtype not in (np.float32, np.float64) or onset_envelope.layout != "c":
-                raise ParameterError("device onset envelope must be a C-ordered float32 or float64 DeviceArray")
-        elif np.asarray(onset_envelope).dtype not in (np.float32, np.float64):
-            raise nat.UnsupportedOnGPU("onset_envelope must be float32 or float64 on the GPU")
+        pl.check_envelope(y, onset_envelope)
         self.mode, self.p = _norm_mode(norm)
         if win_length > MAX_WIN_LENGTH:
             raise nat.UnsupportedOnGPU(f"tempogram: win_length={win_length} exceeds the {MAX_WIN_LENGTH} onset frames "
@@ -71,56 +63,16 @@ class _Front:
         self.win_length = int(win_length)
 
 
-class _Envelope:
-    """The onset envelope of a call on the device, C-ordered (..., n).
-
-    ``y`` runs onset_strength on the device: a host signal is uploaded once and checked like util.valid_audio,
-    the envelope never leaves the GPU.  A host envelope is uploaded as it is.  The status word is cleared for this
-    call's verdict (``verdict``); ``on_device``: the caller passed device data and gets a DeviceArray back.
-    ``aggregate`` is onset_strength's (beat tracking uses np.median)."""
-
-    def __init__(self, y, sr, onset_envelope, hop_length, aggregate=None):
-        from ..onset import onset_strength
-
-        self.audio = None
-        if onset_envelope is None:
-            self.audio = pl.StagedInput(y)
-            self.dev = onset_strength(y=self.audio.dev, sr=sr, hop_length=hop_length, aggregate=aggregate)
-            self.audio.scan_all()
-            self.staged = self.audio
-        else:
-            x = onset_envelope if isinstance(onset_envelope, nat.DeviceArray) else np.asarray(onset_envelope)
-            self.staged = pl.StagedInput(x, dtype=x.dtype)
-            self.dev = self.staged.dev
-        self.on_device = self.staged.on_device
-        self.ctx = self.staged.ctx
-        if self.dev.ndim < 1:
-            raise ParameterError("onset envelope must be at least one-dimensional")
-        if self.on_device:   # a host input was staged after a reset of the status word
-            nat.check(nat.lib().b2l_status_reset(self.ctx.handle))
-
-    def release(self):
-        self.staged.release()
-        self.dev = None   # the envelope onset_strength made goes with its last reference (stream-ordered free)
-
-    def verdict(self):
-        """Raise like the reference when a kernel of this call flagged non-finite data (synchronises)."""
-        flags = pl.status_word(self.ctx)
-        if self.audio is not None and not self.on_device and flags & 1:
-            self.audio.check_finite()
-        if flags & _STATUS_NOT_FINITE:
-            raise ParameterError("Input must be finite")
-
-
-def _launch_tempogram(env: _Envelope, front: _Front, center: bool) -> nat.DeviceArray:
-    """One launch: the float64 tempogram (..., win_length, frames) in layout "ft" (lags contiguous)."""
-    ctx, x = env.ctx, env.dev
+def _launch_tempogram(sc: pl.Scope, x: nat.DeviceArray, front: _Front, center: bool) -> nat.DeviceArray:
+    """One launch on the envelope ``x``: the float64 tempogram (..., win_length, frames) in layout "ft" (lags
+    contiguous)."""
+    ctx = sc.ctx
     W, n, lead = front.win_length, x.shape[-1], x.shape[:-1]
     padded = n + (2 * (W // 2) if center else 0)
     if padded < W:
         raise ParameterError(f"Input is too short (n={padded:d}) for frame_length={W:d}")
     T = n if center else n - W + 1
-    out = nat.DeviceArray.empty(ctx, lead + (W, T), np.float64, layout="ft")
+    out = sc.empty(lead + (W, T), np.float64, layout="ft")
     desc = nat.TempogramDesc(win_length=W, center=int(bool(center)), norm=front.mode,
                              env_f64=int(x.dtype == np.float64), norm_p=front.p)
     d_win = pl.f64_constant(ctx, ("tempogram_window", pl.digest(front.window)), front.window)
@@ -136,17 +88,14 @@ def tempogram(*, y=None, sr: float = 22050, onset_envelope=None, hop_length: int
     Returns float64 ``(..., win_length, n)``: a NumPy array for host input, a DeviceArray in layout "ft" (memory
     ``[...][frame][lag]``) for device input."""
     front = _Front(y, onset_envelope, win_length, window, norm)
-    env = _Envelope(y, sr, onset_envelope, hop_length)
-    try:
-        out = _launch_tempogram(env, front, center)
-    finally:
-        env.release()
-    try:
+    with pl.Scope(y if onset_envelope is None else onset_envelope) as sc:
+        env = _Envelope(y, sr, onset_envelope, hop_length)
+        try:
+            out = _launch_tempogram(sc, env.dev, front, center)
+        finally:
+            env.release()
         env.verdict()
-    except ParameterError:
-        out.free()
-        raise
-    return out if env.on_device else pl.finish(out)
+        return sc.result(out)
 
 
 def fourier_tempogram(*, y=None, sr: float = 22050, onset_envelope=None, hop_length: int = 512,
@@ -198,43 +147,35 @@ def tempo(*, y=None, sr: float = 22050, onset_envelope=None, tg=None, hop_length
         raise nat.UnsupportedOnGPU("tempo: only aggregate=np.mean or None is computed on the GPU (no CPU fallback)")
     bpms, logprior = _prior_tables(win_length, sr=sr, hop_length=hop_length, start_bpm=start_bpm, std_bpm=std_bpm,
                                    max_tempo=max_tempo, prior=prior)
-    env = None
-    own_tg = False
-    if front is not None:
-        env = _Envelope(y, sr, onset_envelope, hop_length)
-        try:
-            d_tg = _launch_tempogram(env, front, center=True)
-        finally:
-            env.release()
-        own_tg, on_device, ctx = True, env.on_device, env.ctx
-    elif isinstance(tg, nat.DeviceArray):
-        if tg.dtype not in (np.float32, np.float64) or tg.layout not in ("c", "ft"):
-            raise ParameterError("device tempogram must be float32 or float64 in layout 'c' or 'ft'")
-        d_tg, on_device, ctx = tg, True, tg.ctx
-    else:
-        tg = np.asarray(tg)
-        dtype = tg.dtype if tg.dtype in (np.float32, np.float64) else np.dtype(np.float64)
-        d_tg, own_tg = pl.to_native(tg, dtype=dtype, host_transpose=True)
-        on_device, ctx = False, d_tg.ctx
-    lead, F = d_tg.shape[:-2], d_tg.shape[-1]
-    mean = aggregate is not None
-    out = nat.DeviceArray.empty(ctx, lead + ((1,) if mean else (F,)), np.float64)
-    ft = d_tg.layout == "ft"
-    desc = nat.TempoDesc(n_lags=win_length, mean=int(mean), tg_f64=int(d_tg.dtype == np.float64), n_frames=F,
-                         row_stride=win_length * F, lag_stride=1 if ft else F, frame_stride=win_length if ft else 1)
-    key = ("tempo", pl.digest(bpms), pl.digest(logprior))
-    d_bpms = pl.f64_constant(ctx, key + ("bpms",), bpms)
-    d_logprior = pl.f64_constant(ctx, key + ("logprior",), logprior)
-    try:
+    source = tg if tg is not None else y if onset_envelope is None else onset_envelope
+    with pl.Scope(source) as sc:
+        env = None
+        if front is not None:
+            env = _Envelope(y, sr, onset_envelope, hop_length)
+            try:
+                d_tg = _launch_tempogram(sc, env.dev, front, center=True)
+            finally:
+                env.release()
+        elif isinstance(tg, nat.DeviceArray):
+            if tg.dtype not in (np.float32, np.float64) or tg.layout not in ("c", "ft"):
+                raise ParameterError("device tempogram must be float32 or float64 in layout 'c' or 'ft'")
+            d_tg = tg
+        else:
+            tg = np.asarray(tg)
+            dtype = tg.dtype if tg.dtype in (np.float32, np.float64) else np.dtype(np.float64)
+            d_tg = sc.own(pl.to_native(tg, dtype=dtype, host_transpose=True)[0])
+        ctx = sc.ctx
+        lead, F = d_tg.shape[:-2], d_tg.shape[-1]
+        mean = aggregate is not None
+        out = sc.empty(lead + ((1,) if mean else (F,)), np.float64)
+        ft = d_tg.layout == "ft"
+        desc = nat.TempoDesc(n_lags=win_length, mean=int(mean), tg_f64=int(d_tg.dtype == np.float64), n_frames=F,
+                             row_stride=win_length * F, lag_stride=1 if ft else F, frame_stride=win_length if ft else 1)
+        key = ("tempo", pl.digest(bpms), pl.digest(logprior))
+        d_bpms = pl.f64_constant(ctx, key + ("bpms",), bpms)
+        d_logprior = pl.f64_constant(ctx, key + ("logprior",), logprior)
         nat.check(nat.lib().b2l_tempo(ctx.handle, C.byref(desc), _vp(d_tg.ptr), pl.clip_count(lead), _vp(d_logprior),
                                       _vp(d_bpms), _vp(out.ptr)))
-    finally:
-        if own_tg:
-            d_tg.free()
-    if env is not None:
-        try:
+        if env is not None:
             env.verdict()
-        except ParameterError:
-            out.free()
-            raise
-    return out if on_device else pl.finish(out)
+        return sc.result(out)

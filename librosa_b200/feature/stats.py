@@ -83,7 +83,7 @@ def _stats_from_S(S, desc, freq, sr, n_fft, what, check_negative=True):
         src.free()
     if not on_device:
         Sd.free()
-    if check_negative and pl.status_word(ctx) & 2:
+    if check_negative and pl.status_word(ctx) & nat.STATUS_NEGATIVE_ENTRY:
         stats.free()
         raise ParameterError(f"{what} is only defined with non-negative energies")
     return stats, ctx, lead, T, on_device, req, fdtype

@@ -74,55 +74,51 @@ def onset_strength_multi(*, y=None, sr: float = 22050, S=None, n_fft: int = 2048
             raise nat.UnsupportedOnGPU(f"median onset aggregation over a channel of {widest} rows: the GPU kernel takes "
                                        f"up to {MAX_MEDIAN_ROWS} (no CPU fallback)")
 
-    staged = None
-    if S is None:
-        if y is None:
-            raise ParameterError("Input signal must be provided to compute a spectrogram")
-        _, req = pl.precheck_signal(y)
-        # one upload, every intermediate on the device; the mel frames are always centred (``center`` only
-        # sets the pad width below)
-        staged = pl.StagedInput(y)
-        mel = melspectrogram(y=staged.dev, sr=sr, n_fft=n_fft, hop_length=hop_length, **kwargs)
-        staged.scan_uncovered(n_fft, hop_length, kwargs.get("win_length"), True, mel.shape[-1])
-        Sd = power_to_db(mel)
-        mel.free()
-        res_dtype = np.dtype(req)
-    else:
-        if not isinstance(S, nat.DeviceArray):
-            S = np.atleast_2d(np.asarray(S))
-        Sd, res_dtype, on_device = pl.spectrogram_input(S)
-        if Sd.layout != "c":
-            raise ParameterError("device spectrogram must be C-ordered (..., rows, frames)")
-    if Sd.ndim < 2:
-        raise ParameterError("spectrogram input must have at least two dimensions")
-    rows, T = Sd.shape[-2], Sd.shape[-1]
-    if T <= lag:
-        raise ParameterError(f"lag={lag} needs more than {T} frames")
-    ctx = Sd.ctx
-    lead = Sd.shape[:-2]
-    desc = nat.OnsetDesc(lag=int(lag), max_size=int(max_size), detrend=int(bool(detrend)),
-                         pad_width=int(lag) + (n_fft // (2 * hop_length) if center else 0))
-    if callable(aggregate):
-        edges = _edges([slice(None)] if channels is None else list(channels), rows, channels is None)
-        if len(edges) - 1 > 32:
-            raise nat.UnsupportedOnGPU("at most 32 onset channels are supported on the GPU")
-        desc.n_channels = len(edges) - 1
-        for i, e in enumerate(edges):
-            desc.bounds[i] = e
-        n_out = len(edges) - 1
-    else:
-        desc.n_channels = 0
-        n_out = rows
-    out = nat.DeviceArray.empty(ctx, tuple(lead) + (n_out, T), np.float32)
-    entry = nat.lib().b2l_onset_median_from_spec if aggregate is np.median else nat.lib().b2l_onset_from_spec
-    nat.check(entry(ctx.handle, C.byref(desc), _vp(Sd.ptr), pl.clip_count(lead), rows, T, _vp(out.ptr)))
-    if staged is not None or not on_device:
-        Sd.free()
-    if detrend:   # scipy.signal.lfilter with float64 coefficients returns float64
-        res_dtype = np.result_type(res_dtype, np.float64)
-    if staged is not None:
-        return staged.result(out, res_dtype)
-    return out if on_device else pl.finish(out, res_dtype)
+    with pl.Scope(y if S is None else S) as sc:
+        if S is None:
+            if y is None:
+                raise ParameterError("Input signal must be provided to compute a spectrogram")
+            _, req = pl.precheck_signal(y)
+            # one upload, every intermediate on the device; the mel frames are always centred (``center`` only
+            # sets the pad width below)
+            staged = pl.StagedInput(y)
+            mel = melspectrogram(y=staged.dev, sr=sr, n_fft=n_fft, hop_length=hop_length, **kwargs)
+            staged.scan_uncovered(n_fft, hop_length, kwargs.get("win_length"), True, mel.shape[-1])
+            Sd = sc.own(power_to_db(mel))
+            mel.free()
+            res_dtype = np.dtype(req)
+        else:
+            if not isinstance(S, nat.DeviceArray):
+                S = np.atleast_2d(np.asarray(S))
+            Sd, res_dtype, _ = pl.spectrogram_input(S)
+            sc.own(Sd)
+            if Sd.layout != "c":
+                raise ParameterError("device spectrogram must be C-ordered (..., rows, frames)")
+        if Sd.ndim < 2:
+            raise ParameterError("spectrogram input must have at least two dimensions")
+        rows, T = Sd.shape[-2], Sd.shape[-1]
+        if T <= lag:
+            raise ParameterError(f"lag={lag} needs more than {T} frames")
+        lead = Sd.shape[:-2]
+        desc = nat.OnsetDesc(lag=int(lag), max_size=int(max_size), detrend=int(bool(detrend)),
+                             pad_width=int(lag) + (n_fft // (2 * hop_length) if center else 0))
+        if callable(aggregate):
+            edges = _edges([slice(None)] if channels is None else list(channels), rows, channels is None)
+            if len(edges) - 1 > 32:
+                raise nat.UnsupportedOnGPU("at most 32 onset channels are supported on the GPU")
+            desc.n_channels = len(edges) - 1
+            for i, e in enumerate(edges):
+                desc.bounds[i] = e
+            n_out = len(edges) - 1
+        else:
+            desc.n_channels = 0
+            n_out = rows
+        out = sc.empty(tuple(lead) + (n_out, T), np.float32)
+        entry = nat.lib().b2l_onset_median_from_spec if aggregate is np.median else nat.lib().b2l_onset_from_spec
+        nat.check(entry(sc.ctx.handle, C.byref(desc), _vp(Sd.ptr), pl.clip_count(lead), rows, T, _vp(out.ptr)))
+        if detrend:   # scipy.signal.lfilter with float64 coefficients returns float64
+            res_dtype = np.result_type(res_dtype, np.float64)
+        return sc.result(out, res_dtype, validate=S is None)
 
 
 def onset_strength(*, y=None, sr: float = 22050, S=None, lag: int = 1, max_size: int = 1, ref=None,
@@ -134,16 +130,12 @@ def onset_strength(*, y=None, sr: float = 22050, S=None, lag: int = 1, max_size:
     odf = onset_strength_multi(y=y, sr=sr, S=S, lag=lag, max_size=max_size, ref=ref, detrend=detrend, center=center,
                                feature=feature, aggregate=aggregate, channels=None, **kwargs)
     if isinstance(odf, nat.DeviceArray):
-        # (..., 1, T) -> (..., T): same memory without the unit axis; the view keeps the owner alive
-        view = nat.DeviceArray(odf.ctx, odf.ptr, odf.shape[:-2] + odf.shape[-1:], odf.dtype, layout="c", owner=False)
-        view._base = odf
-        return view
+        return odf.view(odf.shape[:-2] + odf.shape[-1:])   # (..., 1, T) -> (..., T)
     return odf[..., 0, :]
 
 
 _EMPTY_MATCH = "Attempting to match empty event list"
 _NEGATIVE_MATCH = "Cannot match events with right=False and min(events_to) > min(events_from)"
-_STATUS_NEGATIVE_EVENT = 8   # bit 3 of the status word (b2l_onset_backtrack)
 _PEAK_KEYS = ("pre_max", "post_max", "pre_avg", "post_avg", "delta", "wait", "method")
 
 
@@ -175,12 +167,7 @@ def _empty(shape, sparse, units, ctx, on_device):
     if sparse:
         dtype = np.float64 if units == "time" else np.int64
         return nat.DeviceArray.empty(ctx, (0,), dtype) if on_device else np.array([], dtype=dtype)
-    if on_device:
-        out = nat.DeviceArray.empty(ctx, shape, np.bool_)
-        if out.nbytes:
-            nat.check(nat.lib().b2l_memset(ctx.handle, _vp(out.ptr), 0, out.nbytes))
-        return out
-    return np.zeros(shape, dtype=bool)
+    return ctx.zeros(shape, np.bool_) if on_device else np.zeros(shape, dtype=bool)
 
 
 def _check_units(sparse, units):
@@ -188,12 +175,12 @@ def _check_units(sparse, units):
         raise ParameterError(f"Invalid unit type: {units}")
 
 
-def _normalize(x, normalize):
+def _normalize(sc, x, normalize):
     """One launch: the normalised envelope (None when ``normalize`` is off) and the verdict pair
-    (int64 [2]: flags, pick count)."""
-    ctx = x.ctx
-    flags = nat.DeviceArray.empty(ctx, (2,), np.int64)
-    norm = nat.DeviceArray.empty(ctx, x.shape, x.dtype) if normalize else None
+    (int64 [2]: flags, pick count), owned by the scope ``sc``."""
+    ctx = sc.ctx
+    flags = sc.empty((2,), np.int64)
+    norm = sc.empty(x.shape, x.dtype) if normalize else None
     nat.check(nat.lib().b2l_onset_normalize(ctx.handle, _vp(x.ptr), pl.clip_count(x.shape[:-1]), x.shape[-1],
                                             int(x.dtype == np.float64), float(np.finfo(x.dtype).tiny),
                                             _vp(norm.ptr) if norm is not None else None, _vp(flags.ptr)))
@@ -226,10 +213,10 @@ def _check_energy(energy):
         raise nat.UnsupportedOnGPU("onset_backtrack needs a C-ordered energy DeviceArray")
 
 
-def _backtrack_launch(energy, events, n_events, count, units, hop_length, sr):
-    """One launch; returns the backtracked list (DeviceArray of n_events entries in ``units``)."""
-    ctx = events.ctx
-    out = nat.DeviceArray.empty(ctx, (n_events,), np.float64 if units == "time" else np.int64)
+def _backtrack_launch(sc, energy, events, n_events, count, units, hop_length, sr):
+    """One launch; returns the backtracked list (DeviceArray of n_events entries in ``units``, owned by ``sc``)."""
+    ctx = sc.ctx
+    out = sc.empty((n_events,), np.float64 if units == "time" else np.int64)
     nat.check(nat.lib().b2l_onset_backtrack(ctx.handle, _vp(energy.ptr), energy.shape[0],
                                             int(energy.dtype == np.float64), _vp(events.ptr), n_events,
                                             _vp(count.ptr) if count is not None else None, pk.UNITS[units],
@@ -277,55 +264,41 @@ def onset_detect(*, y=None, sr: float = 22050, onset_envelope=None, hop_length: 
         _check_units(sparse, units)
         return _empty(shape, sparse, units, None, False)
 
-    env = _Envelope(y, sr, onset_envelope, hop_length)
-    try:
-        if env.audio is not None:
-            env.audio.check_finite()
-        x, ctx, on_device = env.dev, env.ctx, env.on_device
-        if onset_envelope is None:
-            pk.check_data(x.dtype, x.shape)
-            _check_normalizable(x.shape, normalize)
-        norm, flags = _normalize(x, normalize)
-        if deferred is not None:
-            verdict = flags.get()
-            if norm is not None:
-                norm.free()
-            if _passes(verdict):
-                raise deferred
-            _check_units(sparse, units)
-            return _empty(x.shape, sparse, units, ctx, on_device)
-        picked = norm if norm is not None else x
-        out_units = ("frames" if backtrack or units not in pk.UNITS else units) if sparse else None
-        dense, lst, count = pk.launch(picked, windows, method, kw["delta"], flags=flags, dense=not sparse,
-                                      units=out_units, hop_length=hop_length, sr=sr)
-        if sparse and backtrack:
-            if energy is None:
-                e_dev = picked
-            elif isinstance(energy, nat.DeviceArray):
-                e_dev = energy
-            else:
-                e_dev = ctx.to_device(np.ascontiguousarray(energy))
-            picks = lst
-            lst = _backtrack_launch(e_dev, picks, x.shape[-1], count, units if units in pk.UNITS else "frames",
-                                    hop_length, sr)
-            picks.free()
-            if e_dev is not picked and e_dev is not energy:
-                e_dev.free()
-        if norm is not None:
-            norm.free()
-    finally:
-        env.release()
-    if not sparse:
-        flags.free()
-        return dense if on_device else pl.finish(dense)
-    verdict = flags.get()   # 16 bytes: the verdict and the pick count
-    k = int(verdict[1]) if _passes(verdict) else 0
-    if _passes(verdict) and backtrack and k == 0:
-        raise ParameterError(_EMPTY_MATCH)
-    _check_units(sparse, units)
-    if on_device:
-        return pk.list_view(lst, k)
-    return lst.get()[:k].copy()
+    with pl.Scope(y if onset_envelope is None else onset_envelope) as sc:
+        env = _Envelope(y, sr, onset_envelope, hop_length)
+        try:
+            if env.audio is not None:
+                env.audio.check_finite()
+            x, ctx, on_device = env.dev, env.ctx, env.on_device
+            if onset_envelope is None:
+                pk.check_data(x.dtype, x.shape)
+                _check_normalizable(x.shape, normalize)
+            norm, flags = _normalize(sc, x, normalize)
+            if deferred is not None:
+                if _passes(flags.get()):
+                    raise deferred
+                _check_units(sparse, units)
+                return _empty(x.shape, sparse, units, ctx, on_device)
+            picked = norm if norm is not None else x
+            out_units = ("frames" if backtrack or units not in pk.UNITS else units) if sparse else None
+            dense, lst, count = pk.launch(sc, picked, windows, method, kw["delta"], flags=flags, dense=not sparse,
+                                          units=out_units, hop_length=hop_length, sr=sr)
+            if sparse and backtrack:
+                e_dev = picked if energy is None else sc.stage(energy)
+                lst = _backtrack_launch(sc, e_dev, lst, x.shape[-1], count, units if units in pk.UNITS else "frames",
+                                        hop_length, sr)
+        finally:
+            env.release()
+        if not sparse:
+            return sc.result(dense)
+        verdict = flags.get()   # 16 bytes: the verdict and the pick count
+        k = int(verdict[1]) if _passes(verdict) else 0
+        if _passes(verdict) and backtrack and k == 0:
+            raise ParameterError(_EMPTY_MATCH)
+        _check_units(sparse, units)
+        if on_device:
+            return sc.keep(lst).view((k,))
+        return lst.get()[:k].copy()
 
 
 def onset_backtrack(events, energy):
@@ -356,27 +329,21 @@ def onset_backtrack(events, energy):
         # the last minimum at or before a frame only depends on the frame's integer part, and frames past the end
         # take the last minimum
         ev = np.minimum(np.floor(ev) if ev.dtype.kind == "f" else ev, max(n, 1)).astype(np.int64)
-    ctx = events.ctx if ev_dev else energy.ctx if isinstance(energy, nat.DeviceArray) else nat.default_context()
-    e_dev = energy if isinstance(energy, nat.DeviceArray) else ctx.to_device(np.ascontiguousarray(energy))
-    d_ev = events if ev_dev else ctx.to_device(ev)
-    if ev_dev:
-        nat.check(nat.lib().b2l_status_reset(ctx.handle))
-    out = _backtrack_launch(e_dev, d_ev, n_events, None, "frames", 512, 22050.0)
-    if e_dev is not energy:
-        e_dev.free()
-    if not ev_dev:
-        d_ev.free()
-    elif pl.status_word(ctx) & _STATUS_NEGATIVE_EVENT:
-        out.free()
-        raise ParameterError(_NEGATIVE_MATCH)
-    return out if on_device else pl.finish(out)
+    with pl.Scope(events, energy) as sc:
+        e_dev = sc.stage(energy)
+        d_ev = sc.stage(events if ev_dev else ev)
+        if ev_dev:
+            nat.check(nat.lib().b2l_status_reset(sc.ctx.handle))
+        out = _backtrack_launch(sc, e_dev, d_ev, n_events, None, "frames", 512, 22050.0)
+        if ev_dev and pl.status_word(sc.ctx) & nat.STATUS_NEGATIVE_EVENT:
+            raise ParameterError(_NEGATIVE_MATCH)
+        return sc.result(out)
 
 
 def detect_stages(onset_envelope, *, normalize: bool = True):
     """The normaliser's output and verdict for a host envelope (testing aid): ``normalized`` (the envelope the
     picker reads) and ``flags`` (bit 0: some value nonzero, bit 1: some value not finite)."""
-    x = nat.default_context().to_device(np.ascontiguousarray(onset_envelope))
-    norm, flags = _normalize(x, normalize)
-    out = {"normalized": norm.get() if norm is not None else np.asarray(onset_envelope), "flags": int(flags.get()[0])}
-    x.free()
-    return out
+    with pl.Scope() as sc:
+        norm, flags = _normalize(sc, sc.stage(onset_envelope), normalize)
+        return {"normalized": norm.get() if norm is not None else np.asarray(onset_envelope),
+                "flags": int(flags.get()[0])}

@@ -14,6 +14,7 @@ from typing import Optional
 import numpy as np
 
 from . import _native as nat
+from . import _pipeline as pl
 from .filters import get_window
 from .util.exceptions import ParameterError
 from .util.utils import is_positive_int, pad_center
@@ -188,42 +189,17 @@ def _zero_lead(lead):
 
 # --------------------------------------------------------------------------------------------- device runner
 class _Run:
-    """One call's device side: the staged ``prob`` (C order, [clip][n_states][n_steps]), the verdict flags and the
-    sliced log-likelihood + decode launches."""
+    """One call's device side: the verdict flags and the sliced log-likelihood + decode launches over ``prob``
+    (C order, [clip][n_states][n_steps])."""
 
     def __init__(self, prob, mode, n_flags):
-        from . import _pipeline as pl
-
         self.on_device = isinstance(prob, nat.DeviceArray)
-        self._ctx = prob.ctx if self.on_device else None
         if self.on_device and prob.layout != "c":
             raise nat.UnsupportedOnGPU("viterbi needs a C-ordered DeviceArray")
-        self.shape, self.dtype, self.mode = prob.shape, np.dtype(prob.dtype), mode
-        self.lead = self.shape[:-2]
-        self.n_clips = pl.clip_count(self.lead)
+        self.prob, self.mode, self.n_flags = prob, mode, n_flags
+        self.shape, self.dtype = prob.shape, np.dtype(prob.dtype)
+        self.n_clips = pl.clip_count(self.shape[:-2])
         self.S, self.T = self.shape[-2], self.shape[-1]
-        self.host = None if self.on_device else np.ascontiguousarray(prob)
-        self.dev = prob if self.on_device else None
-        self.n_flags = n_flags
-        self.flags = None
-        self._owned = []
-
-    @property
-    def ctx(self):
-        """The device context; a host call creates it only when it reaches device work."""
-        if self._ctx is None:
-            self._ctx = nat.default_context()
-        return self._ctx
-
-    def _stage(self):
-        if self.dev is None:
-            self.dev = self.ctx.to_device(self.host)
-            self._owned.append(self.dev)
-
-    def _new_flags(self):
-        flags = nat.DeviceArray.empty(self.ctx, (self.n_flags,), np.int32)
-        nat.check(nat.lib().b2l_memset(self.ctx.handle, _vp(flags.ptr), 0, flags.nbytes))
-        return flags
 
     def _desc(self, eps, d_lm, n_clips):
         return nat.SeqLogObsDesc(mode=self.mode, f64=int(self.dtype == np.float64), n_clips=n_clips,
@@ -231,73 +207,46 @@ class _Run:
 
     def verdict(self):
         """Flags-only launch over the whole batch and one read-back."""
-        self._stage()
-        flags = self._new_flags()
-        nat.check(nat.lib().b2l_seq_logobs(self.ctx.handle, C.byref(self._desc(0.0, None, self.n_clips)),
-                                           _vp(self.dev.ptr), None, _vp(flags.ptr)))
-        return flags.get()
+        with pl.Scope(self.prob) as sc:
+            flags = sc.zeros((self.n_flags,), np.int32)
+            nat.check(nat.lib().b2l_seq_logobs(sc.ctx.handle, C.byref(self._desc(0.0, None, self.n_clips)),
+                                               _vp(sc.stage(self.prob).ptr), None, _vp(flags.ptr)))
+            return flags.get()
 
-    def upload(self, arr, dtype):
-        d = self.ctx.to_device(np.ascontiguousarray(arr, dtype=dtype))
-        self._owned.append(d)
-        return d.ptr
-
-    def decode(self, *, eps, log_marginal, n_models, lt, idx, deg, dense, log_p_init):
-        """Log-likelihoods and decode in slices of whole clips (SCRATCH_BYTES of scratch each).  Returns the states
-        [problem][n_steps] and logp [problem] DeviceArrays, problem = clip * n_models + model."""
-        self._stage()
-        ctx, L = self.ctx, nat.lib()
-        S_dec = 2 if self.mode == nat.SEQ_BINARY else self.S
-        per_clip = n_models * S_dec * self.T * 10
-        clips = max(1, min(self.n_clips, SCRATCH_BYTES // max(per_clip, 1)))
-        n_problems = self.n_clips * n_models
-        states = nat.DeviceArray.empty(ctx, (n_problems, self.T), np.uint16)
-        logp = nat.DeviceArray.empty(ctx, (n_problems,), np.float64)
-        self.flags = self._new_flags()
-        d_lm = self.upload(log_marginal, np.float64) if log_marginal is not None else None
-        model = nat.SeqModel(n_states=S_dec, n_models=n_models, deg=deg, dense=int(dense),
-                             d_lt=self.upload(lt, np.float64), d_idx=self.upload(idx, np.uint16) if idx is not None
-                             else None, d_log_p_init=self.upload(log_p_init, np.float64))
-        lp = ctx.alloc(clips * n_models * S_dec * self.T * 8)
-        try:
+    def decode(self, checks, states_shape, logp_shape, *, eps, log_marginal, n_models, lt, idx, deg, dense,
+               log_p_init):
+        """Log-likelihoods and decode in slices of whole clips (SCRATCH_BYTES of scratch each), then the device data
+        checks (one read-back of the flags).  Returns the states ``states_shape`` and logp ``logp_shape`` of
+        problem = clip * n_models + model, host or device like ``prob``."""
+        with pl.Scope(self.prob) as sc:
+            ctx, L = sc.ctx, nat.lib()
+            dev = sc.stage(self.prob)
+            S_dec = 2 if self.mode == nat.SEQ_BINARY else self.S
+            per_clip = n_models * S_dec * self.T * 10
+            clips = max(1, min(self.n_clips, SCRATCH_BYTES // max(per_clip, 1)))
+            n_problems = self.n_clips * n_models
+            states = sc.empty((n_problems, self.T), np.uint16)
+            logp = sc.empty((n_problems,), np.float64)
+            flags = sc.zeros((self.n_flags,), np.int32)
+            d_lm = sc.stage(log_marginal, np.float64).ptr if log_marginal is not None else None
+            model = nat.SeqModel(n_states=S_dec, n_models=n_models, deg=deg, dense=int(dense),
+                                 d_lt=sc.stage(lt, np.float64).ptr,
+                                 d_idx=sc.stage(idx, np.uint16).ptr if idx is not None else None,
+                                 d_log_p_init=sc.stage(log_p_init, np.float64).ptr)
+            lp = sc.empty((clips * n_models * S_dec * self.T,), np.float64)
             item = self.dtype.itemsize
             for c0 in range(0, self.n_clips, clips):
                 m = min(clips, self.n_clips - c0)
                 nat.check(L.b2l_seq_logobs(ctx.handle, C.byref(self._desc(eps, d_lm, m)),
-                                           _vp(self.dev.ptr + c0 * self.S * self.T * item), _vp(lp),
-                                           _vp(self.flags.ptr)))
+                                           _vp(dev.ptr + c0 * self.S * self.T * item), _vp(lp.ptr), _vp(flags.ptr)))
                 p0 = c0 * n_models
-                nat.check(L.b2l_seq_decode(ctx.handle, C.byref(model), _vp(lp), m * n_models, self.T,
+                nat.check(L.b2l_seq_decode(ctx.handle, C.byref(model), _vp(lp.ptr), m * n_models, self.T,
                                            _vp(states.ptr + p0 * self.T * 2), _vp(logp.ptr + p0 * 8)))
-        finally:
-            ctx.free(lp)
-        return states, logp
-
-    def release(self):
-        for d in self._owned:
-            d.free()
-        self._owned = []
-
-
-def _view(arr, shape):
-    """A reshaped view of a C-ordered DeviceArray that keeps it alive."""
-    out = nat.DeviceArray(arr.ctx, arr.ptr, shape, arr.dtype, layout="c", owner=False)
-    out._base = arr
-    return out
-
-
-def _finish(run, checks, states, logp, states_shape, logp_shape):
-    """Settles the device data checks (one read-back of the flags), then returns host or device results."""
-    if run.on_device:
-        if checks.pending:
-            checks.settle(run.flags.get())
-        run.release()
-        return _view(states, states_shape), _view(logp, logp_shape)
-    run.release()
-    s, lg = states.get().reshape(states_shape), logp.get().reshape(logp_shape)
-    states.free()
-    logp.free()
-    return s, lg
+            if checks.pending:
+                checks.settle(flags.get())
+            if self.on_device:
+                return sc.keep(states).view(states_shape), sc.keep(logp).view(logp_shape)
+            return sc.result(states).reshape(states_shape), sc.result(logp).reshape(logp_shape)
 
 
 def _empty_steps(run, states_shape, return_logp, what):
@@ -305,7 +254,7 @@ def _empty_steps(run, states_shape, return_logp, what):
         raise nat.UnsupportedOnGPU(f"{what} of zero frames with return_logp=True: the reference's log-probability "
                                    "is read past the end of its array")
     if run.on_device:
-        return nat.DeviceArray.empty(run.ctx, states_shape, np.uint16)
+        return run.prob.ctx.empty(states_shape, np.uint16)
     return np.zeros(states_shape, dtype=np.uint16)
 
 
@@ -356,9 +305,8 @@ def viterbi(prob, transition, *, p_init: Optional[np.ndarray] = None, return_log
         if prob.ndim > 2:
             chk.fail(IndexError(f"index 0 is out of bounds for axis {len(lead)} with size 0"))
         return _empty_steps(run, lead + (0,), return_logp, "viterbi")
-    states, logp = run.decode(eps=epsilon, log_marginal=None, n_models=1, lt=lt, idx=idx, deg=deg, dense=dense,
-                              log_p_init=log_p_init)
-    states, logp = _finish(run, chk, states, logp, lead + (n_steps,), logp_shape)
+    states, logp = run.decode(chk, lead + (n_steps,), logp_shape, eps=epsilon, log_marginal=None, n_models=1, lt=lt,
+                              idx=idx, deg=deg, dense=dense, log_p_init=log_p_init)
     if return_logp:
         return states, logp
     return states
@@ -409,9 +357,8 @@ def viterbi_discriminative(prob, transition, *, p_state: Optional[np.ndarray] = 
     lead = prob.shape[:-2]
     if n_steps == 0:
         chk.fail(IndexError(f"index 0 is out of bounds for axis {len(lead)} with size 0"))
-    states, logp = run.decode(eps=epsilon, log_marginal=log_marginal, n_models=1, lt=lt, idx=idx, deg=deg,
-                              dense=dense, log_p_init=log_p_init)
-    states, logp = _finish(run, chk, states, logp, lead + (n_steps,), lead)
+    states, logp = run.decode(chk, lead + (n_steps,), lead, eps=epsilon, log_marginal=log_marginal, n_models=1, lt=lt,
+                              idx=idx, deg=deg, dense=dense, log_p_init=log_p_init)
     if return_logp:
         return states, logp
     return states
@@ -424,7 +371,7 @@ def viterbi_binary(prob, transition, *, p_state=None, p_init=None, return_logp: 
     All labels of all clips are decoded in one launch."""
     prob = _prob_info(prob)
     if prob.ndim < 2:
-        prob = _view(prob, (1,) * (2 - prob.ndim) + prob.shape) if isinstance(prob, nat.DeviceArray) \
+        prob = prob.view((1,) * (2 - prob.ndim) + prob.shape) if isinstance(prob, nat.DeviceArray) \
             else np.atleast_2d(prob)
     _float_dtype(prob.dtype, "viterbi_binary")
     n_states, n_steps = prob.shape[-2:]
@@ -489,9 +436,9 @@ def viterbi_binary(prob, transition, *, p_state=None, p_init=None, return_logp: 
     for label, (d, is_dense, lt_l, idx_l) in enumerate(tables):
         lt[label, :d] = lt_l
         idx[label, :d] = np.arange(2)[:, None] if is_dense else idx_l
-    states, logp = run.decode(eps=eps, log_marginal=log_marginal, n_models=n_states, lt=lt,
-                              idx=None if dense else idx, deg=deg, dense=dense, log_p_init=log_p_init)
-    states, logp = _finish(run, chk, states, logp, lead + (n_states, n_steps), lead + (n_states,))
+    states, logp = run.decode(chk, lead + (n_states, n_steps), lead + (n_states,), eps=eps, log_marginal=log_marginal,
+                              n_models=n_states, lt=lt, idx=None if dense else idx, deg=deg, dense=dense,
+                              log_p_init=log_p_init)
     if return_logp:
         return states, logp
     return states
@@ -555,7 +502,7 @@ def _features(x, what):
         if x.layout != "c" or x.dtype not in (np.float32, np.float64):
             raise nat.UnsupportedOnGPU(f"dtw: {what} must be a C-ordered float32 or float64 DeviceArray")
         if x.ndim < 2:
-            x = _view(x, (1,) * (2 - x.ndim) + x.shape)
+            x = x.view((1,) * (2 - x.ndim) + x.shape)
         return x, x.shape, x.dtype == np.float64
     x = np.atleast_2d(np.asarray(x))
     if np.iscomplexobj(x):
@@ -563,46 +510,6 @@ def _features(x, what):
     if x.dtype != np.float32:
         x = x.astype(np.float64)      # what cdist computes in
     return np.ascontiguousarray(x), x.shape, x.dtype == np.float64
-
-
-class _Align:
-    """Device buffers of one alignment call: what it allocates, freed by release() unless handed to the caller."""
-
-    def __init__(self, ctx=None):
-        self._ctx, self.owned = ctx, []
-
-    @property
-    def ctx(self):
-        """The device context; a host call creates it only when it reaches device work."""
-        if self._ctx is None:
-            self._ctx = nat.default_context()
-        return self._ctx
-
-    def empty(self, shape, dtype):
-        d = nat.DeviceArray.empty(self.ctx, shape, dtype)
-        self.owned.append(d)
-        return d
-
-    def stage(self, x):
-        if isinstance(x, nat.DeviceArray):
-            return x
-        d = self.ctx.to_device(x)
-        self.owned.append(d)
-        return d
-
-    def flags(self):
-        f = self.empty((1,), np.int32)
-        nat.check(nat.lib().b2l_memset(self.ctx.handle, _vp(f.ptr), 0, 4))
-        return f
-
-    def keep(self, d):
-        self.owned.remove(d)
-        return d
-
-    def release(self):
-        for d in self.owned:
-            d.free()
-        self.owned = []
 
 
 def _dtw_desc(shape, steps, w_add, w_mul, *, c_f64=True, subseq=False, band=None):
@@ -633,9 +540,9 @@ def _walk_refusal(status):
         raise nat.UnsupportedOnGPU("dtw: steps holds an index outside the step table")
 
 
-def _path_out(run, buf, length, on_device):
-    if on_device:
-        return _view(run.keep(buf), (length, 2))
+def _path_out(run, buf, length):
+    if run.on_device:
+        return run.keep(buf).view((length, 2))
     return buf.get()[:length].copy()
 
 
@@ -677,9 +584,7 @@ def dtw(X=None, Y=None, *, C=None, metric: str = "euclidean", step_sizes_sigma=N
     if C is not None and (X is not None or Y is not None):
         raise ParameterError("If C is supplied, both X and Y must not be supplied")
 
-    on_device = any(isinstance(a, nat.DeviceArray) for a in (X, Y, C))
-    run = _Align(next((a.ctx for a in (X, Y, C) if isinstance(a, nat.DeviceArray)), None))
-    try:
+    with pl.Scope(X, Y, C) as run:
         transposed = False
         flags = None
         if C is None:
@@ -691,7 +596,7 @@ def dtw(X=None, Y=None, *, C=None, metric: str = "euclidean", step_sizes_sigma=N
                 raise ParameterError(_CDIST_ERROR)
             code = _metric_code(metric)
             if x_f64 != y_f64:        # the kernel reads both in one dtype; widening is exact
-                if on_device:
+                if run.on_device:
                     raise nat.UnsupportedOnGPU("dtw: X and Y must share a dtype when one is a DeviceArray")
                 X, Y, x_f64 = X.astype(np.float64), Y.astype(np.float64), True
             if N == 0 or M == 0 or K == 0:
@@ -700,7 +605,7 @@ def dtw(X=None, Y=None, *, C=None, metric: str = "euclidean", step_sizes_sigma=N
             shape = (M, N) if transposed else (N, M)
             dX, dY = run.stage(X), run.stage(Y)
             d_C = run.empty(shape, np.float64)
-            flags = run.flags()
+            flags = run.zeros((1,), np.int32)
             x_off, y_off = _feature_offsets(x_shape), _feature_offsets(y_shape)
             cdesc = nat.DtwCostDesc(f64=int(x_f64), metric=code, transpose=int(transposed), K=K, N=N, M=M,
                                     h_x_off=x_off.ctypes.data, h_y_off=y_off.ctypes.data)
@@ -711,7 +616,7 @@ def dtw(X=None, Y=None, *, C=None, metric: str = "euclidean", step_sizes_sigma=N
             if isinstance(C, nat.DeviceArray):
                 if C.layout != "c" or C.dtype not in (np.float32, np.float64):
                     raise nat.UnsupportedOnGPU("dtw: C must be a C-ordered float32 or float64 DeviceArray")
-                d_C = C if C.ndim == 2 else _view(C, (1,) * (2 - C.ndim) + C.shape)
+                d_C = C if C.ndim == 2 else C.view((1,) * (2 - C.ndim) + C.shape)
                 if C.ndim > 2:
                     raise nat.UnsupportedOnGPU("dtw: C must be 2-D")
             else:
@@ -730,7 +635,7 @@ def dtw(X=None, Y=None, *, C=None, metric: str = "euclidean", step_sizes_sigma=N
         nan_error = ParameterError("DTW cost matrix C has NaN values. ")
         if C is not None:
             if isinstance(C, nat.DeviceArray):
-                flags = run.flags()
+                flags = run.zeros((1,), np.int32)
                 nat.check(nat.lib().b2l_nan_flag(run.ctx.handle, _vp(d_C.ptr), d_C.size, int(c_f64), _vp(flags.ptr)))
             else:
                 if np.any(np.isnan(C)):
@@ -756,13 +661,11 @@ def dtw(X=None, Y=None, *, C=None, metric: str = "euclidean", step_sizes_sigma=N
                 raise ParameterError("Unable to compute a full DTW warping path. "
                                      "You may want to try again with subseq=True.")
             _walk_refusal(length)
-            out.append(_path_out(run, wp, length, on_device))
+            out.append(_path_out(run, wp, length))
         elif flags is not None and flags.get()[0]:
             raise nan_error
-        D_out = run.keep(D) if on_device else D.get()
-        steps_out = (run.keep(steps) if on_device else steps.get()) if return_steps else None
-    finally:
-        run.release()
+        D_out = run.result(D)
+        steps_out = run.result(steps) if return_steps else None
     ret = [D_out] + out + ([steps_out] if return_steps else [])
     return tuple(ret) if len(ret) > 1 else ret[0]
 
@@ -794,15 +697,12 @@ def dtw_backtracking(steps, *, step_sizes_sigma=None, subseq: bool = False, star
     if start is not None and not 0 <= int(start) < m:
         raise nat.UnsupportedOnGPU(f"dtw_backtracking: start={start} outside the {m} columns (the reference reads "
                                    "outside its array)")
-    run = _Align(steps.ctx if on_device else None)
     zeros = np.zeros(len(table))
-    try:
+    with pl.Scope(steps) as run:
         desc = _dtw_desc((n, m), table, zeros, zeros, subseq=subseq)
         wp, length = _walk(run, desc, run.stage(steps), None, -1 if start is None else int(start), 0, 0, None)
         _walk_refusal(length)
-        return _path_out(run, wp, length, on_device)
-    finally:
-        run.release()
+        return _path_out(run, wp, length)
 
 
 def rqa(sim, *, gap_onset: float = 1, gap_extend: float = 1, knight_moves: bool = True, backtrack: bool = True):
@@ -826,16 +726,15 @@ def rqa(sim, *, gap_onset: float = 1, gap_extend: float = 1, knight_moves: bool 
         raise nat.UnsupportedOnGPU("rqa needs a C-ordered DeviceArray")
     n, m = sim.shape
     f64 = int(sim.dtype == np.float64)
-    run = _Align(sim.ctx if on_device else None)
-    try:
-        d_sim = run.stage(np.ascontiguousarray(sim) if not on_device else sim)
+    with pl.Scope(sim) as run:
+        d_sim = run.stage(sim)
         score = run.empty((n, m), sim.dtype)
         ptr = run.empty((n, m), np.int8)
         L = nat.lib()
         nat.check(L.b2l_rqa(run.ctx.handle, _vp(d_sim.ptr), n, m, f64, float(gap_onset), float(gap_extend),
                             int(bool(knight_moves)), _vp(score.ptr), _vp(ptr.ptr)))
         if not backtrack:
-            return run.keep(score) if on_device else score.get()
+            return run.result(score)
         path = run.empty((n, 2), np.uint64)
         length = run.empty((1,), np.int64)
         nat.check(L.b2l_rqa_path(run.ctx.handle, _vp(score.ptr), _vp(ptr.ptr), n, m, f64, _vp(path.ptr),
@@ -843,10 +742,8 @@ def rqa(sim, *, gap_onset: float = 1, gap_extend: float = 1, knight_moves: bool 
         k = int(length.get()[0])
         if k < 0:
             raise nat.UnsupportedOnGPU("rqa: the path's column index passes -M (the reference raises IndexError)")
-        score_out = run.keep(score) if on_device else score.get()
-        return score_out, _path_out(run, path, k, on_device)
-    finally:
-        run.release()
+        score_out = run.result(score)
+        return score_out, _path_out(run, path, k)
 
 
 def path_to_steps(path, *, inverse: bool = False):

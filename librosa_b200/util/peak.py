@@ -58,39 +58,28 @@ def check_data(dtype, shape):
         raise nat.UnsupportedOnGPU(f"peak picking of rows of {shape[-1]} frames: the GPU takes fewer than 2^31")
 
 
-def launch(x, windows, method, delta, *, flags=None, dense=True, units=None, hop_length=512, sr=22050.0):
-    """One launch of the picker on the C-ordered device data ``x`` (..., n).  ``flags``: the verdict pair of
-    ``onset_normalize`` (picks only where it passed).  Returns the dense picks (DeviceArray of bool, or None) and,
-    with ``units`` (one row only), the list in those units and a count DeviceArray (``flags``'s second word when
-    ``flags`` is given)."""
+def launch(sc, x, windows, method, delta, *, flags=None, dense=True, units=None, hop_length=512, sr=22050.0):
+    """One launch of the picker on the C-ordered device data ``x`` (..., n), its buffers owned by the scope ``sc``.
+    ``flags``: the verdict pair of ``onset_normalize`` (picks only where it passed).  Returns the dense picks
+    (DeviceArray of bool, or None) and, with ``units`` (one row only), the list in those units and a count
+    DeviceArray (``flags``'s second word when ``flags`` is given)."""
     from .. import _pipeline as pl
 
-    ctx, n = x.ctx, x.shape[-1]
+    ctx, n = sc.ctx, x.shape[-1]
     pre_max, post_max, pre_avg, post_avg, wait = (min(v, n) for v in windows)
     desc = nat.PeakDesc(pre_max=pre_max, post_max=max(1, post_max), pre_avg=pre_avg, post_avg=max(1, post_avg),
                         wait=wait, delta=float(delta), method=method, f64=int(x.dtype == np.float64),
                         units=UNITS[units] if units is not None else 0, hop_length=int(hop_length), sr=float(sr))
-    out = nat.DeviceArray.empty(ctx, x.shape, np.bool_) if dense else None
+    out = sc.empty(x.shape, np.bool_) if dense else None
     lst = count = None
     if units is not None:
-        lst = nat.DeviceArray.empty(ctx, (n,), np.float64 if units == "time" else np.int64)
-        if flags is not None:
-            count = nat.DeviceArray(ctx, flags.ptr + 8, (1,), np.int64, layout="c", owner=False)
-            count._base = flags
-        else:
-            count = nat.DeviceArray.empty(ctx, (1,), np.int64)
+        lst = sc.empty((n,), np.float64 if units == "time" else np.int64)
+        count = flags.view((1,), offset=1) if flags is not None else sc.empty((1,), np.int64)
     nat.check(nat.lib().b2l_peak_pick(ctx.handle, C.byref(desc), _vp(x.ptr), pl.clip_count(x.shape[:-1]), n,
                                       _vp(flags.ptr) if flags is not None else None,
                                       _vp(out.ptr) if out is not None else None, _vp(lst.ptr) if lst else None,
                                       _vp(count.ptr) if count else None))
     return out, lst, count
-
-
-def list_view(lst, k):
-    """The first ``k`` entries of a device list, as a view that keeps the list alive."""
-    view = nat.DeviceArray(lst.ctx, lst.ptr, (k,), lst.dtype, layout="c", owner=False)
-    view._base = lst
-    return view
 
 
 def peak_pick(x, *, pre_max, post_max, pre_avg, post_avg, delta, wait, sparse: bool = True, method: str = "greedy",
@@ -112,22 +101,13 @@ def peak_pick(x, *, pre_max, post_max, pre_avg, post_avg, delta, wait, sparse: b
         if x.layout != "c":
             raise nat.UnsupportedOnGPU("peak_pick needs a C-ordered DeviceArray")
         check_data(x.dtype, x.shape)
-        dev = x
     else:
-        moved = np.moveaxis(x, axis, -1)
-        check_data(x.dtype, moved.shape)
-        dev = pl.context_for(None).to_device(np.ascontiguousarray(moved))
-    dense, lst, count = launch(dev, windows, code, delta, dense=not sparse, units="frames" if sparse else None)
-    if not on_device:
-        dev.free()
-    if sparse:
-        k = int(count.get()[0])
-        count.free()
-        if on_device:
-            return list_view(lst, k)
-        out = lst.get()[:k].copy()
-        lst.free()
-        return out
-    if on_device:
-        return dense
-    return np.moveaxis(pl.finish(dense), -1, axis)
+        x = np.moveaxis(x, axis, -1)
+        check_data(x.dtype, x.shape)
+    with pl.Scope(x) as sc:
+        dense, lst, count = launch(sc, sc.stage(x), windows, code, delta, dense=not sparse,
+                                   units="frames" if sparse else None)
+        if sparse:
+            k = int(count.get()[0])
+            return sc.keep(lst).view((k,)) if on_device else lst.get()[:k].copy()
+        return sc.result(dense) if on_device else np.moveaxis(sc.result(dense), -1, axis)

@@ -43,6 +43,63 @@ def test_plan_desc_layout_matches_header():
     assert nat.PlanDesc.h_dct_basis.offset == 48 and nat.PlanDesc.top_db.offset == 64
 
 
+def _header_enumerators():
+    text = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "b2l.h")).read(), flags=re.S)
+    return [n for body in re.findall(r"\benum\b[^{;]*\{(.*?)\}", text, flags=re.S)
+            for n in re.findall(r"\b(B2L_[A-Z0-9_]+)\b", body)]
+
+
+def _mirror(nat, name):
+    """The _native constant that mirrors the header's enumerator ``name``."""
+    short = name[len("B2L_"):]
+    for prefix, table in (("PAD_", nat.PAD_MODES), ("DTW_", nat.DTW_METRICS)):
+        if short.startswith(prefix):
+            return table[short[len(prefix):].lower()]
+    return getattr(nat, name) if hasattr(nat, name) else getattr(nat, short)
+
+
+def test_ctypes_mirror_matches_header(tmp_path):
+    """Every ctypes.Structure of _native has the size and field offsets of the struct its docstring names (field
+    names as in C), and every enumerator of include/b2l.h has the value of its _native constant: a C99 probe
+    compiled against the header prints what C sees."""
+    import shutil
+    import subprocess
+
+    from librosa_b200 import _native as nat
+
+    if shutil.which("gcc") is None:
+        pytest.skip("gcc not available")
+    structs = {}
+    for cls in vars(nat).values():
+        if isinstance(cls, type) and issubclass(cls, ctypes.Structure) and cls is not ctypes.Structure:
+            tag = re.match(r"struct (b2l_\w+) ", cls.__doc__ or "")
+            assert tag, f"{cls.__name__}: the docstring must name its C struct"
+            structs[tag.group(1)] = cls
+    assert len(structs) >= 19
+    enums = _header_enumerators()
+    assert "B2L_STATUS_NEGATIVE_EVENT" in enums
+    lines = ['#include <stddef.h>', '#include <stdio.h>', '#include "b2l.h"', "int main(void) {"]
+    want = {}
+    for tag, cls in structs.items():
+        lines.append(f'  printf("{tag} %zu\\n", sizeof(struct {tag}));')
+        want[tag] = ctypes.sizeof(cls)
+        for field, *_ in cls._fields_:
+            lines.append(f'  printf("{tag}.{field} %zu\\n", offsetof(struct {tag}, {field}));')
+            want[f"{tag}.{field}"] = getattr(cls, field).offset
+    for name in enums:
+        lines.append(f'  printf("{name} %d\\n", (int){name});')
+        want[name] = int(_mirror(nat, name))
+    lines += ["  return 0;", "}"]
+    src = tmp_path / "probe.c"
+    src.write_text("\n".join(lines) + "\n")
+    exe = tmp_path / "probe"
+    subprocess.run(["gcc", "-std=c99", "-Wall", "-Werror", "-I", os.path.join(ROOT, "include"), str(src), "-o",
+                    str(exe)], check=True, capture_output=True)
+    got = dict(line.split() for line in subprocess.run([str(exe)], check=True, capture_output=True,
+                                                       text=True).stdout.splitlines())
+    assert {k: int(v) for k, v in got.items()} == want
+
+
 def _have_gpu():
     from librosa_b200 import _native as nat
 

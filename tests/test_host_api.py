@@ -359,6 +359,38 @@ def test_kernels_launch_only_through_launch():
     assert not stray, stray
 
 
+def test_device_array_view_stays_inside_its_base():
+    base = lb.DeviceArray(None, 4096, (2, 3), np.float64, owner=False)
+    v = base.view((1, 3), offset=3)
+    assert (v.ptr, v.shape, v.dtype, v.layout, v.base) == (4096 + 24, (1, 3), np.float64, "c", base)
+    for shape, offset in (((4,), 3), ((7,), 0), ((1,), -1)):
+        with pytest.raises(ValueError, match="reaches past"):
+            base.view(shape, offset=offset)
+
+
+def test_views_zeroed_buffers_and_status_bits_have_one_home():
+    """Non-owning views and cleared buffers are made only by DeviceArray.view and Context.zeros (_native.py), and the
+    status word's bits are written and read by name (enum b2l_status_bit, nat.STATUS_*), never as digits."""
+    import glob
+    import re
+
+    pkg = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "librosa_b200")
+    stray = []
+    for path in sorted(glob.glob(os.path.join(pkg, "**", "*.py"), recursive=True)):
+        with open(path) as f:
+            text = f.read()
+        name = os.path.relpath(path, pkg)
+        if name != "_native.py":
+            stray += [(name, w) for w in ("owner=False", "b2l_memset") if w in text]
+        stray += [(name, m.group(0)) for m in re.finditer(r"\b_base\b|status_word\([^)]*\)\s*&\s*\d", text)]
+    for path in sorted(glob.glob(os.path.join(pkg, "csrc", "*.cu*")) + glob.glob(os.path.join(pkg, "csrc", "*.h"))):
+        with open(path) as f:
+            text = f.read()
+        pat = r"atomicOr\([^,;]*status[^,;]*,\s*\d|\*\s*[\w.>-]*status\s*=\s*\d"
+        stray += [(os.path.basename(path), m.group(0)) for m in re.finditer(pat, text)]
+    assert not stray, stray
+
+
 def test_polyphase_filter_bookkeeping_matches_scipy():
     """The host half of resample(res_type="polyphase"): the zero-padded low-pass and the crop offset handed to
     b2l_resample_poly, checked by evaluating the kernel's formula  y[j] = sum_m x[m] h[(n_pre_remove + j) down - m up]
