@@ -221,6 +221,26 @@ int b2l_spectral_contrast(b2l_ctx* ctx, const b2l_contrast_desc* desc, const flo
 int b2l_resample_poly(b2l_ctx* ctx, const float* d_x, int64_t n_clips, int64_t n_in, int64_t x_stride, const float* d_h,
                       int32_t n_h, int32_t up, int32_t down, int64_t n_pre_remove, int64_t n_keep, int64_t n_total,
                       float out_scale, float* d_out);
+/* librosa.cqt / vqt (core/constantq.py:820-1266): the filter-bank projection of every octave, stacked as __trim_stack
+ * does (:1169-1194), in one launch per 65 535 clips.  Octave o's STFT d_D [n_clips][n_frames][n_fft_bins] (complex64,
+ * n_frames >= the output's) meets rows indptr_off .. indptr_off + n_rows - 1 of the concatenated complex64 CSR basis
+ * (d_indptr holds absolute positions into d_indices / d_data; nnz: the octave's nonzeros) and fills output rows
+ * row0 .. row0 + n_rows - 1 of d_out [n_clips][n_frames][n_bins].  Each element is SciPy's `csr @ D` for complex64
+ * bit for bit (ascending columns, unfused multiply and add); d_rscale [n_bins] (1 / sqrt(lengths), or NULL when
+ * scale=False) multiplies in double with one rounding, as numpy's complex64 /= float64 does.  Sets no status bit. */
+#define B2L_CQT_MAX_OCTAVES 32
+typedef struct b2l_cqt_octave {
+  const void* d_D;
+  int64_t n_frames;
+  int32_t n_fft_bins;
+  int32_t row0;
+  int32_t n_rows;
+  int32_t indptr_off;
+  int32_t nnz;
+} b2l_cqt_octave;
+int b2l_cqt_project(b2l_ctx* ctx, const b2l_cqt_octave* h_oct, int32_t n_oct, const int32_t* d_indptr,
+                    const int32_t* d_indices, const void* d_data, const double* d_rscale, int64_t n_clips,
+                    int64_t n_frames, int32_t n_bins, void* d_out);
 /* out = x - y over n floats */
 int b2l_sub(b2l_ctx* ctx, const float* d_x, const float* d_y, int64_t n, float* d_out);
 /* Tuning estimation for chroma_stft (feature/spectral.py:1137-1293): librosa.estimate_tuning

@@ -186,6 +186,15 @@ class DtwDesc(C.Structure):
                 ("h_steps", C.c_void_p), ("h_w_add", C.c_void_p), ("h_w_mul", C.c_void_p)]
 
 
+class CqtOctave(C.Structure):
+    """struct b2l_cqt_octave (include/b2l.h): one octave of b2l_cqt_project; d_D is a device pointer."""
+    _fields_ = [("d_D", C.c_void_p), ("n_frames", C.c_int64), ("n_fft_bins", C.c_int32), ("row0", C.c_int32),
+                ("n_rows", C.c_int32), ("indptr_off", C.c_int32), ("nnz", C.c_int32)]
+
+
+CQT_MAX_OCTAVES = 32   # B2L_CQT_MAX_OCTAVES
+
+
 DTW_METRICS = {"euclidean": 0, "sqeuclidean": 1, "cityblock": 2, "chebyshev": 3, "cosine": 4}   # enum b2l_dtw_metric
 BEAT_FRAMES, BEAT_SAMPLES, BEAT_TIME = range(3)   # enum b2l_beat_units
 SEQ_PLAIN, SEQ_DISC, SEQ_BINARY = range(3)        # enum b2l_seq_mode
@@ -289,6 +298,7 @@ def _declare(lib):
         "b2l_dtw_backtrack": (C.c_int, [_vp, P(DtwDesc), _vp, _vp, _i64, C.c_int32, C.c_int32, _vp, _vp, _vp]),
         "b2l_rqa": (C.c_int, [_vp, _vp, _i64, _i64, C.c_int32, C.c_double, C.c_double, C.c_int32, _vp, _vp]),
         "b2l_rqa_path": (C.c_int, [_vp, _vp, _vp, _i64, _i64, C.c_int32, _vp, _vp]),
+        "b2l_cqt_project": (C.c_int, [_vp, P(CqtOctave), C.c_int32, _vp, _vp, _vp, _vp, _i64, _i64, C.c_int32, _vp]),
         "b2l_stft_f64": (C.c_int, [_vp, _vp, _i64, _i64, _i64, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                    P(C.c_double), _vp]),
         "b2l_istft_f64": (C.c_int, [_vp, _vp, _i64, _i64, _i64, C.c_int32, C.c_int32, C.c_int32, P(C.c_double),

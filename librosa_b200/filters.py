@@ -1,5 +1,7 @@
 """Window and filter-bank construction (host side, float64) — mirror of the hot-path parts of
-librosa/filters.py: ``mel`` (:117-251), ``get_window`` (:915-977), ``window_sumsquare`` (:1268-1339).
+librosa/filters.py: ``mel`` (:117-251), ``get_window`` (:915-977), ``window_sumsquare`` (:1268-1339), and the
+constant-Q wavelet basis: ``wavelet_lengths`` (:424-552), ``_relative_bandwidth`` (:555-585), ``wavelet``
+(:589-733), ``window_bandwidth`` (:865-912).
 
 These constants are tiny and parity-critical, so they are computed on the host with the same float64
 expressions as the reference and uploaded once per plan; the GPU only *applies* them.
@@ -100,3 +102,89 @@ def chroma(*, sr: float, n_fft: int, n_chroma: int = 12, tuning: float = 0.0, ct
     if base_c:
         wts = np.roll(wts, -3 * (n_chroma // 12), axis=0)
     return np.ascontiguousarray(wts[:, : int(1 + n_fft / 2)], dtype=dtype)
+
+
+_ENBW_POINTS = 8193   # window_bandwidth's tabulated values are the ENBW of the symmetric 8193-point window
+_ENBW_UNREPRODUCED = ("flattop", "flat", "flt")
+
+
+def window_bandwidth(window, n: int = 1000) -> float:
+    """Equivalent noise bandwidth ``n * sum(w**2) / sum(w)**2`` of a window (librosa/filters.py:865-912).
+
+    Named windows use the symmetric 8193-point window, which reproduces librosa's tabulated value exactly for
+    "hann" (the constant-Q default), "ones", "boxcar", "triangle", "bartlett", "cosine", "parzen", "bohman" and
+    "barthann", and within 1e-15 relative for "hamming", "blackman", "blackmanharris" and "nuttall".  librosa's
+    value for "flattop" is not the ENBW of SciPy's flat-top window (2.78 against 3.77), so it raises
+    ``UnsupportedOnGPU`` rather than move the cutoff of the wavelet basis.  Other specifications use
+    ``get_window(window, n)`` as librosa does."""
+    if isinstance(window, str) and window in _ENBW_UNREPRODUCED:
+        from ._native import UnsupportedOnGPU
+
+        raise UnsupportedOnGPU(f"window_bandwidth({window!r}): librosa's tabulated bandwidth of this window is not "
+                               "reproduced here; use another window")
+    if isinstance(window, str):
+        try:
+            w = scipy.signal.get_window(window, _ENBW_POINTS, fftbins=False)
+        except ValueError:
+            w = None
+        if w is not None:
+            return float(_ENBW_POINTS * np.sum(w ** 2) / (np.sum(w) ** 2))
+    w = get_window(window, n)
+    return float(n * np.sum(w ** 2) / (np.sum(w) ** 2 + np.finfo(np.asarray(w).dtype).tiny))
+
+
+def _relative_bandwidth(*, freqs: np.ndarray) -> np.ndarray:
+    """Relative bandwidth alpha of each frequency from its neighbours on a log2 axis (librosa/filters.py:555-585)."""
+    if len(freqs) <= 1:
+        raise ParameterError(f"2 or more frequencies are required to compute bandwidths. Given freqs={freqs}")
+    logf = np.log2(freqs)
+    bpo = np.empty_like(freqs)
+    bpo[0] = 1 / (logf[1] - logf[0])
+    bpo[-1] = 1 / (logf[-1] - logf[-2])
+    bpo[1:-1] = 2 / (logf[2:] - logf[:-2])
+    return (2.0 ** (2 / bpo) - 1) / (2.0 ** (2 / bpo) + 1)
+
+
+def wavelet_lengths(*, freqs, sr: float = 22050, window="hann", filter_scale: float = 1, gamma=0, alpha=None):
+    """Filter lengths of a wavelet basis and the cutoff frequency of its top filter (librosa/filters.py:424-552)."""
+    freqs = np.asarray(freqs)
+    if filter_scale <= 0:
+        raise ParameterError(f"filter_scale={filter_scale} must be positive")
+    if gamma is not None and gamma < 0:
+        raise ParameterError(f"gamma={gamma} must be non-negative")
+    if np.any(freqs <= 0):
+        raise ParameterError("frequencies must be strictly positive")
+    if len(freqs) > 1 and np.any(freqs[:-1] > freqs[1:]):
+        raise ParameterError(f"Frequency array={freqs} must be in strictly ascending order")
+    alpha = _relative_bandwidth(freqs=freqs) if alpha is None else np.asarray(alpha)
+    offset = alpha * 24.7 / 0.108 if gamma is None else gamma     # ERB-proportional bandwidth offset for None
+    Q = float(filter_scale) / alpha
+    f_cutoff = max(freqs * (1 + 0.5 * window_bandwidth(window) / Q) + 0.5 * offset)
+    return Q * sr / (freqs + offset / alpha), f_cutoff
+
+
+def _fractional_window(window, n: float) -> np.ndarray:
+    """``ceil(n)`` samples: the window of ``floor(n)`` samples, zero from sample ``floor(n)`` on."""
+    lo, hi = int(np.floor(n)), int(np.ceil(n))
+    w = get_window(window, lo)
+    if len(w) < hi:
+        w = np.pad(w, [(0, hi - len(w))], mode="constant")
+    w[lo:] = 0.0
+    return w
+
+
+def wavelet(*, freqs: np.ndarray, sr: float = 22050, window="hann", filter_scale: float = 1, pad_fft: bool = True,
+            norm=1, dtype=np.complex64, gamma=0, alpha=None, **kwargs):
+    """Windowed complex sinusoids at ``freqs``, centred in rows of a common length (a power of two when ``pad_fft``),
+    and their fractional lengths (librosa/filters.py:589-733)."""
+    lengths, _ = wavelet_lengths(freqs=freqs, sr=sr, window=window, filter_scale=filter_scale, gamma=gamma,
+                                 alpha=alpha)
+    rows = []
+    for ilen, freq in zip(lengths, freqs, strict=True):
+        phase = np.arange(-ilen // 2, ilen // 2, dtype=float) * 2 * np.pi * freq / sr
+        sig = np.cos(phase) + 1j * np.sin(phase)
+        sig *= _fractional_window(window, len(sig))
+        rows.append(normalize(sig, norm=norm))
+    size = max(lengths)
+    size = int(2.0 ** (np.ceil(np.log2(size)))) if pad_fft else int(np.ceil(size))
+    return np.asarray([pad_center(r, size=size, **kwargs) for r in rows], dtype=dtype), lengths

@@ -4,7 +4,8 @@ cases through the UNMODIFIED reference; ``--pitch`` writes only tests/golden/pit
 and leaves the other fixtures as they are; ``--rhythm`` likewise writes only tests/golden/rhythm_v1.npz
 (tests/rhythm_cases.py), ``--beat`` only tests/golden/beat_v1.npz (tests/beat_cases.py), ``--onset`` only
 tests/golden/onset_v1.npz (tests/onset_cases.py), ``--sequence`` only tests/golden/sequence_v1.npz
-(tests/sequence_cases.py), and ``--alignment`` only tests/golden/alignment_v1.npz (tests/alignment_cases.py).
+(tests/sequence_cases.py), ``--alignment`` only tests/golden/alignment_v1.npz (tests/alignment_cases.py), and
+``--cqt`` only tests/golden/cqt_v1.npz (tests/cqt_cases.py).
 
 Needs a checkout of the reference (see tools/ref_shim.py); the tests only read the stored fixtures.  Also
 stores a handful of constant tables (mel bases, window sum-square, mel-scale known answers) produced by the
@@ -17,6 +18,7 @@ reference.
     python tools/make_golden.py --onset
     python tools/make_golden.py --sequence
     python tools/make_golden.py --alignment
+    python tools/make_golden.py --cqt
 """
 from __future__ import annotations
 
@@ -316,6 +318,57 @@ def write_alignment():
     print("wrote", path, os.path.getsize(path), "bytes")
 
 
+def write_cqt():
+    """tests/golden/cqt_v1.npz: per case of tests/cqt_cases.py, the reference's C (or ``<name>/error``), its
+    warnings, and what each octave's response step received (signal length, n_fft, hop, the sparse basis; one
+    octave's STFT for the cases in WITH_D), recorded by wrapping the reference's per-octave response function; and
+    the reference's table of window bandwidths (``window_bandwidth/<name>``)."""
+    import cqt_cases as QC
+
+    ref = ref_shim.load_reference()
+    import importlib
+
+    cq = importlib.import_module("librosa.core.constantq")
+    inner = cq.__dict__["__cqt_response"]
+    calls = []
+
+    def recorder(y, n_fft, hop_length, fft_basis, mode, window="ones", phase=True, dtype=None):
+        calls.append((y, n_fft, hop_length, fft_basis, mode, dtype))
+        return inner(y, n_fft, hop_length, fft_basis, mode, window=window, phase=phase, dtype=dtype)
+
+    cq.__dict__["__cqt_response"] = recorder
+    store = {}
+    for case in QC.CASES:
+        name = case["name"]
+        calls.clear()
+        with warnings.catch_warnings(record=True) as caught:
+            warnings.simplefilter("always")
+            try:
+                C = QC.call(ref, case)
+                store[f"{name}/C"] = C
+            except Exception as e:   # the reference's own error, stored as "Class: message"
+                store[f"{name}/error"] = np.array(f"{type(e).__name__}: {e}")
+        store[f"{name}/warnings"] = np.array([str(w.message) for w in caught if "n_fft=" in str(w.message)])
+        store[f"{name}/octaves"] = np.array([(y.shape[-1], n_fft, hop, b.shape[0]) for y, n_fft, hop, b, _, _ in calls],
+                                            dtype=np.int64).reshape(-1, 4)
+        for i, (y, n_fft, hop, b, mode, dtype) in enumerate(calls):
+            if name not in QC.BASIS_ARRAYS:
+                store[f"{name}/basis{i}/sha256"] = np.array(QC.basis_digest(b.indptr, b.indices, b.data))
+            else:
+                store[f"{name}/basis{i}/indptr"] = b.indptr
+                store[f"{name}/basis{i}/indices"] = b.indices
+                store[f"{name}/basis{i}/data"] = b.data
+            if QC.WITH_D.get(name) == i:
+                store[f"{name}/D"] = ref.stft(y, n_fft=n_fft, hop_length=hop, window="ones", pad_mode=mode, dtype=dtype)
+        print(f"{name:32s} {store.get(f'{name}/error', np.shape(store.get(f'{name}/C')))} octaves={len(calls)}")
+    for key, value in sorted(importlib.import_module("librosa.filters").WINDOW_BANDWIDTHS.items()):
+        if isinstance(key, str):   # the reference's tabulated equivalent noise bandwidths
+            store[f"window_bandwidth/{key}"] = np.float64(value)
+    path = os.path.join(ROOT, "tests", "golden", "cqt_v1.npz")
+    np.savez_compressed(path, **store)
+    print("wrote", path, os.path.getsize(path), "bytes")
+
+
 if __name__ == "__main__":
     if "--pitch" in sys.argv[1:]:
         write_pitch()
@@ -329,5 +382,7 @@ if __name__ == "__main__":
         write_sequence()
     elif "--alignment" in sys.argv[1:]:
         write_alignment()
+    elif "--cqt" in sys.argv[1:]:
+        write_cqt()
     else:
         main()
