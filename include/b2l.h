@@ -241,6 +241,56 @@ typedef struct b2l_cqt_octave {
 int b2l_cqt_project(b2l_ctx* ctx, const b2l_cqt_octave* h_oct, int32_t n_oct, const int32_t* d_indptr,
                     const int32_t* d_indices, const void* d_data, const double* d_rscale, int64_t n_clips,
                     int64_t n_frames, int32_t n_bins, void* d_out);
+/* The constant-Q chroma features (feature/spectral.py:1296-1839): chroma_cqt / chroma_vqt (:1296-1423, :1576-1706),
+ * the CENS steps of chroma_cens (:1426-1573) and tonnetz (:1709-1839), in one launch per 65 535 clips.
+ * b2l_chroma_fold reads d_in [n_clips] x (n_bins, n_frames) in the form `input` names (complex64 input is taken as
+ * |x|, correctly rounded) and, per frame, applies the cq_to_chroma map (CSR d_row_ptr [n_chroma + 1], d_cols, d_weights
+ * float64: filters.cq_to_chroma, filters.py:737-861; an identity for tonnetz(chroma=...)), zeroes values below
+ * `threshold` (when has_threshold) and normalises with `norm` (util.normalize, util/utils.py:958-1024: the length in
+ * float64, lengths below tiny(dtype) replaced by 1), all in the chroma precision (out_f64).  The epilogue then:
+ *   PLAIN    writes the chroma to d_out [n_clips][n_chroma][n_frames];
+ *   CENS     L1-normalises, quantises to multiples of 0.25 at the steps 0.4 / 0.2 / 0.1 / 0.05, normalises with
+ *            post_norm (NONE: the quantised values, for b2l_chroma_smooth) and writes as PLAIN;
+ *   TONNETZ  L1-normalises and writes the float64 projection d_phi [6][n_chroma] of it to d_out [n_clips][6][n_frames].
+ * A non-finite value met by a normalisation sets B2L_STATUS_NOT_FINITE_VALUE (normalize's "Input must be finite").
+ * b2l_chroma_smooth is chroma_cens's scipy.ndimage.convolve(x, w, mode="constant") along frames of d_in
+ * [n_clips][n_chroma][n_frames] followed by util.normalize(norm): out[t] = sum_k d_tap_w[k] * x[t - reach +
+ * d_tap_off[k]] in double, ascending k, zero outside the clip, rounded once, with reach = win_len - 1 - win_len / 2;
+ * the taps are the positions of the reversed window whose weight exceeds DBL_EPSILON in magnitude, as ndimage keeps. */
+enum b2l_chroma_input {
+  B2L_CHROMA_IN_C64_FT = 0, /* complex64 [n_frames][n_bins] per clip */
+  B2L_CHROMA_IN_F32_FT = 1,
+  B2L_CHROMA_IN_F32_C = 2,  /* float32 [n_bins][n_frames] per clip */
+  B2L_CHROMA_IN_F64_FT = 3,
+  B2L_CHROMA_IN_F64_C = 4
+};
+enum b2l_chroma_norm { B2L_CHROMA_NORM_NONE = 0, B2L_CHROMA_NORM_INF = 1, B2L_CHROMA_NORM_NEG_INF = 2,
+                       B2L_CHROMA_NORM_ZERO = 3, B2L_CHROMA_NORM_P = 4 };
+enum b2l_chroma_epilogue { B2L_CHROMA_PLAIN = 0, B2L_CHROMA_CENS = 1, B2L_CHROMA_TONNETZ = 2 };
+typedef struct b2l_chroma_desc {
+  int32_t input;          /* enum b2l_chroma_input */
+  int32_t out_f64;        /* chroma precision: float64 (1) or float32 (0) */
+  int32_t n_bins;
+  int32_t n_chroma;
+  int32_t nnz;            /* nonzeros of the map */
+  int32_t norm;           /* enum b2l_chroma_norm */
+  double norm_p;          /* the p of B2L_CHROMA_NORM_P */
+  int32_t has_threshold;
+  int32_t epilogue;       /* enum b2l_chroma_epilogue */
+  double threshold;
+  int32_t post_norm;      /* CENS: enum b2l_chroma_norm after the quantisation */
+  int32_t pad_;
+  double post_p;
+  const int32_t* d_row_ptr;
+  const int32_t* d_cols;
+  const double* d_weights;
+  const double* d_phi;    /* TONNETZ only */
+} b2l_chroma_desc;
+int b2l_chroma_fold(b2l_ctx* ctx, const b2l_chroma_desc* desc, const void* d_in, int64_t n_clips, int64_t n_frames,
+                    void* d_out);
+int b2l_chroma_smooth(b2l_ctx* ctx, const void* d_in, int64_t n_clips, int32_t n_chroma, int64_t n_frames,
+                      int32_t f64, const int32_t* d_tap_off, const double* d_tap_w, int32_t n_taps, int32_t win_len,
+                      int32_t norm, double norm_p, void* d_out);
 /* out = x - y over n floats */
 int b2l_sub(b2l_ctx* ctx, const float* d_x, const float* d_y, int64_t n, float* d_out);
 /* Tuning estimation for chroma_stft (feature/spectral.py:1137-1293): librosa.estimate_tuning

@@ -195,6 +195,20 @@ class CqtOctave(C.Structure):
 CQT_MAX_OCTAVES = 32   # B2L_CQT_MAX_OCTAVES
 
 
+class ChromaDesc(C.Structure):
+    """struct b2l_chroma_desc (include/b2l.h): one b2l_chroma_fold; the d_* fields are device pointers."""
+    _fields_ = [("input", C.c_int32), ("out_f64", C.c_int32), ("n_bins", C.c_int32), ("n_chroma", C.c_int32),
+                ("nnz", C.c_int32), ("norm", C.c_int32), ("norm_p", C.c_double), ("has_threshold", C.c_int32),
+                ("epilogue", C.c_int32), ("threshold", C.c_double), ("post_norm", C.c_int32), ("pad_", C.c_int32),
+                ("post_p", C.c_double), ("d_row_ptr", C.c_void_p), ("d_cols", C.c_void_p), ("d_weights", C.c_void_p),
+                ("d_phi", C.c_void_p)]
+
+
+CHROMA_IN_C64_FT, CHROMA_IN_F32_FT, CHROMA_IN_F32_C, CHROMA_IN_F64_FT, CHROMA_IN_F64_C = range(5)   # enum b2l_chroma_input
+CHROMA_NORM_NONE, CHROMA_NORM_INF, CHROMA_NORM_NEG_INF, CHROMA_NORM_ZERO, CHROMA_NORM_P = range(5)   # enum b2l_chroma_norm
+CHROMA_PLAIN, CHROMA_CENS, CHROMA_TONNETZ = range(3)   # enum b2l_chroma_epilogue
+
+
 DTW_METRICS = {"euclidean": 0, "sqeuclidean": 1, "cityblock": 2, "chebyshev": 3, "cosine": 4}   # enum b2l_dtw_metric
 BEAT_FRAMES, BEAT_SAMPLES, BEAT_TIME = range(3)   # enum b2l_beat_units
 SEQ_PLAIN, SEQ_DISC, SEQ_BINARY = range(3)        # enum b2l_seq_mode
@@ -299,6 +313,9 @@ def _declare(lib):
         "b2l_rqa": (C.c_int, [_vp, _vp, _i64, _i64, C.c_int32, C.c_double, C.c_double, C.c_int32, _vp, _vp]),
         "b2l_rqa_path": (C.c_int, [_vp, _vp, _vp, _i64, _i64, C.c_int32, _vp, _vp]),
         "b2l_cqt_project": (C.c_int, [_vp, P(CqtOctave), C.c_int32, _vp, _vp, _vp, _vp, _i64, _i64, C.c_int32, _vp]),
+        "b2l_chroma_fold": (C.c_int, [_vp, P(ChromaDesc), _vp, _i64, _i64, _vp]),
+        "b2l_chroma_smooth": (C.c_int, [_vp, _vp, _i64, C.c_int32, _i64, C.c_int32, _vp, _vp, C.c_int32, C.c_int32,
+                                        C.c_int32, C.c_double, _vp]),
         "b2l_stft_f64": (C.c_int, [_vp, _vp, _i64, _i64, _i64, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                    P(C.c_double), _vp]),
         "b2l_istft_f64": (C.c_int, [_vp, _vp, _i64, _i64, _i64, C.c_int32, C.c_int32, C.c_int32, P(C.c_double),

@@ -246,3 +246,296 @@ def mfcc(*, y=None, sr: float = 22050, S=None, n_mfcc: int = 20, dct_type: int =
                          n_frames=T, out_tail=(dct.shape[0], T), dtype=np.float32, launch=launch,
                          scratch_per_clip=n_mels * ((T + 63) // 64 * 64))
     return res if isinstance(res, nat.DeviceArray) or res.dtype == res_dtype else res.astype(res_dtype)
+
+
+# --------------------------------------------------------------------------------------------- constant-Q chroma
+# chroma_cqt / chroma_cens / chroma_vqt / tonnetz (feature/spectral.py:1296-1839).  Everything after the CQT is one
+# launch of b2l_chroma_fold (a second, b2l_chroma_smooth, for CENS smoothing); the y= paths run this library's cqt /
+# vqt on the staged signal and fold its complex64 result, so |C| never reaches memory.
+def _chroma_norm(norm):
+    """(enum b2l_chroma_norm, p) of util.normalize's ``norm``, or None for a norm that normalize refuses."""
+    if norm is None:
+        return nat.CHROMA_NORM_NONE, 0.0
+    if norm == np.inf:
+        return nat.CHROMA_NORM_INF, 0.0
+    if norm == -np.inf:
+        return nat.CHROMA_NORM_NEG_INF, 0.0
+    if norm == 0:
+        return nat.CHROMA_NORM_ZERO, 0.0
+    if np.issubdtype(type(norm), np.number) and norm > 0:
+        return nat.CHROMA_NORM_P, float(norm)
+    return None
+
+
+def _map_table(ctx, M):
+    """Device CSR of a dense map (row offsets, columns, float64 weights; ascending columns), cached by the context."""
+    M = np.asarray(M)
+    rows, cols = np.nonzero(M)
+    ptr = np.zeros(M.shape[0] + 1, dtype=np.int32)
+    np.cumsum(np.bincount(rows, minlength=M.shape[0]), out=ptr[1:])
+    key = (pl.digest(M.astype(np.float64)), M.shape)
+    return (pl.f64_constant(ctx, ("chroma_ptr",) + key, ptr),
+            pl.f64_constant(ctx, ("chroma_cols",) + key, cols.astype(np.int32)),
+            pl.f64_constant(ctx, ("chroma_w",) + key, M[rows, cols].astype(np.float64)), len(cols))
+
+
+def _tonnetz_phi(n_chroma: int) -> np.ndarray:
+    """tonnetz's 6 x n_chroma transform (feature/spectral.py:1821-1833)."""
+    dim_map = np.linspace(0, 12, num=n_chroma, endpoint=False)
+    scale = np.asarray([7.0 / 6, 7.0 / 6, 3.0 / 2, 3.0 / 2, 2.0 / 3, 2.0 / 3])
+    V = np.multiply.outer(scale, dim_map)
+    V[::2] -= 0.5
+    R = np.array([1, 1, 1, 1, 0.5, 0.5])
+    return R[:, np.newaxis] * np.cos(np.pi * V)
+
+
+def _smoothing_taps(smoothing_window, win_len_smooth):
+    """chroma_cens's normalised smoothing window of win_len_smooth + 2 points as the taps scipy.ndimage.convolve
+    uses: the window reversed, positions whose weight exceeds DBL_EPSILON in magnitude, ascending."""
+    from .. import filters
+
+    win = filters.get_window(smoothing_window, win_len_smooth + 2, fftbins=False)
+    win = win / np.sum(win)
+    flipped = np.asarray(win, dtype=np.float64)[::-1]
+    keep = np.flatnonzero(np.abs(flipped) > np.finfo(np.float64).eps)
+    return keep.astype(np.int32), np.ascontiguousarray(flipped[keep]), len(win)
+
+
+def _stage_real(sc, X, what: str):
+    """A real ``(..., rows, frames)`` argument on the device, in the layout it has -> (DeviceArray, enum
+    b2l_chroma_input, host copy kept alive until the call has synchronised)."""
+    if isinstance(X, nat.DeviceArray):
+        dt, shape = X.dtype, X.shape
+    else:
+        X = np.asarray(X)
+        dt, shape = X.dtype, X.shape
+    if np.issubdtype(dt, np.complexfloating):
+        raise nat.UnsupportedOnGPU(f"{what}: complex input would give complex chroma; pass the magnitude np.abs({what})")
+    if len(shape) < 2:
+        raise ParameterError(f"{what} must have at least two dimensions (..., bins, frames), given shape={shape}")
+    host = None
+    if isinstance(X, nat.DeviceArray):
+        if dt not in (np.float32, np.float64):
+            raise ParameterError(f"device {what} must be float32 or float64")
+        d = X
+    else:
+        dt = dt if dt in (np.float32, np.float64) else np.result_type(dt, np.float32)
+        mem = np.swapaxes(X, -1, -2)
+        if mem.flags.c_contiguous and not X.flags.c_contiguous and mem.dtype == dt:
+            host, layout = mem, "ft"   # [..., frame, bin] memory, cqt's order="F": uploaded as it is
+        else:
+            host, layout = np.ascontiguousarray(X, dtype=dt), "c"
+        d = sc.empty(shape, dt, layout)
+        if host.nbytes:
+            nat.check(nat.lib().b2l_h2d(sc.ctx.handle, _vp(d.ptr), host.ctypes.data_as(_vp), host.nbytes))
+    f64 = d.dtype == np.float64
+    kind = {(False, "ft"): nat.CHROMA_IN_F32_FT, (False, "c"): nat.CHROMA_IN_F32_C,
+            (True, "ft"): nat.CHROMA_IN_F64_FT, (True, "c"): nat.CHROMA_IN_F64_C}[(f64, d.layout)]
+    return d, kind, host
+
+
+def _chroma_pipeline(*, y, X, what, transform, make_map, norm, threshold, epilogue, post_norm=None, taps=None):
+    """The body of chroma_cqt / chroma_vqt / chroma_cens / tonnetz after their argument checks.
+
+    ``X`` (C, V or chroma) or, when it is None, ``transform(staged device signal)`` (a complex64 "ft" cqt / vqt)
+    is folded with ``make_map(n_rows)``; ``norm`` and ``threshold`` are chroma_cqt's; ``epilogue`` is the
+    b2l_chroma_fold epilogue; CENS: ``post_norm`` is its final norm and ``taps`` its smoothing (None: none).
+    Non-finite data and unsupported norms raise in the reference's order once the device has finished."""
+    staged = None
+    with pl.Scope(y if X is None else X) as sc:
+        if X is None:
+            _, req = pl.precheck_signal(y)
+            staged = pl.StagedInput(y)
+            if staged.on_device:
+                nat.check(nat.lib().b2l_status_reset(staged.ctx.handle))
+            src = sc.own(transform(staged.dev))
+            staged.scan_all()
+            staged.release()
+            kind, req = nat.CHROMA_IN_C64_FT, np.dtype(req)
+        else:
+            src, kind, host = _stage_real(sc, X, what)
+            nat.check(nat.lib().b2l_status_reset(sc.ctx.handle))
+            req = src.dtype
+        ctx, L = sc.ctx, nat.lib()
+        M = make_map(src.shape[-2])
+        prec = np.result_type(M.dtype, np.float32 if kind == nat.CHROMA_IN_C64_FT else src.dtype)
+        lead, T = tuple(src.shape[:-2]), src.shape[-1]
+        d_ptr, d_cols, d_w, nnz = _map_table(ctx, M)
+        nk = _chroma_norm(norm) or (nat.CHROMA_NORM_NONE, 0.0)
+        pk = _chroma_norm(post_norm) or (nat.CHROMA_NORM_NONE, 0.0)
+        d_phi = 0
+        if epilogue == nat.CHROMA_TONNETZ:
+            d_phi = pl.f64_constant(ctx, ("tonnetz_phi", M.shape[0]), _tonnetz_phi(M.shape[0]))
+            out = sc.empty(lead + (6, T), np.float64)
+        else:
+            out = sc.empty(lead + (M.shape[0], T), prec)
+        if taps is not None:
+            pk = (nat.CHROMA_NORM_NONE, 0.0)
+        desc = nat.ChromaDesc(kind, int(prec == np.float64), src.shape[-2], M.shape[0], nnz, nk[0], nk[1],
+                              int(threshold is not None), epilogue, float(threshold or 0.0), pk[0], 0, pk[1],
+                              d_ptr, d_cols, d_w, d_phi or None)
+        n_clips = pl.clip_count(lead)
+        nat.check(L.b2l_chroma_fold(ctx.handle, C.byref(desc), _vp(src.ptr), n_clips, T, _vp(out.ptr)))
+        if taps is not None:
+            off, w, win_len = taps
+            fk = _chroma_norm(post_norm) or (nat.CHROMA_NORM_NONE, 0.0)
+            d_off = pl.f64_constant(ctx, ("cens_off", off.tobytes()), off)
+            d_tw = pl.f64_constant(ctx, ("cens_w", w.tobytes()), w)
+            smoothed = sc.empty(out.shape, prec)
+            nat.check(L.b2l_chroma_smooth(ctx.handle, _vp(out.ptr), n_clips, M.shape[0], T, int(prec == np.float64),
+                                          _vp(d_off), _vp(d_tw), len(off), win_len, fk[0], fk[1], _vp(smoothed.ptr)))
+            out = smoothed
+        flags = pl.status_word(ctx)
+        if staged is not None:
+            staged.check_finite()
+        if flags & nat.STATUS_NOT_FINITE_VALUE:
+            raise ParameterError("Input must be finite")
+        for n in (norm, post_norm):
+            if _chroma_norm(n) is None:
+                raise ParameterError(f"Unsupported norm: {n!r}")
+        if epilogue == nat.CHROMA_TONNETZ:
+            dtype = np.dtype(np.float64)
+        else:
+            dtype = np.result_type(M.dtype, req if kind == nat.CHROMA_IN_C64_FT else src.dtype)
+        return sc.result(out, dtype)
+
+
+def _cqt_transform(*, sr, hop_length, fmin, n_bins, bins_per_octave, tuning, res_type, intervals="equal", gamma=0):
+    """The y= transform of the chroma features: this library's vqt on the staged signal (a DeviceArray result)."""
+    from ..core.constantq import vqt
+
+    return lambda dev: vqt(dev, sr=sr, hop_length=hop_length, fmin=fmin, n_bins=n_bins, intervals=intervals,
+                           gamma=gamma, bins_per_octave=bins_per_octave, tuning=tuning, res_type=res_type)
+
+
+def _refuse_resampling(y, *, sr, hop_length, fmin, n_bins, bins_per_octave, tuning, res_type, intervals="equal",
+                       gamma=0):
+    """Refuse, before any device work, a y= call whose CQT would resample with a resampler other than polyphase
+    (the reference's default res_type is soxr_hq).  Argument errors are left to the CQT, which raises them in the
+    reference's order."""
+    from ..core import constantq as Q
+
+    if res_type == "polyphase":
+        return
+    try:
+        n = y.shape[-1]
+        f0 = Q._default_fmin() if fmin is None else fmin
+        Q.plan(n, sr=sr, hop_length=hop_length, fmin=f0 * 2.0 ** ((tuning or 0.0) / bins_per_octave), n_bins=n_bins,
+               intervals=intervals, gamma=gamma, bins_per_octave=bins_per_octave, filter_scale=1, window="hann",
+               scale=True, res_type=res_type)
+    except nat.UnsupportedOnGPU:
+        raise nat.UnsupportedOnGPU(
+            f"res_type={res_type!r}: this CQT resamples, and only the 'polyphase' resampler runs on the GPU; pass "
+            "res_type='polyphase', or compute the CQT yourself and pass its magnitude as C= (V= for chroma_vqt)") from None
+    except Exception:
+        return
+
+
+def _cqt_chroma_args(y, C, n_chroma, bins_per_octave, cqt_mode):
+    """chroma_cqt's first checks (feature/spectral.py:1378-1393) -> bins_per_octave."""
+    if bins_per_octave is None:
+        bins_per_octave = n_chroma
+    elif np.remainder(bins_per_octave, n_chroma) != 0:
+        raise ParameterError(f"bins_per_octave={bins_per_octave} must be an integer multiple of n_chroma={n_chroma}")
+    if C is None:
+        if y is None:
+            raise ParameterError("At least one of C or y must be provided to compute chroma")
+        if cqt_mode == "hybrid":
+            raise nat.UnsupportedOnGPU("chroma_cqt(cqt_mode='hybrid'): hybrid_cqt is not part of this library; use "
+                                       "cqt_mode='full' or pass C=")
+        if cqt_mode != "full":
+            raise KeyError(cqt_mode)
+    return bins_per_octave
+
+
+def _chroma_cqt(*, y, sr, C, hop_length, fmin, norm, threshold, tuning, n_chroma, n_octaves, window,
+                bins_per_octave, cqt_mode, res_type, epilogue, post_norm=None, taps=None):
+    from .. import filters
+
+    bins_per_octave = _cqt_chroma_args(y, C, n_chroma, bins_per_octave, cqt_mode)
+    cq = dict(sr=sr, hop_length=hop_length, fmin=fmin, n_bins=n_octaves * bins_per_octave,
+              bins_per_octave=bins_per_octave, tuning=tuning, res_type=res_type)
+    if C is None:
+        pl.precheck_signal(y)
+        _refuse_resampling(y, **cq)
+    return _chroma_pipeline(
+        y=y, X=C, what="C", transform=_cqt_transform(**cq),
+        make_map=lambda n: filters.cq_to_chroma(n, bins_per_octave=bins_per_octave, n_chroma=n_chroma, fmin=fmin,
+                                                window=window),
+        norm=norm, threshold=threshold, epilogue=epilogue, post_norm=post_norm, taps=taps)
+
+
+def chroma_cqt(*, y=None, sr: float = 22050, C=None, hop_length: int = 512, fmin=None, norm=np.inf,
+               threshold: float = 0.0, tuning: Optional[float] = None, n_chroma: int = 12, n_octaves: int = 7,
+               window=None, bins_per_octave: Optional[int] = 36, cqt_mode: str = "full", res_type: str = "soxr_hq"):
+    """Constant-Q chromagram, shape ``(..., n_chroma, t)``; same contract as ``librosa.feature.chroma_cqt``
+    (feature/spectral.py:1296-1423), plus ``res_type``, forwarded to ``cqt``: the reference's own cqt call uses its
+    default "soxr_hq", and only "polyphase" resamples on the GPU.  ``C`` is a real CQT magnitude, host or device,
+    float32 or float64; the result is float32, float64 for float64 ``C`` or a ``window``."""
+    return _chroma_cqt(y=y, sr=sr, C=C, hop_length=hop_length, fmin=fmin, norm=norm, threshold=threshold,
+                       tuning=tuning, n_chroma=n_chroma, n_octaves=n_octaves, window=window,
+                       bins_per_octave=bins_per_octave, cqt_mode=cqt_mode, res_type=res_type,
+                       epilogue=nat.CHROMA_PLAIN)
+
+
+def chroma_cens(*, y=None, sr: float = 22050, C=None, hop_length: int = 512, fmin=None,
+                tuning: Optional[float] = None, n_chroma: int = 12, n_octaves: int = 7, bins_per_octave: int = 36,
+                cqt_mode: str = "full", window=None, norm=2, win_len_smooth: Optional[int] = 41,
+                smoothing_window="hann", res_type: str = "soxr_hq"):
+    """Chroma Energy Normalized, shape ``(..., n_chroma, t)``; same contract as ``librosa.feature.chroma_cens``
+    (feature/spectral.py:1426-1573), plus chroma_cqt's ``res_type``.  The chroma, its L1 normalisation and
+    quantisation are one launch; the smoothing (scipy.ndimage.convolve along frames) and the final normalisation
+    another, unless ``win_len_smooth`` is None."""
+    if not ((win_len_smooth is None) or (isinstance(win_len_smooth, (int, np.integer)) and win_len_smooth > 0)):
+        raise ParameterError(f"win_len_smooth={win_len_smooth} must be a positive integer or None")
+    _cqt_chroma_args(y, C, n_chroma, bins_per_octave, cqt_mode)
+    taps = _smoothing_taps(smoothing_window, win_len_smooth) if win_len_smooth else None
+    return _chroma_cqt(y=y, sr=sr, C=C, hop_length=hop_length, fmin=fmin, norm=None, threshold=0.0, tuning=tuning,
+                       n_chroma=n_chroma, n_octaves=n_octaves, window=window, bins_per_octave=bins_per_octave,
+                       cqt_mode=cqt_mode, res_type=res_type, epilogue=nat.CHROMA_CENS, post_norm=norm, taps=taps)
+
+
+def chroma_vqt(*, y=None, sr: float = 22050, V=None, hop_length: int = 512, fmin=None, intervals, norm=np.inf,
+               threshold: float = 0.0, n_octaves: int = 7, bins_per_octave: int = 12, gamma: float = 0,
+               res_type: str = "soxr_hq"):
+    """Variable-Q chromagram, shape ``(..., bins_per_octave, t)``; same contract as
+    ``librosa.feature.chroma_vqt`` (feature/spectral.py:1576-1706), plus chroma_cqt's ``res_type``.  On the y= path
+    ``intervals`` is "equal" or explicit ratios (the named interval sets are not part of this library's vqt)."""
+    from .. import filters
+
+    if not isinstance(intervals, str):
+        bins_per_octave = len(intervals)
+    cq = dict(sr=sr, hop_length=hop_length, fmin=fmin, n_bins=n_octaves * bins_per_octave,
+              bins_per_octave=bins_per_octave, tuning=0.0, res_type=res_type, intervals=intervals, gamma=gamma)
+    if V is None:
+        if y is None:
+            raise ParameterError("At least one of y or V must be provided to compute chroma")
+        if isinstance(intervals, str) and intervals != "equal":
+            raise nat.UnsupportedOnGPU(f"chroma_vqt(y=..., intervals={intervals!r}): only 'equal' and explicit "
+                                       "interval ratios are supported on the y= path; pass V= for named interval sets")
+        pl.precheck_signal(y)
+        _refuse_resampling(y, **cq)
+    return _chroma_pipeline(
+        y=y, X=V, what="V", transform=_cqt_transform(**cq),
+        make_map=lambda n: filters.cq_to_chroma(n, bins_per_octave=bins_per_octave, n_chroma=bins_per_octave,
+                                                fmin=fmin),
+        norm=norm, threshold=threshold, epilogue=nat.CHROMA_PLAIN)
+
+
+def tonnetz(*, y=None, sr: float = 22050, chroma=None, **kwargs):
+    """Tonal centroid features, shape ``(..., 6, t)`` float64; same contract as ``librosa.feature.tonnetz``
+    (feature/spectral.py:1709-1839).  ``kwargs`` go to chroma_cqt when ``chroma`` is None; the chroma, its L1
+    normalisation and the projection are one launch after the CQT."""
+    if y is None and chroma is None:
+        raise ParameterError("Either the audio samples or the chromagram must be passed as an argument.")
+    if chroma is None:
+        kw = dict(sr=sr, C=None, hop_length=512, fmin=None, norm=np.inf, threshold=0.0, tuning=None, n_chroma=12,
+                  n_octaves=7, window=None, bins_per_octave=36, cqt_mode="full", res_type="soxr_hq")
+        unknown = set(kwargs) - set(kw)
+        if unknown:
+            raise TypeError(f"chroma_cqt() got an unexpected keyword argument {sorted(unknown)[0]!r}")
+        kw.update(kwargs)
+        return _chroma_cqt(y=y, epilogue=nat.CHROMA_TONNETZ, **kw)
+    return _chroma_pipeline(y=None, X=chroma, what="chroma", transform=None,
+                            make_map=lambda n: np.eye(n, dtype=np.float32), norm=None, threshold=None,
+                            epilogue=nat.CHROMA_TONNETZ)

@@ -188,3 +188,32 @@ def wavelet(*, freqs: np.ndarray, sr: float = 22050, window="hann", filter_scale
     size = max(lengths)
     size = int(2.0 ** (np.ceil(np.log2(size)))) if pad_fft else int(np.ceil(size))
     return np.asarray([pad_center(r, size=size, **kwargs) for r in rows], dtype=dtype), lengths
+
+
+def _hz_to_midi(frequencies):
+    """MIDI note number of a frequency (librosa/core/convert.py:913-940)."""
+    return (12 * (np.log2(np.asanyarray(frequencies)) - np.log2(440.0)) + 69)[()]
+
+
+def cq_to_chroma(n_input: int, *, bins_per_octave: int = 12, n_chroma: int = 12, fmin=None, window=None,
+                 base_c: bool = True, dtype=np.float32) -> np.ndarray:
+    """Map of constant-Q bins onto chroma bins, shape ``(n_chroma, n_input)`` (librosa/filters.py:737-861): the
+    identity tiled ``bins_per_octave / n_chroma`` times, rolled to centre on each target bin, repeated over the
+    octaves, rolled so that the first chroma bin is C (A when not ``base_c``), then convolved with ``window`` when
+    one is given (float64 then).  ``fmin`` None is C1."""
+    n_merge = float(bins_per_octave) / n_chroma
+    if fmin is None:
+        fmin = 440.0 * (2.0 ** ((np.asanyarray(24) - 69.0) / 12.0))   # note_to_hz("C1")
+    if np.mod(n_merge, 1) != 0:
+        raise ParameterError("Incompatible CQ merge: input bins must be an integer multiple of output bins.")
+    cq_to_ch = np.repeat(np.eye(n_chroma), int(n_merge), axis=1)
+    cq_to_ch = np.roll(cq_to_ch, -int(n_merge // 2), axis=1)
+    n_octaves = np.ceil(float(n_input) / bins_per_octave)
+    cq_to_ch = np.tile(cq_to_ch, int(n_octaves))[:, :n_input]
+    midi_0 = np.mod(_hz_to_midi(fmin), 12)
+    roll = midi_0 if base_c else midi_0 - 9
+    roll = int(np.round(roll * (n_chroma / 12.0)))
+    cq_to_ch = np.roll(cq_to_ch, roll, axis=0).astype(dtype)
+    if window is not None:
+        cq_to_ch = scipy.signal.convolve(cq_to_ch, np.atleast_2d(window), mode="same")
+    return cq_to_ch

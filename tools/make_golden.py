@@ -4,8 +4,9 @@ cases through the UNMODIFIED reference; ``--pitch`` writes only tests/golden/pit
 and leaves the other fixtures as they are; ``--rhythm`` likewise writes only tests/golden/rhythm_v1.npz
 (tests/rhythm_cases.py), ``--beat`` only tests/golden/beat_v1.npz (tests/beat_cases.py), ``--onset`` only
 tests/golden/onset_v1.npz (tests/onset_cases.py), ``--sequence`` only tests/golden/sequence_v1.npz
-(tests/sequence_cases.py), ``--alignment`` only tests/golden/alignment_v1.npz (tests/alignment_cases.py), and
-``--cqt`` only tests/golden/cqt_v1.npz (tests/cqt_cases.py).
+(tests/sequence_cases.py), ``--alignment`` only tests/golden/alignment_v1.npz (tests/alignment_cases.py),
+``--cqt`` only tests/golden/cqt_v1.npz (tests/cqt_cases.py), and ``--chroma`` only tests/golden/chroma_v1.npz
+(tests/chroma_cases.py).
 
 Needs a checkout of the reference (see tools/ref_shim.py); the tests only read the stored fixtures.  Also
 stores a handful of constant tables (mel bases, window sum-square, mel-scale known answers) produced by the
@@ -19,6 +20,7 @@ reference.
     python tools/make_golden.py --sequence
     python tools/make_golden.py --alignment
     python tools/make_golden.py --cqt
+    python tools/make_golden.py --chroma
 """
 from __future__ import annotations
 
@@ -369,6 +371,78 @@ def write_cqt():
     print("wrote", path, os.path.getsize(path), "bytes")
 
 
+def write_chroma():
+    """tests/golden/chroma_v1.npz: per case of tests/chroma_cases.py, the reference's result (or ``<name>/error``);
+    the y= cases run with the reference's feature module calling the reference's own cqt / vqt with
+    res_type="polyphase" (rebound only while they run).  For WITH_STEPS, |C| (the argument of the reference's
+    cq_to_chroma einsum), the raw chroma (recorded around util.normalize) and CENS's quantised input (recorded
+    around scipy.ndimage.convolve); and the cq_to_chroma maps of MAPS."""
+    import functools
+    import importlib
+
+    import scipy.ndimage
+
+    import chroma_cases as HC
+
+    ref = ref_shim.load_reference()
+    spectral = importlib.import_module("librosa.feature.spectral")
+    store = {}
+    for name, kw in HC.MAPS.items():
+        kw = dict(kw)
+        store[f"map/{name}"] = ref.filters.cq_to_chroma(kw.pop("n_input"), **kw)
+    store["tonnetz_chroma_stft/input"] = ref.feature.chroma_stft(y=HC.stft_chroma_signal(), sr=22050, hop_length=512,
+                                                                 tuning=0.0)
+    orig = {k: spectral.__dict__[k] for k in ("cqt", "vqt", "np")}
+    for case in HC.CASES:
+        if case["refuse"]:
+            continue
+        name = case["name"]
+        rec = {}
+        polyphase = case["kw"].get("res_type") == "polyphase"
+
+        class _Np:   # np as the feature module sees it, with einsum recorded (its second operand is |C|)
+            def __getattr__(self, attr):
+                return getattr(np, attr)
+
+            @staticmethod
+            def einsum(spec, *ops, **kw):
+                out = np.einsum(spec, *ops, **kw)
+                if spec == "cf,...ft->...ct":
+                    rec.setdefault("absC", ops[1])
+                    rec.setdefault("raw", out.copy())
+                return out
+
+        conv = scipy.ndimage.convolve
+
+        def convolve(x, w, **kw):
+            rec.setdefault("quant", np.array(x))
+            return conv(x, w, **kw)
+
+        if polyphase:
+            spectral.cqt = functools.partial(orig["cqt"], res_type="polyphase")
+            spectral.vqt = functools.partial(orig["vqt"], res_type="polyphase")
+        spectral.np = _Np()
+        scipy.ndimage.convolve = convolve
+        try:
+            with warnings.catch_warnings():
+                warnings.simplefilter("ignore")
+                out = HC.call(ref, case, golden=store, drop_res_type=True)
+            store[f"{name}/out"] = out
+        except Exception as e:   # the reference's own error, stored as "Class: message"
+            store[f"{name}/error"] = np.array(f"{type(e).__name__}: {e}")
+        finally:
+            spectral.__dict__.update(orig)
+            scipy.ndimage.convolve = conv
+        if name in HC.WITH_STEPS:
+            for k, v in rec.items():
+                if k != "absC" or case["inp"] is None:   # a C= case's |C| is its seeded input
+                    store[f"{name}/{k}"] = v
+        print(f"{name:32s} {store.get(f'{name}/error', np.shape(store.get(f'{name}/out')))} {sorted(rec)}")
+    path = os.path.join(ROOT, "tests", "golden", "chroma_v1.npz")
+    np.savez_compressed(path, **store)
+    print("wrote", path, os.path.getsize(path), "bytes")
+
+
 if __name__ == "__main__":
     if "--pitch" in sys.argv[1:]:
         write_pitch()
@@ -384,5 +458,7 @@ if __name__ == "__main__":
         write_alignment()
     elif "--cqt" in sys.argv[1:]:
         write_cqt()
+    elif "--chroma" in sys.argv[1:]:
+        write_chroma()
     else:
         main()
