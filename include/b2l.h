@@ -156,7 +156,7 @@ int b2l_melspectrogram(b2l_ctx* ctx, const b2l_plan* plan, const float* d_y, int
 /* librosa.feature.mfcc(y=...) — feature/spectral.py:1843-2019 incl. power_to_db
  * (core/spectrum.py:1735-1883, per-clip top_db reference max).  d_logmel is scratch of
  * n_clips * n_mels * (n_frames rounded up to a multiple of 64) floats (internal tiled layout; NULL: allocated
- * and freed internally). */
+ * and freed internally); like d_y and d_mfcc it needs only the 4-byte alignment of a float. */
 int b2l_mfcc(b2l_ctx* ctx, const b2l_plan* plan, const float* d_y, int64_t n_clips, int64_t n,
              int64_t y_stride, float* d_mfcc, float* d_logmel);
 

@@ -50,6 +50,9 @@ __global__ void __launch_bounds__(KS == 2 ? 640 : 512) dct_clamp4_kernel(const f
   const int m_lo = kset == 0 ? 0 : m_split, m_hi = kset == 0 ? m_split : n_mels;
   for (int i = tid; i < n_mels * KP; i += blockDim.x) s_dct[i] = dctT[i];
   const bool vec_ok = (T % 4 == 0) && ((reinterpret_cast<uintptr_t>(L) & 15) == 0);
+  // tiled: every 64-frame block is 256 * n_mels bytes, so the blocks are 16-byte aligned exactly when L is (a
+  // caller's b2l_mfcc scratch need not be)
+  const bool tile_vec = (reinterpret_cast<uintptr_t>(L) & 15) == 0;
   const bool vec_out = (T % 4 == 0) && ((reinterpret_cast<uintptr_t>(C) & 15) == 0);
   const int blocks64 = (T + 63) >> 6;
   const float* xlane = s_tile + (lane >> 4) * blk_words + (lane & 15) * 4;
@@ -61,7 +64,10 @@ __global__ void __launch_bounds__(KS == 2 ? 640 : 512) dct_clamp4_kernel(const f
       const int b0 = t0 >> 6;
       const int words = (blocks64 - b0 >= 2 ? 2 : 1) * blk_words;   // the clip's last tile may hold one block only
       const float* Lt = L + ((long long)clip * blocks64 + b0) * blk_words;
-      for (int i = tid; i < words / 4; i += blockDim.x) cp_async16(s_tile + 4 * i, Lt + 4 * i);
+      if (tile_vec)
+        for (int i = tid; i < words / 4; i += blockDim.x) cp_async16(s_tile + 4 * i, Lt + 4 * i);
+      else
+        for (int i = tid; i < words; i += blockDim.x) cp_async4(s_tile + i, Lt + i);
     } else {
       const float* Lc = L + (long long)clip * n_mels * T + t0;
       if (vec_ok && t0 + DCT4_TILE <= T) {
