@@ -173,9 +173,10 @@ def _smooth_even_sizes(limit=4096):
 
 
 def test_mixed_radix_every_size(lb, oracle):
-    """All 96 frame lengths mr_kernel / mr_inv_kernel serve (even, 12 .. 4096, half = 2^a 3^b 5^c, not a power of
-    two) — every radix schedule the host can produce: stft against the oracle, and istft of the oracle's spectrum
-    (length given) against the signal at the float32 bound the power-of-two path is held to (SNR >= 60 dB)."""
+    """All 96 frame lengths mr_inv_kernel serves (even, 12 .. 4096, half = 2^a 3^b 5^c, not a power of two) — every
+    radix schedule the host can produce: istft of the oracle's spectrum (length given) against the signal at the
+    float32 bound the power-of-two path is held to (SNR >= 60 dB).  The forward direction (mr_kernel modes 0 and 1)
+    is held to a float64 reference at every size by test_gpu_forward_spectrum.test_mixed_radix_sizes."""
     import signals
 
     sizes = _smooth_even_sizes()
@@ -186,8 +187,7 @@ def test_mixed_radix_every_size(lb, oracle):
         kw = dict(n_fft=n_fft, hop_length=hop, pad_mode=("constant", "reflect", "edge")[idx % 3])
         with warnings.catch_warnings():
             warnings.simplefilter("ignore")
-            D, Do = lb.stft(y, **kw), oracle.stft(y, **kw)
-        close(D, Do, **TOL["stft"])
+            Do = oracle.stft(y, **kw)
         yr = lb.istft(Do, hop_length=hop, n_fft=n_fft, length=y.shape[-1])
         err = yr - y
         snr = 10 * np.log10(float((y ** 2).sum()) / max(float((err ** 2).sum()), 1e-30))

@@ -149,9 +149,15 @@ def tw_count_split(log2m):
     return count
 
 
-def forward_choice(n_fft, hop, basis, smem_optin=H100_SMEM_OPTIN):
-    """(variant, FT, halves, shared-memory bytes, per-half exchange bytes) of run_forward in MODE_MEL, or None
-    (refused)."""
+MODE_STFT, MODE_MEL, MODE_SPEC, MODE_STATS = 0, 1, 2, 3                   # FwdMode (common.cuh)
+
+
+def forward_choice(n_fft, hop, basis, smem_optin=H100_SMEM_OPTIN, mode=MODE_MEL):
+    """(variant, FT, halves, shared-memory bytes, per-half exchange bytes) of run_forward in `mode`, or None
+    (refused).  The modes differ in the tables after the mbarriers (the MelRow table in MODE_MEL, the M + 1 bin
+    frequencies in MODE_STATS, nothing in MODE_STFT / MODE_SPEC) and in the exchange region: the MelLayout group
+    stride where the power rows are parked (MODE_MEL, MODE_STATS), the plain FT (M + M / 32) float2 otherwise.
+    `basis` is only read in MODE_MEL."""
     log2m = int(np.log2(n_fft)) - 1
     M, N = n_fft // 2, n_fft
     tpf = M // 32 if M >= 32 else 1
@@ -166,16 +172,22 @@ def forward_choice(n_fft, hop, basis, smem_optin=H100_SMEM_OPTIN):
         span = (f - 1) * hop + N
         if span > 0x3fffffff:
             continue
-        t = table_for(basis, rows_per_warp(f))
         off = align_up(N * 4, 16)
         off = align_up(off + tw_count_split(log2m) * 8, 16)
         off = align_up(off + 8 * nh, 16)
-        off = align_up(off + len(t.w) * 4, 16)
-        off = align_up(off + t.n_rows * 8, 16)                           # sizeof(MelRow) == 8
+        if mode == MODE_MEL:
+            t = table_for(basis, rows_per_warp(f))
+            off = align_up(off + len(t.w) * 4, 16)
+            off = align_up(off + t.n_rows * 8, 16)                       # sizeof(MelRow) == 8
+        if mode == MODE_STATS:
+            off = align_up(off + (M + 1) * 4, 16)                        # bin frequencies
         off = align_up(off, 128)
         off += align_up(span * 4, 128) * nh
         off = align_up(off, 128)
-        xbytes = align_up(f * group_stride(M, f) * 8 + ((M + 16) * 4 if M < 128 else 0), 128)
+        if mode in (MODE_MEL, MODE_STATS):
+            xbytes = align_up(f * group_stride(M, f) * 8 + ((M + 16) * 4 if M < 128 else 0), 128)
+        else:
+            xbytes = align_up(f * (M + M // 32) * 8, 128)
         off += xbytes * nh
         if off <= smem_optin:
             return v, f, nh, off, xbytes
@@ -192,22 +204,22 @@ def table_for(basis, H):
     return _tables[key][1]
 
 
-def first_refused_hop(n_fft, basis, smem_optin=H100_SMEM_OPTIN):
+def first_refused_hop(n_fft, basis, smem_optin=H100_SMEM_OPTIN, mode=MODE_MEL):
     lo, hi = 1, 1 << 16                                                 # fits at lo, refused at hi (monotone)
-    assert forward_choice(n_fft, hi, basis, smem_optin) is None
+    assert forward_choice(n_fft, hi, basis, smem_optin, mode) is None
     while hi - lo > 1:
         mid = (lo + hi) // 2
-        lo, hi = (mid, hi) if forward_choice(n_fft, mid, basis, smem_optin) else (lo, mid)
+        lo, hi = (mid, hi) if forward_choice(n_fft, mid, basis, smem_optin, mode) else (lo, mid)
     return hi
 
 
-def variant_runs(n_fft, basis, smem_optin=H100_SMEM_OPTIN):
-    """[(first hop, last hop, variant, FT)] of the instances MODE_MEL selects, hop by hop, and the first refused
+def variant_runs(n_fft, basis, smem_optin=H100_SMEM_OPTIN, mode=MODE_MEL):
+    """[(first hop, last hop, variant, FT)] of the instances `mode` selects, hop by hop, and the first refused
     hop."""
-    stop = first_refused_hop(n_fft, basis, smem_optin)
+    stop = first_refused_hop(n_fft, basis, smem_optin, mode)
     runs = []
     for hop in range(1, stop):
-        v, f = forward_choice(n_fft, hop, basis, smem_optin)[:2]
+        v, f = forward_choice(n_fft, hop, basis, smem_optin, mode)[:2]
         if runs and tuple(runs[-1][2:]) == (v, f):
             runs[-1][1] = hop
         else:

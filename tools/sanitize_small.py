@@ -47,4 +47,20 @@ nat.check(nat.lib().b2l_mfcc(ctx.handle, plan.handle, ctypes.c_void_p(d_y.ptr), 
                              ctypes.c_void_p(out.ptr + 4), ctypes.c_void_p(scr.ptr + 4)))
 Cu = out.get()[1:].reshape(y.shape[0], 20, T)
 print("mfcc unaligned scratch", Cu.shape, bool(np.array_equal(Cu, lb.feature.mfcc(y=y, sr=22050, n_fft=512, hop_length=128))))
+# stft / spectrogram / fused statistics: one hop per instance window of MODE_STFT / MODE_SPEC and of MODE_STATS (the
+# last hop of each), and stats_kernel at the top of its warp ladder (29 056 bins, one warp per block)
+from librosa_b200.core.spectrum import _spectrogram
+for n_fft, hop in [(1024, 674), (1024, 686), (2048, 1248), (2048, 1303), (2048, 5206), (4096, 1546), (4096, 1915),
+                   (4096, 10101), (8192, 16672)]:
+    yb = (0.1 * rng.standard_normal((2, 4 * hop + n_fft))).astype(np.float32)
+    D = lb.stft(yb, n_fft=n_fft, hop_length=hop)
+    Sp, _ = _spectrogram(y=yb, n_fft=n_fft, hop_length=hop, power=1.5)
+    print("stft", n_fft, hop, D.shape, bool(np.isfinite(D).all() and np.isfinite(Sp).all()))
+for n_fft, hop in [(1024, 652), (1024, 665), (2048, 1165), (2048, 1230), (2048, 5051), (4096, 1194), (4096, 1613),
+                   (4096, 9408), (8192, 12544)]:
+    yb = (0.1 * rng.standard_normal((2, 4 * hop + n_fft))).astype(np.float32)
+    c = lb.feature.spectral_centroid(y=yb, sr=22050, n_fft=n_fft, hop_length=hop)
+    print("stats", n_fft, hop, c.shape, bool(np.isfinite(c).all()))
+Sb = np.abs(rng.standard_normal((2, 29056, 3))).astype(np.float32)
+print("stats_kernel 29056 bins", bool(np.isfinite(lb.feature.spectral_centroid(S=Sb, sr=22050)).all()))
 print("sanitize_small done")
