@@ -241,6 +241,42 @@ typedef struct b2l_cqt_octave {
 int b2l_cqt_project(b2l_ctx* ctx, const b2l_cqt_octave* h_oct, int32_t n_oct, const int32_t* d_indptr,
                     const int32_t* d_indices, const void* d_data, const double* d_rscale, int64_t n_clips,
                     int64_t n_frames, int32_t n_bins, void* d_out);
+/* librosa.iirt (core/spectrum.py:1522-1713).  b2l_pad_center: np.pad(y, pad, mode) of each clip of d_x [n_clips][n]
+ * into d_out [n_clips][n + 2 pad] (enum b2l_pad_mode; an empty signal takes only "constant" / "empty").
+ * b2l_iirt_filter: scipy.signal.sosfiltfilt (padtype "odd", SciPy's default padlen) of every (clip, band) chain,
+ * one thread per chain, bit for bit in float64: the odd extension formed in float32, then SciPy's _sosfilt loop with
+ * unfused multiplies and adds.  Chain (clip, j) of rate r reads d_x + clip * x_stride (n samples; n must exceed the
+ * band's padlen) and band d_bands[j]; its scratch column is d_scratch + clip * n_bands + j, with rows scratch_stride
+ * doubles apart, n + padlen rows of which are written; rows 0 .. n-1 hold the filtered signal afterwards.
+ * d_coef [bands][B2L_IIRT_MAX_SECTIONS][8] holds per section b0 b1 b2 a1 a2 and sosfilt_zi's two entries (a0 == 1);
+ * sections 0 .. max_sections - 1 run for every band, so a band with fewer fills the rest with pass-through sections
+ * (b0 = 1, all else 0).  d_info [bands][2] holds the section count and padlen.
+ * b2l_iirt_stmsp: d_out [n_clips][n_bands][n_frames] float32, element (clip, d_bands[j], t) of rate r =
+ * factor * sum_{i < w} x[d_starts[t] + i]^2 over the filtered signal in the scratch (rows at or past n read as the
+ * zeros of util.fix_length), summed in NumPy's pairwise order as given by the leaf program d_leaves [n_leaves][4]
+ * (row offset, length <= 128, partial sums combined after it, 0), rounded once to float32.  Both set no status bit. */
+#define B2L_IIRT_MAX_SECTIONS 10
+#define B2L_IIRT_MAX_RATES 16
+#define B2L_IIRT_MAX_DEPTH 32 /* partial sums held at once by a leaf program */
+typedef struct b2l_iirt_rate {
+  const float* d_x;
+  int64_t x_stride;
+  int64_t n;
+  double* d_scratch;
+  int64_t scratch_stride;
+  const int32_t* d_bands;
+  int32_t n_bands;
+  int32_t n_leaves;
+  const int32_t* d_starts;
+  const int32_t* d_leaves;
+  double factor;
+} b2l_iirt_rate;
+int b2l_pad_center(b2l_ctx* ctx, const float* d_x, int64_t n_clips, int64_t n, int32_t pad, int32_t pad_mode,
+                   float* d_out);
+int b2l_iirt_filter(b2l_ctx* ctx, const b2l_iirt_rate* h_rates, int32_t n_rates, const double* d_coef,
+                    const int32_t* d_info, int32_t max_sections, int64_t n_clips);
+int b2l_iirt_stmsp(b2l_ctx* ctx, const b2l_iirt_rate* h_rates, int32_t n_rates, int64_t n_clips, int64_t n_frames,
+                   int32_t n_bands, float* d_out);
 /* The constant-Q chroma features (feature/spectral.py:1296-1839): chroma_cqt / chroma_vqt (:1296-1423, :1576-1706),
  * the CENS steps of chroma_cens (:1426-1573) and tonnetz (:1709-1839), in one launch per 65 535 clips.
  * b2l_chroma_fold reads d_in [n_clips] x (n_bins, n_frames) in the form `input` names (complex64 input is taken as

@@ -195,6 +195,17 @@ class CqtOctave(C.Structure):
 CQT_MAX_OCTAVES = 32   # B2L_CQT_MAX_OCTAVES
 
 
+class IirtRate(C.Structure):
+    """struct b2l_iirt_rate (include/b2l.h): the chains of one sampling rate of b2l_iirt_filter / b2l_iirt_stmsp;
+    the d_* fields are device pointers."""
+    _fields_ = [("d_x", C.c_void_p), ("x_stride", C.c_int64), ("n", C.c_int64), ("d_scratch", C.c_void_p),
+                ("scratch_stride", C.c_int64), ("d_bands", C.c_void_p), ("n_bands", C.c_int32),
+                ("n_leaves", C.c_int32), ("d_starts", C.c_void_p), ("d_leaves", C.c_void_p), ("factor", C.c_double)]
+
+
+IIRT_MAX_SECTIONS, IIRT_MAX_RATES, IIRT_MAX_DEPTH = 10, 16, 32   # B2L_IIRT_MAX_SECTIONS / _RATES / _DEPTH
+
+
 class ChromaDesc(C.Structure):
     """struct b2l_chroma_desc (include/b2l.h): one b2l_chroma_fold; the d_* fields are device pointers."""
     _fields_ = [("input", C.c_int32), ("out_f64", C.c_int32), ("n_bins", C.c_int32), ("n_chroma", C.c_int32),
@@ -313,6 +324,9 @@ def _declare(lib):
         "b2l_rqa": (C.c_int, [_vp, _vp, _i64, _i64, C.c_int32, C.c_double, C.c_double, C.c_int32, _vp, _vp]),
         "b2l_rqa_path": (C.c_int, [_vp, _vp, _vp, _i64, _i64, C.c_int32, _vp, _vp]),
         "b2l_cqt_project": (C.c_int, [_vp, P(CqtOctave), C.c_int32, _vp, _vp, _vp, _vp, _i64, _i64, C.c_int32, _vp]),
+        "b2l_pad_center": (C.c_int, [_vp, _vp, _i64, _i64, C.c_int32, C.c_int32, _vp]),
+        "b2l_iirt_filter": (C.c_int, [_vp, P(IirtRate), C.c_int32, _vp, _vp, C.c_int32, _i64]),
+        "b2l_iirt_stmsp": (C.c_int, [_vp, P(IirtRate), C.c_int32, _i64, _i64, C.c_int32, _vp]),
         "b2l_chroma_fold": (C.c_int, [_vp, P(ChromaDesc), _vp, _i64, _i64, _vp]),
         "b2l_chroma_smooth": (C.c_int, [_vp, _vp, _i64, C.c_int32, _i64, C.c_int32, _vp, _vp, C.c_int32, C.c_int32,
                                         C.c_int32, C.c_double, _vp]),

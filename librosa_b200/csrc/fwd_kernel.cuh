@@ -55,41 +55,6 @@ __device__ __forceinline__ void tma_load_1d(void* dst_smem, const void* src_gmem
       : "memory");
 }
 
-// ------------------------------------------------------------------ padded sample fetch
-// Virtual sample j of a clip of n samples under np.pad semantics (librosa/core/spectrum.py:252-328,
-// equivalence to np.pad(y, n_fft//2, mode) per SURVEY Appendix A.2).
-__device__ __forceinline__ float load_padded(const float* __restrict__ y, int n, long long j, int mode, int pad) {
-  if (j >= 0 && j < n) return __ldg(y + j);
-  switch (mode) {
-    case PAD_EDGE:
-      return __ldg(y + (j < 0 ? 0 : n - 1));
-    case PAD_REFLECT: {
-      if (n == 1) return __ldg(y);
-      long long P = 2LL * (n - 1);
-      long long m = j % P;
-      if (m < 0) m += P;
-      if (m >= n) m = P - m;
-      return __ldg(y + m);
-    }
-    case PAD_SYMMETRIC: {
-      long long P = 2LL * n;
-      long long m = j % P;
-      if (m < 0) m += P;
-      if (m >= n) m = P - 1 - m;
-      return __ldg(y + m);
-    }
-    case PAD_LINEAR_RAMP: {
-      long long d = j < 0 ? -j : j - (n - 1);          // distance from the edge sample, 1..pad
-      float edge = __ldg(y + (j < 0 ? 0 : n - 1));
-      long long i = pad - d;                           // np.linspace(0, edge, pad, endpoint=False)[i]
-      if (i <= 0) return 0.0f;
-      return (float)((double)i * ((double)edge / (double)pad));
-    }
-    default:
-      return 0.0f;
-  }
-}
-
 // |X|^power from |X|^2 for power != 2 (kept out of line: the default power-2 path never executes it)
 static __device__ __noinline__ float power_from_sq(float p2, int power_mode, float power) {
   float mag = sqrtf(p2);

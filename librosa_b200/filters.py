@@ -1,7 +1,8 @@
 """Window and filter-bank construction (host side, float64) — mirror of the hot-path parts of
 librosa/filters.py: ``mel`` (:117-251), ``get_window`` (:915-977), ``window_sumsquare`` (:1268-1339), and the
 constant-Q wavelet basis: ``wavelet_lengths`` (:424-552), ``_relative_bandwidth`` (:555-585), ``wavelet``
-(:589-733), ``window_bandwidth`` (:865-912).
+(:589-733), ``window_bandwidth`` (:865-912), and the multirate semitone filter bank of ``iirt``:
+``mr_frequencies`` (:1075-1117) and ``semitone_filterbank`` (:1120-1230).
 
 These constants are tiny and parity-critical, so they are computed on the host with the same float64
 expressions as the reference and uploaded once per plan; the GPU only *applies* them.
@@ -217,3 +218,42 @@ def cq_to_chroma(n_input: int, *, bins_per_octave: int = 12, n_chroma: int = 12,
     if window is not None:
         cq_to_ch = scipy.signal.convolve(cq_to_ch, np.atleast_2d(window), mode="same")
     return cq_to_ch
+
+
+def _multirate_fb(center_freqs=None, sample_rates=None, Q: float = 25.0, passband_ripple: float = 1,
+                  stopband_attenuation: float = 50, ftype: str = "ellip", flayout: str = "sos"):
+    """One ``scipy.signal.iirdesign`` band-pass per centre frequency (librosa/filters.py:981-1072): passband centre
+    +- bw/2, stopband centre +- bw, bw = centre / Q, edges relative to each band's Nyquist rate."""
+    if center_freqs is None:
+        raise ParameterError("center_freqs must be provided.")
+    if sample_rates is None:
+        raise ParameterError("sample_rates must be provided.")
+    if center_freqs.shape != sample_rates.shape:
+        raise ParameterError("Number of provided center_freqs and sample_rates must be equal.")
+    nyquist = 0.5 * sample_rates
+    bandwidths = center_freqs / float(Q)
+    bank = []
+    for f0, nyq, bw in zip(center_freqs, nyquist, bandwidths, strict=True):
+        wp = [f0 - 0.5 * bw, f0 + 0.5 * bw] / nyq
+        ws = [f0 - bw, f0 + bw] / nyq
+        bank.append(scipy.signal.iirdesign(wp, ws, passband_ripple, stopband_attenuation, analog=False, ftype=ftype,
+                                           output=flayout))
+    return bank, sample_rates
+
+
+def mr_frequencies(tuning: float):
+    """Centre frequencies of MIDI pitches 24 .. 108 (shifted by ``tuning`` semitones) and the rate each band runs at:
+    36 at 882 Hz, 34 at 4 410 Hz, 15 at 22 050 Hz (librosa/filters.py:1075-1117)."""
+    notes = np.arange(24 + tuning, 109 + tuning)
+    center_freqs = 440.0 * (2.0 ** ((np.asanyarray(notes)[()] - 69.0) / 12.0))
+    sample_rates = np.asarray(36 * [882.0] + 34 * [4410.0] + 15 * [22050.0])
+    return center_freqs, sample_rates
+
+
+def semitone_filterbank(*, center_freqs=None, tuning: float = 0.0, sample_rates=None, flayout: str = "ba", **kwargs):
+    """Multirate IIR band-pass filter bank (librosa/filters.py:1120-1230): ``mr_frequencies(tuning)`` unless
+    centre frequencies or rates are given; ``kwargs`` (Q, passband_ripple, stopband_attenuation, ftype) go to the
+    design.  Returns (one filter per band in ``flayout``, the rate of each band)."""
+    if center_freqs is None and sample_rates is None:
+        center_freqs, sample_rates = mr_frequencies(tuning)
+    return _multirate_fb(center_freqs=center_freqs, sample_rates=sample_rates, flayout=flayout, **kwargs)

@@ -5,8 +5,8 @@ and leaves the other fixtures as they are; ``--rhythm`` likewise writes only tes
 (tests/rhythm_cases.py), ``--beat`` only tests/golden/beat_v1.npz (tests/beat_cases.py), ``--onset`` only
 tests/golden/onset_v1.npz (tests/onset_cases.py), ``--sequence`` only tests/golden/sequence_v1.npz
 (tests/sequence_cases.py), ``--alignment`` only tests/golden/alignment_v1.npz (tests/alignment_cases.py),
-``--cqt`` only tests/golden/cqt_v1.npz (tests/cqt_cases.py), and ``--chroma`` only tests/golden/chroma_v1.npz
-(tests/chroma_cases.py).
+``--cqt`` only tests/golden/cqt_v1.npz (tests/cqt_cases.py), ``--chroma`` only tests/golden/chroma_v1.npz
+(tests/chroma_cases.py), and ``--iirt`` only tests/golden/iirt_v1.npz (tests/iirt_cases.py).
 
 Needs a checkout of the reference (see tools/ref_shim.py); the tests only read the stored fixtures.  Also
 stores a handful of constant tables (mel bases, window sum-square, mel-scale known answers) produced by the
@@ -21,6 +21,7 @@ reference.
     python tools/make_golden.py --alignment
     python tools/make_golden.py --cqt
     python tools/make_golden.py --chroma
+    python tools/make_golden.py --iirt
 """
 from __future__ import annotations
 
@@ -443,6 +444,66 @@ def write_chroma():
     print("wrote", path, os.path.getsize(path), "bytes")
 
 
+def write_iirt():
+    """tests/golden/iirt_v1.npz: per case of tests/iirt_cases.py, the reference's result (or ``<name>/error``); for
+    WITH_STEPS, what its resample returned for each rate other than sr and what its sosfiltfilt returned for one
+    band, recorded by wrapping the two functions only while the case runs."""
+    import importlib
+
+    import scipy.signal
+
+    import iirt_cases as IC
+
+    ref = ref_shim.load_reference()
+    spectrum = importlib.import_module("librosa.core.spectrum")
+    resample, sosfiltfilt = spectrum.resample, scipy.signal.sosfiltfilt
+    store = {}
+    for case in IC.CASES:
+        name = case["name"]
+        if case["refuse"]:   # only the refusal is checked
+            continue
+        seen = {"y": {}, "bands": []}
+
+        def rec_resample(y, *, orig_sr, target_sr, **kw):
+            out = resample(y, orig_sr=orig_sr, target_sr=target_sr, **kw)
+            if target_sr != orig_sr:
+                seen["y"][float(target_sr)] = out
+            return out
+
+        def rec_sosfiltfilt(sos, x, *a, **kw):
+            out = sosfiltfilt(sos, x, *a, **kw)
+            seen["bands"].append(out)
+            return out
+
+        spectrum.resample, scipy.signal.sosfiltfilt = rec_resample, rec_sosfiltfilt
+        try:
+            with warnings.catch_warnings():
+                warnings.simplefilter("ignore")
+                store[f"{name}/S"] = IC.call(ref, case)
+        except Exception as e:   # the reference's own error, stored as "Class: message"
+            store[f"{name}/error"] = np.array(f"{type(e).__name__}: {e}")
+        finally:
+            spectrum.resample, scipy.signal.sosfiltfilt = resample, sosfiltfilt
+        if name in IC.WITH_STEPS and f"{name}/S" in store:
+            for rate, y in seen["y"].items():
+                store[f"{name}/y{rate:g}"] = y
+            b = IC.WITH_STEPS[name]
+            store[f"{name}/band{b}"] = seen["bands"][b]
+        print(f"{name:32s} {store.get(f'{name}/error', np.shape(store.get(f'{name}/S')))}")
+    for cfg, kw in IC.BANKS.items():   # the designed filter banks: sections stacked, sections per band, rates
+        sos, srs = ref.filters.semitone_filterbank(flayout="sos", **kw)
+        store[f"bank/{cfg}/sos"] = np.concatenate(sos)
+        store[f"bank/{cfg}/sections"] = np.array([len(s) for s in sos])
+        store[f"bank/{cfg}/rates"] = srs
+    ba, _ = ref.filters.semitone_filterbank(flayout="ba")
+    store["bank/defaults/b"] = np.stack([b for b, _ in ba])
+    store["bank/defaults/a"] = np.stack([a for _, a in ba])
+    store["mr_frequencies/0.3"] = np.stack(ref.filters.mr_frequencies(0.3))
+    path = os.path.join(ROOT, "tests", "golden", "iirt_v1.npz")
+    np.savez_compressed(path, **store)
+    print("wrote", path, os.path.getsize(path), "bytes")
+
+
 if __name__ == "__main__":
     if "--pitch" in sys.argv[1:]:
         write_pitch()
@@ -460,5 +521,7 @@ if __name__ == "__main__":
         write_cqt()
     elif "--chroma" in sys.argv[1:]:
         write_chroma()
+    elif "--iirt" in sys.argv[1:]:
+        write_iirt()
     else:
         main()
