@@ -871,15 +871,25 @@ extern "C" int b2l_pcen(b2l_ctx* c, const b2l_pcen_desc* d, const float* d_S, in
   if (!(d->b >= 0.0f && d->b <= 1.0f)) return fail(B2L_ERR_INVALID, "b=%g must be between 0 and 1", d->b);
   if (d->max_size < 1) return fail(B2L_ERR_INVALID, "max_size=%d must be a positive integer", d->max_size);
   if (n_clips <= 0 || n_rows <= 0 || n_frames <= 0) return B2L_OK;
-  if (n_frames > 0x7fffffffLL || n_rows > kMaxGridY || n_clips > kMaxGridY)
+  const long long rows = (long long)n_clips * n_rows;
+  if (n_frames > 0x7fffffffLL || n_rows > 0x7fffffffLL || (rows + 127) / 128 > 0x7fffffffLL)
     return fail(B2L_ERR_UNSUPPORTED, "pcen: batch too large");
   DeviceGuard g(c->device);
   const float* ref = d_S;
   if (d->max_size > 1) {
     if (!d_scratch) return fail(B2L_ERR_INVALID, "max_size > 1 needs a scratch buffer of the size of S");
-    const dim3 grid((unsigned)((n_frames + 127) / 128), (unsigned)n_rows, (unsigned)n_clips);
-    if (int rc = launch(c, maxfilter_rows_kernel, grid, 128, 0, d_S, (int)n_rows, (int)n_frames, d->max_size, d_scratch))
-      return rc;
+    // rows on grid.y and clips on grid.z: slices of at most 65 535 of each
+    const int rc = for_clip_slices(n_clips, [&](int64_t c0, int64_t m) {
+      const size_t off = (size_t)c0 * (size_t)n_rows * (size_t)n_frames;
+      for (int64_t r0 = 0; r0 < n_rows; r0 += kMaxGridY) {
+        const dim3 grid((unsigned)((n_frames + 127) / 128), (unsigned)std::min(kMaxGridY, n_rows - r0), (unsigned)m);
+        if (int rc = launch(c, maxfilter_rows_kernel, grid, 128, 0, d_S + off, (int)n_rows, (int)n_frames, d->max_size,
+                            (int)r0, d_scratch + off))
+          return rc;
+      }
+      return (int)B2L_OK;
+    });
+    if (rc) return rc;
     ref = d_scratch;
   }
   PcenArgs a;
@@ -889,7 +899,6 @@ extern "C" int b2l_pcen(b2l_ctx* c, const b2l_pcen_desc* d, const float* d_S, in
   a.eps = d->eps;
   a.b = d->b;
   a.mode = d->power == 0.0f ? 0 : (d->bias == 0.0f ? 1 : 2);
-  const long long rows = (long long)n_clips * n_rows;
   return launch(c, pcen_kernel, (unsigned)((rows + 127) / 128), 128, 0, d_S, ref, rows, (int)n_frames, a, d_zi, d_zf,
                 d_out);
 }
@@ -1006,8 +1015,7 @@ extern "C" int b2l_hpss(b2l_ctx* c, const b2l_hpss_desc* d, const float* d_mag, 
     return fail(B2L_ERR_INVALID, "Margins must be >= 1.0. A typical range is between 1 and 10.");
   if (!(d->power > 0.0f)) return fail(B2L_ERR_INVALID, "power must be strictly positive");
   if (n_clips <= 0 || n_frames <= 0 || n_bins <= 0) return B2L_OK;
-  if (n_frames > kMaxGridY || n_clips > kMaxGridY || n_bins > 0x7fffffffLL)
-    return fail(B2L_ERR_UNSUPPORTED, "hpss: batch too large");
+  if (n_frames > 0x7fffffffLL || n_bins > 0x7fffffffLL) return fail(B2L_ERR_UNSUPPORTED, "hpss: batch too large");
   HpssArgs a;
   a.T = (int)n_frames;
   a.F = (int)n_bins;
@@ -1021,9 +1029,21 @@ extern "C" int b2l_hpss(b2l_ctx* c, const b2l_hpss_desc* d, const float* d_mag, 
   DeviceGuard g(c->device);
   const int w = std::max(d->win_harm, d->win_perc);
   auto kern = w <= 8 ? hpss_kernel<8> : w <= 16 ? hpss_kernel<16> : w <= 32 ? hpss_kernel<32> : hpss_kernel<64>;
-  const dim3 grid((unsigned)((n_bins + 127) / 128), (unsigned)n_frames, (unsigned)n_clips);
   const float2* sc = d->mask_only ? nullptr : (const float2*)d_S_complex;
-  return launch(c, kern, grid, 128, 0, d_mag, sc, a, (float*)d_out_harm, (float*)d_out_perc);
+  // complex masked components are float2 elements, masks and real components float
+  const size_t out_words = sc ? 2 : 1;
+  // frames on grid.y and clips on grid.z: slices of at most 65 535 of each, the frame slice passed as a.t0
+  return for_clip_slices(n_clips, [&](int64_t c0, int64_t m) {
+    const size_t off = (size_t)c0 * (size_t)n_frames * (size_t)n_bins;
+    for (int64_t t0 = 0; t0 < n_frames; t0 += kMaxGridY) {
+      a.t0 = (int)t0;
+      const dim3 grid((unsigned)((n_bins + 127) / 128), (unsigned)std::min(kMaxGridY, n_frames - t0), (unsigned)m);
+      if (int rc = launch(c, kern, grid, 128, 0, d_mag + off, sc ? sc + off : nullptr, a,
+                          (float*)d_out_harm + out_words * off, (float*)d_out_perc + out_words * off))
+        return rc;
+    }
+    return (int)B2L_OK;
+  });
 }
 
 extern "C" int b2l_reassign(b2l_ctx* c, const b2l_reassign_desc* d, const void* d_Sh, const void* d_Sdh,

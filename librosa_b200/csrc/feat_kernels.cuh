@@ -379,11 +379,13 @@ __global__ void pcen_kernel(const float* __restrict__ S, const float* __restrict
   }
   if (zf && my_row < n_rows) zf[my_row] = z;
 }
-// scipy.ndimage.maximum_filter1d along the row axis of [clip][rows][T] blocks (reflect boundary)
-__global__ void maxfilter_rows_kernel(const float* __restrict__ S, int rows, int T, int size, float* __restrict__ out) {
+// scipy.ndimage.maximum_filter1d along the row axis of [clip][rows][T] blocks (reflect boundary); grid.y covers
+// rows m0 .. m0 + gridDim.y - 1
+__global__ void maxfilter_rows_kernel(const float* __restrict__ S, int rows, int T, int size, int m0,
+                                      float* __restrict__ out) {
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
   if (t >= T) return;
-  const int m = blockIdx.y;
+  const int m = m0 + blockIdx.y;
   const float* Sc = S + (long long)blockIdx.z * rows * T;
   float v = -INFINITY;
   const int lo = m - size / 2;
@@ -710,11 +712,13 @@ __device__ __forceinline__ int reflect_index(int i, int n) {
   while (i < 0 || i >= n) i = i < 0 ? -i - 1 : 2 * n - i - 1;
   return i;
 }
+// util.softmask: an infinite power is the hard mask X > X_ref everywhere, also where both lie below tiny(float32)
+// (the reference splits or zeroes those cells only for a finite power)
 __device__ __forceinline__ float soft_mask(float x, float x_ref, float power, int split_zeros) {
+  if (isinf(power)) return x > x_ref ? 1.0f : 0.0f;
   float z = fmaxf(x, x_ref);
   const bool bad = z < 1.17549435e-38f;
   if (bad) return split_zeros ? 0.5f : 0.0f;
-  if (isinf(power)) return x > x_ref ? 1.0f : 0.0f;
   const float a = x / z, b = x_ref / z;
   const float pa = power == 2.0f ? a * a : (power == 1.0f ? a : powf(a, power));
   const float pb = power == 2.0f ? b * b : (power == 1.0f ? b : powf(b, power));
@@ -722,6 +726,7 @@ __device__ __forceinline__ float soft_mask(float x, float x_ref, float power, in
 }
 struct HpssArgs {
   int T, F, win_h, win_p;
+  int t0;                    // frame of grid.y == 0 (launches of at most 65 535 frames)
   float margin_h, margin_p, power;
   int split_zeros, mode;     // mode 0: masked components, 1: the masks
 };
@@ -729,7 +734,7 @@ template <int NS>
 __global__ void hpss_kernel(const float* __restrict__ M, const float2* __restrict__ Sc, HpssArgs a,
                             float* __restrict__ out_h, float* __restrict__ out_p) {
   const int f = blockIdx.x * blockDim.x + threadIdx.x;
-  const int t = blockIdx.y;
+  const int t = a.t0 + blockIdx.y;
   if (f >= a.F) return;
   const long long base = (long long)blockIdx.z * a.T * a.F;
   const float* Mc = M + base;

@@ -184,6 +184,26 @@ def spectral_flatness(*, y=None, S=None, n_fft: int = 2048, hop_length: int = 51
                       window=window, center=center, pad_mode=pad_mode)
 
 
+def _contrast_bands(freq, octa, quantile):
+    """The reference's octave-band masks (feature/spectral.py:483-499) reduced to (first bin, bin count, tail
+    length) per band, the three numbers contrast_kernel reads.  ``octa`` holds the n_bands + 2 band edges."""
+    n_bands = len(octa) - 2
+    bands = []
+    for k in range(n_bands + 1):
+        band = np.logical_and(freq >= octa[k], freq <= octa[k + 1])
+        idx = np.flatnonzero(band)
+        if k > 0:
+            band[idx[0] - 1] = True
+        if k == n_bands:
+            band[idx[-1] + 1:] = True
+        sel = np.flatnonzero(band)
+        if sel.size and sel[-1] - sel[0] + 1 != sel.size:
+            raise nat.UnsupportedOnGPU("spectral_contrast: non-contiguous band (freq must be increasing)")
+        count = sel.size - (1 if k < n_bands else 0)
+        bands.append((int(sel[0]) if sel.size else 0, max(int(count), 0), int(max(np.rint(quantile * np.sum(band)), 1))))
+    return bands
+
+
 def spectral_contrast(*, y=None, sr: float = 22050, S=None, n_fft: int = 2048, hop_length: int = 512,
                       win_length: Optional[int] = None, window="hann", center: bool = True, pad_mode="constant",
                       freq=None, fmin: float = 200.0, n_bands: int = 6, quantile: float = 0.02,
@@ -230,21 +250,8 @@ def spectral_contrast(*, y=None, sr: float = 22050, S=None, n_fft: int = 2048, h
     if n_bands + 1 > 16:
         raise nat.UnsupportedOnGPU("spectral_contrast: at most 15 octave bands on the GPU")
     desc = nat.ContrastDesc(n_bands=n_bands + 1)
-    for k in range(n_bands + 1):
-        # the reference's band mask (feature/spectral.py:483-499), reduced to (first bin, count, tail length)
-        band = np.logical_and(freq >= octa[k], freq <= octa[k + 1])
-        idx = np.flatnonzero(band)
-        if k > 0:
-            band[idx[0] - 1] = True
-        if k == n_bands:
-            band[idx[-1] + 1:] = True
-        sel = np.flatnonzero(band)
-        if sel.size and sel[-1] - sel[0] + 1 != sel.size:
-            raise nat.UnsupportedOnGPU("spectral_contrast: non-contiguous band (freq must be increasing)")
-        count = sel.size - (1 if k < n_bands else 0)
-        desc.lo[k] = int(sel[0]) if sel.size else 0
-        desc.count[k] = max(int(count), 0)
-        desc.k[k] = int(max(np.rint(quantile * np.sum(band)), 1))
+    for k, (lo, count, tail) in enumerate(_contrast_bands(freq, octa, quantile)):
+        desc.lo[k], desc.count[k], desc.k[k] = lo, count, tail
     lead = Sd.shape[:-2]
     n_clips = pl.clip_count(lead)
     L = nat.lib()
