@@ -227,8 +227,19 @@ int b2l_resample_poly(b2l_ctx* ctx, const float* d_x, int64_t n_clips, int64_t n
  * (d_indptr holds absolute positions into d_indices / d_data; nnz: the octave's nonzeros) and fills output rows
  * row0 .. row0 + n_rows - 1 of d_out [n_clips][n_frames][n_bins].  Each element is SciPy's `csr @ D` for complex64
  * bit for bit (ascending columns, unfused multiply and add); d_rscale [n_bins] (1 / sqrt(lengths), or NULL when
- * scale=False) multiplies in double with one rounding, as numpy's complex64 /= float64 does.  Sets no status bit. */
+ * scale=False) multiplies in double with one rounding, as numpy's complex64 /= float64 does.  Sets no status bit.
+ *
+ * kind: B2L_CQT_FULL for such an octave.  B2L_CQT_PSEUDO (pseudo_cqt, :474-590) marks an octave whose table holds the
+ * float32 |basis| in the real parts (imaginary parts 0) and whose rows project |D| (np.abs of complex64 as NumPy's
+ * vectorised x86 loop computes it: larger part * sqrtf(fmaf(r, r, 1)), r = smaller / larger): SciPy's float32
+ * `csr @ np.abs(D)` bit for bit.  B2L_CQT_DIVIDE, or'd in, makes the octave's rows divide
+ * by d_rscale in double (one rounding) instead of multiplying.  b2l_cqt_project refuses pseudo octaves
+ * (B2L_ERR_INVALID); b2l_cqt_project_abs takes both kinds and writes float32 into d_out [n_clips][n_frames][n_bins]:
+ * a pseudo row its scaled sum, a full row the np.abs of the complex64 value b2l_cqt_project would store. */
 #define B2L_CQT_MAX_OCTAVES 32
+#define B2L_CQT_FULL 0
+#define B2L_CQT_PSEUDO 1
+#define B2L_CQT_DIVIDE 0x10
 typedef struct b2l_cqt_octave {
   const void* d_D;
   int64_t n_frames;
@@ -237,10 +248,14 @@ typedef struct b2l_cqt_octave {
   int32_t n_rows;
   int32_t indptr_off;
   int32_t nnz;
-} b2l_cqt_octave;
+  int32_t kind;
+} b2l_cqt_octave;   /* 40 bytes */
 int b2l_cqt_project(b2l_ctx* ctx, const b2l_cqt_octave* h_oct, int32_t n_oct, const int32_t* d_indptr,
                     const int32_t* d_indices, const void* d_data, const double* d_rscale, int64_t n_clips,
                     int64_t n_frames, int32_t n_bins, void* d_out);
+int b2l_cqt_project_abs(b2l_ctx* ctx, const b2l_cqt_octave* h_oct, int32_t n_oct, const int32_t* d_indptr,
+                        const int32_t* d_indices, const void* d_data, const double* d_rscale, int64_t n_clips,
+                        int64_t n_frames, int32_t n_bins, float* d_out);
 /* librosa.iirt (core/spectrum.py:1522-1713).  b2l_pad_center: np.pad(y, pad, mode) of each clip of d_x [n_clips][n]
  * into d_out [n_clips][n + 2 pad] (enum b2l_pad_mode; an empty signal takes only "constant" / "empty").
  * b2l_iirt_filter: scipy.signal.sosfiltfilt (padtype "odd", SciPy's default padlen) of every (clip, band) chain,

@@ -187,12 +187,14 @@ class DtwDesc(C.Structure):
 
 
 class CqtOctave(C.Structure):
-    """struct b2l_cqt_octave (include/b2l.h): one octave of b2l_cqt_project; d_D is a device pointer."""
+    """struct b2l_cqt_octave (include/b2l.h): one octave of b2l_cqt_project / b2l_cqt_project_abs; d_D is a device
+    pointer."""
     _fields_ = [("d_D", C.c_void_p), ("n_frames", C.c_int64), ("n_fft_bins", C.c_int32), ("row0", C.c_int32),
-                ("n_rows", C.c_int32), ("indptr_off", C.c_int32), ("nnz", C.c_int32)]
+                ("n_rows", C.c_int32), ("indptr_off", C.c_int32), ("nnz", C.c_int32), ("kind", C.c_int32)]
 
 
 CQT_MAX_OCTAVES = 32   # B2L_CQT_MAX_OCTAVES
+CQT_FULL, CQT_PSEUDO, CQT_DIVIDE = 0, 1, 0x10   # B2L_CQT_FULL / B2L_CQT_PSEUDO / B2L_CQT_DIVIDE
 
 
 class IirtRate(C.Structure):
@@ -324,6 +326,8 @@ def _declare(lib):
         "b2l_rqa": (C.c_int, [_vp, _vp, _i64, _i64, C.c_int32, C.c_double, C.c_double, C.c_int32, _vp, _vp]),
         "b2l_rqa_path": (C.c_int, [_vp, _vp, _vp, _i64, _i64, C.c_int32, _vp, _vp]),
         "b2l_cqt_project": (C.c_int, [_vp, P(CqtOctave), C.c_int32, _vp, _vp, _vp, _vp, _i64, _i64, C.c_int32, _vp]),
+        "b2l_cqt_project_abs": (C.c_int, [_vp, P(CqtOctave), C.c_int32, _vp, _vp, _vp, _vp, _i64, _i64, C.c_int32,
+                                          _vp]),
         "b2l_pad_center": (C.c_int, [_vp, _vp, _i64, _i64, C.c_int32, C.c_int32, _vp]),
         "b2l_iirt_filter": (C.c_int, [_vp, P(IirtRate), C.c_int32, _vp, _vp, C.c_int32, _i64]),
         "b2l_iirt_stmsp": (C.c_int, [_vp, P(IirtRate), C.c_int32, _i64, _i64, C.c_int32, _vp]),

@@ -1,11 +1,16 @@
-"""``cqt`` / ``vqt`` with librosa's signatures, executed by libb2l.so on an H100 (reference:
-librosa/core/constantq.py:620-1266).
+"""``cqt`` / ``vqt`` / ``pseudo_cqt`` / ``hybrid_cqt`` with librosa's signatures, executed by libb2l.so on an H100
+(reference: librosa/core/constantq.py:209-590, 620-1266).
 
 The octave pyramid runs on the device with one staging of the input and no host round trip: an optional early
 downsample by 2^k (polyphase resampler), then per octave, from the top down, a centred STFT with a rectangular
 window into frame-major scratch and a halving of the signal for the next octave.  One launch of
 ``b2l_cqt_project`` then applies every octave's sparse complex filter basis and writes the stacked result.  The
 filter bases, frequencies and lengths are host constants built with the reference's float64 expressions.
+
+``pseudo_cqt`` is one centred Hann STFT at a single n_fft whose magnitudes meet the magnitudes of one filter basis;
+``hybrid_cqt`` stacks such a pseudo part (the high bins, whose filters fit in two hops) on top of ``np.abs`` of a
+``cqt`` of the remaining low bins.  Both run as the same staged pass: the pseudo part's STFT, the full part's
+pyramid, and one launch of ``b2l_cqt_project_abs`` writing every row as float32 magnitudes (DESIGN §4.19).
 """
 from __future__ import annotations
 
@@ -20,10 +25,10 @@ from .. import _native as nat
 from .. import _pipeline as pl
 from .. import filters
 from ..util.exceptions import ParameterError
-from ..util.utils import dtype_r2c
+from ..util.utils import dtype_c2r, dtype_r2c
 from .audio import _poly_filter
 
-__all__ = ["cqt", "vqt", "cqt_frequencies"]
+__all__ = ["cqt", "vqt", "pseudo_cqt", "hybrid_cqt", "cqt_frequencies"]
 
 _vp = C.c_void_p
 
@@ -69,6 +74,12 @@ def _clip_freqs(freqs, window, filter_scale, gamma, sr) -> np.ndarray:
     return freqs[:idx]
 
 
+def _et_relative_bw(bins_per_octave: int) -> np.ndarray:
+    """The relative bandwidth of one bin of an equal-tempered scale (librosa/core/constantq.py:1577-1598)."""
+    r = 2 ** (1 / bins_per_octave)
+    return np.atleast_1d((r ** 2 - 1) / (r ** 2 + 1))
+
+
 def _two_factors(x: int) -> int:
     n = 0
     while x > 0 and x % 2 == 0:
@@ -98,17 +109,26 @@ def _sparsify(x: np.ndarray, quantile: float, dtype) -> np.ndarray:
     return (x * (mags >= thresh[:, np.newaxis])).astype(dtype, copy=False)
 
 
-def filter_basis(sr, freqs, alpha, filter_scale, norm, sparsity, window, gamma, rescale) -> Basis:
+def _pseudo_n_fft(lengths, hop_length: int) -> int:
+    """pseudo_cqt's transform size: the longest filter's power of two, at least two hops (constantq.py:1144-1145)."""
+    return max(int(2.0 ** (np.ceil(np.log2(np.max(lengths))))), int(2.0 ** (1 + np.ceil(np.log2(hop_length)))))
+
+
+def filter_basis(sr, freqs, alpha, filter_scale, norm, sparsity, window, gamma, rescale, hop_length=None) -> Basis:
     """The FFT of one octave's wavelets at rate ``sr``, rescaled by ``lengths / n_fft``, non-negative bins only,
-    sparsified and multiplied by ``rescale`` (sqrt of the top rate over this octave's rate) (librosa/core/constantq.py:1067-1080, 1123-1166)."""
+    sparsified and multiplied by ``rescale`` (sqrt of the top rate over this octave's rate) (librosa/core/constantq.py:1067-1080, 1123-1166).
+
+    With ``hop_length`` (pseudo_cqt): n_fft covers at least two hops, and the table holds ``np.abs`` of the sparse
+    basis (float32 magnitudes in the real parts)."""
     basis, lengths = filters.wavelet(freqs=freqs, sr=sr, filter_scale=filter_scale, norm=norm, pad_fft=True,
                                      window=window, gamma=gamma, alpha=alpha)
-    n_fft = basis.shape[1]
+    n_fft = basis.shape[1] if hop_length is None else _pseudo_n_fft(lengths, hop_length)
     basis *= lengths[:, np.newaxis] / float(n_fft)
     fft_basis = scipy.fft.fft(basis, n=n_fft, axis=1)[:, : (n_fft // 2) + 1]
     dense = _sparsify(fft_basis, sparsity, np.complex64)
     rows, cols = np.nonzero(dense)
-    data = (dense[rows, cols] * np.float64(rescale)).astype(np.complex64)
+    data = dense[rows, cols]
+    data = (np.abs(data) if hop_length is not None else data * np.float64(rescale)).astype(np.complex64)
     indptr = np.zeros(dense.shape[0] + 1, dtype=np.int32)
     np.cumsum(np.bincount(rows, minlength=dense.shape[0]), out=indptr[1:])
     return Basis(indptr, cols.astype(np.int32), data, int(n_fft))
@@ -150,11 +170,7 @@ def plan(n: int, *, sr, hop_length, fmin, n_bins, intervals, gamma, bins_per_oct
     if auto_n_bins:
         freqs = _clip_freqs(freqs, window, filter_scale, gamma, sr)
         n_bins = len(freqs)
-    if n_bins == 1:
-        r = 2 ** (1 / bins_per_octave)
-        alpha = np.atleast_1d((r ** 2 - 1) / (r ** 2 + 1))
-    else:
-        alpha = filters._relative_bandwidth(freqs=freqs)
+    alpha = _et_relative_bw(bins_per_octave) if n_bins == 1 else filters._relative_bandwidth(freqs=freqs)
     lengths, filter_cutoff = filters.wavelet_lengths(freqs=freqs, sr=sr, window=window, filter_scale=filter_scale,
                                                      gamma=gamma, alpha=alpha)
     nyquist = sr / 2.0
@@ -238,6 +254,110 @@ def _resample_half(ctx, d_x, n_clips: int, n: int, down: int, out_scale: float, 
                                           n_out, n_out, out_scale, _vp(d_out)))
 
 
+class PseudoPlan(NamedTuple):
+    sr: float
+    freqs: np.ndarray
+    alpha: np.ndarray
+    lengths: np.ndarray
+    n_bins: int
+    n_fft: int
+    hop: int
+    n_frames: int
+
+
+def _equal_bins(*, sr, fmin, n_bins, bins_per_octave, filter_scale, window):
+    """pseudo_cqt's and hybrid_cqt's (freqs, alpha, lengths) for a resolved ``fmin``, with the reference's checks in
+    its order (librosa/core/constantq.py:318-358, 519-555)."""
+    if fmin >= sr / 2:
+        raise ParameterError(f"fmin={fmin} must be less than sr/2={sr/2}")
+    auto_n_bins = n_bins is None
+    if auto_n_bins:
+        n_bins = int(np.ceil(bins_per_octave * (np.log2(sr) - np.log2(fmin))))
+    freqs = cqt_frequencies(n_bins, fmin=fmin, bins_per_octave=bins_per_octave)
+    if auto_n_bins:
+        freqs = _clip_freqs(freqs, window, filter_scale, 0, sr)
+        n_bins = len(freqs)
+    alpha = _et_relative_bw(bins_per_octave) if n_bins == 1 else filters._relative_bandwidth(freqs=freqs)
+    lengths, filter_cutoff = filters.wavelet_lengths(freqs=freqs, sr=sr, window=window, filter_scale=filter_scale,
+                                                     alpha=alpha)
+    if filter_cutoff > sr / 2:
+        raise ParameterError(f"Filter cutoff frequency {filter_cutoff} exceeds Nyquist frequency {sr/2}. "
+                             "Try reducing the number of frequency bins.")
+    return freqs, alpha, lengths
+
+
+def pseudo_plan(n: int, *, sr, hop_length, fmin, n_bins, bins_per_octave, filter_scale, window) -> PseudoPlan:
+    """The host half of pseudo_cqt (librosa/core/constantq.py:519-590) for a signal of ``n`` samples and a resolved
+    ``fmin``: its checks, its bins and its single n_fft."""
+    freqs, alpha, lengths = _equal_bins(sr=sr, fmin=fmin, n_bins=n_bins, bins_per_octave=bins_per_octave,
+                                        filter_scale=filter_scale, window=window)
+    return PseudoPlan(sr, freqs, alpha, lengths, len(freqs), _pseudo_n_fft(lengths, hop_length), hop_length,
+                      1 + n // hop_length)
+
+
+def hybrid_split(lengths, hop_length: int) -> np.ndarray:
+    """hybrid_cqt's pseudo bins: those whose filter, padded to a power of two, is shorter than two hops
+    (librosa/core/constantq.py:360-366)."""
+    return 2.0 ** np.ceil(np.log2(lengths)) < 2 * hop_length
+
+
+def _check_pseudo_stft(pp: PseudoPlan, n: int, pad_mode):
+    """The pseudo part's stft checks (its "n_fft=... is too large" warning) and the GPU's limit on its n_fft."""
+    pl.check_stft_geometry(n, pp.n_fft, True, pad_mode)
+    if pp.n_fft > pl.MAX_N_FFT:
+        raise nat.UnsupportedOnGPU(f"pseudo_cqt: n_fft={pp.n_fft} (the longest filter of fmin={pp.freqs[0]:.2f} Hz, "
+                                   f"or two hops); the float32 STFT kernels stop at n_fft={pl.MAX_N_FFT}: raise fmin "
+                                   "or lower the hop")
+    pl.require_supported_n_fft(pp.n_fft)
+
+
+def _check_full_stft(p: Plan, pad_mode):
+    for o in p.octaves:
+        pl.check_stft_geometry(o.n, o.n_fft, True, pad_mode)
+        pl.require_supported_n_fft(o.n_fft)
+
+
+def _staged(y, *, what, real, sr, bins_per_octave, tuning, dtype, prepare, **kw):
+    """What every constant-Q entry point does around the device pass: the signal's checks, ``tuning``
+    (estimate_tuning on the staged signal when None), ``prepare(n, tuning) -> (full Plan or None, PseudoPlan or
+    None)`` with the reference's checks, then ``_run``; with a given tuning nothing touches the device before
+    ``prepare`` has passed.  The stft's "n_fft=... is too large" warnings are held back until the finite
+    verdict, because the reference's stft raises on non-finite audio before it warns.  ``real``: float32
+    magnitudes (the reference's real dtype of ``dtype``), else complex64."""
+    n, req = pl.precheck_signal(y, stacklevel=5)
+    on_device = isinstance(y, nat.DeviceArray)
+    out_dtype = np.dtype(dtype) if dtype is not None else dtype_r2c(req)
+    if real:
+        out_dtype = np.dtype(dtype_c2r(out_dtype))
+    dev_dtype = np.dtype(np.float32 if real else np.complex64)
+    if on_device and out_dtype != dev_dtype:
+        raise nat.UnsupportedOnGPU(f"{what} dtype={out_dtype}: device results are {dev_dtype}")
+    staged = None
+    try:
+        if tuning is None:
+            from .pitch import estimate_tuning
+
+            staged = pl.StagedInput(y)
+            tuning = estimate_tuning(y=staged.dev, sr=sr, bins_per_octave=bins_per_octave)
+        with warnings.catch_warnings(record=True) as held:
+            warnings.simplefilter("always")
+            full, pseudo = prepare(n, tuning)
+        n_oct = (len(full.octaves) if full else 0) + (1 if pseudo else 0)
+        if n_oct > nat.CQT_MAX_OCTAVES:
+            raise nat.UnsupportedOnGPU(f"{what}: {n_oct} octaves; the GPU projection takes at most "
+                                       f"{nat.CQT_MAX_OCTAVES}")
+        if staged is None:
+            staged = pl.StagedInput(y)
+        out = _run(staged, full, pseudo, mag=real, **kw)
+    finally:
+        if staged is not None:
+            staged.release()
+    res = staged.result(out, out_dtype)
+    for w in held:
+        warnings.warn(w.message, w.category, stacklevel=3)
+    return res
+
+
 def vqt(y, *, sr: float = 22050, hop_length: int = 512, fmin: Optional[float] = None, n_bins: Optional[int] = 84,
         intervals="equal", gamma: Optional[float] = None, bins_per_octave: int = 12, tuning: Optional[float] = 0.0,
         filter_scale: float = 1, norm: Optional[float] = 1, sparsity: float = 0.01, window="hann",
@@ -251,101 +371,131 @@ def vqt(y, *, sr: float = 22050, hop_length: int = 512, fmin: Optional[float] = 
         bins_per_octave = len(intervals)
     if fmin is None:
         fmin = _default_fmin()
-    n, req = pl.precheck_signal(y)
-    on_device = isinstance(y, nat.DeviceArray)
-    out_dtype = np.dtype(dtype) if dtype is not None else dtype_r2c(req)
-    if on_device and out_dtype != np.complex64:
-        raise nat.UnsupportedOnGPU(f"cqt/vqt dtype={out_dtype}: device results are complex64")
-    staged = pl.StagedInput(y)
-    try:
-        if tuning is None:
-            from .pitch import estimate_tuning
 
-            tuning = estimate_tuning(y=staged.dev, sr=sr, bins_per_octave=bins_per_octave)
-        fmin = fmin * 2.0 ** (tuning / bins_per_octave)
-        p = plan(n, sr=sr, hop_length=hop_length, fmin=fmin, n_bins=n_bins, intervals=intervals, gamma=gamma,
-                 bins_per_octave=bins_per_octave, filter_scale=filter_scale, window=window, scale=scale,
-                 res_type=res_type)
-        # stft's "n_fft=... is too large" warning, once per octave: held back until the finite verdict, because the
-        # reference's stft raises on non-finite audio before it warns
-        with warnings.catch_warnings(record=True) as held:
-            warnings.simplefilter("always")
-            for o in p.octaves:
-                pl.check_stft_geometry(o.n, o.n_fft, True, pad_mode)
-                pl.require_supported_n_fft(o.n_fft)
-        if len(p.octaves) > nat.CQT_MAX_OCTAVES:
-            raise nat.UnsupportedOnGPU(f"cqt/vqt: {len(p.octaves)} octaves; the GPU projection takes at most "
-                                       f"{nat.CQT_MAX_OCTAVES}")
-        out = _run(staged, p, filter_scale=filter_scale, norm=norm, sparsity=sparsity, window=window, gamma=gamma,
-                   scale=scale, pad_mode=pad_mode)
-    finally:
-        staged.release()
-    res = staged.result(out, out_dtype)
-    for w in held:
-        warnings.warn(w.message, w.category, stacklevel=2)
-    return res
+    def prepare(n, tuning):
+        p = plan(n, sr=sr, hop_length=hop_length, fmin=fmin * 2.0 ** (tuning / bins_per_octave), n_bins=n_bins,
+                 intervals=intervals, gamma=gamma, bins_per_octave=bins_per_octave, filter_scale=filter_scale,
+                 window=window, scale=scale, res_type=res_type)
+        _check_full_stft(p, pad_mode)
+        return p, None
+
+    return _staged(y, what="cqt/vqt", real=False, sr=sr, bins_per_octave=bins_per_octave, tuning=tuning, dtype=dtype,
+                   prepare=prepare, filter_scale=filter_scale, norm=norm, sparsity=sparsity, window=window,
+                   gamma=gamma, scale=scale, pad_mode=pad_mode)
 
 
-def _run(staged, p: Plan, *, filter_scale, norm, sparsity, window, gamma, scale, pad_mode):
-    """Enqueue the octave pyramid and the projection for a staged signal; returns the (..., n_bins, T) "ft" result."""
+def _run(staged, full: Optional[Plan], pseudo: Optional[PseudoPlan], *, mag, filter_scale, norm, sparsity, window,
+         gamma, scale, pad_mode):
+    """Enqueue one pass for a staged signal: the pseudo part's centred Hann STFT, the full part's octave pyramid,
+    then one projection launch writing every row; the pseudo part's rows are the top (highest) bins, after the
+    full part's.  Returns the (..., n_bins, T) "ft"
+    result: complex64 (b2l_cqt_project), or float32 magnitudes with ``mag`` (b2l_cqt_project_abs)."""
     ctx, m = staged.ctx, staged.n_clips
-    key, bs = _bases_cached(p, filter_scale=filter_scale, norm=norm, sparsity=sparsity, window=window, gamma=gamma)
-    rows = octave_rows(p)
+    n_low = full.n_bins if full is not None else 0
+    parts, keys, rscale = [], [], []   # parts: (basis, output row0, rows kept, first kept row, kind)
+    if pseudo is not None:
+        key, b = _pseudo_basis_cached(pseudo, filter_scale=filter_scale, norm=norm, sparsity=sparsity, window=window)
+        keys.append(key)
+        parts.append((b, n_low, pseudo.n_bins, 0, nat.CQT_PSEUDO | (nat.CQT_DIVIDE if scale else 0)))
+        # pseudo_cqt's C /= np.sqrt(n_fft) or C *= np.sqrt(lengths / n_fft), each in float64 with one rounding
+        rscale.append(np.full(pseudo.n_bins, np.sqrt(pseudo.n_fft)) if scale else np.sqrt(pseudo.lengths / pseudo.n_fft))
+    if full is not None:
+        key, bs = _bases_cached(full, filter_scale=filter_scale, norm=norm, sparsity=sparsity, window=window,
+                                gamma=gamma)
+        keys.append(key)
+        parts += [(b, row0, keep, first, nat.CQT_FULL) for b, (row0, keep, first) in zip(bs, octave_rows(full))]
+        rscale.insert(0, 1.0 / np.sqrt(full.lengths) if scale else np.ones(full.n_bins))
+    n_bins = n_low + (pseudo.n_bins if pseudo is not None else 0)
+    T = min(x.n_frames for x in (full, pseudo) if x is not None)
     indptr, nnz_off, ip_off, descs = [], 0, 0, []
-    for b, (row0, keep, first) in zip(bs, rows):
+    for b, row0, keep, first, kind in parts:
         indptr.append(b.indptr + nnz_off)
-        descs.append((row0, keep, ip_off + first, int(b.indptr[first + keep] - b.indptr[first])))
+        descs.append((row0, keep, ip_off + first, int(b.indptr[first + keep] - b.indptr[first]), kind))
         ip_off += len(b.indptr)
         nnz_off += len(b.data)
+    key = tuple(keys)
     d_indptr = _table(ctx, ("cqt_indptr",) + key, np.concatenate(indptr).astype(np.int32))
-    d_indices = _table(ctx, ("cqt_indices",) + key, np.concatenate([b.indices for b in bs]).astype(np.int32))
-    d_data = _table(ctx, ("cqt_data",) + key, np.concatenate([b.data for b in bs]).astype(np.complex64))
-    d_rscale = _table(ctx, ("cqt_rscale", p.lengths.tobytes()), 1.0 / np.sqrt(p.lengths)) if scale else 0
+    d_indices = _table(ctx, ("cqt_indices",) + key, np.concatenate([p[0].indices for p in parts]).astype(np.int32))
+    d_data = _table(ctx, ("cqt_data",) + key, np.concatenate([p[0].data for p in parts]).astype(np.complex64))
+    rs = np.concatenate(rscale)
+    scaled = scale or pseudo is not None   # unscaled full rows multiply by 1.0: exact
+    d_rscale = _table(ctx, ("cqt_rscale", rs.tobytes()), rs) if scaled else 0
+    octs = (nat.CqtOctave * len(parts))()
     with pl.Scope(staged.dev) as sc:
         staged.scan_all()
-        cur, n_cur = staged.dev.ptr, staged.n
-        if p.early > 1:
-            d = sc.empty((m, -(-n_cur // p.early)), np.float32)
-            _resample_half(ctx, cur, m, n_cur, p.early, p.early_scale, d.ptr)
-            cur, n_cur = d.ptr, d.shape[-1]
-        octs = (nat.CqtOctave * len(p.octaves))()
-        for i, (o, b) in enumerate(zip(p.octaves, bs)):
-            assert n_cur == o.n
-            F = o.n_fft // 2 + 1
-            D = sc.empty((m, o.n_frames, F), np.complex64)
-            plan_ = nat.make_plan(ctx, ("stft", o.n_fft, o.hop, True, pad_mode, "ones"), n_fft=o.n_fft,
-                                  hop_length=o.hop, center=True, pad_mode=pad_mode, window=np.ones(o.n_fft))
-            nat.check(nat.lib().b2l_stft(ctx.handle, plan_.handle, _vp(cur), m, n_cur, n_cur, _vp(D.ptr)))
-            row0, keep, ip, nnz = descs[i]
-            octs[i] = nat.CqtOctave(D.ptr, o.n_frames, F, row0, keep, ip, nnz)
-            if o.resample_after:
-                d = sc.empty((m, -(-n_cur // 2)), np.float32)
-                _resample_half(ctx, cur, m, n_cur, 2, float(np.sqrt(2.0)), d.ptr)
+        i = 0
+        if pseudo is not None:
+            F = pseudo.n_fft // 2 + 1
+            D = sc.empty((m, pseudo.n_frames, F), np.complex64)
+            win, wkey = pl.resolve_window("hann", pseudo.n_fft, pseudo.n_fft)
+            plan_ = nat.make_plan(ctx, ("stft", pseudo.n_fft, pseudo.hop, True, pad_mode, wkey), n_fft=pseudo.n_fft,
+                                  hop_length=pseudo.hop, center=True, pad_mode=pad_mode, window=win)
+            nat.check(nat.lib().b2l_stft(ctx.handle, plan_.handle, _vp(staged.dev.ptr), m, staged.n, staged.n,
+                                         _vp(D.ptr)))
+            row0, keep, ip, nnz, kind = descs[0]
+            octs[0] = nat.CqtOctave(D.ptr, pseudo.n_frames, F, row0, keep, ip, nnz, kind)
+            i = 1
+        if full is not None:
+            cur, n_cur = staged.dev.ptr, staged.n
+            if full.early > 1:
+                d = sc.empty((m, -(-n_cur // full.early)), np.float32)
+                _resample_half(ctx, cur, m, n_cur, full.early, full.early_scale, d.ptr)
                 cur, n_cur = d.ptr, d.shape[-1]
-        out = sc.empty(tuple(staged.lead) + (p.n_bins, p.n_frames), np.complex64, layout="ft")
-        nat.check(nat.lib().b2l_cqt_project(ctx.handle, octs, len(p.octaves), _vp(d_indptr), _vp(d_indices),
-                                            _vp(d_data), _vp(d_rscale) if scale else None, m, p.n_frames, p.n_bins,
-                                            _vp(out.ptr)))
+            for o in full.octaves:
+                assert n_cur == o.n
+                F = o.n_fft // 2 + 1
+                D = sc.empty((m, o.n_frames, F), np.complex64)
+                plan_ = nat.make_plan(ctx, ("stft", o.n_fft, o.hop, True, pad_mode, "ones"), n_fft=o.n_fft,
+                                      hop_length=o.hop, center=True, pad_mode=pad_mode, window=np.ones(o.n_fft))
+                nat.check(nat.lib().b2l_stft(ctx.handle, plan_.handle, _vp(cur), m, n_cur, n_cur, _vp(D.ptr)))
+                row0, keep, ip, nnz, kind = descs[i]
+                octs[i] = nat.CqtOctave(D.ptr, o.n_frames, F, row0, keep, ip, nnz, kind)
+                i += 1
+                if o.resample_after:
+                    d = sc.empty((m, -(-n_cur // 2)), np.float32)
+                    _resample_half(ctx, cur, m, n_cur, 2, float(np.sqrt(2.0)), d.ptr)
+                    cur, n_cur = d.ptr, d.shape[-1]
+        out = sc.empty(tuple(staged.lead) + (n_bins, T), np.float32 if mag else np.complex64, layout="ft")
+        project = nat.lib().b2l_cqt_project_abs if mag else nat.lib().b2l_cqt_project
+        nat.check(project(ctx.handle, octs, len(parts), _vp(d_indptr), _vp(d_indices), _vp(d_data),
+                          _vp(d_rscale) if scaled else None, m, T, n_bins, _vp(out.ptr)))
         return sc.keep(out)
 
 
 _BASES = {}
 
 
-def _bases_cached(p: Plan, *, filter_scale, norm, sparsity, window, gamma):
-    """(key, bases()) memoised per configuration, as the reference caches __vqt_filter_fft.  The key holds everything
-    a basis depends on: the frequencies and bandwidths, the rate after early downsampling, and every octave's rows,
-    rate and n_fft (which follow from the hop: the signal is halved only while the hop stays even)."""
-    key = (p.freqs.tobytes(), p.alpha.tobytes(), p.sr,
-           tuple((o.rows.start, o.rows.stop, o.sr, o.n_fft) for o in p.octaves),
-           str(filter_scale), str(norm), str(sparsity), repr(window), str(gamma))
+def _cached(key, build):
+    """(key, build()) memoised per configuration, as the reference caches __vqt_filter_fft."""
     got = _BASES.get(key)
     if got is None:
         if len(_BASES) >= 32:
             _BASES.clear()
-        got = _BASES[key] = bases(p, filter_scale=filter_scale, norm=norm, sparsity=sparsity, window=window,
-                                  gamma=gamma)
+        got = _BASES[key] = build()
     return key, got
+
+
+def pseudo_basis(pp: PseudoPlan, *, filter_scale, norm, sparsity, window) -> Basis:
+    """pseudo_cqt's |basis| (librosa/core/constantq.py:557-571)."""
+    return filter_basis(pp.sr, pp.freqs, pp.alpha, filter_scale, norm, sparsity, window, 0, 1.0, hop_length=pp.hop)
+
+
+def _pseudo_basis_cached(pp: PseudoPlan, *, filter_scale, norm, sparsity, window):
+    key = ("pseudo", pp.freqs.tobytes(), pp.alpha.tobytes(), pp.sr, pp.n_fft, str(filter_scale), str(norm),
+           str(sparsity), repr(window))
+    return _cached(key, lambda: pseudo_basis(pp, filter_scale=filter_scale, norm=norm, sparsity=sparsity,
+                                             window=window))
+
+
+def _bases_cached(p: Plan, *, filter_scale, norm, sparsity, window, gamma):
+    """(key, bases()) memoised per configuration.  The key holds everything a basis depends on: the frequencies and
+    bandwidths, the rate after early downsampling, and every octave's rows, rate and n_fft (which follow from the
+    hop: the signal is halved only while the hop stays even)."""
+    key = (p.freqs.tobytes(), p.alpha.tobytes(), p.sr,
+           tuple((o.rows.start, o.rows.stop, o.sr, o.n_fft) for o in p.octaves),
+           str(filter_scale), str(norm), str(sparsity), repr(window), str(gamma))
+    return _cached(key, lambda: bases(p, filter_scale=filter_scale, norm=norm, sparsity=sparsity, window=window,
+                                      gamma=gamma))
 
 
 def cqt(y, *, sr: float = 22050, hop_length: int = 512, fmin: Optional[float] = None, n_bins: Optional[int] = 84,
@@ -356,3 +506,73 @@ def cqt(y, *, sr: float = 22050, hop_length: int = 512, fmin: Optional[float] = 
     return vqt(y, sr=sr, hop_length=hop_length, fmin=fmin, n_bins=n_bins, intervals="equal", gamma=0,
                bins_per_octave=bins_per_octave, tuning=tuning, filter_scale=filter_scale, norm=norm,
                sparsity=sparsity, window=window, scale=scale, pad_mode=pad_mode, res_type=res_type, dtype=dtype)
+
+
+def pseudo_cqt(y, *, sr: float = 22050, hop_length: int = 512, fmin: Optional[float] = None,
+               n_bins: Optional[int] = 84, bins_per_octave: int = 12, tuning: Optional[float] = 0.0,
+               filter_scale: float = 1, norm: Optional[float] = 1, sparsity: float = 0.01, window="hann",
+               scale: bool = True, pad_mode="constant", dtype=None):
+    """Pseudo constant-Q transform; same contract as ``librosa.pseudo_cqt`` (core/constantq.py:430-590).
+
+    One centred Hann STFT at n_fft = the longest filter's power of two, at least two hops, and the magnitude of one
+    filter basis applied to its magnitude.  Returns ``(..., n_bins, T)`` float32 (float64 for float64 audio or
+    ``dtype=complex128``, computed in float32), C-ordered like the reference's.  A DeviceArray in gives a float32
+    DeviceArray out whose memory is ``[..., frame, bin]`` (layout "ft").
+
+    n_fft above 8192 is refused (UnsupportedOnGPU): the float32 STFT kernels stop there.  That includes the
+    defaults (fmin C1, 84 bins), whose longest filter needs n_fft=16384; from about fmin=65.4 Hz (C2) up, with
+    hops up to 4096, the transform runs."""
+    if fmin is None:
+        fmin = _default_fmin()
+
+    def prepare(n, tuning):
+        pp = pseudo_plan(n, sr=sr, hop_length=hop_length, fmin=fmin * 2.0 ** (tuning / bins_per_octave),
+                         n_bins=n_bins, bins_per_octave=bins_per_octave, filter_scale=filter_scale, window=window)
+        _check_pseudo_stft(pp, n, pad_mode)
+        return None, pp
+
+    res = _staged(y, what="pseudo_cqt", real=True, sr=sr, bins_per_octave=bins_per_octave, tuning=tuning,
+                  dtype=dtype, prepare=prepare, filter_scale=filter_scale, norm=norm, sparsity=sparsity,
+                  window=window, gamma=0, scale=scale, pad_mode=pad_mode)
+    return res if isinstance(res, nat.DeviceArray) else np.ascontiguousarray(res)
+
+
+def hybrid_cqt(y, *, sr: float = 22050, hop_length: int = 512, fmin: Optional[float] = None,
+               n_bins: Optional[int] = 84, bins_per_octave: int = 12, tuning: Optional[float] = 0.0,
+               filter_scale: float = 1, norm: Optional[float] = 1, sparsity: float = 0.01, window="hann",
+               scale: bool = True, pad_mode="constant", res_type: str = "soxr_hq", dtype=None):
+    """Hybrid constant-Q transform; same contract as ``librosa.hybrid_cqt`` (core/constantq.py:208-428).
+
+    The bins whose filters, padded to a power of two, are shorter than two hops take ``pseudo_cqt`` (the highest rows),
+    the others ``np.abs(cqt(...))``, trimmed to the shorter frame count.  Returns ``(..., n_bins, T)`` float32
+    (float64 for float64 audio, computed in float32) with memory ``[..., frame, bin]``, the reference's
+    ``order="F"``; a DeviceArray in gives a float32 DeviceArray out (layout "ft").
+
+    Refused (UnsupportedOnGPU): a pseudo part whose n_fft exceeds 8192 (a hop above 4096), and whatever ``cqt``
+    refuses for the full part: a resampler other than ``res_type="polyphase"`` where the pyramid resamples, an
+    octave n_fft above 8192 (an odd hop stops the halving early)."""
+    if fmin is None:
+        fmin = _default_fmin()
+
+    def prepare(n, tuning):
+        fmin_t = fmin * 2.0 ** (tuning / bins_per_octave)
+        freqs, _, lengths = _equal_bins(sr=sr, fmin=fmin_t, n_bins=n_bins, bins_per_octave=bins_per_octave,
+                                        filter_scale=filter_scale, window=window)
+        is_pseudo = hybrid_split(lengths, hop_length)
+        n_pseudo = int(np.sum(is_pseudo))
+        n_full = len(freqs) - n_pseudo
+        full = pseudo = None
+        if n_pseudo > 0:
+            pseudo = pseudo_plan(n, sr=sr, hop_length=hop_length, fmin=np.min(freqs[is_pseudo]), n_bins=n_pseudo,
+                                 bins_per_octave=bins_per_octave, filter_scale=filter_scale, window=window)
+            _check_pseudo_stft(pseudo, n, pad_mode)
+        if n_full > 0:
+            full = plan(n, sr=sr, hop_length=hop_length, fmin=fmin_t, n_bins=n_full, intervals="equal", gamma=0,
+                        bins_per_octave=bins_per_octave, filter_scale=filter_scale, window=window, scale=scale,
+                        res_type=res_type)
+            _check_full_stft(full, pad_mode)
+        return full, pseudo
+
+    return _staged(y, what="hybrid_cqt", real=True, sr=sr, bins_per_octave=bins_per_octave, tuning=tuning,
+                   dtype=dtype, prepare=prepare, filter_scale=filter_scale, norm=norm, sparsity=sparsity,
+                   window=window, gamma=0, scale=scale, pad_mode=pad_mode)

@@ -1,5 +1,5 @@
-// cqt_api.cu — C ABI of the constant-Q filter-bank projection (cqt_kernels.cuh): librosa.cqt / vqt
-// (librosa/core/constantq.py:820-1266).  The only unit that includes cqt_kernels.cuh.
+// cqt_api.cu — C ABI of the constant-Q filter-bank projection (cqt_kernels.cuh): librosa.cqt / vqt / pseudo_cqt /
+// hybrid_cqt (librosa/core/constantq.py:209-590, 820-1266).  The only unit that includes cqt_kernels.cuh.
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -18,11 +18,11 @@ const size_t kStageCap = 48 * 1024;
 
 size_t table_bytes(const b2l_cqt_octave& o) { return (size_t)o.nnz * (sizeof(float2) + sizeof(int)) + (o.n_rows + 1) * 4; }
 
-}  // namespace
 
-extern "C" int b2l_cqt_project(b2l_ctx* c, const b2l_cqt_octave* h_oct, int32_t n_oct, const int32_t* d_indptr,
-                               const int32_t* d_indices, const void* d_data, const double* d_rscale, int64_t n_clips,
-                               int64_t n_frames, int32_t n_bins, void* d_out) {
+// b2l_cqt_project (complex64 out, complex octaves only) and b2l_cqt_project_abs (float32 magnitudes out).
+int project(b2l_ctx* c, const b2l_cqt_octave* h_oct, int32_t n_oct, const int32_t* d_indptr, const int32_t* d_indices,
+            const void* d_data, const double* d_rscale, int64_t n_clips, int64_t n_frames, int32_t n_bins, void* d_out,
+            bool mag) {
   if (!c || !h_oct || !d_indptr || !d_indices || !d_data || !d_out) return fail(B2L_ERR_INVALID, "NULL argument");
   if (n_oct < 1 || n_oct > B2L_CQT_MAX_OCTAVES)
     return fail(B2L_ERR_UNSUPPORTED, "cqt: %d octaves; the projection takes 1 to %d", n_oct, B2L_CQT_MAX_OCTAVES);
@@ -33,8 +33,10 @@ extern "C" int b2l_cqt_project(b2l_ctx* c, const b2l_cqt_octave* h_oct, int32_t 
   for (int o = 0; o < n_oct; ++o) {
     const b2l_cqt_octave& h = h_oct[o];
     if (!h.d_D || h.n_rows < 1 || h.row0 < 0 || h.row0 + h.n_rows > n_bins || h.nnz < 0 || h.indptr_off < 0 ||
-        h.n_fft_bins < 1 || h.n_frames < n_frames)
+        h.n_fft_bins < 1 || h.n_frames < n_frames || (h.kind & ~(B2L_CQT_PSEUDO | B2L_CQT_DIVIDE)) != 0)
       return fail(B2L_ERR_INVALID, "cqt: bad descriptor of octave %d", o);
+    if ((h.kind & B2L_CQT_PSEUDO) && !mag)
+      return fail(B2L_ERR_INVALID, "cqt: octave %d is a pseudo (magnitude) octave; use b2l_cqt_project_abs", o);
     b2l_cqt::Octave& d = a.oct[o];
     d.D = (const float2*)h.d_D;
     d.T_o = h.n_frames;
@@ -43,6 +45,7 @@ extern "C" int b2l_cqt_project(b2l_ctx* c, const b2l_cqt_octave* h_oct, int32_t 
     d.n_rows = h.n_rows;
     d.indptr_off = h.indptr_off;
     d.nnz = h.nnz;
+    d.kind = h.kind;
     d.tile0 = tiles;
     tiles += (n_frames * h.n_rows + b2l_cqt::kThreads - 1) / b2l_cqt::kThreads;
     smem = std::max(smem, table_bytes(h));
@@ -56,7 +59,8 @@ extern "C" int b2l_cqt_project(b2l_ctx* c, const b2l_cqt_octave* h_oct, int32_t 
   a.rscale = d_rscale;
   a.T = n_frames;
   a.n_bins = n_bins;
-  a.out = (float2*)d_out;
+  a.mag = mag;
+  a.out = d_out;
   a.staged = smem <= kStageCap;
   if (!a.staged) smem = 0;
   DeviceGuard g(c->device);
@@ -65,4 +69,21 @@ extern "C" int b2l_cqt_project(b2l_ctx* c, const b2l_cqt_octave* h_oct, int32_t 
     a.clip0 = c0;
     return launch(c, b2l_cqt::cqt_project_kernel, dim3((unsigned)tiles, (unsigned)m), b2l_cqt::kThreads, smem, a);
   });
+}
+
+}  // namespace
+
+static_assert(sizeof(b2l_cqt_octave) == 40, "b2l_cqt_octave is part of the C ABI");
+static_assert(b2l_cqt::kPseudo == B2L_CQT_PSEUDO && b2l_cqt::kDivide == B2L_CQT_DIVIDE, "octave kind bits");
+
+extern "C" int b2l_cqt_project(b2l_ctx* c, const b2l_cqt_octave* h_oct, int32_t n_oct, const int32_t* d_indptr,
+                               const int32_t* d_indices, const void* d_data, const double* d_rscale, int64_t n_clips,
+                               int64_t n_frames, int32_t n_bins, void* d_out) {
+  return project(c, h_oct, n_oct, d_indptr, d_indices, d_data, d_rscale, n_clips, n_frames, n_bins, d_out, false);
+}
+
+extern "C" int b2l_cqt_project_abs(b2l_ctx* c, const b2l_cqt_octave* h_oct, int32_t n_oct, const int32_t* d_indptr,
+                                   const int32_t* d_indices, const void* d_data, const double* d_rscale,
+                                   int64_t n_clips, int64_t n_frames, int32_t n_bins, float* d_out) {
+  return project(c, h_oct, n_oct, d_indptr, d_indices, d_data, d_rscale, n_clips, n_frames, n_bins, d_out, true);
 }

@@ -441,8 +441,9 @@ def _cqt_chroma_args(y, C, n_chroma, bins_per_octave, cqt_mode):
         if y is None:
             raise ParameterError("At least one of C or y must be provided to compute chroma")
         if cqt_mode == "hybrid":
-            raise nat.UnsupportedOnGPU("chroma_cqt(cqt_mode='hybrid'): hybrid_cqt is not part of this library; use "
-                                       "cqt_mode='full' or pass C=")
+            raise nat.UnsupportedOnGPU("chroma_cqt(cqt_mode='hybrid') does not compute the CQT itself; pass "
+                                       "C=hybrid_cqt(y, ...) (its float32 result is taken as it is) or use "
+                                       "cqt_mode='full'")
         if cqt_mode != "full":
             raise KeyError(cqt_mode)
     return bins_per_octave

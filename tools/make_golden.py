@@ -6,7 +6,8 @@ and leaves the other fixtures as they are; ``--rhythm`` likewise writes only tes
 tests/golden/onset_v1.npz (tests/onset_cases.py), ``--sequence`` only tests/golden/sequence_v1.npz
 (tests/sequence_cases.py), ``--alignment`` only tests/golden/alignment_v1.npz (tests/alignment_cases.py),
 ``--cqt`` only tests/golden/cqt_v1.npz (tests/cqt_cases.py), ``--chroma`` only tests/golden/chroma_v1.npz
-(tests/chroma_cases.py), and ``--iirt`` only tests/golden/iirt_v1.npz (tests/iirt_cases.py).
+(tests/chroma_cases.py), ``--iirt`` only tests/golden/iirt_v1.npz (tests/iirt_cases.py), and ``--hybrid-cqt`` only
+tests/golden/hybrid_cqt_v1.npz (tests/hybrid_cqt_cases.py).
 
 Needs a checkout of the reference (see tools/ref_shim.py); the tests only read the stored fixtures.  Also
 stores a handful of constant tables (mel bases, window sum-square, mel-scale known answers) produced by the
@@ -22,6 +23,7 @@ reference.
     python tools/make_golden.py --cqt
     python tools/make_golden.py --chroma
     python tools/make_golden.py --iirt
+    python tools/make_golden.py --hybrid-cqt
 """
 from __future__ import annotations
 
@@ -504,6 +506,75 @@ def write_iirt():
     print("wrote", path, os.path.getsize(path), "bytes")
 
 
+def write_hybrid_cqt():
+    """tests/golden/hybrid_cqt_v1.npz: per case of tests/hybrid_cqt_cases.py, the reference's C (or
+    ``<name>/error``), its stft warnings, the split of hybrid_cqt (recorded around the reference's pseudo_cqt and cqt,
+    which hybrid_cqt calls through the module's globals), and what the pseudo part's response step received
+    (n_fft, the |basis| or its digest, and the STFT for WITH_D), recorded around the reference's __cqt_response."""
+    import hybrid_cqt_cases as HC
+
+    ref = ref_shim.load_reference()
+    import importlib
+
+    cq = importlib.import_module("librosa.core.constantq")
+    inner = {k: cq.__dict__[k] for k in ("__cqt_response", "pseudo_cqt", "cqt")}
+    calls, parts = [], []
+
+    def recorder(y, n_fft, hop_length, fft_basis, mode, window="ones", phase=True, dtype=None):
+        if not phase:
+            calls.append((y, n_fft, hop_length, fft_basis, mode, dtype))
+        return inner["__cqt_response"](y, n_fft, hop_length, fft_basis, mode, window=window, phase=phase, dtype=dtype)
+
+    def rec_pseudo(y, **kw):
+        parts.append(("pseudo", kw["fmin"], kw["n_bins"]))
+        return inner["pseudo_cqt"](y, **kw)
+
+    def rec_cqt(y, **kw):
+        parts.append(("full", kw["fmin"], kw["n_bins"]))
+        return inner["cqt"](y, **kw)
+
+    cq.__dict__["__cqt_response"] = recorder
+    store = {}
+    for case in HC.CASES:
+        name = case["name"]
+        calls.clear()
+        parts.clear()
+        hybrid = case["fn"] == "hybrid_cqt"
+        if hybrid:
+            cq.__dict__["pseudo_cqt"], cq.__dict__["cqt"] = rec_pseudo, rec_cqt
+        with warnings.catch_warnings(record=True) as caught:
+            warnings.simplefilter("always")
+            try:
+                store[f"{name}/C"] = HC.call(ref, case)
+            except Exception as e:   # the reference's own error, stored as "Class: message"
+                store[f"{name}/error"] = np.array(f"{type(e).__name__}: {e}")
+            finally:
+                cq.__dict__["pseudo_cqt"], cq.__dict__["cqt"] = inner["pseudo_cqt"], inner["cqt"]
+        store[f"{name}/warnings"] = np.array([str(w.message) for w in caught if "n_fft=" in str(w.message)])
+        if hybrid:
+            got = {kind: (fmin, n) for kind, fmin, n in parts}
+            store[f"{name}/n_pseudo"] = np.int64(got.get("pseudo", (0, 0))[1])
+            store[f"{name}/n_full"] = np.int64(got.get("full", (0, 0))[1])
+            if "pseudo" in got:
+                store[f"{name}/fmin_pseudo"] = np.float64(got["pseudo"][0])
+        for y, n_fft, hop, b, mode, dtype in calls[:1]:
+            store[f"{name}/n_fft"] = np.int64(n_fft)
+            if name in HC.BASIS_DIGEST:
+                store[f"{name}/basis/sha256"] = np.array(HC.basis_digest(b.indptr, b.indices, b.data))
+            else:
+                store[f"{name}/basis/indptr"] = b.indptr
+                store[f"{name}/basis/indices"] = b.indices
+                store[f"{name}/basis/data"] = b.data
+            if name in HC.WITH_D:
+                store[f"{name}/D"] = ref.stft(y, n_fft=n_fft, hop_length=hop, window="hann", pad_mode=mode, dtype=dtype)
+        print(f"{name:32s} {store.get(f'{name}/error', np.shape(store.get(f'{name}/C')))} "
+              f"pseudo calls={len(calls)} parts={[(k, n) for k, _, n in parts]}")
+    cq.__dict__["__cqt_response"] = inner["__cqt_response"]
+    path = os.path.join(ROOT, "tests", "golden", "hybrid_cqt_v1.npz")
+    np.savez_compressed(path, **store)
+    print("wrote", path, os.path.getsize(path), "bytes")
+
+
 if __name__ == "__main__":
     if "--pitch" in sys.argv[1:]:
         write_pitch()
@@ -523,5 +594,7 @@ if __name__ == "__main__":
         write_chroma()
     elif "--iirt" in sys.argv[1:]:
         write_iirt()
+    elif "--hybrid-cqt" in sys.argv[1:]:
+        write_hybrid_cqt()
     else:
         main()
