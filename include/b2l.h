@@ -292,6 +292,44 @@ int b2l_iirt_filter(b2l_ctx* ctx, const b2l_iirt_rate* h_rates, int32_t n_rates,
                     const int32_t* d_info, int32_t max_sections, int64_t n_clips);
 int b2l_iirt_stmsp(b2l_ctx* ctx, const b2l_iirt_rate* h_rates, int32_t n_rates, int64_t n_clips, int64_t n_frames,
                    int32_t n_bands, float* d_out);
+/* librosa.feature.delta (feature/utils.py:20-130): scipy.signal.savgol_filter along the middle axis of
+ * d_x [outer][n][inner] (float32, or float64 with f64) into d_y of the same geometry and type, in one launch.
+ * Bit for bit scipy.ndimage.convolve1d: d_taps [width] are the reversed coefficients (savgol_coeffs(...)[::-1]),
+ * `sym` ndimage's classification of them (1 symmetric, -1 antisymmetric, 0 neither), the sum runs in double in
+ * ndimage's order with unfused operations and is rounded once.  d_pad [width - 1] is the padded-index table of the
+ * line: the source sample of positions -h .. -1 and n .. n + h - 1 (h = width / 2), -1 for cval.  interp: outputs
+ * 0 .. h-1 and n-h .. n-1 of each line are d_edge [width - 1][width] (rows 0 .. h-1 over samples 0 .. width-1, rows
+ * h .. width-2 over samples n-width .. n-1) applied in ascending order; a non-finite sample in those windows sets
+ * B2L_STATUS_NOT_FINITE_VALUE.  Widths above B2L_DELTA_MAX_WIDTH return B2L_ERR_UNSUPPORTED. */
+#define B2L_DELTA_MAX_WIDTH 255
+typedef struct b2l_delta_desc {
+  int32_t width;
+  int32_t sym;
+  int32_t interp;
+  int32_t f64;
+  double cval;
+  const double* d_taps;
+  const double* d_edge;
+  const int64_t* d_pad;
+} b2l_delta_desc;
+int b2l_delta(b2l_ctx* ctx, const b2l_delta_desc* desc, const void* d_x, int64_t outer, int64_t n, int64_t inner,
+              void* d_y);
+/* librosa.feature.stack_memory (feature/utils.py:133-315): d_out [n_clips][n_steps * d][t], C order, element
+ * (c, s * d + r, i) = input (c, r, i - s * delay), where element (c, r, i) of d_x is at c * clip_stride + r * row_stride
+ * + i * col_stride (elements of elem_size bytes: 1, 2, 4, 8 or 16).  Columns outside [0, t) are np.pad's padded
+ * positions: d_pad [(n_steps - 1) * |delay|] holds the source column of positions -len .. -1 (delay > 0) or
+ * t .. t + len - 1 (delay < 0), -1 for the constant, whose bytes are fill.  One launch; no status bit. */
+typedef struct b2l_stack_desc {
+  int32_t elem_size;
+  int32_t n_steps;
+  int64_t delay;
+  int64_t clip_stride;
+  int64_t row_stride;
+  int64_t col_stride;
+  uint8_t fill[16];
+} b2l_stack_desc;
+int b2l_stack_memory(b2l_ctx* ctx, const b2l_stack_desc* desc, const void* d_x, int64_t n_clips, int64_t d, int64_t t,
+                     const int64_t* d_pad, void* d_out);
 /* The constant-Q chroma features (feature/spectral.py:1296-1839): chroma_cqt / chroma_vqt (:1296-1423, :1576-1706),
  * the CENS steps of chroma_cens (:1426-1573) and tonnetz (:1709-1839), in one launch per 65 535 clips.
  * b2l_chroma_fold reads d_in [n_clips] x (n_bins, n_frames) in the form `input` names (complex64 input is taken as

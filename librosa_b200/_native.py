@@ -208,6 +208,21 @@ class IirtRate(C.Structure):
 IIRT_MAX_SECTIONS, IIRT_MAX_RATES, IIRT_MAX_DEPTH = 10, 16, 32   # B2L_IIRT_MAX_SECTIONS / _RATES / _DEPTH
 
 
+class DeltaDesc(C.Structure):
+    """struct b2l_delta_desc (include/b2l.h); the d_* fields are device pointers."""
+    _fields_ = [("width", C.c_int32), ("sym", C.c_int32), ("interp", C.c_int32), ("f64", C.c_int32),
+                ("cval", C.c_double), ("d_taps", C.c_void_p), ("d_edge", C.c_void_p), ("d_pad", C.c_void_p)]
+
+
+class StackDesc(C.Structure):
+    """struct b2l_stack_desc (include/b2l.h)."""
+    _fields_ = [("elem_size", C.c_int32), ("n_steps", C.c_int32), ("delay", C.c_int64), ("clip_stride", C.c_int64),
+                ("row_stride", C.c_int64), ("col_stride", C.c_int64), ("fill", C.c_uint8 * 16)]
+
+
+DELTA_MAX_WIDTH = 255   # B2L_DELTA_MAX_WIDTH
+
+
 class ChromaDesc(C.Structure):
     """struct b2l_chroma_desc (include/b2l.h): one b2l_chroma_fold; the d_* fields are device pointers."""
     _fields_ = [("input", C.c_int32), ("out_f64", C.c_int32), ("n_bins", C.c_int32), ("n_chroma", C.c_int32),
@@ -331,6 +346,8 @@ def _declare(lib):
         "b2l_pad_center": (C.c_int, [_vp, _vp, _i64, _i64, C.c_int32, C.c_int32, _vp]),
         "b2l_iirt_filter": (C.c_int, [_vp, P(IirtRate), C.c_int32, _vp, _vp, C.c_int32, _i64]),
         "b2l_iirt_stmsp": (C.c_int, [_vp, P(IirtRate), C.c_int32, _i64, _i64, C.c_int32, _vp]),
+        "b2l_delta": (C.c_int, [_vp, P(DeltaDesc), _vp, _i64, _i64, _i64, _vp]),
+        "b2l_stack_memory": (C.c_int, [_vp, P(StackDesc), _vp, _i64, _i64, _i64, _vp, _vp]),
         "b2l_chroma_fold": (C.c_int, [_vp, P(ChromaDesc), _vp, _i64, _i64, _vp]),
         "b2l_chroma_smooth": (C.c_int, [_vp, _vp, _i64, C.c_int32, _i64, C.c_int32, _vp, _vp, C.c_int32, C.c_int32,
                                         C.c_int32, C.c_double, _vp]),

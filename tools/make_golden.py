@@ -6,8 +6,9 @@ and leaves the other fixtures as they are; ``--rhythm`` likewise writes only tes
 tests/golden/onset_v1.npz (tests/onset_cases.py), ``--sequence`` only tests/golden/sequence_v1.npz
 (tests/sequence_cases.py), ``--alignment`` only tests/golden/alignment_v1.npz (tests/alignment_cases.py),
 ``--cqt`` only tests/golden/cqt_v1.npz (tests/cqt_cases.py), ``--chroma`` only tests/golden/chroma_v1.npz
-(tests/chroma_cases.py), ``--iirt`` only tests/golden/iirt_v1.npz (tests/iirt_cases.py), and ``--hybrid-cqt`` only
-tests/golden/hybrid_cqt_v1.npz (tests/hybrid_cqt_cases.py).
+(tests/chroma_cases.py), ``--iirt`` only tests/golden/iirt_v1.npz (tests/iirt_cases.py), ``--hybrid-cqt`` only
+tests/golden/hybrid_cqt_v1.npz (tests/hybrid_cqt_cases.py), and ``--feature-utils`` only
+tests/golden/feature_utils_v1.npz (tests/feature_utils_cases.py).
 
 Needs a checkout of the reference (see tools/ref_shim.py); the tests only read the stored fixtures.  Also
 stores a handful of constant tables (mel bases, window sum-square, mel-scale known answers) produced by the
@@ -24,6 +25,7 @@ reference.
     python tools/make_golden.py --chroma
     python tools/make_golden.py --iirt
     python tools/make_golden.py --hybrid-cqt
+    python tools/make_golden.py --feature-utils
 """
 from __future__ import annotations
 
@@ -575,6 +577,29 @@ def write_hybrid_cqt():
     print("wrote", path, os.path.getsize(path), "bytes")
 
 
+def write_feature_utils():
+    """tests/golden/feature_utils_v1.npz: per case of tests/feature_utils_cases.py that the GPU does not refuse, the
+    reference's delta / stack_memory output (``<name>/out``) or its error (``<name>/error``)."""
+    import feature_utils_cases as FU
+
+    ref = ref_shim.load_reference()
+    store = {}
+    for case in FU.CASES:
+        if case["refuse"]:
+            continue
+        name = case["name"]
+        with warnings.catch_warnings():
+            warnings.simplefilter("ignore")
+            try:
+                store[f"{name}/out"] = np.asarray(FU.call(ref, case))
+            except Exception as e:   # the reference's own error, stored as "Class: message"
+                store[f"{name}/error"] = np.array(f"{type(e).__name__}: {e}")
+        print(f"{name:40s} {store.get(f'{name}/error', np.shape(store.get(f'{name}/out')))}")
+    path = os.path.join(ROOT, "tests", "golden", "feature_utils_v1.npz")
+    np.savez_compressed(path, **store)
+    print("wrote", path, os.path.getsize(path), "bytes")
+
+
 if __name__ == "__main__":
     if "--pitch" in sys.argv[1:]:
         write_pitch()
@@ -596,5 +621,7 @@ if __name__ == "__main__":
         write_iirt()
     elif "--hybrid-cqt" in sys.argv[1:]:
         write_hybrid_cqt()
+    elif "--feature-utils" in sys.argv[1:]:
+        write_feature_utils()
     else:
         main()
