@@ -389,11 +389,64 @@ class Scope:
             self._owned.append(d)
         return d
 
+    def free(self, *ds):
+        """Free those of ``ds`` that this scope owns now rather than on exit (stream-ordered: safe right after their
+        last launch), so that later allocations of the call can reuse the blocks.  The caller's arrays stay."""
+        for d in ds:
+            if any(d is o for o in self._owned):
+                d.free()
+
     def stage(self, x, dtype=None) -> nat.DeviceArray:
         """A DeviceArray as it is; a host array uploaded C-ordered as ``dtype`` (default: its own)."""
         if isinstance(x, nat.DeviceArray):
             return x
         return self.own(self.ctx.to_device(np.ascontiguousarray(x, dtype=dtype)))
+
+    def spectrogram(self, S, what: str = "S", stacklevel: int = 4):
+        """A real spectrogram-like argument ``(..., rows, frames)`` on the device -> (DeviceArray, requested dtype).
+        A device array must be float32 and keeps its layout; a host array is uploaded C-ordered as float32.
+        ``what`` and ``stacklevel`` go to check_real_dtype (``stacklevel`` counted as there: 4 names the line that
+        calls this method, 5 the line that calls that function)."""
+        if isinstance(S, nat.DeviceArray):
+            if S.dtype != np.float32:
+                raise ParameterError(f"device {what} must be float32")
+            return S, np.dtype(np.float32)
+        S = np.asarray(S)
+        if np.iscomplexobj(S):
+            raise ParameterError("spectrogram input must be real")
+        dtype = S.dtype if np.issubdtype(S.dtype, np.floating) else np.float32
+        req = check_real_dtype(dtype, what, stacklevel=stacklevel)
+        return self.stage(S, np.float32), req
+
+    def native(self, S, dtype=None, host_transpose: bool = False) -> nat.DeviceArray:
+        """A spectrogram-like array ``(..., bins, frames)``, host or device, real or complex, in any layout, in the
+        kernels' native [frame][bin] "ft" layout.
+
+        A device array already in "ft" comes back as it is; any other goes through the transpose kernel, host arrays
+        after a C-ordered upload as ``dtype`` (freed as soon as the transpose is enqueued).  ``host_transpose``:
+        reorder a host array with NumPy instead (no copy when its memory already is [frame][bin]) — for complex128,
+        which the transpose kernel does not take."""
+        if isinstance(S, nat.DeviceArray):
+            if S.layout == "ft":
+                return S
+            out = self.own(S.ctx.empty(S.shape, S.dtype, layout="ft"))
+            nat.check(nat.lib().b2l_transpose(S.ctx.handle, C.c_void_p(S.ptr), clip_count(S.shape[:-2]), S.shape[-2],
+                                              S.shape[-1], S.dtype.itemsize, C.c_void_p(out.ptr)))
+            return out
+        if not host_transpose:
+            raw = self.stage(S, dtype)
+            out = self.native(raw)
+            raw.free()
+            return out
+        view = np.swapaxes(S, -1, -2)
+        mem = np.ascontiguousarray(view, dtype=dtype)
+        out = self.empty(S.shape, mem.dtype, layout="ft")
+        if mem.nbytes:
+            nat.check(nat.lib().b2l_h2d(self.ctx.handle, C.c_void_p(out.ptr), mem.ctypes.data_as(C.c_void_p),
+                                        mem.nbytes))
+            if mem is not view:   # a staging copy made here must outlive the upload
+                self.ctx.synchronize()
+        return out
 
     def empty(self, shape, dtype, layout: str = "c") -> nat.DeviceArray:
         return self.own(self.ctx.empty(shape, dtype, layout))
@@ -463,52 +516,6 @@ class Envelope:
             self.audio.check_finite()
         if flags & nat.STATUS_NOT_FINITE_VALUE:
             raise ParameterError("Input must be finite")
-
-
-# --------------------------------------------------------------------------------------------- spectrogram inputs
-def spectrogram_input(S):
-    """A real spectrogram-like argument ``(..., rows, frames)``, host or device -> (DeviceArray, requested dtype,
-    input was on the device).  Host arrays are uploaded C-ordered; device arrays keep their layout."""
-    if isinstance(S, nat.DeviceArray):
-        if S.dtype != np.float32:
-            raise ParameterError("device spectrogram must be float32")
-        return S, np.dtype(np.float32), True
-    S = np.asarray(S)
-    if np.iscomplexobj(S):
-        raise ParameterError("spectrogram input must be real")
-    req = check_real_dtype(S.dtype if np.issubdtype(S.dtype, np.floating) else np.float32, "S")
-    return nat.default_context().to_device(np.ascontiguousarray(S, dtype=np.float32)), req, False
-
-
-def to_native(S, dtype=None, host_transpose: bool = False, ctx=None):
-    """A spectrogram-like array ``(..., bins, frames)``, host or device, real or complex, in any layout ->
-    (DeviceArray in the kernels' native [frame][bin] "ft" layout, whether the caller owns it).
-
-    A device array already in "ft" comes back as it is; any other goes through the transpose kernel, host arrays
-    after a C-ordered upload as ``dtype``.  ``host_transpose``: reorder a host array with NumPy instead (no copy
-    when its memory already is [frame][bin]) — for complex128, which the transpose kernel does not take.  Host
-    arrays go to ``ctx`` (default: the default context)."""
-    if not isinstance(S, nat.DeviceArray):
-        ctx = ctx or nat.default_context()
-        if not host_transpose:
-            raw = ctx.to_device(np.ascontiguousarray(S, dtype=dtype))
-            out, _ = to_native(raw)
-            raw.free()
-            return out, True
-        view = np.swapaxes(S, -1, -2)
-        mem = np.ascontiguousarray(view, dtype=dtype)
-        out = nat.DeviceArray.empty(ctx, S.shape, dtype, layout="ft")
-        if mem.nbytes:
-            nat.check(nat.lib().b2l_h2d(ctx.handle, C.c_void_p(out.ptr), mem.ctypes.data_as(C.c_void_p), mem.nbytes))
-            if mem is not view:   # a staging copy made here must outlive the upload
-                ctx.synchronize()
-        return out, True
-    if S.layout == "ft":
-        return S, False
-    out = nat.DeviceArray.empty(S.ctx, S.shape, S.dtype, layout="ft")
-    nat.check(nat.lib().b2l_transpose(S.ctx.handle, C.c_void_p(S.ptr), clip_count(S.shape[:-2]), S.shape[-2],
-                                      S.shape[-1], S.dtype.itemsize, C.c_void_p(out.ptr)))
-    return out, True
 
 
 # --------------------------------------------------------------------------------------------- forward ops

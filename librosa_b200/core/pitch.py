@@ -29,35 +29,35 @@ def _key_to_float(key: int) -> np.float32:
     return np.array([u], dtype=np.uint32).view(np.float32)[0]
 
 
-def _tuning_from_device_spec(ctx, Sd, sr, n_fft, *, resolution, bins_per_octave, fmin, fmax, threshold, ref):
+def _tuning_from_device_spec(Sd, sr, n_fft, *, resolution, bins_per_octave, fmin, fmax, threshold, ref):
     """Sd: float32 DeviceArray (..., bins, frames), any layout.  Returns the tuning estimate (float)."""
     F, T = Sd.shape[-2], Sd.shape[-1]
     L = nat.lib()
-    src, own = pl.to_native(Sd)
-    freqs = fft_frequencies(sr=sr, n_fft=n_fft)
-    fmin = np.maximum(fmin, 0)
-    fmax = np.minimum(fmax, float(sr) / 2)
-    mask = np.flatnonzero((fmin <= freqs) & (freqs < fmax))
-    desc = nat.PipDesc(k_lo=int(mask[0]) if mask.size else 0, k_hi=int(mask[-1]) + 1 if mask.size else 0,
-                       threshold=float(threshold), ref_abs=-1.0, hz_per_bin=float(sr) / n_fft,
-                       bins_per_octave=float(bins_per_octave))
-    if ref is not None and ref is not np.max:
-        if callable(ref):
-            raise nat.UnsupportedOnGPU("piptrack(ref=callable) other than np.max is not supported on the GPU")
-        desc.ref_abs = float(np.abs(ref))
-    rows = pl.clip_count(Sd.shape[:-2]) * T
-    hist = (C.c_uint64 * 2048)()
+    with pl.Scope(Sd) as sc:
+        src = sc.native(Sd)
+        freqs = fft_frequencies(sr=sr, n_fft=n_fft)
+        fmin = np.maximum(fmin, 0)
+        fmax = np.minimum(fmax, float(sr) / 2)
+        mask = np.flatnonzero((fmin <= freqs) & (freqs < fmax))
+        desc = nat.PipDesc(k_lo=int(mask[0]) if mask.size else 0, k_hi=int(mask[-1]) + 1 if mask.size else 0,
+                           threshold=float(threshold), ref_abs=-1.0, hz_per_bin=float(sr) / n_fft,
+                           bins_per_octave=float(bins_per_octave))
+        if ref is not None and ref is not np.max:
+            if callable(ref):
+                raise nat.UnsupportedOnGPU("piptrack(ref=callable) other than np.max is not supported on the GPU")
+            desc.ref_abs = float(np.abs(ref))
+        rows = pl.clip_count(Sd.shape[:-2]) * T
+        hist = (C.c_uint64 * 2048)()
 
-    def run(mode, prefix=0, mag_threshold=0.0, edges=None, n_res=0):
-        desc.mode, desc.prefix, desc.mag_threshold, desc.n_res_bins = mode, prefix, float(mag_threshold), n_res
-        e = edges.ctypes.data_as(_vp) if edges is not None else None
-        nat.check(L.b2l_pip_pass(ctx.handle, C.byref(desc), _vp(src.ptr), rows, F, e, hist))
-        n = n_res if mode == 3 else (1024 if mode == 2 else 2048)
-        return np.frombuffer(hist, dtype=np.uint64, count=n).astype(np.int64)
+        def run(mode, prefix=0, mag_threshold=0.0, edges=None, n_res=0):
+            desc.mode, desc.prefix, desc.mag_threshold, desc.n_res_bins = mode, prefix, float(mag_threshold), n_res
+            e = edges.ctypes.data_as(_vp) if edges is not None else None
+            nat.check(L.b2l_pip_pass(sc.ctx.handle, C.byref(desc), _vp(src.ptr), rows, F, e, hist))
+            n = n_res if mode == 3 else (1024 if mode == 2 else 2048)
+            return np.frombuffer(hist, dtype=np.uint64, count=n).astype(np.int64)
 
-    h0 = run(0)
-    n_peaks = int(h0.sum())
-    try:
+        h0 = run(0)
+        n_peaks = int(h0.sum())
         if n_peaks == 0:
             warnings.warn("Trying to estimate tuning from empty frequency set.", stacklevel=3)
             return 0.0
@@ -84,9 +84,6 @@ def _tuning_from_device_spec(ctx, Sd, sr, n_fft, *, resolution, bins_per_octave,
             raise nat.UnsupportedOnGPU("tuning resolution finer than 1/2048 is not supported on the GPU")
         counts = run(3, mag_threshold=med, edges=np.ascontiguousarray(edges, dtype=np.float64), n_res=len(edges) - 1)
         return edges[int(np.argmax(counts))]
-    finally:
-        if own:
-            src.free()
 
 
 def estimate_tuning(*, y=None, sr: float = 22050, S=None, n_fft: Optional[int] = 2048, resolution: float = 0.01,
@@ -102,34 +99,30 @@ def estimate_tuning(*, y=None, sr: float = 22050, S=None, n_fft: Optional[int] =
         raise TypeError(f"piptrack() got an unexpected keyword argument '{sorted(extra)[0]}'")
     pip = dict(fmin=kwargs.get("fmin", 150.0), fmax=kwargs.get("fmax", 4000.0), threshold=kwargs.get("threshold", 0.1),
                ref=kwargs.get("ref", None))
-    staged = None
-    if S is None:
-        if y is None:
-            raise ParameterError("Input signal must be provided to compute a spectrogram")
-        pl.precheck_signal(y)
-        staged = pl.StagedInput(y)
-        Sd, n_fft = _spectrogram(y=staged.dev, n_fft=n_fft, hop_length=kwargs.get("hop_length"), power=1,
-                                 win_length=kwargs.get("win_length"), window=kwargs.get("window", "hann"),
-                                 center=kwargs.get("center", True), pad_mode=kwargs.get("pad_mode", "constant"))
-        own = True
-        staged.scan_uncovered(n_fft, kwargs.get("hop_length"), kwargs.get("win_length"), kwargs.get("center", True),
-                              Sd.shape[-1])
-    else:
-        if not isinstance(S, nat.DeviceArray) and np.iscomplexobj(S):
-            S = np.abs(S)
-        Sd, _, on_device = pl.spectrogram_input(S)
-        own = not on_device
-        if n_fft is None or n_fft // 2 + 1 != Sd.shape[-2]:
-            n_fft = 2 * (Sd.shape[-2] - 1)
-    try:
-        est = _tuning_from_device_spec(Sd.ctx, Sd, sr, n_fft, resolution=resolution, bins_per_octave=bins_per_octave,
-                                       **pip)
-    finally:
-        if own:
-            Sd.free()
-    if staged is not None:
-        staged.check_finite()
-    return est
+    with pl.Scope(y if S is None else S) as sc:
+        staged = None
+        if S is None:
+            if y is None:
+                raise ParameterError("Input signal must be provided to compute a spectrogram")
+            pl.precheck_signal(y)
+            staged = pl.StagedInput(y)
+            sc.own(staged.dev)
+            Sd, n_fft = _spectrogram(y=staged.dev, n_fft=n_fft, hop_length=kwargs.get("hop_length"), power=1,
+                                     win_length=kwargs.get("win_length"), window=kwargs.get("window", "hann"),
+                                     center=kwargs.get("center", True), pad_mode=kwargs.get("pad_mode", "constant"))
+            sc.own(Sd)
+            staged.scan_uncovered(n_fft, kwargs.get("hop_length"), kwargs.get("win_length"),
+                                  kwargs.get("center", True), Sd.shape[-1])
+        else:
+            if not isinstance(S, nat.DeviceArray) and np.iscomplexobj(S):
+                S = np.abs(S)
+            Sd, _ = sc.spectrogram(S)
+            if n_fft is None or n_fft // 2 + 1 != Sd.shape[-2]:
+                n_fft = 2 * (Sd.shape[-2] - 1)
+        est = _tuning_from_device_spec(Sd, sr, n_fft, resolution=resolution, bins_per_octave=bins_per_octave, **pip)
+        if staged is not None:
+            staged.check_finite()
+        return est
 
 
 # --------------------------------------------------------------------------------------------- yin / pyin

@@ -119,8 +119,20 @@ def _check_istft_out(out, shape):
             raise ParameterError(f"Shape mismatch for provided output array out.shape={out.shape} != {list(shape)}")
 
 
-def _istft_f64(stft_matrix, on_device, n_frames, T_stored, F, n_fft, hop_length, win_length, window, win, center,
-               dtype, length, out):
+def _istft_result(sc, y, dtype, out):
+    """istft's return value: the device signal for a device call without ``out``, else ``y`` copied to the host as
+    ``dtype`` (written into ``out`` when given)."""
+    if sc.on_device and out is None:
+        return sc.keep(y)
+    res = pl.finish(y, dtype)
+    if out is None:
+        return res
+    out[...] = res
+    return out
+
+
+def _istft_f64(stft_matrix, n_frames, T_stored, F, n_fft, hop_length, win_length, window, win, center, dtype, length,
+               out):
     """complex128 STFT -> float64 signal in FP64 on the device (core/spectrum.py:506-626 in double)."""
     if dtype is None:
         dtype = np.float64
@@ -130,23 +142,15 @@ def _istft_f64(stft_matrix, on_device, n_frames, T_stored, F, n_fft, hop_length,
     out_len = _istft_out_len(n_fft, hop_length, n_frames, center, length)
     _check_istft_out(out, tuple(stft_matrix.shape[:-2]) + (out_len,))
     f64.require_supported(n_fft)
-    if on_device and stft_matrix.layout != "ft":
-        raise ParameterError("device complex128 stft_matrix must be in the native [frame][bin] layout")
-    Dd, own = pl.to_native(stft_matrix, np.complex128, host_transpose=True)
-    ctx = Dd.ctx
-    start = n_fft // 2 if center else 0
-    inv = f64.inv_wss(window, n_frames, win_length, n_fft, hop_length, start, out_len)
-    y = f64.istft(ctx, Dd, n_frames_used=n_frames, n_fft=n_fft, hop_length=hop_length, center=center, win=win,
-                  inv=inv, out_len=out_len)
-    if own:
-        Dd.free()
-    if on_device and out is None:
-        return y
-    res = pl.finish(y, dtype)
-    if out is None:
-        return res
-    out[...] = res
-    return out
+    with pl.Scope(stft_matrix) as sc:
+        if sc.on_device and stft_matrix.layout != "ft":
+            raise ParameterError("device complex128 stft_matrix must be in the native [frame][bin] layout")
+        Dd = sc.native(stft_matrix, np.complex128, host_transpose=True)
+        start = n_fft // 2 if center else 0
+        inv = f64.inv_wss(window, n_frames, win_length, n_fft, hop_length, start, out_len)
+        y = sc.own(f64.istft(sc.ctx, Dd, n_frames_used=n_frames, n_fft=n_fft, hop_length=hop_length, center=center,
+                             win=win, inv=inv, out_len=out_len))
+        return _istft_result(sc, y, dtype, out)
 
 
 def istft(stft_matrix, *, hop_length: Optional[int] = None, win_length: Optional[int] = None,
@@ -177,8 +181,8 @@ def istft(stft_matrix, *, hop_length: Optional[int] = None, win_length: Optional
     if (in_dtype == np.complex128 and pl.native_float64(in_dtype)) or \
             (in_dtype == np.complex64 and not on_device and not pl.f32_kernels_cover(n_fft) and f64.supported(n_fft)):
         wide = stft_matrix if in_dtype == np.complex128 else stft_matrix.astype(np.complex128)
-        return _istft_f64(wide, on_device, n_frames, T_stored, F, n_fft, hop_length, win_length, window, win,
-                          center, dtype if dtype is not None else dtype_c2r(in_dtype), length, out)
+        return _istft_f64(wide, n_frames, T_stored, F, n_fft, hop_length, win_length, window, win, center,
+                          dtype if dtype is not None else dtype_c2r(in_dtype), length, out)
     if in_dtype != np.complex64:
         if in_dtype.kind == "c" and pl.wide_complex_ok("istft input"):
             pass
@@ -194,29 +198,22 @@ def istft(stft_matrix, *, hop_length: Optional[int] = None, win_length: Optional
     lead = tuple(stft_matrix.shape[:-2])
     _check_istft_out(out, lead + (out_len,))
     pl.require_supported_n_fft(n_fft, inverse=True)
-    ctx = pl.context_for(stft_matrix)
-    key = ("stft", n_fft, hop_length, bool(center), "constant", wkey)
-    plan = nat.make_plan(ctx, key, n_fft=n_fft, hop_length=hop_length, center=center, pad_mode="constant",
-                         window=win)
-    if on_device and stft_matrix.dtype != np.complex64:
-        raise ParameterError("device stft_matrix must be complex64")
-    # a host matrix whose memory already is [.., frame, bin] complex64 (stft's own output) uploads as it is
-    zero_copy = not on_device and in_dtype == np.complex64 and np.swapaxes(stft_matrix, -1, -2).flags.c_contiguous
-    Dd, own = pl.to_native(stft_matrix, np.complex64, host_transpose=zero_copy)
-    start = n_fft // 2 if center else 0
-    inv_ptr = _inv_wss(ctx, window, n_frames, win_length, n_fft, hop_length, start, out_len, wkey)
-    y = nat.DeviceArray.empty(ctx, lead + (out_len,), np.float32)
-    nat.check(nat.lib().b2l_istft(ctx.handle, plan.handle, _vp(Dd.ptr), pl.clip_count(lead), T_stored, n_frames,
-                                  _vp(inv_ptr), out_len, _vp(y.ptr), out_len))
-    if own:
-        Dd.free()   # stream-ordered pool: safe right after the launch
-    if on_device and out is None:
-        return y
-    res = pl.finish(y, dtype)
-    if out is None:
-        return res
-    out[...] = res
-    return out
+    with pl.Scope(stft_matrix) as sc:
+        ctx = sc.ctx
+        key = ("stft", n_fft, hop_length, bool(center), "constant", wkey)
+        plan = nat.make_plan(ctx, key, n_fft=n_fft, hop_length=hop_length, center=center, pad_mode="constant",
+                             window=win)
+        if on_device and stft_matrix.dtype != np.complex64:
+            raise ParameterError("device stft_matrix must be complex64")
+        # a host matrix whose memory already is [.., frame, bin] complex64 (stft's own output) uploads as it is
+        zero_copy = not on_device and in_dtype == np.complex64 and np.swapaxes(stft_matrix, -1, -2).flags.c_contiguous
+        Dd = sc.native(stft_matrix, np.complex64, host_transpose=zero_copy)
+        start = n_fft // 2 if center else 0
+        inv_ptr = _inv_wss(ctx, window, n_frames, win_length, n_fft, hop_length, start, out_len, wkey)
+        y = sc.empty(lead + (out_len,), np.float32)
+        nat.check(nat.lib().b2l_istft(ctx.handle, plan.handle, _vp(Dd.ptr), pl.clip_count(lead), T_stored, n_frames,
+                                      _vp(inv_ptr), out_len, _vp(y.ptr), out_len))
+        return _istft_result(sc, y, dtype, out)
 
 
 def _spectrogram(*, y=None, S=None, n_fft: Optional[int] = 2048, hop_length: Optional[int] = 512,
@@ -233,10 +230,10 @@ def _spectrogram(*, y=None, S=None, n_fft: Optional[int] = 2048, hop_length: Opt
         raise ParameterError("Input signal must be provided to compute a spectrogram")
     fr = pl.forward_front(y, n_fft, hop_length, win_length, window, center, pad_mode)
     if pl.wide_route(y, fr.dtype, n_fft):
-        staged, D = f64.stft(y, n_fft=n_fft, hop_length=fr.hop, center=center, mode=fr.mode, win=fr.window)
-        Sd = f64.abs_pow(staged.ctx, D, power)
-        D.free()
-        return staged.result(Sd, fr.dtype), n_fft
+        with pl.Scope(y) as sc:
+            _, D = f64.stft(y, n_fft=n_fft, hop_length=fr.hop, center=center, mode=fr.mode, win=fr.window)
+            Sd = sc.own(f64.abs_pow(sc.ctx, sc.own(D), power))
+            return sc.result(Sd, fr.dtype, validate=True), n_fft
     pl.require_supported_n_fft(n_fft)
 
     def launch(ctx, plan, d_in, m, n_, d_out, d_scr):
@@ -298,61 +295,55 @@ def _to_db(S, ref, amin, top_db, axes, amplitude: bool):
         flat = np.ascontiguousarray(Sp).reshape(n_keep, 1, -1)
         res = _to_db(flat, ref, amin, top_db, "auto", amplitude)
         return np.transpose(np.asarray(res).reshape(Sp.shape), np.argsort(perm))[()]
-    ctx = S.ctx if on_device else nat.default_context()
-    if not on_device and S.dtype == np.float64 and pl.native_float64(S.dtype) and S.ndim >= 1:
-        return _to_db_f64(ctx, S, ref, amin, top_db, amplitude)
-    if on_device:
-        if S.dtype != np.float32:
-            raise ParameterError("device input must be float32")
-        dev = S
-        req = np.dtype(np.float32)
-    else:
-        if not np.issubdtype(S.dtype, np.floating):
+    with pl.Scope(S) as sc:
+        if not on_device and S.dtype == np.float64 and pl.native_float64(S.dtype) and S.ndim >= 1:
+            return _to_db_f64(sc, S, ref, amin, top_db, amplitude)
+        if not on_device and not np.issubdtype(S.dtype, np.floating):
             S = S.astype(np.float32)
-        req = pl.check_real_dtype(S.dtype, f"{name} input")
-        dev = ctx.to_device(np.ascontiguousarray(S, dtype=np.float32))
-    ndim = len(dev.shape)
-    if ndim >= 2:
-        lead = dev.shape[:-2]
-        per = dev.shape[-2] * dev.shape[-1]
-    else:
-        lead = ()
-        per = dev.size
-    n_lead = pl.clip_count(lead)
-    out = nat.DeviceArray.empty(ctx, dev.shape, np.float32, layout=dev.layout)
-    tdb = -1.0 if top_db is None else float(top_db)
-    L = nat.lib()
-    src = dev
-    if amplitude:
-        # power = |S|**2 (written into the output buffer, converted in place), amin**2, ref**2
-        nat.check(L.b2l_unary(ctx.handle, nat.UNARY_SQUARE, _vp(dev.ptr), dev.size, 0.0, _vp(out.ptr)))
-        src = out
-        amin = float(amin) ** 2
-    if callable(ref):
-        if on_device:
-            raise nat.UnsupportedOnGPU("callable ref needs a host array")
-        ax = (-2, -1) if ndim >= 2 else ((-1,) if ndim == 1 else None)
-        try:
-            ref_value = np.asarray(ref(np.abs(S) if amplitude else S, axis=ax, keepdims=True), dtype=np.float64).reshape(-1)
-        except TypeError as exc:
-            raise ParameterError("The provided reference function must support 'axis' and 'keepdims' "
-                                 "arguments for proper multichannel processing.") from exc
+        dev, req = sc.spectrogram(S, f"{name} input", stacklevel=5)
+        ctx = sc.ctx
+        ndim = len(dev.shape)
+        if ndim >= 2:
+            lead = dev.shape[:-2]
+            per = dev.shape[-2] * dev.shape[-1]
+        else:
+            lead = ()
+            per = dev.size
+        n_lead = pl.clip_count(lead)
+        out = sc.empty(dev.shape, np.float32, layout=dev.layout)
+        tdb = -1.0 if top_db is None else float(top_db)
+        L = nat.lib()
+        src = dev
         if amplitude:
-            ref_value = ref_value ** 2
-        for i in range(n_lead):   # one reference level per leading index
-            nat.check(L.b2l_power_to_db(ctx.handle, _vp(src.ptr + 4 * i * per), 1, per, float(amin),
-                                        float(ref_value[i if ref_value.size > 1 else 0]), tdb,
-                                        _vp(out.ptr + 4 * i * per)))
-    else:
-        ref_value = float(np.abs(ref)) ** 2 if amplitude else float(np.abs(ref))
-        nat.check(L.b2l_power_to_db(ctx.handle, _vp(src.ptr), n_lead, per, float(amin), ref_value, tdb,
-                                    _vp(out.ptr)))
-    if on_device:
-        return out
-    return pl.finish(out, req)[()]
+            # power = |S|**2 (written into the output buffer, converted in place), amin**2, ref**2
+            nat.check(L.b2l_unary(ctx.handle, nat.UNARY_SQUARE, _vp(dev.ptr), dev.size, 0.0, _vp(out.ptr)))
+            src = out
+            amin = float(amin) ** 2
+        if callable(ref):
+            if on_device:
+                raise nat.UnsupportedOnGPU("callable ref needs a host array")
+            ax = (-2, -1) if ndim >= 2 else ((-1,) if ndim == 1 else None)
+            try:
+                ref_value = np.asarray(ref(np.abs(S) if amplitude else S, axis=ax, keepdims=True),
+                                       dtype=np.float64).reshape(-1)
+            except TypeError as exc:
+                raise ParameterError("The provided reference function must support 'axis' and 'keepdims' "
+                                     "arguments for proper multichannel processing.") from exc
+            if amplitude:
+                ref_value = ref_value ** 2
+            for i in range(n_lead):   # one reference level per leading index
+                nat.check(L.b2l_power_to_db(ctx.handle, _vp(src.ptr + 4 * i * per), 1, per, float(amin),
+                                            float(ref_value[i if ref_value.size > 1 else 0]), tdb,
+                                            _vp(out.ptr + 4 * i * per)))
+        else:
+            ref_value = float(np.abs(ref)) ** 2 if amplitude else float(np.abs(ref))
+            nat.check(L.b2l_power_to_db(ctx.handle, _vp(src.ptr), n_lead, per, float(amin), ref_value, tdb,
+                                        _vp(out.ptr)))
+        res = sc.result(out, req)
+        return res if on_device else res[()]
 
 
-def _to_db_f64(ctx, S, ref, amin, top_db, amplitude):
+def _to_db_f64(sc, S, ref, amin, top_db, amplitude):
     """power_to_db / amplitude_to_db of a float64 host array in FP64 (core/spectrum.py:1866-1881, :1990-2038)."""
     shape = S.shape
     work = S if S.ndim >= 2 else S.reshape(1, -1)
@@ -370,38 +361,32 @@ def _to_db_f64(ctx, S, ref, amin, top_db, amplitude):
         power, amin, ref_value = mag ** 2, float(amin) ** 2, ref_value ** 2
     else:
         power = mag
-    dev = ctx.to_device(np.ascontiguousarray(power, dtype=np.float64).reshape((n_lead,) + work.shape[-2:]))
+    dev = sc.stage(np.reshape(power, (n_lead,) + work.shape[-2:]), np.float64)
     if ref_value.size > 1:
         parts = []
         for i in range(n_lead):                     # one reference level per leading index
             one = dev.view((1,) + work.shape[-2:], offset=i * work.shape[-2] * work.shape[-1])
-            parts.append(f64.power_to_db(ctx, one, ref_value=float(ref_value[i]), amin=amin, top_db=top_db))
+            parts.append(sc.own(f64.power_to_db(sc.ctx, one, ref_value=float(ref_value[i]), amin=amin, top_db=top_db)))
         res = np.concatenate([pl.finish(p) for p in parts], axis=0)
     else:
-        res = pl.finish(f64.power_to_db(ctx, dev, ref_value=float(ref_value[0]), amin=amin, top_db=top_db))
-    dev.free()
+        res = pl.finish(sc.own(f64.power_to_db(sc.ctx, dev, ref_value=float(ref_value[0]), amin=amin, top_db=top_db)))
     return res.reshape(shape)[()]
 
 
 def _db_inverse(S_db, op, param):
     on_device = isinstance(S_db, nat.DeviceArray)
-    ctx = S_db.ctx if on_device else nat.default_context()
-    if on_device:
-        if S_db.dtype != np.float32:
-            raise ParameterError("device input must be float32")
-        dev, req = S_db, np.dtype(np.float32)
-    else:
+    if not on_device:
         S_db = np.asarray(S_db)
         if np.iscomplexobj(S_db):
             raise nat.UnsupportedOnGPU("complex dB values are not supported on the GPU")
-        req = np.dtype(np.float64) if not np.issubdtype(S_db.dtype, np.floating) else \
-            pl.check_real_dtype(S_db.dtype, "dB input")
-        dev = ctx.to_device(np.ascontiguousarray(S_db, dtype=np.float32))
-    out = nat.DeviceArray.empty(ctx, dev.shape, np.float32, layout=dev.layout)
-    nat.check(nat.lib().b2l_unary(ctx.handle, op, _vp(dev.ptr), dev.size, float(param), _vp(out.ptr)))
-    if on_device:
-        return out
-    return pl.finish(out, req)[()]
+    with pl.Scope(S_db) as sc:
+        dev, req = sc.spectrogram(S_db, "dB input", stacklevel=5)
+        if not on_device and not np.issubdtype(S_db.dtype, np.floating):
+            req = np.dtype(np.float64)
+        out = sc.empty(dev.shape, np.float32, layout=dev.layout)
+        nat.check(nat.lib().b2l_unary(sc.ctx.handle, op, _vp(dev.ptr), dev.size, float(param), _vp(out.ptr)))
+        res = sc.result(out, req)
+        return res if on_device else res[()]
 
 
 def db_to_power(S_db, *, ref: float = 1.0):
@@ -458,50 +443,37 @@ def pcen(S, *, sr: float = 22050, hop_length: int = 512, gain: float = 0.98, bia
             max_axis = 0
         if max_axis not in (-2, ndim - 2):
             raise nat.UnsupportedOnGPU("pcen on the GPU max-filters along the second-to-last axis (max_axis=-2)")
-    ctx = S.ctx if on_device else nat.default_context()
-    if on_device:
-        if S.dtype != np.float32 or S.layout != "c":
-            raise ParameterError("device input must be a C-ordered float32 DeviceArray")
-        dev, req = S, np.dtype(np.float32)
-    else:
-        if not np.issubdtype(S.dtype, np.floating):
+    with pl.Scope(S) as sc:
+        if not on_device and not np.issubdtype(S.dtype, np.floating):
             S = S.astype(np.float32)
-        req = pl.check_real_dtype(S.dtype, "pcen input")
-        dev = ctx.to_device(np.ascontiguousarray(S, dtype=np.float32))
-    T = dev.shape[-1]
-    rows = dev.shape[-2] if ndim >= 2 else 1
-    lead = dev.shape[:-2] if ndim >= 2 else ()
-    n_lead = pl.clip_count(lead)
-    state_shape = dev.shape[:-1] + (1,)
-    d_zi = None
-    if zi is not None:
-        zi = np.asarray(zi, dtype=np.float64)
-        try:
-            zi_full = np.broadcast_to(zi, state_shape)
-        except ValueError as exc:
-            raise ValueError(f"zi has shape {zi.shape}, expected a shape broadcastable to {state_shape}") from exc
-        d_zi = ctx.to_device(np.ascontiguousarray(zi_full, dtype=np.float32))
-    d_zf = nat.DeviceArray.empty(ctx, state_shape, np.float32) if return_zf else None
-    out = nat.DeviceArray.empty(ctx, dev.shape, np.float32)
-    scratch = nat.DeviceArray.empty(ctx, dev.shape, np.float32) if max_size > 1 else None
-    desc = nat.PcenDesc(gain=float(gain), bias=float(bias), power=float(power), eps=float(eps), b=float(b),
-                        max_size=int(max_size))
-    nat.check(nat.lib().b2l_pcen(ctx.handle, C.byref(desc), _vp(dev.ptr), n_lead, rows, T,
-                                 _vp(d_zi.ptr if d_zi is not None else None),
-                                 _vp(d_zf.ptr if d_zf is not None else None),
-                                 _vp(scratch.ptr if scratch is not None else None), _vp(out.ptr)))
-    if scratch is not None:
-        scratch.free()
-    if d_zi is not None:
-        d_zi.free()
-    if on_device:
-        return (out, d_zf) if return_zf else out
-    dev.free()
-    res_dtype = np.result_type(req, np.float64)
-    res = pl.finish(out, res_dtype)
-    if return_zf:
-        return res, pl.finish(d_zf, res_dtype)
-    return res
+        dev, req = sc.spectrogram(S, "pcen input", stacklevel=5)
+        if dev.layout != "c":
+            raise ParameterError("device pcen input must be C-ordered")
+        T = dev.shape[-1]
+        rows = dev.shape[-2] if ndim >= 2 else 1
+        lead = dev.shape[:-2] if ndim >= 2 else ()
+        n_lead = pl.clip_count(lead)
+        state_shape = dev.shape[:-1] + (1,)
+        d_zi = None
+        if zi is not None:
+            zi = np.asarray(zi, dtype=np.float64)
+            try:
+                zi_full = np.broadcast_to(zi, state_shape)
+            except ValueError as exc:
+                raise ValueError(f"zi has shape {zi.shape}, expected a shape broadcastable to {state_shape}") from exc
+            d_zi = sc.stage(zi_full, np.float32)
+        d_zf = sc.empty(state_shape, np.float32) if return_zf else None
+        out = sc.empty(dev.shape, np.float32)
+        scratch = sc.empty(dev.shape, np.float32) if max_size > 1 else None
+        desc = nat.PcenDesc(gain=float(gain), bias=float(bias), power=float(power), eps=float(eps), b=float(b),
+                            max_size=int(max_size))
+        nat.check(nat.lib().b2l_pcen(sc.ctx.handle, C.byref(desc), _vp(dev.ptr), n_lead, rows, T,
+                                     _vp(d_zi.ptr if d_zi is not None else None),
+                                     _vp(d_zf.ptr if d_zf is not None else None),
+                                     _vp(scratch.ptr if scratch is not None else None), _vp(out.ptr)))
+        res_dtype = np.result_type(req, np.float64)
+        res = sc.result(out, res_dtype)
+        return (res, sc.result(d_zf, res_dtype)) if return_zf else res
 
 
 def reassigned_spectrogram(y, *, sr: float = 22050, S=None, n_fft: int = 2048, hop_length: Optional[int] = None,
@@ -529,42 +501,40 @@ def reassigned_spectrogram(y, *, sr: float = 22050, S=None, n_fft: int = 2048, h
         hop_length = int(win_length // 4)
     n, req = pl.precheck_signal(y)
     w = pad_center(filters.get_window(window, win_length, fftbins=True), size=n_fft)
-    staged = pl.StagedInput(y)
-    ctx, yd = staged.ctx, staged.dev
-    kw = dict(n_fft=n_fft, hop_length=hop_length, center=center, pad_mode=pad_mode)
-    if S is None:
-        Sh = stft(yd, window=w, **kw)
-    else:
-        Sh, _ = pl.to_native(np.asarray(S), np.complex64, host_transpose=True, ctx=ctx)
-    F, T = Sh.shape[-2], Sh.shape[-1]
-    staged.scan_uncovered(n_fft, hop_length, win_length, center, T)
-    Sdh = stft(yd, window=cyclic_gradient(w), **kw) if reassign_frequencies else None
-    Sth = None
-    if reassign_times:
-        half = n_fft // 2
-        window_times = np.arange(-half, half + 1) if n_fft % 2 else np.arange(0.5 - half, half)
-        Sth = stft(yd, window=w * window_times, **kw)
-    offset = 0 if center else int(n_fft // 2)
-    frame_times = (np.arange(T) * hop_length + offset).astype(int) / float(sr)
-    from .convert import fft_frequencies
+    with pl.Scope(y) as sc:
+        staged = pl.StagedInput(y)
+        ctx, yd = sc.ctx, sc.own(staged.dev)
+        kw = dict(n_fft=n_fft, hop_length=hop_length, center=center, pad_mode=pad_mode)
+        if S is None:
+            Sh = sc.own(stft(yd, window=w, **kw))
+        else:
+            Sh = sc.native(np.asarray(S), np.complex64, host_transpose=True)
+        F, T = Sh.shape[-2], Sh.shape[-1]
+        staged.scan_uncovered(n_fft, hop_length, win_length, center, T)
+        Sdh = sc.own(stft(yd, window=cyclic_gradient(w), **kw)) if reassign_frequencies else None
+        Sth = None
+        if reassign_times:
+            half = n_fft // 2
+            window_times = np.arange(-half, half + 1) if n_fft % 2 else np.arange(0.5 - half, half)
+            Sth = sc.own(stft(yd, window=w * window_times, **kw))
+        offset = 0 if center else int(n_fft // 2)
+        frame_times = (np.arange(T) * hop_length + offset).astype(int) / float(sr)
+        from .convert import fft_frequencies
 
-    d_bf = ctx.constant(("fftfreq", float(sr), int(n_fft)), lambda: fft_frequencies(sr=sr, n_fft=n_fft))
-    d_ft = ctx.constant(("frametimes", float(sr), int(hop_length), int(offset), int(T)), lambda: frame_times)
-    n_clips = pl.clip_count(Sh.shape[:-2])
-    outs = [nat.DeviceArray.empty(ctx, Sh.shape, np.float32, layout="ft") for _ in range(3)]
-    desc = nat.ReassignDesc(sr=float(sr), mag_threshold=float(ref_power) ** 0.5, max_time=float(n) / float(sr),
-                            reassign_frequencies=int(bool(reassign_frequencies)), reassign_times=int(bool(reassign_times)),
-                            apply_threshold=int(ref_power > 0), fill_nan=int(bool(fill_nan)), clip=int(bool(clip)))
-    nat.check(nat.lib().b2l_reassign(ctx.handle, C.byref(desc), _vp(Sh.ptr), _vp(Sdh.ptr if Sdh is not None else None),
-                                     _vp(Sth.ptr if Sth is not None else None), n_clips, T, F, _vp(d_bf), _vp(d_ft),
-                                     _vp(outs[0].ptr), _vp(outs[1].ptr), _vp(outs[2].ptr)))
-    for tmp in (Sh, Sdh, Sth):
-        if tmp is not None:
-            tmp.free()
-    if staged.on_device:
-        return tuple(outs)
-    wide = np.result_type(req, np.float64)
-    return staged.result(outs[0], wide), pl.finish(outs[1], wide), pl.finish(outs[2], req)
+        d_bf = ctx.constant(("fftfreq", float(sr), int(n_fft)), lambda: fft_frequencies(sr=sr, n_fft=n_fft))
+        d_ft = ctx.constant(("frametimes", float(sr), int(hop_length), int(offset), int(T)), lambda: frame_times)
+        n_clips = pl.clip_count(Sh.shape[:-2])
+        outs = [sc.empty(Sh.shape, np.float32, layout="ft") for _ in range(3)]
+        desc = nat.ReassignDesc(sr=float(sr), mag_threshold=float(ref_power) ** 0.5, max_time=float(n) / float(sr),
+                                reassign_frequencies=int(bool(reassign_frequencies)),
+                                reassign_times=int(bool(reassign_times)), apply_threshold=int(ref_power > 0),
+                                fill_nan=int(bool(fill_nan)), clip=int(bool(clip)))
+        nat.check(nat.lib().b2l_reassign(ctx.handle, C.byref(desc), _vp(Sh.ptr),
+                                         _vp(Sdh.ptr if Sdh is not None else None),
+                                         _vp(Sth.ptr if Sth is not None else None), n_clips, T, F, _vp(d_bf),
+                                         _vp(d_ft), _vp(outs[0].ptr), _vp(outs[1].ptr), _vp(outs[2].ptr)))
+        wide = np.result_type(req, np.float64)
+        return sc.result(outs[0], wide, validate=True), sc.result(outs[1], wide), sc.result(outs[2], req)
 
 
 class _Deprecated:
@@ -611,30 +581,25 @@ def phase_vocoder(D, *, rate: Optional[float] = None, t_out=None, kind="linear",
         res_dtype = np.dtype(D.dtype)
         if res_dtype == np.complex128 and not pl.wide_complex_ok("phase_vocoder input"):
             raise ParameterError("complex128 input refused (B2L_FLOAT64=error)")
-    src, own = pl.to_native(D, np.complex64, host_transpose=True)
-    ctx = src.ctx
-    F = D.shape[-2]
-    lead = tuple(D.shape[:-2])
-    n_clips = pl.clip_count(lead)
-    n_out = int(t_out.shape[0])
-    # phase increments: frames floor(t), floor(t) + 1 (:1498-1512); magnitudes: the segment scipy's interp1d
-    # picks — searchsorted(x, t) clipped to [1, n - 1], minus one — and the offset inside it (:1517-1527)
-    i0 = np.floor(t_out).astype(np.int32)
-    i1 = np.minimum(i0 + 1, n_frames - 1).astype(np.int32)
-    hi = np.clip(np.searchsorted(np.arange(n_frames, dtype=float), t_out), 1, n_frames - 1)
-    lo = (hi - 1).astype(np.int32)
-    dx = np.ascontiguousarray(t_out - lo, dtype=np.float64)
-    tables = [ctx.to_device(np.ascontiguousarray(a)) for a in (i0, i1, lo, dx)]
-    out = nat.DeviceArray.empty(ctx, lead + (F, n_out), np.complex64, layout="ft")
-    nat.check(nat.lib().b2l_phase_vocoder(ctx.handle, _vp(src.ptr), n_clips, n_frames, F, n_out, _vp(tables[0].ptr),
-                                          _vp(tables[1].ptr), _vp(tables[2].ptr), _vp(tables[3].ptr), _vp(out.ptr)))
-    for tb in tables:
-        tb.free()
-    if own:
-        src.free()
-    if on_device:
-        return out
-    return pl.finish(out, res_dtype)
+    with pl.Scope(D) as sc:
+        src = sc.native(D, np.complex64, host_transpose=True)
+        F = D.shape[-2]
+        lead = tuple(D.shape[:-2])
+        n_clips = pl.clip_count(lead)
+        n_out = int(t_out.shape[0])
+        # phase increments: frames floor(t), floor(t) + 1 (:1498-1512); magnitudes: the segment scipy's interp1d
+        # picks — searchsorted(x, t) clipped to [1, n - 1], minus one — and the offset inside it (:1517-1527)
+        i0 = np.floor(t_out).astype(np.int32)
+        i1 = np.minimum(i0 + 1, n_frames - 1).astype(np.int32)
+        hi = np.clip(np.searchsorted(np.arange(n_frames, dtype=float), t_out), 1, n_frames - 1)
+        lo = (hi - 1).astype(np.int32)
+        dx = np.ascontiguousarray(t_out - lo, dtype=np.float64)
+        tables = [sc.stage(a) for a in (i0, i1, lo, dx)]
+        out = sc.empty(lead + (F, n_out), np.complex64, layout="ft")
+        nat.check(nat.lib().b2l_phase_vocoder(sc.ctx.handle, _vp(src.ptr), n_clips, n_frames, F, n_out,
+                                              _vp(tables[0].ptr), _vp(tables[1].ptr), _vp(tables[2].ptr),
+                                              _vp(tables[3].ptr), _vp(out.ptr)))
+        return sc.result(out, res_dtype)
 
 
 def griffinlim(S, *, n_iter: int = 32, hop_length: Optional[int] = None, win_length: Optional[int] = None,
@@ -664,42 +629,40 @@ def griffinlim(S, *, n_iter: int = 32, hop_length: Optional[int] = None, win_len
     F, T = S.shape[-2], S.shape[-1]
     n_clips = pl.clip_count(S.shape[:-2])
     pl.require_supported_n_fft(n_fft, inverse=True)
-    ctx = pl.context_for(S)
-    L = nat.lib()
-    S_ft, _ = pl.to_native(S, np.float32, ctx=ctx)
-    S_host_shape = S.shape
-    if init == "random":
-        # same generator calls as the reference, so a given seed gives the same starting phases
-        ph = 2 * np.pi * rng.random(size=S_host_shape)
-        a0 = (np.cos(ph) + 1j * np.sin(ph)).astype(np.complex64)
-        a0 = a0 * (np.asarray(S.get()) if on_device else S.astype(np.float32))
-        angles, _ = pl.to_native(a0, np.complex64, ctx=ctx)
-    else:
-        angles = nat.DeviceArray.empty(ctx, S_host_shape, np.complex64, layout="ft")
-        ones, _ = pl.to_native(np.ones(S_host_shape, dtype=np.complex64), np.complex64, ctx=ctx)
-        nat.check(L.b2l_gl_update(ctx.handle, _vp(ones.ptr), None, _vp(S_ft.ptr), 0.0, 0.0, _vp(angles.ptr),
-                                  n_clips * F * T))
-    kw_i = dict(hop_length=hop_length, win_length=win_length, n_fft=n_fft, window=window, center=center, length=length)
-    kw_f = dict(n_fft=n_fft, hop_length=hop_length, win_length=win_length, window=window, center=center,
-                pad_mode=pad_mode)
-    scale = float(momentum / (1 + momentum))
-    tprev = None
-    for _ in range(int(n_iter)):
-        inverse = istft(angles, **kw_i)
-        rebuilt = stft(inverse, **kw_f)
-        inverse.free()
-        if tuple(rebuilt.shape) != tuple(S_host_shape):
-            # a `length` that does not correspond to T frames: the reference fails at `angles[:] = rebuilt`
-            # (core/spectrum.py:2884) with a broadcast error; the update kernel would run out of bounds
-            shape = tuple(rebuilt.shape)
-            rebuilt.free()
-            raise ParameterError(f"length={length} gives an STFT of shape {shape}, expected {tuple(S_host_shape)}")
-        nat.check(L.b2l_gl_update(ctx.handle, _vp(rebuilt.ptr), _vp(tprev.ptr) if tprev is not None else None,
-                                  _vp(S_ft.ptr), scale, eps, _vp(angles.ptr), n_clips * F * T))
-        if tprev is not None:
-            tprev.free()
-        tprev = rebuilt
-    y = istft(angles, **kw_i)
-    if on_device:
-        return y
-    return pl.finish(y, np.dtype(dtype) if dtype is not None else s_dtype)
+    with pl.Scope(S) as sc:
+        ctx = sc.ctx
+        L = nat.lib()
+        S_ft = sc.native(S, np.float32)
+        S_host_shape = S.shape
+        if init == "random":
+            # same generator calls as the reference, so a given seed gives the same starting phases
+            ph = 2 * np.pi * rng.random(size=S_host_shape)
+            a0 = (np.cos(ph) + 1j * np.sin(ph)).astype(np.complex64)
+            a0 = a0 * (np.asarray(S.get()) if on_device else S.astype(np.float32))
+            angles = sc.native(a0, np.complex64)
+        else:
+            angles = sc.empty(S_host_shape, np.complex64, layout="ft")
+            ones = sc.native(np.ones(S_host_shape, dtype=np.complex64), np.complex64)
+            nat.check(L.b2l_gl_update(ctx.handle, _vp(ones.ptr), None, _vp(S_ft.ptr), 0.0, 0.0, _vp(angles.ptr),
+                                      n_clips * F * T))
+        kw_i = dict(hop_length=hop_length, win_length=win_length, n_fft=n_fft, window=window, center=center,
+                    length=length)
+        kw_f = dict(n_fft=n_fft, hop_length=hop_length, win_length=win_length, window=window, center=center,
+                    pad_mode=pad_mode)
+        scale = float(momentum / (1 + momentum))
+        tprev = None
+        for _ in range(int(n_iter)):
+            inverse = sc.own(istft(angles, **kw_i))
+            rebuilt = sc.own(stft(inverse, **kw_f))
+            inverse.free()
+            if tuple(rebuilt.shape) != tuple(S_host_shape):
+                # a `length` that does not correspond to T frames: the reference fails at `angles[:] = rebuilt`
+                # (core/spectrum.py:2884) with a broadcast error; the update kernel would run out of bounds
+                raise ParameterError(f"length={length} gives an STFT of shape {tuple(rebuilt.shape)}, expected "
+                                     f"{tuple(S_host_shape)}")
+            nat.check(L.b2l_gl_update(ctx.handle, _vp(rebuilt.ptr), _vp(tprev.ptr) if tprev is not None else None,
+                                      _vp(S_ft.ptr), scale, eps, _vp(angles.ptr), n_clips * F * T))
+            if tprev is not None:
+                tprev.free()
+            tprev = rebuilt
+        return sc.result(istft(angles, **kw_i), np.dtype(dtype) if dtype is not None else s_dtype)

@@ -22,18 +22,20 @@ def _separate(y, want, *, kernel_size, power, mask, margin, n_fft, hop_length, w
     if mask:
         raise nat.UnsupportedOnGPU("effects.hpss(mask=True) inverts the masks themselves; not supported on the GPU")
     n, req = pl.precheck_signal(y)
-    staged = pl.StagedInput(y)
-    D = stft(staged.dev, n_fft=n_fft, hop_length=hop_length, win_length=win_length, center=center, pad_mode=pad_mode)
-    staged.scan_uncovered(n_fft, hop_length, win_length, center, D.shape[-1])
-    harm, perc = _hpss_device(D, kernel_size=kernel_size, power=power, mask=False, margin=margin)
-    D.free()
-    outs = []
-    for name, comp in (("harm", harm), ("perc", perc)):
-        if name in want:
-            yd_out = istft(comp, n_fft=n_fft, hop_length=hop_length, win_length=win_length, center=center, length=n)
-            outs.append(staged.result(yd_out, req))
-        comp.free()
-    return outs
+    with pl.Scope(y) as sc:
+        staged = pl.StagedInput(y)
+        D = sc.own(stft(sc.own(staged.dev), n_fft=n_fft, hop_length=hop_length, win_length=win_length, center=center,
+                        pad_mode=pad_mode))
+        staged.scan_uncovered(n_fft, hop_length, win_length, center, D.shape[-1])
+        harm, perc = _hpss_device(sc, D, kernel_size=kernel_size, power=power, mask=False, margin=margin)
+        D.free()
+        outs = []
+        for name, comp in (("harm", harm), ("perc", perc)):
+            if name in want:
+                yd_out = istft(comp, n_fft=n_fft, hop_length=hop_length, win_length=win_length, center=center, length=n)
+                outs.append(sc.result(yd_out, req, validate=True))
+            comp.free()
+        return outs
 
 
 def hpss(y, *, kernel_size=31, power: float = 2.0, mask: bool = False, margin=1.0, n_fft: int = 2048,
@@ -67,16 +69,15 @@ def time_stretch(y, *, rate: float, **kwargs):
     if rate <= 0:
         raise ParameterError("rate must be a positive number")
     n, req = pl.precheck_signal(y)
-    staged = pl.StagedInput(y)
-    D = stft(staged.dev, **kwargs)
-    staged.scan_uncovered(kwargs.get("n_fft", 2048), kwargs.get("hop_length"), kwargs.get("win_length"),
-                          kwargs.get("center", True), D.shape[-1])
-    # the reference forwards these two (deprecated, unused) arguments, so its call always warns; same here
-    Ds = phase_vocoder(D, rate=rate, hop_length=kwargs.get("hop_length"), n_fft=kwargs.get("n_fft"))
-    D.free()
-    out = istft(Ds, length=round(n / rate), **kwargs)
-    Ds.free()
-    return staged.result(out, req)
+    with pl.Scope(y) as sc:
+        staged = pl.StagedInput(y)
+        D = sc.own(stft(sc.own(staged.dev), **kwargs))
+        staged.scan_uncovered(kwargs.get("n_fft", 2048), kwargs.get("hop_length"), kwargs.get("win_length"),
+                              kwargs.get("center", True), D.shape[-1])
+        # the reference forwards these two (deprecated, unused) arguments, so its call always warns; same here
+        Ds = sc.own(phase_vocoder(D, rate=rate, hop_length=kwargs.get("hop_length"), n_fft=kwargs.get("n_fft")))
+        D.free()
+        return sc.result(istft(Ds, length=round(n / rate), **kwargs), req, validate=True)
 
 
 def pitch_shift(y, *, sr: float, n_steps: float, bins_per_octave: int = 12, res_type: str = "soxr_hq",
@@ -93,27 +94,21 @@ def pitch_shift(y, *, sr: float, n_steps: float, bins_per_octave: int = 12, res_
         raise ParameterError(f"bins_per_octave={bins_per_octave} must be a positive integer.")
     rate = 2.0 ** (-float(n_steps) / bins_per_octave)
     n, req = pl.precheck_signal(y)
-    staged = pl.StagedInput(y)
-    staged.scan_all()
-    stretched = time_stretch(staged.dev, rate=rate, **kwargs)
-    try:
-        shifted = resample(stretched, orig_sr=float(sr) / rate, target_sr=sr, res_type=res_type, scale=scale)
-    finally:
+    with pl.Scope(y) as sc:
+        staged = pl.StagedInput(y)
+        staged.scan_all()
+        stretched = sc.own(time_stretch(sc.own(staged.dev), rate=rate, **kwargs))
+        shifted = sc.own(resample(stretched, orig_sr=float(sr) / rate, target_sr=sr, res_type=res_type, scale=scale))
         stretched.free()
-        if "shifted" not in locals():
-            staged.release()
-    # util.fix_length(y_shift, size=y.shape[-1]) on the device
-    m = shifted.shape[-1]
-    if m == n:
-        out = shifted
-    else:
-        ctx = shifted.ctx
-        lead = shifted.shape[:-1]
-        rows = pl.clip_count(lead)
-        out = (ctx.zeros if m < n else ctx.empty)(tuple(lead) + (n,), np.float32)
-        if rows and min(m, n):
-            nat.check(nat.lib().b2l_copy2d(ctx.handle, C.c_void_p(out.ptr), n * 4, C.c_void_p(shifted.ptr), m * 4,
-                                           min(m, n) * 4, rows))
-        shifted.free()
-    staged.release()
-    return staged.result(out, req)
+        # util.fix_length(y_shift, size=y.shape[-1]) on the device
+        m = shifted.shape[-1]
+        if m == n:
+            out = shifted
+        else:
+            lead = shifted.shape[:-1]
+            rows = pl.clip_count(lead)
+            out = (sc.zeros if m < n else sc.empty)(tuple(lead) + (n,), np.float32)
+            if rows and min(m, n):
+                nat.check(nat.lib().b2l_copy2d(sc.ctx.handle, C.c_void_p(out.ptr), n * 4, C.c_void_p(shifted.ptr),
+                                               m * 4, min(m, n) * 4, rows))
+        return sc.result(out, req, validate=True)

@@ -52,7 +52,6 @@ def mel_to_stft(M, *, sr: float = 22050, n_fft: int = 2048, power: float = 2.0, 
         raise ParameterError("mel spectrogram must have at least two dimensions (n_mels, frames)")
     if not (power > 0):
         raise ParameterError(f"power={power} must be strictly positive")
-    req = np.dtype(np.float32) if on_device else pl.check_real_dtype(M.dtype, "mel_to_stft input")
     n_mels, T = M.shape[-2], M.shape[-1]
     kwargs.pop("dtype", None)
     try:
@@ -60,23 +59,16 @@ def mel_to_stft(M, *, sr: float = 22050, n_fft: int = 2048, power: float = 2.0, 
     except TypeError:   # unhashable kwarg
         basis, pinv, step = _nnls_constants.__wrapped__(float(sr), int(n_fft), int(n_mels), tuple(kwargs.items()))
     F = basis.shape[1]
-    ctx = M.ctx if on_device else nat.default_context()
-    if on_device:
-        if M.dtype != np.float32 or M.layout != "c":
-            raise ParameterError("device mel spectrogram must be C-ordered float32")
-        Md = M
-    else:
-        Md = ctx.to_device(np.ascontiguousarray(M, dtype=np.float32))
-    lead = tuple(M.shape[:-2])
-    out = nat.DeviceArray.empty(ctx, lead + (F, T), np.float32)
-    nat.check(nat.lib().b2l_nnls_mel(ctx.handle, _vp(Md.ptr), pl.clip_count(lead), T, n_mels, F,
-                                     basis.ctypes.data_as(_fp), pinv.ctypes.data_as(_fp), float(step), NNLS_ITERATIONS,
-                                     float(1.0 / power), _vp(out.ptr)))
-    if on_device:
-        return out
-    res = pl.finish(out, req)
-    Md.free()
-    return res
+    with pl.Scope(M) as sc:
+        Md, req = sc.spectrogram(M, "mel_to_stft input", stacklevel=5)
+        if Md.layout != "c":
+            raise ParameterError("device mel spectrogram must be C-ordered")
+        lead = tuple(M.shape[:-2])
+        out = sc.empty(lead + (F, T), np.float32)
+        nat.check(nat.lib().b2l_nnls_mel(sc.ctx.handle, _vp(Md.ptr), pl.clip_count(lead), T, n_mels, F,
+                                         basis.ctypes.data_as(_fp), pinv.ctypes.data_as(_fp), float(step),
+                                         NNLS_ITERATIONS, float(1.0 / power), _vp(out.ptr)))
+        return sc.result(out, req)
 
 
 def mel_to_audio(M, *, sr: float = 22050, n_fft: int = 2048, hop_length: Optional[int] = None,
@@ -119,28 +111,19 @@ def mfcc_to_mel(mfcc, *, n_mels: int = 128, dct_type: int = 2, norm="ortho", ref
         raise ParameterError("MFCC to mel lifter must be a non-negative number.")
     n_mfcc, T = mfcc.shape[-2], mfcc.shape[-1]
     basis = _idct_basis(n_mfcc, n_mels, dct_type, norm, lifter, np.float32 if on_device else mfcc.dtype)
-    req = np.dtype(np.float32) if on_device else pl.check_real_dtype(mfcc.dtype, "mfcc_to_mel input")
-    ctx = mfcc.ctx if on_device else nat.default_context()
-    if on_device:
-        if mfcc.dtype != np.float32 or mfcc.layout != "c":
-            raise ParameterError("device mfcc must be C-ordered float32")
-        Cd = mfcc
-    else:
-        Cd = ctx.to_device(np.ascontiguousarray(mfcc, dtype=np.float32))
-    # the matrix product runs on the DCT kernel: "mel rows" = n_mfcc inputs, "coefficients" = n_mels outputs
-    plan = nat.make_plan(ctx, ("idct", n_mfcc, pl.digest(basis)), n_fft=8, hop_length=1, center=True,
-                         pad_mode="constant", window=np.ones(8),
-                         mel_basis=np.zeros((n_mfcc, 5), dtype=np.float32), dct_basis=basis)
-    lead = tuple(mfcc.shape[:-2])
-    logmel = nat.DeviceArray.empty(ctx, lead + (n_mels, T), np.float32)
-    nat.check(nat.lib().b2l_dct_project(ctx.handle, plan.handle, _vp(Cd.ptr), pl.clip_count(lead), T,
-                                        _vp(logmel.ptr)))
-    mel = db_to_power(logmel, ref=ref)
-    logmel.free()
-    if on_device:
-        return mel
-    Cd.free()
-    return pl.finish(mel, req)
+    with pl.Scope(mfcc) as sc:
+        Cd, req = sc.spectrogram(mfcc, "mfcc_to_mel input", stacklevel=5)
+        if Cd.layout != "c":
+            raise ParameterError("device mfcc must be C-ordered")
+        # the matrix product runs on the DCT kernel: "mel rows" = n_mfcc inputs, "coefficients" = n_mels outputs
+        plan = nat.make_plan(sc.ctx, ("idct", n_mfcc, pl.digest(basis)), n_fft=8, hop_length=1, center=True,
+                             pad_mode="constant", window=np.ones(8),
+                             mel_basis=np.zeros((n_mfcc, 5), dtype=np.float32), dct_basis=basis)
+        lead = tuple(mfcc.shape[:-2])
+        logmel = sc.empty(lead + (n_mels, T), np.float32)
+        nat.check(nat.lib().b2l_dct_project(sc.ctx.handle, plan.handle, _vp(Cd.ptr), pl.clip_count(lead), T,
+                                            _vp(logmel.ptr)))
+        return sc.result(db_to_power(logmel, ref=ref), req)
 
 
 def mfcc_to_audio(mfcc, *, n_mels: int = 128, dct_type: int = 2, norm="ortho", ref: float = 1.0, lifter: float = 0,

@@ -163,7 +163,7 @@ def tempo(*, y=None, sr: float = 22050, onset_envelope=None, tg=None, hop_length
         else:
             tg = np.asarray(tg)
             dtype = tg.dtype if tg.dtype in (np.float32, np.float64) else np.dtype(np.float64)
-            d_tg = sc.own(pl.to_native(tg, dtype=dtype, host_transpose=True)[0])
+            d_tg = sc.native(tg, dtype=dtype, host_transpose=True)
         ctx = sc.ctx
         lead, F = d_tg.shape[:-2], d_tg.shape[-1]
         mean = aggregate is not None

@@ -29,22 +29,21 @@ def melspectrogram(*, y=None, sr: float = 22050, S=None, n_fft: int = 2048, hop_
     ``librosa.feature.melspectrogram``.  ``kwargs`` go to ``filters.mel`` (n_mels, fmin, fmax, htk, norm, dtype)."""
     if S is not None:
         # mel_basis . S for a caller-supplied spectrogram (feature/spectral.py:2158-2160)
-        Sd, req, on_device = pl.spectrogram_input(S)
-        F, T = Sd.shape[-2], Sd.shape[-1]
-        if n_fft is None or n_fft // 2 + 1 != F:
-            n_fft = 2 * (F - 1)
-        basis, bkey = pl.mel_basis(sr, n_fft, kwargs)
-        ctx = Sd.ctx
-        plan = nat.make_plan(ctx, ("melproj", n_fft, bkey), n_fft=n_fft, hop_length=1, center=True,
-                             pad_mode="constant", window=np.ones(n_fft), mel_basis=basis)
-        lead = Sd.shape[:-2]
-        src, own = pl.to_native(Sd)
-        out = nat.DeviceArray.empty(ctx, lead + (basis.shape[0], T), np.float32)
-        nat.check(nat.lib().b2l_mel_project(ctx.handle, plan.handle, _vp(src.ptr), pl.clip_count(lead), T,
-                                            _vp(out.ptr)))
-        if own:
-            src.free()
-        return out if on_device else pl.finish(out, np.result_type(req, basis.dtype))
+        with pl.Scope(S) as sc:
+            Sd, req = sc.spectrogram(S)
+            F, T = Sd.shape[-2], Sd.shape[-1]
+            if n_fft is None or n_fft // 2 + 1 != F:
+                n_fft = 2 * (F - 1)
+            basis, bkey = pl.mel_basis(sr, n_fft, kwargs)
+            ctx = sc.ctx
+            plan = nat.make_plan(ctx, ("melproj", n_fft, bkey), n_fft=n_fft, hop_length=1, center=True,
+                                 pad_mode="constant", window=np.ones(n_fft), mel_basis=basis)
+            lead = Sd.shape[:-2]
+            src = sc.native(Sd)
+            out = sc.empty(lead + (basis.shape[0], T), np.float32)
+            nat.check(nat.lib().b2l_mel_project(ctx.handle, plan.handle, _vp(src.ptr), pl.clip_count(lead), T,
+                                                _vp(out.ptr)))
+            return sc.result(out, np.result_type(req, basis.dtype))
     if n_fft is None:
         raise ParameterError(f"Unable to compute spectrogram with n_fft={n_fft}")
     if y is None:
@@ -53,8 +52,8 @@ def melspectrogram(*, y=None, sr: float = 22050, S=None, n_fft: int = 2048, hop_
     basis, bkey = pl.mel_basis(sr, n_fft, kwargs)
     res_dtype = np.result_type(fr.dtype, basis.dtype)
     if pl.wide_route(y, fr.dtype, n_fft):
-        staged, mel_d = _mel_f64(y, n_fft, fr, center, power, basis)
-        return staged.result(mel_d, res_dtype)
+        with pl.Scope(y) as sc:
+            return sc.result(_mel_f64(sc, y, n_fft, fr, center, power, basis), res_dtype, validate=True)
     pl.require_supported_n_fft(n_fft)
     if not pl.fused_front_end(n_fft):
         # chirp-z frames: |STFT|**power on the device, then the band-sparse projection (two kernels)
@@ -73,15 +72,15 @@ def melspectrogram(*, y=None, sr: float = 22050, S=None, n_fft: int = 2048, hop_
     return res if isinstance(res, nat.DeviceArray) or res.dtype == res_dtype else res.astype(res_dtype)
 
 
-def _mel_f64(y, n_fft, fr, center, power, basis):
+def _mel_f64(sc, y, n_fft, fr, center, power, basis):
     """float64 signal -> float64 mel spectrogram on the device in FP64: stft, |.|**power, band projection
-    (feature/spectral.py:2145-2160 in the input's precision).  Returns (StagedInput, DeviceArray)."""
-    staged, D = f64.stft(y, n_fft=n_fft, hop_length=fr.hop, center=center, mode=fr.mode, win=fr.window)
-    Sd = f64.abs_pow(staged.ctx, D, power)
+    (feature/spectral.py:2145-2160 in the input's precision), owned by the scope ``sc`` of ``y``."""
+    _, D = f64.stft(y, n_fft=n_fft, hop_length=fr.hop, center=center, mode=fr.mode, win=fr.window)
+    Sd = sc.own(f64.abs_pow(sc.ctx, sc.own(D), power))
     D.free()
-    mel_d = f64.mel(staged.ctx, Sd, basis)
+    mel_d = sc.own(f64.mel(sc.ctx, Sd, basis))
     Sd.free()
-    return staged, mel_d
+    return mel_d
 
 
 def _compose_nonpow2(y, tail, res_dtype, **spec_kw):
@@ -107,60 +106,54 @@ def chroma_stft(*, y=None, sr: float = 22050, S=None, norm=np.inf, n_fft: int = 
     from ..core.pitch import _tuning_from_device_spec
     from ..core.spectrum import _spectrogram
 
-    staged = None
-    if S is None:
-        if y is None:
-            raise ParameterError("Input signal must be provided to compute a spectrogram")
-        _, req = pl.precheck_signal(y)
-        staged = pl.StagedInput(y)
-        Sd, n_fft = _spectrogram(y=staged.dev, n_fft=n_fft, hop_length=hop_length, power=2, win_length=win_length,
-                                 window=window, center=center, pad_mode=pad_mode)
-        staged.scan_uncovered(n_fft, hop_length, win_length, center, Sd.shape[-1])
-        src, own = Sd, True
-    else:
-        Sd, req, on_device = pl.spectrogram_input(S)
-        if n_fft is None or n_fft // 2 + 1 != Sd.shape[-2]:
-            n_fft = 2 * (Sd.shape[-2] - 1)
-        src, own = pl.to_native(Sd)
-    ctx = src.ctx
-    F, T = src.shape[-2], src.shape[-1]
-    lead = src.shape[:-2]
-    n_clips = pl.clip_count(lead)
-    L = nat.lib()
-    try:
+    with pl.Scope(y if S is None else S) as sc:
+        if S is None:
+            if y is None:
+                raise ParameterError("Input signal must be provided to compute a spectrogram")
+            _, req = pl.precheck_signal(y)
+            staged = pl.StagedInput(y)
+            sc.own(staged.dev)
+            Sd, n_fft = _spectrogram(y=staged.dev, n_fft=n_fft, hop_length=hop_length, power=2, win_length=win_length,
+                                     window=window, center=center, pad_mode=pad_mode)
+            staged.scan_uncovered(n_fft, hop_length, win_length, center, Sd.shape[-1])
+            src = sc.own(Sd)
+        else:
+            Sd, req = sc.spectrogram(S)
+            if n_fft is None or n_fft // 2 + 1 != Sd.shape[-2]:
+                n_fft = 2 * (Sd.shape[-2] - 1)
+            src = sc.native(Sd)
+        ctx = sc.ctx
+        F, T = src.shape[-2], src.shape[-1]
+        lead = src.shape[:-2]
+        n_clips = pl.clip_count(lead)
+        L = nat.lib()
         if tuning is None:
-            tuning = _tuning_from_device_spec(ctx, src, sr, n_fft, resolution=0.01, bins_per_octave=n_chroma,
-                                              fmin=150.0, fmax=4000.0, threshold=0.1, ref=None)
+            tuning = _tuning_from_device_spec(src, sr, n_fft, resolution=0.01, bins_per_octave=n_chroma, fmin=150.0,
+                                              fmax=4000.0, threshold=0.1, ref=None)
         fb = filters.chroma(sr=sr, n_fft=n_fft, tuning=tuning, n_chroma=n_chroma, **kwargs)
         if fb.shape[1] != F:
             raise ParameterError(f"chroma filter bank has {fb.shape[1]} bins, the spectrogram {F}")
         plan = nat.make_plan(ctx, ("chroma", n_fft, pl.digest(fb)), n_fft=n_fft, hop_length=1, center=True,
                              pad_mode="constant", window=np.ones(n_fft), mel_basis=fb)
-        raw = nat.DeviceArray.empty(ctx, tuple(lead) + (fb.shape[0], T), np.float32)
+        raw = sc.empty(tuple(lead) + (fb.shape[0], T), np.float32)
         nat.check(L.b2l_mel_project(ctx.handle, plan.handle, _vp(src.ptr), n_clips, T, _vp(raw.ptr)))
-    finally:
-        if own:
-            src.free()
-    if norm is None:
-        out = raw
-    else:
-        if norm == np.inf:
-            kind, p = 0, 0.0
-        elif norm == -np.inf:
-            kind, p = 1, 0.0
-        elif norm == 0:
-            kind, p = 2, 0.0
-        elif np.issubdtype(type(norm), np.number) and norm > 0:
-            kind, p = 3, float(norm)
+        sc.free(src)
+        if norm is None:
+            out = raw
         else:
-            raise ParameterError(f"Unsupported norm: {repr(norm)}")
-        out = nat.DeviceArray.empty(ctx, raw.shape, np.float32)
-        nat.check(L.b2l_normalize_rows(ctx.handle, _vp(raw.ptr), n_clips, fb.shape[0], T, kind, p, _vp(out.ptr)))
-        raw.free()
-    res_dtype = np.result_type(req, fb.dtype)
-    if staged is not None:
-        return staged.result(out, res_dtype)
-    return out if on_device else pl.finish(out, res_dtype)
+            if norm == np.inf:
+                kind, p = 0, 0.0
+            elif norm == -np.inf:
+                kind, p = 1, 0.0
+            elif norm == 0:
+                kind, p = 2, 0.0
+            elif np.issubdtype(type(norm), np.number) and norm > 0:
+                kind, p = 3, float(norm)
+            else:
+                raise ParameterError(f"Unsupported norm: {repr(norm)}")
+            out = sc.empty(raw.shape, np.float32)
+            nat.check(L.b2l_normalize_rows(ctx.handle, _vp(raw.ptr), n_clips, fb.shape[0], T, kind, p, _vp(out.ptr)))
+        return sc.result(out, np.result_type(req, fb.dtype), validate=S is None)
 
 
 def _dct_basis(n_mels: int, n_mfcc: int, dct_type: int, norm, lifter: float, dtype=np.float32) -> np.ndarray:
@@ -182,20 +175,20 @@ def mfcc(*, y=None, sr: float = 22050, S=None, n_mfcc: int = 20, dct_type: int =
     if not (lifter >= 0):   # also catches NaN, like the reference's final else-branch
         raise ParameterError(f"MFCC lifter={lifter} must be a non-negative number")
     if S is not None:
-        Sd, req, on_device = pl.spectrogram_input(S)
-        if Sd.layout != "c":
-            raise ParameterError("device log-mel input must be C-ordered (..., n_mels, frames)")
-        ctx = Sd.ctx
-        n_mels, T = Sd.shape[-2], Sd.shape[-1]
-        dct = _dct_basis(n_mels, n_mfcc, dct_type, norm, lifter)
-        plan = nat.make_plan(ctx, ("dct", n_mels, pl.digest(dct)), n_fft=8, hop_length=1, center=True,
-                             pad_mode="constant", window=np.ones(8),
-                             mel_basis=np.zeros((n_mels, 5), dtype=np.float32), dct_basis=dct)
-        lead = Sd.shape[:-2]
-        out = nat.DeviceArray.empty(ctx, lead + (dct.shape[0], T), np.float32)
-        nat.check(nat.lib().b2l_dct_project(ctx.handle, plan.handle, _vp(Sd.ptr), pl.clip_count(lead), T,
-                                            _vp(out.ptr)))
-        return out if on_device else pl.finish(out, req)
+        with pl.Scope(S) as sc:
+            Sd, req = sc.spectrogram(S)
+            if Sd.layout != "c":
+                raise ParameterError("device log-mel input must be C-ordered (..., n_mels, frames)")
+            n_mels, T = Sd.shape[-2], Sd.shape[-1]
+            dct = _dct_basis(n_mels, n_mfcc, dct_type, norm, lifter)
+            plan = nat.make_plan(sc.ctx, ("dct", n_mels, pl.digest(dct)), n_fft=8, hop_length=1, center=True,
+                                 pad_mode="constant", window=np.ones(8),
+                                 mel_basis=np.zeros((n_mels, 5), dtype=np.float32), dct_basis=dct)
+            lead = Sd.shape[:-2]
+            out = sc.empty(lead + (dct.shape[0], T), np.float32)
+            nat.check(nat.lib().b2l_dct_project(sc.ctx.handle, plan.handle, _vp(Sd.ptr), pl.clip_count(lead), T,
+                                                _vp(out.ptr)))
+            return sc.result(out, req)
     # y path: fused stft -> |.|^power -> mel -> dB (+ per-clip max), then clamp + DCT
     n_fft = kwargs.pop("n_fft", 2048)
     hop_length = kwargs.pop("hop_length", 512)
@@ -217,12 +210,13 @@ def mfcc(*, y=None, sr: float = 22050, S=None, n_mfcc: int = 20, dct_type: int =
     if pl.wide_route(y, fr.dtype, n_fft):
         # float64 signal (or a frame length only the FP64 kernels cover): mel -> power_to_db (ref 1.0, amin 1e-10,
         # top_db 80) -> DCT, all in FP64
-        staged, mel_d = _mel_f64(y, n_fft, fr, center, power, basis)
-        db_d = f64.power_to_db(staged.ctx, mel_d, ref_value=1.0, amin=1e-10, top_db=80.0)
-        mel_d.free()
-        out = f64.dct(staged.ctx, db_d, _dct_basis(n_mels, n_mfcc, dct_type, norm, lifter, dtype=np.float64))
-        db_d.free()
-        return staged.result(out, res_dtype)
+        with pl.Scope(y) as sc:
+            mel_d = _mel_f64(sc, y, n_fft, fr, center, power, basis)
+            db_d = sc.own(f64.power_to_db(sc.ctx, mel_d, ref_value=1.0, amin=1e-10, top_db=80.0))
+            mel_d.free()
+            out = sc.own(f64.dct(sc.ctx, db_d, _dct_basis(n_mels, n_mfcc, dct_type, norm, lifter, dtype=np.float64)))
+            db_d.free()
+            return sc.result(out, res_dtype, validate=True)
     dct = _dct_basis(n_mels, n_mfcc, dct_type, norm, lifter)
     pl.require_supported_n_fft(n_fft)
     if not pl.fused_front_end(n_fft):

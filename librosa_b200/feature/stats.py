@@ -43,54 +43,51 @@ def _desc(row, *, roll_percent=0.85, amin=1e-10, power=2.0, p=2.0, norm=True, fr
                          bw_p=float(p), bw_norm=int(bool(norm)), frame_length=int(frame_length), want=1 << row)
 
 
-def _take_row(ctx, stats, lead, T, row, on_device, res_dtype):
-    """Row ``row`` of a [clip][N_STATS][T] block -> array of shape lead + (1, T)."""
+def _take_row(sc, stats, row, res_dtype):
+    """Row ``row`` of a stats block (..., N_STATS, T) -> array of shape (..., 1, T)."""
+    lead, T = tuple(stats.shape[:-2]), stats.shape[-1]
     n_clips = pl.clip_count(lead)
     if isinstance(stats, np.ndarray):
-        out = stats.reshape(n_clips, nat.N_STATS, T)[:, row:row + 1, :].reshape(tuple(lead) + (1, T))
+        out = stats.reshape(n_clips, nat.N_STATS, T)[:, row:row + 1, :].reshape(lead + (1, T))
         return np.ascontiguousarray(out).astype(res_dtype, copy=False)
-    dst = nat.DeviceArray.empty(ctx, tuple(lead) + (1, T), np.float32)
+    dst = sc.empty(lead + (1, T), np.float32)
     if n_clips and T:
-        nat.check(nat.lib().b2l_copy2d(ctx.handle, _vp(dst.ptr), T * 4, _vp(stats.ptr + row * T * 4),
+        nat.check(nat.lib().b2l_copy2d(sc.ctx.handle, _vp(dst.ptr), T * 4, _vp(stats.ptr + row * T * 4),
                                        nat.N_STATS * T * 4, T * 4, n_clips))
-    stats.free()                      # stream-ordered pool: safe right after the copy has been enqueued
-    return dst if on_device else pl.finish(dst, res_dtype)
+    stats.free()                      # this call's own block; stream-ordered pool: safe once the copy is enqueued
+    return sc.result(dst, res_dtype)
 
 
-def _stats_from_S(S, desc, freq, sr, n_fft, what, check_negative=True):
-    """S= form: stats_kernel over a stored spectrogram.  Returns (stats block, ctx, lead, T, on_device,
-    S dtype, freq dtype).  ``check_negative``: fetch the kernel's "negative entry" verdict and raise like the
-    reference (skipped for spectrograms this package has just computed itself)."""
+def _stats_from_S(sc, S, desc, freq, sr, n_fft, what, check_negative=True):
+    """S= form: stats_kernel over a stored spectrogram.  Returns (stats block (..., N_STATS, T), S dtype, freq
+    dtype).  ``check_negative``: fetch the kernel's "negative entry" verdict and raise like the reference (skipped
+    for spectrograms this package has just computed itself)."""
     if not isinstance(S, nat.DeviceArray) and np.iscomplexobj(S):
         raise ParameterError(f"{what} is only defined with real-valued input")
-    ctx = pl.context_for(S)
     if check_negative:
-        nat.check(nat.lib().b2l_status_reset(ctx.handle))
-    Sd, req, on_device = pl.spectrogram_input(S)
+        nat.check(nat.lib().b2l_status_reset(sc.ctx.handle))
+    Sd, req = sc.spectrogram(S)
     if Sd.ndim < 2:
         raise ParameterError("spectrogram input must have at least two dimensions")
     F, T = Sd.shape[-2], Sd.shape[-1]
     if n_fft is None or n_fft // 2 + 1 != F:
         n_fft = 2 * (F - 1)
     table, fkey, fdtype = _freq_table(freq, sr, n_fft, F)
-    d_freq = ctx.constant(fkey, lambda: table)
+    d_freq = sc.ctx.constant(fkey, lambda: table)
     lead = Sd.shape[:-2]
-    src, own = pl.to_native(Sd)
-    stats = nat.DeviceArray.empty(ctx, tuple(lead) + (nat.N_STATS, T), np.float32)
-    nat.check(nat.lib().b2l_spectral_stats_from_spec(ctx.handle, C.byref(desc), _vp(src.ptr), pl.clip_count(lead), T,
-                                                     F, _vp(d_freq), _vp(stats.ptr)))
-    if own:
-        src.free()
-    if not on_device:
-        Sd.free()
-    if check_negative and pl.status_word(ctx) & nat.STATUS_NEGATIVE_ENTRY:
-        stats.free()
+    src = sc.native(Sd)
+    stats = sc.empty(tuple(lead) + (nat.N_STATS, T), np.float32)
+    nat.check(nat.lib().b2l_spectral_stats_from_spec(sc.ctx.handle, C.byref(desc), _vp(src.ptr), pl.clip_count(lead),
+                                                     T, F, _vp(d_freq), _vp(stats.ptr)))
+    sc.free(src, Sd)
+    if check_negative and pl.status_word(sc.ctx) & nat.STATUS_NEGATIVE_ENTRY:
         raise ParameterError(f"{what} is only defined with non-negative energies")
-    return stats, ctx, lead, T, on_device, req, fdtype
+    return stats, req, fdtype
 
 
-def _stats_from_y(y, desc, freq, sr, *, n_fft, hop_length, win_length, window, center, pad_mode, what):
-    """y= form: the fused kernel (power-of-two n_fft) or chirp-z spectrogram + stats_kernel."""
+def _stats_from_y(sc, y, desc, freq, sr, *, n_fft, hop_length, win_length, window, center, pad_mode, what):
+    """y= form: the fused kernel (power-of-two n_fft) or chirp-z spectrogram + stats_kernel.  Returns (stats block
+    (..., N_STATS, T), signal dtype, freq dtype)."""
     if n_fft is None:
         raise ParameterError(f"Unable to compute spectrogram with n_fft={n_fft}")
     if y is None:
@@ -101,18 +98,12 @@ def _stats_from_y(y, desc, freq, sr, *, n_fft, hop_length, win_length, window, c
     if not pl.is_pow2(n_fft):
         from .spectral import _compose_nonpow2
 
-        box = {}
-
         def tail(Sd):
-            stats, ctx, lead, T_, _, _, _ = _stats_from_S(Sd, desc, freq, sr, n_fft, what, check_negative=False)
-            box["v"] = (ctx, lead, T_)
-            return stats
+            return _stats_from_S(sc, Sd, desc, freq, sr, n_fft, what, check_negative=False)[0]
 
-        on_device = isinstance(y, nat.DeviceArray)
         stats = _compose_nonpow2(y, tail, np.float32, n_fft=n_fft, hop_length=fr.hop, power=1, win_length=win_length,
                                  window=window, center=center, pad_mode=pad_mode)
-        ctx, lead, T_ = box["v"]
-        return stats, ctx, lead, T_, on_device, fr.dtype, fdtype
+        return stats, fr.dtype, fdtype
 
     def launch(ctx, plan, d_in, m, n_, d_out, d_scr):
         nat.check(nat.lib().b2l_spectral_stats(ctx.handle, plan.handle, C.byref(desc), _vp(d_in), m, n_, n_,
@@ -123,18 +114,18 @@ def _stats_from_y(y, desc, freq, sr, *, n_fft, hop_length, win_length, window, c
                            plan_kw=dict(n_fft=n_fft, hop_length=fr.hop, center=center, pad_mode=fr.mode,
                                         window=fr.window, power=1.0),
                            n_frames=T, out_tail=(nat.N_STATS, T), dtype=np.float32, launch=launch)
-    on_device = isinstance(y, nat.DeviceArray)
-    return stats, pl.context_for(y), tuple(y.shape[:-1]), T, on_device, fr.dtype, fdtype
+    return stats, fr.dtype, fdtype
 
 
 def _statistic(row, what, desc, res_of, *, y, S, sr, n_fft, hop_length, freq, win_length, window, center, pad_mode):
-    if S is not None:
-        stats, ctx, lead, T, on_device, sdt, fdt = _stats_from_S(S, desc, freq, sr, n_fft, what)
-    else:
-        stats, ctx, lead, T, on_device, sdt, fdt = _stats_from_y(
-            y, desc, freq, sr, n_fft=n_fft, hop_length=hop_length, win_length=win_length, window=window,
-            center=center, pad_mode=pad_mode, what=what)
-    return _take_row(ctx, stats, lead, T, row, on_device, res_of(sdt, fdt))
+    with pl.Scope(y if S is None else S) as sc:
+        if S is not None:
+            stats, sdt, fdt = _stats_from_S(sc, S, desc, freq, sr, n_fft, what)
+        else:
+            stats, sdt, fdt = _stats_from_y(sc, y, desc, freq, sr, n_fft=n_fft, hop_length=hop_length,
+                                            win_length=win_length, window=window, center=center, pad_mode=pad_mode,
+                                            what=what)
+        return _take_row(sc, stats, row, res_of(sdt, fdt))
 
 
 def spectral_centroid(*, y=None, sr: float = 22050, S=None, n_fft: int = 2048, hop_length: int = 512, freq=None,
@@ -213,71 +204,64 @@ def spectral_contrast(*, y=None, sr: float = 22050, S=None, n_fft: int = 2048, h
     any increasing ``freq``)."""
     from ..core.spectrum import _spectrogram, power_to_db
 
-    staged = None
-    if S is None:
-        if y is None:
-            raise ParameterError("Input signal must be provided to compute a spectrogram")
-        _, req = pl.precheck_signal(y)
-        staged = pl.StagedInput(y)
-        Sd, n_fft = _spectrogram(y=staged.dev, n_fft=n_fft, hop_length=hop_length, power=1, win_length=win_length,
-                                 window=window, center=center, pad_mode=pad_mode)
-        staged.scan_uncovered(n_fft, hop_length, win_length, center, Sd.shape[-1])
-        own_S = True
-    else:
-        if not isinstance(S, nat.DeviceArray) and np.iscomplexobj(S):
-            raise nat.UnsupportedOnGPU("spectral_contrast of a complex S is not supported on the GPU: pass np.abs(S)")
-        Sd, req, on_device = pl.spectrogram_input(S)
-        own_S = not on_device
-        if n_fft is None or n_fft // 2 + 1 != Sd.shape[-2]:
-            n_fft = 2 * (Sd.shape[-2] - 1)
-    ctx = Sd.ctx
-    F, T = Sd.shape[-2], Sd.shape[-1]
-    if freq is None:
-        freq = fft_frequencies(sr=sr, n_fft=n_fft)
-    freq = np.atleast_1d(freq)
-    if freq.ndim != 1 or len(freq) != F:
-        raise ParameterError(f"freq.shape mismatch: expected ({F:d},)")
-    if n_bands < 1 or not isinstance(n_bands, (int, np.integer)):
-        raise ParameterError("n_bands must be a positive integer")
-    if not 0.0 < quantile < 1.0:
-        raise ParameterError("quantile must lie in the range (0, 1)")
-    if fmin <= 0:
-        raise ParameterError("fmin must be a positive number")
-    octa = np.zeros(n_bands + 2)
-    octa[1:] = fmin * (2.0 ** np.arange(0, n_bands + 1))
-    if np.any(octa[:-1] >= 0.5 * sr):
-        raise ParameterError("Frequency band exceeds Nyquist. Reduce either fmin or n_bands.")
-    if n_bands + 1 > 16:
-        raise nat.UnsupportedOnGPU("spectral_contrast: at most 15 octave bands on the GPU")
-    desc = nat.ContrastDesc(n_bands=n_bands + 1)
-    for k, (lo, count, tail) in enumerate(_contrast_bands(freq, octa, quantile)):
-        desc.lo[k], desc.count[k], desc.k[k] = lo, count, tail
-    lead = Sd.shape[:-2]
-    n_clips = pl.clip_count(lead)
-    L = nat.lib()
-    src, own = pl.to_native(Sd)
-    shape = tuple(lead) + (n_bands + 1, T)
-    peak = nat.DeviceArray.empty(ctx, shape, np.float32)
-    valley = nat.DeviceArray.empty(ctx, shape, np.float32)
-    nat.check(L.b2l_spectral_contrast(ctx.handle, C.byref(desc), _vp(src.ptr), n_clips, T, F, _vp(peak.ptr),
-                                      _vp(valley.ptr)))
-    if own:
-        src.free()
-    if own_S:
-        Sd.free()
-    if not linear:
-        p_db, v_db = power_to_db(peak), power_to_db(valley)
-        peak.free()
-        valley.free()
-        peak, valley = p_db, v_db
-    out = nat.DeviceArray.empty(ctx, shape, np.float32)
-    nat.check(L.b2l_sub(ctx.handle, _vp(peak.ptr), _vp(valley.ptr), peak.size, _vp(out.ptr)))
-    peak.free()
-    valley.free()
-    res_dtype = np.result_type(req, np.float64)
-    if staged is not None:
-        return staged.result(out, res_dtype)
-    return out if on_device else pl.finish(out, res_dtype)
+    with pl.Scope(y if S is None else S) as sc:
+        if S is None:
+            if y is None:
+                raise ParameterError("Input signal must be provided to compute a spectrogram")
+            _, req = pl.precheck_signal(y)
+            staged = pl.StagedInput(y)
+            sc.own(staged.dev)
+            Sd, n_fft = _spectrogram(y=staged.dev, n_fft=n_fft, hop_length=hop_length, power=1, win_length=win_length,
+                                     window=window, center=center, pad_mode=pad_mode)
+            sc.own(Sd)
+            staged.scan_uncovered(n_fft, hop_length, win_length, center, Sd.shape[-1])
+        else:
+            if not isinstance(S, nat.DeviceArray) and np.iscomplexobj(S):
+                raise nat.UnsupportedOnGPU(
+                    "spectral_contrast of a complex S is not supported on the GPU: pass np.abs(S)")
+            Sd, req = sc.spectrogram(S)
+            if n_fft is None or n_fft // 2 + 1 != Sd.shape[-2]:
+                n_fft = 2 * (Sd.shape[-2] - 1)
+        ctx = sc.ctx
+        F, T = Sd.shape[-2], Sd.shape[-1]
+        if freq is None:
+            freq = fft_frequencies(sr=sr, n_fft=n_fft)
+        freq = np.atleast_1d(freq)
+        if freq.ndim != 1 or len(freq) != F:
+            raise ParameterError(f"freq.shape mismatch: expected ({F:d},)")
+        if n_bands < 1 or not isinstance(n_bands, (int, np.integer)):
+            raise ParameterError("n_bands must be a positive integer")
+        if not 0.0 < quantile < 1.0:
+            raise ParameterError("quantile must lie in the range (0, 1)")
+        if fmin <= 0:
+            raise ParameterError("fmin must be a positive number")
+        octa = np.zeros(n_bands + 2)
+        octa[1:] = fmin * (2.0 ** np.arange(0, n_bands + 1))
+        if np.any(octa[:-1] >= 0.5 * sr):
+            raise ParameterError("Frequency band exceeds Nyquist. Reduce either fmin or n_bands.")
+        if n_bands + 1 > 16:
+            raise nat.UnsupportedOnGPU("spectral_contrast: at most 15 octave bands on the GPU")
+        desc = nat.ContrastDesc(n_bands=n_bands + 1)
+        for k, (lo, count, tail) in enumerate(_contrast_bands(freq, octa, quantile)):
+            desc.lo[k], desc.count[k], desc.k[k] = lo, count, tail
+        lead = Sd.shape[:-2]
+        n_clips = pl.clip_count(lead)
+        L = nat.lib()
+        src = sc.native(Sd)
+        shape = tuple(lead) + (n_bands + 1, T)
+        peak = sc.empty(shape, np.float32)
+        valley = sc.empty(shape, np.float32)
+        nat.check(L.b2l_spectral_contrast(ctx.handle, C.byref(desc), _vp(src.ptr), n_clips, T, F, _vp(peak.ptr),
+                                          _vp(valley.ptr)))
+        sc.free(src, Sd)
+        if not linear:
+            p_db, v_db = power_to_db(peak), power_to_db(valley)
+            peak.free()
+            valley.free()
+            peak, valley = sc.own(p_db), sc.own(v_db)
+        out = sc.empty(shape, np.float32)
+        nat.check(L.b2l_sub(ctx.handle, _vp(peak.ptr), _vp(valley.ptr), peak.size, _vp(out.ptr)))
+        return sc.result(out, np.result_type(req, np.float64), validate=S is None)
 
 
 # --------------------------------------------------------------------------------------------- time-domain framings
@@ -293,20 +277,18 @@ def _frame_feature(what, y, frame_length, hop_length, center, pad_mode, *, thres
     if hop_length < 1:
         raise ParameterError(f"Invalid hop_length: {hop_length}")
     T = pl.frame_count(n, frame_length, hop_length, center)
-    staged = pl.StagedInput(y)
-    ctx = staged.ctx
-    out = nat.DeviceArray.empty(ctx, staged.lead + (1, T), np.float32)
-    nat.check(nat.lib().b2l_frame_feature(ctx.handle, what, _vp(staged.dev.ptr), staged.n_clips, staged.n, staged.n,
-                                          frame_length, hop_length, int(bool(center)), nat.PAD_MODES[pad_mode],
-                                          float(threshold), int(zero_pos), int(pad_first), float(out_scale),
-                                          _vp(out.ptr)))
-    if staged.on_device:
-        return out, True
-    if validate:
-        staged.scan_uncovered(frame_length, hop_length, None, center, T)
-    res = pl.finish(out, validate=validate)
-    staged.release()
-    return res, False
+    with pl.Scope(y) as sc:
+        staged = pl.StagedInput(y)
+        out = sc.empty(staged.lead + (1, T), np.float32)
+        nat.check(nat.lib().b2l_frame_feature(sc.ctx.handle, what, _vp(staged.dev.ptr), staged.n_clips, staged.n,
+                                              staged.n, frame_length, hop_length, int(bool(center)),
+                                              nat.PAD_MODES[pad_mode], float(threshold), int(zero_pos), int(pad_first),
+                                              float(out_scale), _vp(out.ptr)))
+        if validate:
+            staged.scan_uncovered(frame_length, hop_length, None, center, T)
+        res = sc.result(out, validate=validate)
+        staged.release()
+        return res, sc.on_device
 
 
 def rms(*, y=None, S=None, frame_length: int = 2048, hop_length: int = 512, center: bool = True,
@@ -342,9 +324,10 @@ def rms(*, y=None, S=None, frame_length: int = 2048, hop_length: int = 512, cent
         if not isinstance(S, nat.DeviceArray) and np.iscomplexobj(S):
             raise nat.UnsupportedOnGPU("rms(S=...) with a complex S is not supported on the GPU: pass np.abs(S)")
         # rms only squares S, so the sign of an entry is irrelevant (no non-negativity requirement)
-        stats, ctx, lead, T, on_device, _, _ = _stats_from_S(S, _desc(nat.STAT_RMS, frame_length=frame_length), None, 22050,
-                                                             frame_length, "rms", check_negative=False)
-        return _take_row(ctx, stats, lead, T, nat.STAT_RMS, on_device, np.dtype(dtype))
+        with pl.Scope(S) as sc:
+            desc = _desc(nat.STAT_RMS, frame_length=frame_length)
+            stats, _, _ = _stats_from_S(sc, S, desc, None, 22050, frame_length, "rms", check_negative=False)
+            return _take_row(sc, stats, nat.STAT_RMS, np.dtype(dtype))
     raise ParameterError("Either `y` or `S` must be input.")
 
 

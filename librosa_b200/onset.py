@@ -90,8 +90,7 @@ def onset_strength_multi(*, y=None, sr: float = 22050, S=None, n_fft: int = 2048
         else:
             if not isinstance(S, nat.DeviceArray):
                 S = np.atleast_2d(np.asarray(S))
-            Sd, res_dtype, _ = pl.spectrogram_input(S)
-            sc.own(Sd)
+            Sd, res_dtype = sc.spectrogram(S)
             if Sd.layout != "c":
                 raise ParameterError("device spectrogram must be C-ordered (..., rows, frames)")
         if Sd.ndim < 2:

@@ -173,15 +173,17 @@ def test_zero_envelope_returns_before_bpm_checks(monkeypatch):
     assert bpm.shape == (2,) and bpm.dtype == np.float64 and beats.shape == (2, 50) and beats.dtype == bool
 
 
-def test_median_refusal_before_device_work(monkeypatch):
+def test_median_refusal_before_any_device_work(monkeypatch):
     """Channels wider than the median kernel's 512 rows, and other aggregates, are refused from the shapes alone."""
+    from librosa_b200 import _native as nat
     from librosa_b200 import _pipeline as pl
 
     def no_device(*a, **k):
         raise AssertionError("device work before the refusal")
 
     monkeypatch.setattr(pl, "StagedInput", no_device)
-    monkeypatch.setattr(pl, "spectrogram_input", no_device)
+    monkeypatch.setattr(nat, "default_context", no_device)
+    monkeypatch.setattr(nat, "lib", no_device)
     with pytest.raises(lb.UnsupportedOnGPU, match="600 rows"):
         lb.onset.onset_strength(S=np.zeros((600, 20), np.float32), aggregate=np.median)
     with pytest.raises(lb.UnsupportedOnGPU, match="513 rows"):

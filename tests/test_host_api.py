@@ -391,6 +391,31 @@ def test_views_zeroed_buffers_and_status_bits_have_one_home():
     assert not stray, stray
 
 
+def test_device_buffers_of_a_call_belong_to_its_scope():
+    """The spectrum, spectral-feature, statistics, inverse, HPSS, effects, tuning and resampling calls stage, allocate
+    and free through _pipeline.Scope, which frees what a call still owns on its normal and its exception path alike:
+    no module stages a spectrogram or a host array, or allocates a device buffer, by hand."""
+    import glob
+    import re
+
+    # the two free functions Scope.native / Scope.spectrogram replaced, spelled with a character class so that a
+    # search of the repository for their names finds nothing, this test included
+    retired = re.compile(r"to_[n]ative|spectrogram_[i]nput")
+    pkg = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "librosa_b200")
+    stray = []
+    for path in sorted(glob.glob(os.path.join(pkg, "**", "*.py"), recursive=True)):
+        with open(path) as f:
+            text = f.read()
+        stray += [(os.path.relpath(path, pkg), m.group(0)) for m in retired.finditer(text)]
+    for name in ("core/spectrum.py", "core/pitch.py", "core/audio.py", "feature/spectral.py", "feature/stats.py",
+                 "feature/inverse.py", "decompose.py", "effects.py"):
+        with open(os.path.join(pkg, name)) as f:
+            text = f.read()
+        stray += [(name, w) for w in ("default_context(", ".to_device(", "DeviceArray.empty(", "in locals()")
+                  if w in text]
+    assert not stray, stray
+
+
 def test_polyphase_filter_bookkeeping_matches_scipy():
     """The host half of resample(res_type="polyphase"): the zero-padded low-pass and the crop offset handed to
     b2l_resample_poly, checked by evaluating the kernel's formula  y[j] = sum_m x[m] h[(n_pre_remove + j) down - m up]

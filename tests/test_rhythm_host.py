@@ -77,15 +77,17 @@ _ERRORS = [
 
 
 @pytest.mark.parametrize("fn,kw,exc,msg", _ERRORS, ids=[f"{e[0]}-{i}" for i, e in enumerate(_ERRORS)])
-def test_errors_before_device_work(monkeypatch, fn, kw, exc, msg):
+def test_errors_before_any_device_work(monkeypatch, fn, kw, exc, msg):
     """The reference's argument errors (and the GPU's refusals) come before any staging: a device touch fails."""
+    from librosa_b200 import _native as nat
     from librosa_b200 import _pipeline as pl
 
     def no_device(*a, **k):
         raise AssertionError("device work before the argument checks")
 
     monkeypatch.setattr(pl, "StagedInput", no_device)
-    monkeypatch.setattr(pl, "to_native", no_device)
+    monkeypatch.setattr(nat, "default_context", no_device)
+    monkeypatch.setattr(nat, "lib", no_device)
     with pytest.raises(exc, match=msg):
         getattr(lb.feature, fn)(**kw)
 
