@@ -16,7 +16,6 @@
 #pragma once
 #include "common.cuh"
 #include "fft_engine.cuh"
-#include "fwd_kernel.cuh"   // load_padded, power_from_sq, sqmag
 
 namespace b2l {
 

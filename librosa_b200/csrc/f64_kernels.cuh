@@ -15,7 +15,7 @@
 
 namespace b2l {
 
-// np.pad index map in double (same modes as load_padded in fwd_kernel.cuh)
+// np.pad index map in double (same modes as load_padded in common.cuh)
 __device__ __forceinline__ double load_padded64(const double* __restrict__ y, int n, long long j, int mode, int pad) {
   if (j >= 0 && j < n) return y[j];
   switch (mode) {

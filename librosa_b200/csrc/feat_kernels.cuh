@@ -1,10 +1,11 @@
 // feat_kernels.cuh — frame-wise features that sit next to the FFT path: spectral statistics of a stored
 // magnitude spectrogram (the S= form of librosa.feature.spectral_centroid / bandwidth / rolloff / flatness /
 // rms; the y= form is fused into fwd_kernel, MODE_STATS) and the two time-domain framings that need no FFT
-// (rms(y=...), zero_crossing_rate).
+// (rms(y=...), zero_crossing_rate), then the plan-free kernels over spectrograms and signals: onset strength, pcen,
+// spectral contrast, piptrack, HPSS, reassignment, phase vocoder, resampling, power_to_db, the Griffin-Lim update
+// and a batched transpose used as a layout adapter.  Included by feature_api.cu only.
 #pragma once
 #include "common.cuh"
-#include "fwd_kernel.cuh"   // load_padded
 #include "stats.cuh"
 
 namespace b2l {
@@ -864,6 +865,101 @@ __global__ void unary_kernel(const float* __restrict__ in, long long n, int op, 
       if (op == UNARY_DB_TO_AMPLITUDE) r = sqrtf(r);
     }
     out[i] = r;
+  }
+}
+
+// ------------------------------------------------------------------ polyphase resampling
+// librosa.resample(res_type="polyphase") = scipy.signal.resample_poly(y, up, down) (librosa/core/audio.py:1129-1145):
+// upfirdn(h, x, up, down) cropped to [n_pre_remove, n_pre_remove + n_out) with the zero-padded low-pass h the host
+// designs exactly as SciPy does (firwin(2 * 10 * max(up, down) + 1, 1 / max(up, down), window=("kaiser", 5.0)) * up,
+// float32 for float32 data).  Output sample j is
+//     y[j] = sum_m x[m] * h[(n_pre_remove + j) * down - m * up],
+// accumulated over increasing m like SciPy's upfirdn loop; one thread per output sample (about 20 * max(1, down / up)
+// taps each).  Samples j >= n_keep of a row are the zeros of util.fix_length; out_scale carries 1 / sqrt(ratio).
+__global__ void resample_poly_kernel(const float* __restrict__ x, long long x_stride, int n_in, const float* __restrict__ h,
+                                     int n_h, int up, int down, long long n_pre_remove, int n_keep, int n_total,
+                                     long long n_clips, float out_scale, float* __restrict__ out) {
+  const long long total = n_clips * n_total;
+  for (long long o = (long long)blockIdx.x * blockDim.x + threadIdx.x; o < total; o += (long long)gridDim.x * blockDim.x) {
+    const long long clip = o / n_total;
+    const int j = (int)(o - clip * n_total);
+    float acc = 0.0f;
+    if (j < n_keep) {
+      const long long t = (n_pre_remove + j) * (long long)down;          // position in the up-sampled stream
+      long long m_hi = t / up;
+      if (m_hi > n_in - 1) m_hi = n_in - 1;
+      long long m_lo = t - (n_h - 1);                                    // smallest m with t - m * up <= n_h - 1
+      m_lo = m_lo <= 0 ? 0 : (m_lo + up - 1) / up;
+      const float* xc = x + clip * x_stride;
+      long long k = t - m_lo * up;
+      for (long long m = m_lo; m <= m_hi; ++m, k -= up) acc = fmaf(__ldg(h + k), __ldg(xc + m), acc);
+      acc *= out_scale;
+    }
+    out[o] = acc;
+  }
+}
+
+// ------------------------------------------------------------------ power_to_db
+__global__ void db_kernel(const float* __restrict__ in, long long per_clip, float amin, float db_sub,
+                          unsigned int* __restrict__ clip_max, float* __restrict__ out) {
+  const int clip = blockIdx.y;
+  const float* ic = in + (long long)clip * per_clip;
+  float* oc = out + (long long)clip * per_clip;
+  float mx = -INFINITY;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < per_clip;
+       i += (long long)gridDim.x * blockDim.x) {
+    float v = 10.0f * log10f(fmaxf(amin, ic[i])) - db_sub;
+    oc[i] = v;
+    mx = fmaxf(mx, v);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+  if ((threadIdx.x & 31) == 0 && mx > -INFINITY) atomicMax(clip_max + clip, float_to_key(mx));
+}
+
+__global__ void db_clamp_kernel(float* __restrict__ x, long long per_clip, const unsigned int* __restrict__ clip_max,
+                                float top_db) {
+  const int clip = blockIdx.y;
+  float* xc = x + (long long)clip * per_clip;
+  const float floor_v = key_to_float(clip_max[clip]) - top_db;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < per_clip;
+       i += (long long)gridDim.x * blockDim.x)
+    xc[i] = fmaxf(xc[i], floor_v);
+}
+
+// ------------------------------------------------------------------ Griffin-Lim phase update
+// angles <- rebuilt - scale * tprev ;  angles <- angles / (|angles| + eps) * S      (elementwise)
+// librosa/core/spectrum.py:2898-2903 (scale = momentum / (1 + momentum), eps = tiny(complex64)).
+__global__ void gl_update_kernel(const float2* __restrict__ rebuilt, const float2* __restrict__ tprev,
+                                 const float* __restrict__ S, float scale, float eps, float2* __restrict__ out,
+                                 long long n) {
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    float2 a = rebuilt[i];
+    if (tprev != nullptr) {
+      const float2 p = tprev[i];
+      a.x = fmaf(-scale, p.x, a.x);
+      a.y = fmaf(-scale, p.y, a.y);
+    }
+    const float mag = hypotf(a.x, a.y) + eps;
+    const float s = S[i];
+    out[i] = make_float2(a.x / mag * s, a.y / mag * s);
+  }
+}
+
+// ------------------------------------------------------------------ batched transpose
+template <typename T>
+__global__ void transpose_kernel(const T* __restrict__ in, int rows, int cols, T* __restrict__ out) {
+  __shared__ T tile[32][33];
+  const long long base = (long long)blockIdx.z * rows * cols;
+  const int c0 = blockIdx.x * 32, r0 = blockIdx.y * 32;
+  for (int j = threadIdx.y; j < 32; j += blockDim.y) {
+    int r = r0 + j, c = c0 + threadIdx.x;
+    if (r < rows && c < cols) tile[j][threadIdx.x] = in[base + (long long)r * cols + c];
+  }
+  __syncthreads();
+  for (int j = threadIdx.y; j < 32; j += blockDim.y) {
+    int c = c0 + j, r = r0 + threadIdx.x;
+    if (r < rows && c < cols) out[base + (long long)c * rows + r] = tile[threadIdx.x][j];
   }
 }
 

@@ -55,23 +55,6 @@ __device__ __forceinline__ void tma_load_1d(void* dst_smem, const void* src_gmem
       : "memory");
 }
 
-// |X|^power from |X|^2 for power != 2 (kept out of line: the default power-2 path never executes it)
-static __device__ __noinline__ float power_from_sq(float p2, int power_mode, float power) {
-  float mag = sqrtf(p2);
-  return power_mode == 1 ? mag : powf(mag, power);
-}
-__device__ __forceinline__ float sqmag(float2 x) { return fmaf(x.x, x.x, x.y * x.y); }
-// 10 * log10(x) through the hardware base-2 logarithm (MUFU.LG2: about 2 ulp of the result, so the error grows with
-// |dB|: within 1e-6 dB + 2^-22 |dB|, up to 1.7e-5 dB near the -100 dB floor of amin 1e-10, measured on an H100):
-// the library log10f is 28 instructions per value, and the dB epilogue runs once
-// per mel row and frame — for the short rows of n_fft = 1024 it was a third of the projection phase.
-__device__ __forceinline__ float db10(float x) { return 3.0102999566398120f * __log2f(x); }
-__device__ __forceinline__ float sqrt_approx(float x) {
-  float r;
-  asm("sqrt.approx.f32 %0, %1;" : "=f"(r) : "f"(x));
-  return r;
-}
-
 // Exchange-buffer slot of Z[M - k] for k = t + TPF*c (the partner of bin k in the real-FFT un-mix).
 // For warp-multiple groups the padded index is affine in the lane with a compile-time offset.
 template <int M, int TPF, int C>

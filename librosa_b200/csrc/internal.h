@@ -1,5 +1,5 @@
-// internal.h — host-side state and helpers shared by the C ABI units (runtime.cu, plan.cu, api.cu, f64_api.cu,
-// inverse_api.cu, rhythm_api.cu) and the per-size kernel instantiations (fwd_inst.cu, inv_inst.cu, czt_inst.cu).
+// internal.h — host-side state and helpers shared by the C ABI units (runtime.cu, plan.cu and the *_api.cu units:
+// spectrum, feature, pitch, f64, inverse, ...) and the per-size kernel instantiations (fwd_inst.cu, inv_inst.cu, czt_inst.cu).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -198,6 +198,11 @@ std::vector<double2> f64_twiddles(int n, int count);
 
 // Grows the context's per-clip maximum scratch to at least n_clips entries.
 int ensure_clip_max(b2l_ctx* c, size_t n_clips);
+// Grows the context's scratch array to at least `bytes` (the contents are not kept).
+int ensure_scratch(b2l_ctx* c, size_t bytes);
+
+// Checks a spectral-statistics descriptor and converts it to the kernels' StatsParams (feature_api.cu).
+int check_stats_desc(const b2l_stats_desc* d, StatsParams* sp);
 
 // ------------------------------------------------------------------ launches
 // Resident blocks per SM of kernel `fn` with `threads` threads and `smem` bytes of dynamic shared memory, cached per

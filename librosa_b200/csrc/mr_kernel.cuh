@@ -18,7 +18,6 @@
 #pragma once
 #include "common.cuh"
 #include "fft_engine.cuh"
-#include "fwd_kernel.cuh"   // load_padded, power_from_sq, sqmag, db10, sqrt_approx
 
 namespace b2l {
 

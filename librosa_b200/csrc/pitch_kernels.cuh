@@ -12,7 +12,6 @@
 #include "argmax.cuh"
 #include "common.cuh"
 #include "fft_engine.cuh"
-#include "fwd_kernel.cuh"   // load_padded
 
 namespace b2l {
 
@@ -241,7 +240,7 @@ struct PyinObsArgs {
   double* voiced_prob;        // [row]
 };
 
-// Per-warp shared slice of pyin_obs_kernel, in bytes (host mirror in api.cu).
+// Per-warp shared slice of pyin_obs_kernel, in bytes (host mirror in pitch_api.cu).
 __host__ __device__ inline size_t pyin_obs_slice(int n_lags, int max_cand, int n_thresholds) {
   size_t b = (size_t)max_cand * 8;                   // probability of each trough
   b += ((size_t)n_lags * 4 + 7) / 8 * 8;             // the CMND row

@@ -214,6 +214,19 @@ int b2l::ensure_clip_max(b2l_ctx* c, size_t n_clips) {
   return B2L_OK;
 }
 
+int b2l::ensure_scratch(b2l_ctx* c, size_t bytes) {
+  if (c->scratch_bytes >= bytes) return B2L_OK;
+  if (c->d_scratch) {
+    CUDA_TRY(cudaStreamSynchronize(c->stream));
+    CUDA_TRY(cudaFree(c->d_scratch));
+    c->d_scratch = nullptr;
+    c->scratch_bytes = 0;
+  }
+  CUDA_TRY(cudaMalloc((void**)&c->d_scratch, bytes));
+  c->scratch_bytes = bytes;
+  return B2L_OK;
+}
+
 extern "C" int b2l_alloc(b2l_ctx* c, size_t bytes, void** d_ptr) {
   if (!c || !d_ptr) return fail(B2L_ERR_INVALID, "NULL argument");
   DeviceGuard g(c->device);

@@ -6,19 +6,19 @@ reflect index map of hpss_kernel.  This file is the specification the kernels ar
 tests/test_gpu_feature_kernels.py runs them, with the case lists generated here.
 
 Restated here:
-    b2l_spectral_contrast (api.cu)  sort capacity cap = next power of two >= max(32, largest band count); per warp
-                                    (Fp + cap) 4 bytes, Fp = (F + 3) & ~3; warps per block 8 -> 4 -> 2 -> 1, the first
+    b2l_spectral_contrast           sort capacity cap = next power of two >= max(32, largest band count); per warp
+      (feature_api.cu)              (Fp + cap) 4 bytes, Fp = (F + 3) & ~3; warps per block 8 -> 4 -> 2 -> 1, the first
                                     that fits the opt-in shared memory; refused when one warp does not fit
     contrast_kernel paths           kk = min(k, n);  kk <= 16 and n <= 512: sorted runs (lane l owns band bins l,
                                     l + 32, ...; sort_keys<2|4|8|16> by per = ceil(n / 32), none for per = 1), then
                                     the head walk (minima) and the s_top[-32 used] walk (maxima);  kk <= 16, n > 512:
                                     knock-out extraction;  kk > 16: bitonic sort of the band in shared memory
-    b2l_frame_feature (api.cu)      frame_td_block_kernel when frame_length % hop == 0, R = frame_length / hop <= 64,
-                                    n_clips <= 65 535 (clips on grid.y); frame_td_kernel otherwise
+    b2l_frame_feature               frame_td_block_kernel when frame_length % hop == 0, R = frame_length / hop <= 64,
+      (feature_api.cu)              n_clips <= 65 535 (clips on grid.y); frame_td_kernel otherwise
     frame_td_block_kernel           tiles of 64 frames; block g covers padded positions g hop - pad + [0, hop); a
                                     frame's count is the sum of its R blocks minus the crossing at its first position
                                     plus pad_first
-    b2l_hpss (api.cu)               hpss_kernel<NS>, NS = 8 / 16 / 32 / 64 by max(win_harm, win_perc)
+    b2l_hpss (feature_api.cu)       hpss_kernel<NS>, NS = 8 / 16 / 32 / 64 by max(win_harm, win_perc)
     reflect_index                   the np.pad "symmetric" extension, repeated for windows longer than the axis
 
 The sizing tables are H100 constants (232 448 bytes of opt-in shared memory).  Last, the comparisons of the GPU test

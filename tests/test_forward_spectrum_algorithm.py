@@ -4,17 +4,17 @@ a row over the lanes of a warp, and how many warps mr_kernel runs in modes 0 and
 the kernels are read against; tests/test_gpu_forward_spectrum.py runs them.
 
 Restated here:
-    run_forward (csrc/api.cu)        forward_choice of tests/test_mel_front_end_algorithm.py with its `mode`: no
-                                     MelRow table outside MODE_MEL, the M + 1 bin frequencies in MODE_STATS, and an
+    run_forward                      forward_choice of tests/test_mel_front_end_algorithm.py with its `mode`: no
+      (csrc/spectrum_api.cu)         MelRow table outside MODE_MEL, the M + 1 bin frequencies in MODE_STATS, and an
                                      exchange region of FT (M + M/32) float2 in MODE_STFT / MODE_SPEC against the
                                      MelLayout group stride in MODE_STATS
     b2l_spectral_stats_from_spec     stats_kernel's warp ladder nw = 8 -> 4 -> 2 -> 1: the first nw whose block,
-      (csrc/api.cu)                  (nw + 1) Fp 4 bytes with Fp = (F + 3) & ~3, fits the opt-in shared memory
+      (csrc/feature_api.cu)          (nw + 1) Fp 4 bytes with Fp = (F + 3) & ~3, fits the opt-in shared memory
     frame_stats (csrc/stats.cuh)     lane l owns bins [l c, (l + 1) c) clipped to F, c = ((F + 31) / 32) | 1; the
                                      running sum of bin k is the exclusive warp scan of the chunk totals (shfl_up,
                                      Hillis-Steele) plus the lane-local walk
-    mr_block (csrc/api.cu)           warps per block of mr_kernel<0 | 1, G> (no mel tables), G = 16 lanes per frame for
-                                     M <= 512, 32 above
+    mr_block                         warps per block of mr_kernel<0 | 1, G> (no mel tables), G = 16 lanes per frame for
+      (csrc/spectrum_api.cu)         M <= 512, 32 above
 
 The selection tables are H100 constants (232 448 bytes of opt-in shared memory).  Last, the comparisons the GPU test
 uses must reject subtly wrong kernels simulated in float64 on that test's own signals.
@@ -69,7 +69,7 @@ H100_MR_SPECTRUM_WARPS = [
 ]
 
 
-# ------------------------------------------------------------------ b2l_spectral_stats_from_spec (api.cu)
+# ------------------------------------------------------------------ b2l_spectral_stats_from_spec (feature_api.cu)
 def stats_block(F, smem_optin=H100_SMEM_OPTIN):
     """(warps per block, shared-memory bytes) of stats_kernel for rows of F bins, or None (refused)."""
     Fp = (F + 3) & ~3
@@ -108,7 +108,7 @@ def warp_exclusive_scan(x):
     return incl - x, incl[..., 31]
 
 
-# ------------------------------------------------------------------ mr_block (api.cu), modes 0 and 1
+# ------------------------------------------------------------------ mr_block (spectrum_api.cu), modes 0 and 1
 def mr_spectrum_block(n_fft, smem_optin=H100_SMEM_OPTIN):
     """(lanes per frame G, warps per block, shared-memory bytes) of run_mr in modes 0 / 1 (n_mels 0), or None."""
     M = n_fft // 2

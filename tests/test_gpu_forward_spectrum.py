@@ -408,9 +408,9 @@ def tile_frames(n_fft, hop, kind):
 
 
 def tma_staging(n_fft, hop, y_stride, offset, kind):
-    """run_forward's tma_ok (api.cu) for a clip `offset` floats past a 16-byte aligned allocation, with FT taken from
-    the instance `kind` selects: base, row stride and staged span (FT - 1) hop + n_fft all 16-byte aligned.  Interior
-    tiles then stage by TMA bulk copy (TILE_TMA), edge tiles with constant padding by TILE_TMA_ZERO."""
+    """run_forward's tma_ok (spectrum_api.cu) for a clip `offset` floats past a 16-byte aligned allocation, with FT
+    taken from the instance `kind` selects: base, row stride and staged span (FT - 1) hop + n_fft all 16-byte aligned.
+    Interior tiles then stage by TMA bulk copy (TILE_TMA), edge tiles with constant padding by TILE_TMA_ZERO."""
     return offset % 4 == 0 and y_stride % 4 == 0 and ((tile_frames(n_fft, hop, kind) - 1) * hop + n_fft) % 4 == 0
 
 

@@ -1,7 +1,8 @@
-"""GPU (-m gpu): the power-of-two inverse kernel (csrc/inv_kernel.cuh, launched by run_inverse in csrc/api.cu) at all
-eleven sizes n_fft = 8 ... 8192, against a float64 reference built here: scipy.fft.irfft of the complex64 input widened
-to complex128, the float64 window (get_window + pad_center), a plain overlap-add, and the oracle's window-sum-square.
-The slot / piece / halo / carry schedule itself is restated for the CPU in tests/test_inverse_gather_algorithm.py.
+"""GPU (-m gpu): the power-of-two inverse kernel (csrc/inv_kernel.cuh, launched by run_inverse in csrc/spectrum_api.cu)
+at all eleven sizes n_fft = 8 ... 8192, against a float64 reference built here: scipy.fft.irfft of the complex64 input
+widened to complex128, the float64 window (get_window + pad_center), a plain overlap-add, and the oracle's
+window-sum-square.  The slot / piece / halo / carry schedule itself is restated for the CPU in
+tests/test_inverse_gather_algorithm.py.
 
 Most tests call b2l_istft the way core/spectrum.py::istft does (plan, reciprocal window-sum-square, device
 pointers) but into an output buffer the test filled with NaN, with a row stride of its choosing: every sample

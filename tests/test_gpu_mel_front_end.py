@@ -92,8 +92,8 @@ def tile_frames(n_fft, hop, n_mels=128):
 
 
 def bulk_copy(n_fft, hop, y_stride, offset):
-    """run_forward's tma_ok (api.cu) for a clip `offset` floats past a 16-byte aligned allocation: base, row stride
-    and staged span (FT - 1) hop + n_fft all 16-byte aligned.  Interior tiles then stage by TMA bulk copy
+    """run_forward's tma_ok (spectrum_api.cu) for a clip `offset` floats past a 16-byte aligned allocation: base, row
+    stride and staged span (FT - 1) hop + n_fft all 16-byte aligned.  Interior tiles then stage by TMA bulk copy
     (TILE_TMA; edge tiles TILE_TMA_ZERO or the gather); otherwise every tile takes the per-sample gather."""
     return offset % 4 == 0 and y_stride % 4 == 0 and ((tile_frames(n_fft, hop) - 1) * hop + n_fft) % 4 == 0
 

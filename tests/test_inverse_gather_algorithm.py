@@ -1,4 +1,4 @@
-"""The scheduling of the power-of-two inverse (run_inverse in csrc/api.cu, inv_kernel in csrc/inv_kernel.cuh)
+"""The scheduling of the power-of-two inverse (run_inverse in csrc/spectrum_api.cu, inv_kernel in csrc/inv_kernel.cuh)
 restated in integer-indexed NumPy, in float64, on the CPU.  The windowed frames w * irfft(D) are taken as given, so
 no FFT is involved: what is checked is the slot / piece / halo / round / carry scheme that turns frames into output
 samples.  This file is the specification the kernel is read against.

@@ -8,10 +8,12 @@ Restated here:
                                      rule lo == 4 (j mod G) mod max(H, 4)), shared trip count `quads` per work item,
                                      zero-padded weights at `off`
     MelLayout (csrc/common.cuh)      rows per warp H, group stride GS, row stride RS = 2 GS
-    run_forward (csrc/api.cu)        MODE_MEL: CTA variant (116 = two 8-warp halves, then 16, then 8 warps), frames
-                                     per tile FT, halves and the shared-memory bytes, the first that fits wins
-    mr_block / run_mr (csrc/api.cu)  warps per block and lanes per frame G of mr_kernel
-    launch_dct (csrc/api.cu)         dct_clamp4_kernel with KS = 2 or 1 warp sets, dct_generic_kernel, or refused
+    run_forward                      MODE_MEL: CTA variant (116 = two 8-warp halves, then 16, then 8 warps), frames
+      (csrc/spectrum_api.cu)         per tile FT, halves and the shared-memory bytes, the first that fits wins
+    mr_block / run_mr                warps per block and lanes per frame G of mr_kernel
+      (csrc/spectrum_api.cu)
+    launch_dct                       dct_clamp4_kernel with KS = 2 or 1 warp sets, dct_generic_kernel, or refused
+      (csrc/spectrum_api.cu)
 
 Asserted over a grid of mel configurations crossed with every (n_fft, FT) an H100 reaches: every shared-memory word a
 row reads is one the same tile wrote for the same frame (its power row, bins 0 .. M + 3, or a non-padding word of the
@@ -133,7 +135,7 @@ def dense_rows(t, M, RS):
     return out
 
 
-# ------------------------------------------------------------------ run_forward (api.cu), MODE_MEL
+# ------------------------------------------------------------------ run_forward (spectrum_api.cu), MODE_MEL
 def tw_count_split(log2m):
     """HostFftCfg::tw_count(true): fwd_kernel's split inter-pass table."""
     M = 1 << log2m
@@ -244,7 +246,7 @@ H100_MEL_VARIANTS = {
 }
 
 
-# ------------------------------------------------------------------ run_mr / mr_block (api.cu), mode 2
+# ------------------------------------------------------------------ run_mr / mr_block (spectrum_api.cu), mode 2
 def mr_sizes():
     """Even n_fft of 12 ... 4096, not a power of two, whose half has no prime factor above 5 (pl.mr_covers)."""
     out = []
@@ -290,7 +292,7 @@ def mr_choice(n_fft, basis, smem_optin=H100_SMEM_OPTIN):
     return 32 // fpw, w, tables + w * per_warp
 
 
-# ------------------------------------------------------------------ launch_dct (api.cu)
+# ------------------------------------------------------------------ launch_dct (spectrum_api.cu)
 def dct_choice(n_mels, n_mfcc, tiled, smem_optin=H100_SMEM_OPTIN):
     """"ks2" / "ks1" (dct_clamp4_kernel<KS>), "generic" (dct_generic_kernel) or "refused"."""
     KG = (n_mfcc + 7) // 8
