@@ -330,6 +330,16 @@ typedef struct b2l_stack_desc {
 } b2l_stack_desc;
 int b2l_stack_memory(b2l_ctx* ctx, const b2l_stack_desc* desc, const void* d_x, int64_t n_clips, int64_t d, int64_t t,
                      const int64_t* d_pad, void* d_out);
+/* librosa.util.localmax / localmin (util/utils.py:1029-1178) along the middle axis of d_x [outer][n][inner], n >= 2,
+ * elements of `type` (enum b2l_elem_type), into d_out of the same geometry, one byte (0 / 1) per element: never at
+ * position 0; x[i] > x[i-1] and x[i] >= x[i+1] inside the line (mirrored when !is_max); x[n-1] > x[n-2] at its end.
+ * NaN compares false.  One launch. */
+enum b2l_elem_type {
+  B2L_ELEM_I8 = 0, B2L_ELEM_U8 = 1, B2L_ELEM_I16 = 2, B2L_ELEM_U16 = 3, B2L_ELEM_I32 = 4, B2L_ELEM_U32 = 5,
+  B2L_ELEM_I64 = 6, B2L_ELEM_U64 = 7, B2L_ELEM_F32 = 8, B2L_ELEM_F64 = 9, B2L_ELEM_BOOL = 10
+};
+int b2l_localext(b2l_ctx* ctx, const void* d_x, int32_t type, int32_t is_max, int64_t outer, int64_t n, int64_t inner,
+                 uint8_t* d_out);
 /* The constant-Q chroma features (feature/spectral.py:1296-1839): chroma_cqt / chroma_vqt (:1296-1423, :1576-1706),
  * the CENS steps of chroma_cens (:1426-1573) and tonnetz (:1709-1839), in one launch per 65 535 clips.
  * b2l_chroma_fold reads d_in [n_clips] x (n_bins, n_frames) in the form `input` names (complex64 input is taken as
@@ -553,6 +563,31 @@ int b2l_pyin_obs(b2l_ctx* ctx, const b2l_pyin_desc* desc, const float* d_cmnd, i
 int b2l_viterbi(b2l_ctx* ctx, const b2l_pyin_desc* desc, const int32_t* d_count, const int32_t* d_cand_bin,
                 const double* d_cand_prob, const double* d_voiced_prob, int64_t n_clips, int64_t n_frames,
                 uint16_t* d_states, double* d_f0, uint8_t* d_voiced);
+/* librosa.piptrack (core/pitch.py:182-366) over d_S [n_clips] x (n_bins, n_frames), float32 or float64 (f64), in
+ * memory [clip][frame][bin] ("ft") or, with layout_c, [clip][bin][frame], into d_pitches / d_mags [n_clips][n_frames]
+ * [n_bins] of the same type (every bin written, zero off the peaks).  abs_mode: 0 takes S as it is, 1 takes |S|, 2
+ * takes |S| when S holds a value < 0 and no NaN (the reference's S.min() < 0), which one extra launch decides on the
+ * device.  The frame reference is threshold * max over the frame's bins (ref_frame; in float64 when thr_wide, else
+ * in the data type; a NaN bin makes it NaN) or ref_abs; peaks are the bins k_lo <= k < k_hi where
+ * localmax(S * (S > ref)) holds along the bins.  Interpolation in the reference's precision: the parabolic shift in
+ * float64 from sums in the data type, pitch = (k + shift) * sr / n_fft in float64, mag = S + 0.5 * avg * shift in the
+ * data type, unfused.  A row of more than B2L_PIPTRACK_MAX_ROW_BYTES (bins rounded up to 4, times the element size)
+ * returns B2L_ERR_UNSUPPORTED. */
+#define B2L_PIPTRACK_MAX_ROW_BYTES (200 * 1024)
+typedef struct b2l_piptrack_desc {
+  int32_t f64, layout_c;
+  int32_t k_lo, k_hi;
+  int32_t abs_mode, ref_frame, thr_wide, pad_;
+  double threshold, ref_abs, sr, n_fft;
+} b2l_piptrack_desc;
+int b2l_piptrack(b2l_ctx* ctx, const b2l_piptrack_desc* desc, const void* d_S, int64_t n_clips, int32_t n_bins,
+                 int64_t n_frames, void* d_pitches, void* d_mags);
+/* librosa.pitch_tuning's histogram (core/pitch.py:112-179) over the n values of d_f (float32, or float64 with f64), in
+ * one launch: h_counts[b] for b < n_bins counts the residuals mod(bins_per_octave * log2(f / 27.5), 1) folded to
+ * [-0.5, 0.5) of the values f > 0 that fall in [h_edges[b], h_edges[b + 1]) (np.histogram; the last bin closed), and
+ * h_counts[n_bins] counts the values > 0.  1 <= n_bins <= 2048.  Synchronises. */
+int b2l_pitch_tuning(b2l_ctx* ctx, const void* d_f, int64_t n, int32_t f64, double bins_per_octave, int32_t n_bins,
+                     const double* h_edges, uint64_t* h_counts);
 
 /* ---- rhythm: librosa.feature.tempogram / tempo (feature/rhythm.py:38-470) ---------------------------------------
  * b2l_tempogram: onset envelopes d_env [n_rows][n] (float32, or float64 when env_f64) -> the normalised local

@@ -21,7 +21,7 @@ from .core.audio import resample, stream
 from .core.constantq import cqt, cqt_frequencies, hybrid_cqt, pseudo_cqt, vqt
 from .core.convert import (fft_frequencies, fourier_tempo_frequencies, frames_to_samples, frames_to_time, hz_to_mel,
                            hz_to_octs, mel_frequencies, mel_to_hz, samples_to_time, tempo_frequencies)
-from .core.pitch import estimate_tuning, pyin, yin
+from .core.pitch import estimate_tuning, pitch_tuning, piptrack, pyin, yin
 from .core.semitone import iirt
 from .core.spectrum import (_spectrogram, amplitude_to_db, db_to_amplitude, db_to_power, griffinlim, istft,
                             pcen, phase_vocoder, power_to_db, reassigned_spectrogram, stft)
@@ -49,7 +49,7 @@ def to_device(arr, device=None):
 
 __all__ = [
     "stream", "resample", "stft", "istft", "griffinlim", "power_to_db", "amplitude_to_db", "pcen", "phase_vocoder", "reassigned_spectrogram", "db_to_power", "db_to_amplitude", "_spectrogram", "feature", "filters", "util", "core", "onset", "beat", "decompose", "effects", "sequence",
-    "hz_to_mel", "mel_to_hz", "hz_to_octs", "estimate_tuning", "yin", "pyin", "cqt", "vqt", "pseudo_cqt", "hybrid_cqt", "cqt_frequencies", "iirt", "mel_frequencies", "fft_frequencies", "tempo_frequencies", "fourier_tempo_frequencies", "frames_to_samples", "frames_to_time", "samples_to_time", "ParameterError", "LibrosaError",
+    "hz_to_mel", "mel_to_hz", "hz_to_octs", "estimate_tuning", "pitch_tuning", "piptrack", "yin", "pyin", "cqt", "vqt", "pseudo_cqt", "hybrid_cqt", "cqt_frequencies", "iirt", "mel_frequencies", "fft_frequencies", "tempo_frequencies", "fourier_tempo_frequencies", "frames_to_samples", "frames_to_time", "samples_to_time", "ParameterError", "LibrosaError",
     "Context", "DeviceArray", "default_context", "device_count", "pinned_empty", "to_device", "device_copy",
     "NativeLibraryError", "UnsupportedOnGPU", "bind_host_to_device",
 ]

@@ -208,6 +208,20 @@ class IirtRate(C.Structure):
 IIRT_MAX_SECTIONS, IIRT_MAX_RATES, IIRT_MAX_DEPTH = 10, 16, 32   # B2L_IIRT_MAX_SECTIONS / _RATES / _DEPTH
 
 
+class PiptrackDesc(C.Structure):
+    """struct b2l_piptrack_desc (include/b2l.h)."""
+    _fields_ = [("f64", C.c_int32), ("layout_c", C.c_int32), ("k_lo", C.c_int32), ("k_hi", C.c_int32),
+                ("abs_mode", C.c_int32), ("ref_frame", C.c_int32), ("thr_wide", C.c_int32), ("pad_", C.c_int32),
+                ("threshold", C.c_double), ("ref_abs", C.c_double), ("sr", C.c_double), ("n_fft", C.c_double)]
+
+
+PIPTRACK_MAX_ROW_BYTES = 200 * 1024   # B2L_PIPTRACK_MAX_ROW_BYTES
+(ELEM_I8, ELEM_U8, ELEM_I16, ELEM_U16, ELEM_I32, ELEM_U32, ELEM_I64, ELEM_U64, ELEM_F32, ELEM_F64,
+ ELEM_BOOL) = range(11)   # enum b2l_elem_type: the element types of b2l_localext
+ELEM_TYPES = {np.dtype(t): i for i, t in enumerate((np.int8, np.uint8, np.int16, np.uint16, np.int32, np.uint32,
+                                                     np.int64, np.uint64, np.float32, np.float64, np.bool_))}
+
+
 class DeltaDesc(C.Structure):
     """struct b2l_delta_desc (include/b2l.h); the d_* fields are device pointers."""
     _fields_ = [("width", C.c_int32), ("sym", C.c_int32), ("interp", C.c_int32), ("f64", C.c_int32),
@@ -321,6 +335,8 @@ def _declare(lib):
         "b2l_yin_pick": (C.c_int, [_vp, P(YinDesc), _vp, _i64, _vp]),
         "b2l_pyin_obs": (C.c_int, [_vp, P(PyinDesc), _vp, _i64, _vp, _vp, _vp, _vp]),
         "b2l_viterbi": (C.c_int, [_vp, P(PyinDesc), _vp, _vp, _vp, _vp, _i64, _i64, _vp, _vp, _vp]),
+        "b2l_piptrack": (C.c_int, [_vp, P(PiptrackDesc), _vp, _i64, C.c_int32, _i64, _vp, _vp]),
+        "b2l_pitch_tuning": (C.c_int, [_vp, _vp, _i64, C.c_int32, C.c_double, C.c_int32, _vp, _vp]),
         "b2l_tempogram": (C.c_int, [_vp, P(TempogramDesc), _vp, _i64, _i64, _vp, _vp]),
         "b2l_tempo": (C.c_int, [_vp, P(TempoDesc), _vp, _i64, _vp, _vp, _vp]),
         "b2l_beat_track": (C.c_int, [_vp, P(BeatDesc), _vp, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp]),
@@ -348,6 +364,7 @@ def _declare(lib):
         "b2l_iirt_stmsp": (C.c_int, [_vp, P(IirtRate), C.c_int32, _i64, _i64, C.c_int32, _vp]),
         "b2l_delta": (C.c_int, [_vp, P(DeltaDesc), _vp, _i64, _i64, _i64, _vp]),
         "b2l_stack_memory": (C.c_int, [_vp, P(StackDesc), _vp, _i64, _i64, _i64, _vp, _vp]),
+        "b2l_localext": (C.c_int, [_vp, _vp, C.c_int32, C.c_int32, _i64, _i64, _i64, _vp]),
         "b2l_chroma_fold": (C.c_int, [_vp, P(ChromaDesc), _vp, _i64, _i64, _vp]),
         "b2l_chroma_smooth": (C.c_int, [_vp, _vp, _i64, C.c_int32, _i64, C.c_int32, _vp, _vp, C.c_int32, C.c_int32,
                                         C.c_int32, C.c_double, _vp]),

@@ -1,10 +1,12 @@
 """``librosa.estimate_tuning`` (reference: librosa/core/pitch.py:28-109, on top of ``piptrack`` :182-366 and
-``pitch_tuning`` :112-179), as needed by ``feature.chroma_stft``; the pitch trackers ``yin`` and ``pyin``
-(:369-968) further down.
+``pitch_tuning`` :112-179), as needed by ``feature.chroma_stft``; the public ``piptrack`` and ``pitch_tuning``; the
+pitch trackers ``yin`` and ``pyin`` (:369-968) further down.
 
-The peak picking and parabolic interpolation of ``piptrack`` run on the GPU over the whole spectrogram; the
-peak list is never materialised.  The median magnitude that gates the peaks is found exactly by radix selection
-over three histogram passes, the tuning by one residual-histogram pass; the host only reads those histograms."""
+Inside ``estimate_tuning`` the peak picking and parabolic interpolation of ``piptrack`` run on the GPU over the whole
+spectrogram and the peak list is never materialised.  The median magnitude that gates the peaks is found exactly by
+radix selection over three histogram passes, the tuning by one residual-histogram pass; the host only reads those
+histograms.  The public ``piptrack`` writes the dense ``(pitches, mags)`` pair in one launch, in the reference's
+roundings (csrc/pitch_kernels.cuh piptrack_kernel); ``pitch_tuning`` is one histogram launch."""
 from __future__ import annotations
 
 import ctypes as C
@@ -123,6 +125,158 @@ def estimate_tuning(*, y=None, sr: float = 22050, S=None, n_fft: Optional[int] =
         if staged is not None:
             staged.check_finite()
         return est
+
+
+# --------------------------------------------------------------------------------------------- piptrack
+_GRADIENT_TOO_SMALL = ("Shape of array too small to calculate a numerical gradient, at least (edge_order + 1) elements "
+                       "are required.")
+
+
+def _piptrack_desc(F, n_fft, dtype, *, sr, fmin, fmax, threshold, ref):
+    """The b2l_piptrack_desc of one call, after the reference's checks in its order (fft_frequencies, np.gradient's
+    length check, then the reference value); refuses a callable ``ref`` other than np.max and rows too long for
+    shared memory, all before any device work."""
+    fmin = np.maximum(fmin, 0)
+    fmax = np.minimum(fmax, float(sr) / 2)
+    freqs = fft_frequencies(sr=sr, n_fft=n_fft)
+    if F < 2:
+        raise ValueError(_GRADIENT_TOO_SMALL)
+    mask = np.flatnonzero((fmin <= freqs) & (freqs < fmax))
+    desc = nat.PiptrackDesc(f64=int(dtype == np.float64), k_lo=int(mask[0]) if mask.size else 0,
+                            k_hi=int(mask[-1]) + 1 if mask.size else 0, sr=float(sr), n_fft=float(n_fft))
+    if ref is None or ref is np.max:
+        # threshold * np.max(S, axis=-2) in NumPy's promotion: a Python float stays in S's dtype, a float64 scalar
+        # widens the product of a float32 spectrogram
+        desc.ref_frame, desc.threshold = 1, float(threshold)
+        desc.thr_wide = int(dtype == np.float32 and np.result_type(threshold, np.float32) == np.float64)
+    elif callable(ref):
+        raise nat.UnsupportedOnGPU("piptrack(ref=callable) other than np.max is not supported on the GPU")
+    else:
+        desc.ref_abs = float(np.abs(ref))   # S > |ref| compares in float64 (|ref| is a float64 or int64 scalar)
+    if ((F + 3) & ~3) * dtype.itemsize > nat.PIPTRACK_MAX_ROW_BYTES:
+        raise nat.UnsupportedOnGPU(f"piptrack: a row of {F} {dtype} bins does not fit in shared memory on the GPU")
+    return desc
+
+
+def piptrack(*, y=None, sr: float = 22050, S=None, n_fft: Optional[int] = 2048, hop_length: Optional[int] = None,
+             fmin: float = 150.0, fmax: float = 4000.0, threshold: float = 0.1, win_length: Optional[int] = None,
+             window="hann", center: bool = True, pad_mode="constant", ref=None):
+    """Pitch tracking on the thresholded, parabolically interpolated STFT; same contract as ``librosa.piptrack``.
+
+    ``S`` (..., bins, frames) is a host array (float32, float64, or complex: taken as ``|S|``) or a float32 / float64
+    DeviceArray in layout "c" or "ft"; ``y`` a host or device signal (float64 is computed in float32, see
+    ``B2L_FLOAT64``).  ``ref`` is None / ``np.max`` (``threshold`` times the frame maximum) or a number; other
+    callables are refused with UnsupportedOnGPU.  Returns ``(pitches, mags)`` shaped like ``S`` and zero off the
+    peaks: C-ordered NumPy arrays for host input, "ft" DeviceArrays for device input."""
+    from .spectrum import _spectrogram
+
+    on_device = isinstance(S if S is not None else y, nat.DeviceArray)
+    staged = None
+    layout_c = 0
+    if S is None:
+        if n_fft is None:
+            raise ParameterError(f"Unable to compute spectrogram with n_fft={n_fft}")
+        if y is None:
+            raise ParameterError("Input signal must be provided to compute a spectrogram")
+        fr = pl.forward_front(y, n_fft, hop_length, win_length, window, center, pad_mode, native_ok=False)
+        pl.require_supported_n_fft(n_fft)
+        out_dtype, dtype, abs_mode = fr.dtype, np.dtype(np.float32), 0
+        shape = tuple(y.shape[:-1]) + (1 + n_fft // 2, fr.n_frames)
+    else:
+        if not on_device:
+            S = np.asarray(S)
+        if n_fft is None or n_fft // 2 + 1 != S.shape[-2]:
+            n_fft = 2 * (S.shape[-2] - 1)
+        dtype = np.dtype(S.dtype)
+        if on_device:
+            if dtype not in (np.float32, np.float64):
+                raise nat.UnsupportedOnGPU(f"piptrack: device S must be float32 or float64, got {dtype}")
+            if S.size == 0:
+                raise ValueError("zero-size array to reduction operation minimum which has no identity")
+            abs_mode, layout_c = 2, int(S.layout == "c")          # S.min() < 0 is decided on the device
+        else:
+            if np.iscomplexobj(S):
+                S, abs_mode = np.abs(S), 0
+            else:
+                abs_mode = int(bool(S.min() < 0))               # the reference's test, and its error on empty S
+            dtype = np.dtype(S.dtype)
+            if dtype not in (np.float32, np.float64):
+                raise nat.UnsupportedOnGPU(f"piptrack: S of dtype {dtype} is not supported on the GPU (float32, "
+                                           "float64 or complex)")
+        out_dtype, shape = dtype, tuple(S.shape)
+    desc = _piptrack_desc(shape[-2], n_fft, dtype, sr=sr, fmin=fmin, fmax=fmax, threshold=threshold, ref=ref)
+    desc.abs_mode = abs_mode
+    with pl.Scope(y if S is None else S) as sc:
+        if S is None:
+            staged = pl.StagedInput(y)
+            sc.own(staged.dev)
+            Sd, _ = _spectrogram(y=staged.dev, n_fft=n_fft, hop_length=hop_length, power=1, win_length=win_length,
+                                 window=window, center=center, pad_mode=pad_mode)
+            sc.own(Sd)
+            staged.scan_uncovered(n_fft, hop_length, win_length, center, Sd.shape[-1])
+        elif on_device:
+            Sd = S
+        else:
+            ft = np.swapaxes(S, -1, -2)
+            layout_c = int(not ft.flags.c_contiguous)          # upload the memory as it is when it is [frame][bin]
+            Sd = sc.stage(S if layout_c else ft, dtype)
+        desc.layout_c = layout_c
+        pitches = sc.empty(shape, dtype, layout="ft")
+        mags = sc.empty(shape, dtype, layout="ft")
+        nat.check(nat.lib().b2l_piptrack(sc.ctx.handle, C.byref(desc), _vp(Sd.ptr), pl.clip_count(shape[:-2]),
+                                         shape[-2], shape[-1], _vp(pitches.ptr), _vp(mags.ptr)))
+        if on_device:
+            return sc.result(pitches), sc.result(mags)
+        out = tuple(np.ascontiguousarray(sc.result(d), dtype=out_dtype) for d in (pitches, mags))
+        if staged is not None:
+            staged.check_finite()
+        return out
+
+
+_EMPTY_TUNING = "Trying to estimate tuning from empty frequency set."
+
+
+def pitch_tuning(frequencies, *, resolution: float = 0.01, bins_per_octave: int = 12) -> float:
+    """Tuning offset (fractions of a bin) of a collection of frequencies; same contract as ``librosa.pitch_tuning``.
+
+    ``frequencies``: a host array of any shape (integer input is taken as float64, as NumPy promotes it) or a float32
+    / float64 DeviceArray.  The residual histogram is one launch; resolutions finer than 1/2048 are refused with
+    UnsupportedOnGPU."""
+    on_device = isinstance(frequencies, nat.DeviceArray)
+    if not on_device:
+        frequencies = np.atleast_1d(frequencies)
+        if frequencies.dtype.kind in "biu":
+            frequencies = frequencies.astype(np.float64)
+    dtype = np.dtype(frequencies.dtype)
+    if dtype not in (np.float32, np.float64):
+        raise nat.UnsupportedOnGPU(f"pitch_tuning: frequencies of dtype {dtype} are not supported on the GPU")
+    deferred = None   # the reference raises these only after finding the frequency set non-empty
+    try:
+        edges = np.linspace(-0.5, 0.5, int(np.ceil(1.0 / resolution)) + 1)
+        if len(edges) < 2:
+            raise ValueError("attempt to get argmax of an empty sequence")
+    except Exception as e:
+        if not on_device:   # decided on the host, before any device work
+            if not np.any(frequencies > 0):
+                warnings.warn(_EMPTY_TUNING, stacklevel=2)
+                return 0.0
+            raise
+        edges, deferred = np.linspace(-0.5, 0.5, 2), e
+    if len(edges) - 1 > 2048:
+        raise nat.UnsupportedOnGPU("tuning resolution finer than 1/2048 is not supported on the GPU")
+    n_bins = len(edges) - 1
+    counts = (C.c_uint64 * (n_bins + 1))()
+    with pl.Scope(frequencies) as sc:
+        d = sc.stage(frequencies)
+        nat.check(nat.lib().b2l_pitch_tuning(sc.ctx.handle, _vp(d.ptr), d.size, int(dtype == np.float64),
+                                             float(bins_per_octave), n_bins, edges.ctypes.data_as(_vp), counts))
+    counts = np.frombuffer(counts, dtype=np.uint64).astype(np.int64)
+    if counts[n_bins] == 0:
+        warnings.warn(_EMPTY_TUNING, stacklevel=2)
+        return 0.0
+    if deferred is not None:
+        raise deferred
+    return edges[int(np.argmax(counts[:n_bins]))]
 
 
 # --------------------------------------------------------------------------------------------- yin / pyin

@@ -1,5 +1,6 @@
 // featutil_api.cu — C ABI of the feature-stacking utilities (featutil_kernels.cuh): librosa.feature.delta and
-// librosa.feature.stack_memory (librosa/feature/utils.py).  The only unit that includes featutil_kernels.cuh.
+// librosa.feature.stack_memory (librosa/feature/utils.py), and the peak test librosa.util.localmax / localmin.  The
+// only unit that includes featutil_kernels.cuh.
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <string.h>
@@ -29,6 +30,17 @@ int launch_stack(b2l_ctx* c, const b2l_featutil::StackArgs& a) {
   namespace F = b2l_featutil;
   const long long grid = grid_stride_blocks(a.rows * a.chunks, F::kWarps, 32LL * c->sm_count);
   return launch(c, F::stack_memory_kernel<S>, dim3((unsigned)grid), F::kThreads, 0, a);
+}
+
+template <class T>
+int launch_localext(b2l_ctx* c, const void* d_x, bool is_max, long long outer, long long n, long long inner,
+                    uint8_t* d_out) {
+  namespace F = b2l_featutil;
+  const long long total = outer * n * inner;
+  const unsigned grid = (unsigned)grid_stride_blocks(total, F::kThreads * 4, 32LL * c->sm_count);
+  if (inner == 1)
+    return launch(c, F::localext_kernel<T, true>, dim3(grid), F::kThreads, 0, (const T*)d_x, total, n, inner, is_max, d_out);
+  return launch(c, F::localext_kernel<T, false>, dim3(grid), F::kThreads, 0, (const T*)d_x, total, n, inner, is_max, d_out);
 }
 
 }  // namespace
@@ -95,5 +107,29 @@ extern "C" int b2l_stack_memory(b2l_ctx* c, const b2l_stack_desc* desc, const vo
     case 4: return launch_stack<4>(c, a);
     case 8: return launch_stack<8>(c, a);
     default: return launch_stack<16>(c, a);
+  }
+}
+
+extern "C" int b2l_localext(b2l_ctx* c, const void* d_x, int32_t type, int32_t is_max, int64_t outer, int64_t n,
+                            int64_t inner, uint8_t* d_out) {
+  if (!c) return fail(B2L_ERR_INVALID, "NULL argument");
+  if (outer < 0 || n < 2 || inner < 0) return fail(B2L_ERR_INVALID, "localext: bad geometry (the axis needs 2 or more values)");
+  if (outer == 0 || inner == 0) return B2L_OK;
+  if (!d_x || !d_out) return fail(B2L_ERR_INVALID, "NULL device pointer");
+  DeviceGuard g(c->device);
+  const bool mx = is_max != 0;
+  switch (type) {
+    case B2L_ELEM_I8: return launch_localext<int8_t>(c, d_x, mx, outer, n, inner, d_out);
+    case B2L_ELEM_U8: return launch_localext<uint8_t>(c, d_x, mx, outer, n, inner, d_out);
+    case B2L_ELEM_I16: return launch_localext<int16_t>(c, d_x, mx, outer, n, inner, d_out);
+    case B2L_ELEM_U16: return launch_localext<uint16_t>(c, d_x, mx, outer, n, inner, d_out);
+    case B2L_ELEM_I32: return launch_localext<int32_t>(c, d_x, mx, outer, n, inner, d_out);
+    case B2L_ELEM_U32: return launch_localext<uint32_t>(c, d_x, mx, outer, n, inner, d_out);
+    case B2L_ELEM_I64: return launch_localext<long long>(c, d_x, mx, outer, n, inner, d_out);
+    case B2L_ELEM_U64: return launch_localext<unsigned long long>(c, d_x, mx, outer, n, inner, d_out);
+    case B2L_ELEM_F32: return launch_localext<float>(c, d_x, mx, outer, n, inner, d_out);
+    case B2L_ELEM_F64: return launch_localext<double>(c, d_x, mx, outer, n, inner, d_out);
+    case B2L_ELEM_BOOL: return launch_localext<bool>(c, d_x, mx, outer, n, inner, d_out);
+    default: return fail(B2L_ERR_UNSUPPORTED, "localext: element type %d", type);
   }
 }

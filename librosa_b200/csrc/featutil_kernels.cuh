@@ -4,6 +4,7 @@
 //                         halo in its own shared-memory slot
 //   delta_strided_kernel  savgol_filter along a strided axis (inner > 1): one output per thread, threads along inner
 //   stack_memory_kernel   the gather of stack_memory: output (clip, step * d + row, i) <- input column i - step * delay
+//   localext_kernel       librosa.util.localmax / localmin along one axis (librosa/util/utils.py), one byte per element
 //
 // delta reproduces scipy.ndimage.convolve1d (which savgol_filter calls) bit for bit: every line is widened to double,
 // the reversed taps fw are applied in ndimage's fixed order with separately rounded multiplies and adds, and the sum is
@@ -224,6 +225,22 @@ __global__ void __launch_bounds__(kThreads) stack_memory_kernel(StackArgs a) {
 #pragma unroll
     for (int k = 0; k < kPer; ++k)
       if (i0 + 32 * k < a.t) yr[i0 + 32 * k] = v[k];
+  }
+}
+
+// librosa.util.localmax / localmin along the middle axis of x [outer][n][inner] (n >= 2) into one byte per element:
+// local_extremum (common.cuh) of each element and its neighbours on the line.  One output per thread in memory order;
+// CONTIG (inner == 1) spares the division by inner, as delta's row path does.
+template <class T, bool CONTIG>
+__global__ void __launch_bounds__(kThreads) localext_kernel(const T* __restrict__ x, long long total, long long n,
+                                                            long long inner, bool is_max, uint8_t* __restrict__ out) {
+  for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.x * blockDim.x) {
+    const long long j = CONTIG ? e % n : (e / inner) % n;
+    const long long s = CONTIG ? 1 : inner;
+    const T cur = x[e];
+    const T prev = j > 0 ? x[e - s] : cur;
+    const T next = j < n - 1 ? x[e + s] : cur;
+    out[e] = b2l::local_extremum(is_max, j, n, prev, cur, next);
   }
 }
 

@@ -1,5 +1,5 @@
 // pitch_api.cu — C ABI of the pitch trackers (pitch_kernels.cuh, include/b2l.h): librosa.yin and librosa.pyin as the
-// CMND, yin decision, pyin observation and Viterbi decoding launches.
+// CMND, yin decision, pyin observation and Viterbi decoding launches; librosa.piptrack and librosa.pitch_tuning.
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -189,4 +189,87 @@ extern "C" int b2l_viterbi(b2l_ctx* c, const b2l_pyin_desc* d, const int32_t* d_
   if ((rc = blocks_per_sm(c, viterbi_kernel, 256, smem, &occ, smem_limit))) return rc;
   if (occ < 1) return fail(B2L_ERR_UNSUPPORTED, "viterbi: %lld states do not fit on an SM", S);
   return launch(c, viterbi_kernel, (unsigned)n_clips, 256, smem, a);
+}
+
+template <class T>
+static int launch_piptrack(b2l_ctx* c, const b2l_piptrack_desc* d, const void* d_S, int64_t n_clips, int32_t F,
+                           int64_t n_frames, void* d_pitches, void* d_mags) {
+  const size_t per_warp = (size_t)((F + 3) & ~3) * sizeof(T);
+  if (per_warp > B2L_PIPTRACK_MAX_ROW_BYTES || per_warp > c->smem_optin)
+    return fail(B2L_ERR_UNSUPPORTED, "piptrack: a row of %d bins does not fit in shared memory", F);
+  int nw = 8;
+  while (nw > 1 && per_warp * nw > c->smem_optin) nw >>= 1;
+  const size_t smem = per_warp * nw;
+  PiptrackArgs<T> a;
+  a.S = (const T*)d_S;
+  a.n_rows = n_clips * n_frames;
+  a.n_frames = n_frames;
+  a.frame_stride = d->layout_c ? 1 : F;
+  a.bin_stride = d->layout_c ? n_frames : 1;
+  a.F = F;
+  a.k_lo = d->k_lo;
+  a.k_hi = d->k_hi;
+  a.abs_mode = d->abs_mode;
+  a.sign = nullptr;
+  a.ref_frame = d->ref_frame;
+  a.thr_wide = d->thr_wide;
+  a.threshold = d->threshold;
+  a.ref_abs = d->ref_abs;
+  a.sr = d->sr;
+  a.n_fft = d->n_fft;
+  a.pitches = (T*)d_pitches;
+  a.mags = (T*)d_mags;
+  if (d->abs_mode == 2) {   // S.min() < 0, decided on the device: one pass sets the sign word the main kernel reads
+    if (int rc = ensure_scratch(c, sizeof(unsigned))) return rc;
+    unsigned* word = reinterpret_cast<unsigned*>(c->d_scratch);
+    CUDA_TRY(cudaMemsetAsync(word, 0, sizeof(unsigned), c->stream));
+    const long long n = a.n_rows * F;
+    if (int rc = launch(c, sign_scan_kernel<T>, (unsigned)grid_stride_blocks(n, 256, 32LL * c->sm_count), 256, 0,
+                        a.S, n, word))
+      return rc;
+    a.sign = word;
+  }
+  long long grid = 0;
+  if (int rc = resident_grid(c, piptrack_kernel<T>, nw * 32, smem, (a.n_rows + nw - 1) / nw, &grid)) return rc;
+  if (!grid) return fail(B2L_ERR_UNSUPPORTED, "piptrack: a row of %d bins does not fit on an SM", F);
+  return launch(c, piptrack_kernel<T>, (unsigned)grid, nw * 32, smem, a);
+}
+
+extern "C" int b2l_piptrack(b2l_ctx* c, const b2l_piptrack_desc* d, const void* d_S, int64_t n_clips, int32_t n_bins,
+                            int64_t n_frames, void* d_pitches, void* d_mags) {
+  if (!c || !d) return fail(B2L_ERR_INVALID, "NULL argument");
+  if (n_clips < 0 || n_frames < 0 || n_bins < 2) return fail(B2L_ERR_INVALID, "piptrack: bad geometry");
+  if (d->k_lo < 0 || d->k_hi > n_bins) return fail(B2L_ERR_INVALID, "piptrack: bad bin range");
+  if (d->abs_mode < 0 || d->abs_mode > 2) return fail(B2L_ERR_INVALID, "piptrack: bad abs_mode %d", d->abs_mode);
+  if (n_clips == 0 || n_frames == 0) return B2L_OK;
+  if (!d_S || !d_pitches || !d_mags) return fail(B2L_ERR_INVALID, "NULL device pointer");
+  DeviceGuard g(c->device);
+  return d->f64 ? launch_piptrack<double>(c, d, d_S, n_clips, n_bins, n_frames, d_pitches, d_mags)
+                : launch_piptrack<float>(c, d, d_S, n_clips, n_bins, n_frames, d_pitches, d_mags);
+}
+
+extern "C" int b2l_pitch_tuning(b2l_ctx* c, const void* d_f, int64_t n, int32_t f64, double bins_per_octave,
+                                int32_t n_bins, const double* h_edges, uint64_t* h_counts) {
+  if (!c || !h_edges || !h_counts) return fail(B2L_ERR_INVALID, "NULL argument");
+  if (n_bins < 1 || n_bins > 2048) return fail(B2L_ERR_INVALID, "pitch_tuning: %d bins; 1 .. 2048 are supported", n_bins);
+  if (n < 0) return fail(B2L_ERR_INVALID, "pitch_tuning: bad length");
+  for (int i = 0; i <= n_bins; ++i) h_counts[i] = 0;
+  if (n == 0) return B2L_OK;
+  if (!d_f) return fail(B2L_ERR_INVALID, "NULL device pointer");
+  DeviceGuard g(c->device);
+  if (int rc = ensure_scratch(c, 2049 * sizeof(unsigned long long) + 2049 * sizeof(double))) return rc;
+  unsigned long long* d_counts = reinterpret_cast<unsigned long long*>(c->d_scratch);
+  double* d_edges = reinterpret_cast<double*>(d_counts + 2049);
+  CUDA_TRY(cudaMemsetAsync(d_counts, 0, (size_t)(n_bins + 1) * sizeof(unsigned long long), c->stream));
+  CUDA_TRY(cudaMemcpyAsync(d_edges, h_edges, (size_t)(n_bins + 1) * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+  const unsigned grid = (unsigned)grid_stride_blocks(n, 256, 16LL * c->sm_count);
+  int rc = f64 ? launch(c, tuning_hist_kernel<double>, grid, 256, 0, (const double*)d_f, (long long)n, bins_per_octave,
+                        (int)n_bins, (const double*)d_edges, d_counts)
+               : launch(c, tuning_hist_kernel<float>, grid, 256, 0, (const float*)d_f, (long long)n,
+                        (float)bins_per_octave, (int)n_bins, (const double*)d_edges, d_counts);
+  if (rc) return rc;
+  CUDA_TRY(cudaMemcpyAsync(h_counts, d_counts, (size_t)(n_bins + 1) * sizeof(unsigned long long), cudaMemcpyDeviceToHost,
+                           c->stream));
+  CUDA_TRY(cudaStreamSynchronize(c->stream));
+  return B2L_OK;
 }

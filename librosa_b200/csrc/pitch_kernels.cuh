@@ -1,9 +1,13 @@
-// pitch_kernels.cuh — librosa.yin / librosa.pyin (librosa/core/pitch.py:369-931, sequence.py:1174-1259).
+// pitch_kernels.cuh — librosa.yin / librosa.pyin (librosa/core/pitch.py:369-931, sequence.py:1174-1259), librosa.piptrack
+// and librosa.pitch_tuning (core/pitch.py:112-366).
 //
 //   yin_cmnd_kernel   frames -> cumulative mean normalised difference (CMND), float32 [row][lag]
 //   yin_pick_kernel   CMND -> f0 of yin (first threshold trough, else the global minimum, + parabolic shift)
 //   pyin_obs_kernel   CMND -> the voiced observation candidates of pyin (compact) and voiced_prob
 //   viterbi_kernel    candidates -> decoded state path, f0 and voiced flag of pyin (one CTA per clip, float64)
+//   piptrack_kernel   spectrogram rows -> the dense (pitches, mags) of librosa.piptrack (one warp per frame row)
+//   sign_scan_kernel  the S.min() < 0 verdict of a device spectrogram, for piptrack_kernel
+//   tuning_hist_kernel  frequencies -> the residual histogram of librosa.pitch_tuning
 //
 // A row is one (clip, frame) pair.  n_lags = max_period - min_period + 1 lags per row.
 #pragma once
@@ -478,6 +482,157 @@ __global__ void __launch_bounds__(256) viterbi_kernel(const ViterbiArgs a) {
       if (t > 0) s = a.ptr[row * S + s];
     }
   }
+}
+
+// ------------------------------------------------------------------ piptrack / pitch_tuning
+// librosa.piptrack (core/pitch.py:182-366) and librosa.pitch_tuning (:112-179) in the reference's roundings: every
+// operation the reference does in the spectrogram's type T is one separately rounded operation here (no contracted
+// FMA), and what it promotes to float64 is computed in float64 and rounded once.
+__device__ __forceinline__ float add_rn(float a, float b) { return __fadd_rn(a, b); }
+__device__ __forceinline__ double add_rn(double a, double b) { return __dadd_rn(a, b); }
+__device__ __forceinline__ float sub_rn(float a, float b) { return __fsub_rn(a, b); }
+__device__ __forceinline__ double sub_rn(double a, double b) { return __dsub_rn(a, b); }
+__device__ __forceinline__ float mul_rn(float a, float b) { return __fmul_rn(a, b); }
+__device__ __forceinline__ double mul_rn(double a, double b) { return __dmul_rn(a, b); }
+__device__ __forceinline__ float div_rn(float a, float b) { return __fdiv_rn(a, b); }
+__device__ __forceinline__ double div_rn(double a, double b) { return __ddiv_rn(a, b); }
+template <class T> __device__ __forceinline__ T from_double(double v);
+template <> __device__ __forceinline__ float from_double<float>(double v) { return __double2float_rn(v); }
+template <> __device__ __forceinline__ double from_double<double>(double v) { return v; }
+
+// Bits of b2l_piptrack's sign word: what S.min() < 0 needs (a NaN makes the minimum NaN, which is not < 0).
+constexpr unsigned kSignNegative = 1u, kSignNaN = 2u;
+
+// One pass over n values: sets kSignNegative when one is < 0 and kSignNaN when one is NaN.
+template <class T>
+__global__ void __launch_bounds__(256) sign_scan_kernel(const T* __restrict__ x, long long n, unsigned* __restrict__ word) {
+  unsigned bits = 0;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    const T v = __ldg(x + i);
+    bits |= (v < T(0) ? kSignNegative : 0u) | (v != v ? kSignNaN : 0u);
+  }
+  bits = __reduce_or_sync(0xffffffffu, bits);
+  if ((threadIdx.x & 31) == 0 && bits) atomicOr(word, bits);
+}
+
+// The reference's _parabolic_interpolation stencil at an interior bin with neighbours l and r: numba evaluates
+// a = (r + l) - 2 * c and b = (r - l) / 2 with the sums in T and the rest promoted to float64, returns 0 when
+// |b| >= |a| (NaN fails the test), else -b / a, and rounds the shift to T once when it is stored.
+template <class T>
+__device__ __forceinline__ T parabolic_shift(T l, T c, T r) {
+  const double a = __dsub_rn((double)add_rn(r, l), __dmul_rn(2.0, (double)c));
+  const double b = __dmul_rn((double)sub_rn(r, l), 0.5);
+  return fabs(b) >= fabs(a) ? T(0) : from_double<T>(__ddiv_rn(-b, a));
+}
+
+template <class T>
+struct PiptrackArgs {
+  const T* S;                // [clip] x (F bins, n_frames frames); bin k of frame t at t * frame_stride + k * bin_stride
+  long long n_rows;          // n_clips * n_frames
+  long long n_frames;
+  long long frame_stride, bin_stride;
+  int F;
+  int k_lo, k_hi;            // bins with fmin <= f < fmax
+  int abs_mode;              // 0 S as it is, 1 |S|, 2 |S| when the sign word says S.min() < 0
+  const unsigned* sign;      // abs_mode 2: the word sign_scan_kernel wrote
+  int ref_frame;             // 1: ref = threshold * max over the frame (np.max: NaN propagates), 0: ref_abs
+  int thr_wide;              // threshold * max in float64 (threshold a float64 scalar) rather than in T
+  double threshold, ref_abs;
+  double sr, n_fft;
+  T* pitches;                // [row][F]: zero off the peaks
+  T* mags;
+};
+
+// One warp per (clip, frame) row: the row goes through the warp's slot of shared memory (|.| applied), the frame
+// reference is formed, and every bin of both output rows is written: the interpolated peak where freq_mask &
+// localmax(S * (S > ref)) holds, zero elsewhere.  The product is formed literally, so inf * 0 is NaN.
+template <class T>
+__global__ void __launch_bounds__(256) piptrack_kernel(const PiptrackArgs<T> a) {
+  extern __shared__ __align__(16) unsigned char pip_smem[];
+  const int nw = blockDim.x >> 5, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int F = a.F;
+  T* s_row = reinterpret_cast<T*>(pip_smem) + (size_t)warp * ((F + 3) & ~3);
+  const bool use_abs = a.abs_mode == 1 || (a.abs_mode == 2 && (*a.sign & (kSignNegative | kSignNaN)) == kSignNegative);
+  const T thr_t = from_double<T>(a.threshold);   // NumPy's threshold * max in T (a Python float is cast to T)
+  for (long long r = (long long)blockIdx.x * nw + warp; r < a.n_rows; r += (long long)gridDim.x * nw) {
+    const long long clip = r / a.n_frames, t = r - clip * a.n_frames;
+    const T* src = a.S + clip * F * a.n_frames + t * a.frame_stride;
+    T mx = T(-INFINITY);
+    bool nan = false;
+    for (int i = lane; i < F; i += 32) {
+      T v = __ldg(src + i * a.bin_stride);
+      if (use_abs) v = fabs(v);
+      s_row[i] = v;
+      nan |= v != v;
+      mx = fmax(mx, v);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) mx = fmax(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+    if (__any_sync(0xffffffffu, nan)) mx = T(NAN);
+    __syncwarp();
+    double ref = a.ref_abs;
+    if (a.ref_frame) ref = a.thr_wide ? __dmul_rn(a.threshold, (double)mx) : (double)mul_rn(thr_t, mx);
+    T* po = a.pitches + r * F;
+    T* mo = a.mags + r * F;
+    for (int k = lane; k < F; k += 32) {
+      T pitch = T(0), mag = T(0);
+      if (k >= a.k_lo && k < a.k_hi && k > 0) {
+        const bool last = k == F - 1;
+        const T l = s_row[k - 1], c = s_row[k], rr = last ? c : s_row[k + 1];
+        auto thr = [&](T v) { return (double)v > ref ? v : mul_rn(v, T(0)); };   // S * (S > ref)
+        if (local_extremum(true, k, F, thr(l), thr(c), thr(rr))) {
+          T shift = T(0), avg;
+          if (last) {
+            avg = sub_rn(c, l);                                     // np.gradient: one-sided at the edge
+          } else {
+            avg = mul_rn(sub_rn(rr, l), T(0.5));                    // (S[k+1] - S[k-1]) / 2
+            shift = parabolic_shift(l, c, rr);
+          }
+          mag = add_rn(c, mul_rn(mul_rn(T(0.5), avg), shift));    // S + 0.5 * avg * shift
+          pitch = from_double<T>(__ddiv_rn(__dmul_rn(__dadd_rn((double)k, (double)shift), a.sr), a.n_fft));
+        }
+      }
+      po[k] = pitch;
+      mo[k] = mag;
+    }
+    __syncwarp();
+  }
+}
+
+// pitch_tuning's residual histogram: over the n values of f, count those > 0 (counts[n_bins]) and bin the residual
+// mod(bins_per_octave * log2(f / 27.5), 1), folded to [-0.5, 0.5), into n_bins <= 2048 bins with float64 edges and
+// np.histogram's rule (edges[b] <= x < edges[b + 1], the last bin closed).  The residual is computed in T with
+// np.mod's rounding (fmod, then + 1 when negative); log2 is the float64 log2 rounded to T.  A NaN residual (f = inf)
+// is dropped, as np.histogram drops it.
+template <class T>
+__global__ void __launch_bounds__(256) tuning_hist_kernel(const T* __restrict__ f, long long n, T bins_per_octave,
+                                                          int n_bins, const double* __restrict__ edges,
+                                                          unsigned long long* __restrict__ counts) {
+  __shared__ unsigned int s_cnt[2048];
+  for (int i = threadIdx.x; i < n_bins; i += blockDim.x) s_cnt[i] = 0;
+  __syncthreads();
+  unsigned int positive = 0;
+  for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (long long)gridDim.x * blockDim.x) {
+    const T v = __ldg(f + e);
+    if (!(v > T(0))) continue;
+    ++positive;
+    const T x = mul_rn(bins_per_octave, from_double<T>(log2((double)div_rn(v, T(27.5)))));
+    T res = fmod(x, T(1));
+    if (res < T(0)) res = add_rn(res, T(1));
+    else if (res == T(0)) res = T(0);
+    if (res >= T(0.5)) res = sub_rn(res, T(1));
+    if (res != res) continue;
+    int b = (int)floor(((double)res + 0.5) * n_bins);
+    b = max(0, min(n_bins - 1, b));
+    while (b > 0 && (double)res < edges[b]) --b;
+    while (b < n_bins - 1 && (double)res >= edges[b + 1]) ++b;
+    atomicAdd(&s_cnt[b], 1u);
+  }
+  positive = __reduce_add_sync(0xffffffffu, positive);
+  if ((threadIdx.x & 31) == 0 && positive) atomicAdd(&counts[n_bins], (unsigned long long)positive);
+  __syncthreads();
+  for (int i = threadIdx.x; i < n_bins; i += blockDim.x)
+    if (s_cnt[i]) atomicAdd(&counts[i], (unsigned long long)s_cnt[i]);
 }
 
 }  // namespace b2l

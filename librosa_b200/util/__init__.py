@@ -1,4 +1,5 @@
-"""``librosa.util`` names used on the FFT time-frequency path, ``peak_pick`` and ``fill_off_diagonal``."""
+"""``librosa.util`` names used on the FFT time-frequency path, ``peak_pick``, ``fill_off_diagonal`` and the peak test
+``localmax`` / ``localmin``."""
 from .exceptions import LibrosaError, ParameterError
 from .peak import peak_pick
 from .utils import (
@@ -11,6 +12,8 @@ from .utils import (
     fix_length,
     frame,
     is_positive_int,
+    localmax,
+    localmin,
     normalize,
     pad_center,
     tiny,
@@ -19,5 +22,5 @@ from .utils import (
 
 __all__ = [
     "LibrosaError", "ParameterError", "MAX_MEM_BLOCK", "abs2", "dtype_c2r", "dtype_r2c", "expand_to",
-    "fill_off_diagonal", "fix_length", "frame", "is_positive_int", "normalize", "pad_center", "peak_pick", "tiny", "valid_audio",
+    "fill_off_diagonal", "fix_length", "frame", "is_positive_int", "localmax", "localmin", "normalize", "pad_center", "peak_pick", "tiny", "valid_audio",
 ]

@@ -218,3 +218,49 @@ def fill_off_diagonal(x: np.ndarray, *, radius: float, value: float = 0) -> None
         idx_l = np.tril_indices_from(x, k=-radius - offset)
     x[idx_u] = value
     x[idx_l] = value
+
+
+def _localext(x, axis: int, is_max: bool):
+    """localmax / localmin on the GPU: one launch over ``x`` viewed as [outer][n][inner] along the logical ``axis``."""
+    import ctypes as C
+
+    from numpy.lib.array_utils import normalize_axis_index
+
+    from .. import _native as nat
+    from .. import _pipeline as pl
+
+    on_device = isinstance(x, nat.DeviceArray)
+    if not on_device:
+        x = np.asarray(x)
+    shape, dtype = tuple(x.shape), np.dtype(x.dtype)
+    ax = normalize_axis_index(axis, len(shape), msg_prefix="axis2")   # the AxisError of x.swapaxes(-1, axis)
+    if dtype not in nat.ELEM_TYPES:
+        raise nat.UnsupportedOnGPU(f"localmax / localmin: dtype {dtype} is not supported on the GPU (integers, float32, "
+                                   "float64, bool)")
+    if shape[ax] < 2:   # the reference's x[..., -2] on the rotated axis
+        raise IndexError(f"index -2 is out of bounds for axis {len(shape) - 1} with size {shape[ax]}")
+    layout = x.layout if on_device else "c"
+    mem = shape[:-2] + (shape[-1], shape[-2]) if layout == "ft" else shape
+    m = {len(shape) - 1: len(shape) - 2, len(shape) - 2: len(shape) - 1}.get(ax, ax) if layout == "ft" else ax
+    outer, n, inner = pl.clip_count(mem[:m]), mem[m], pl.clip_count(mem[m + 1:])
+    with pl.Scope(x) as sc:
+        out = sc.empty(shape, np.bool_, layout=layout)
+        if out.size:
+            d_x = sc.stage(x)
+            nat.check(nat.lib().b2l_localext(sc.ctx.handle, C.c_void_p(d_x.ptr), nat.ELEM_TYPES[dtype], int(is_max),
+                                             outer, n, inner, C.c_void_p(out.ptr)))
+        return sc.result(out)
+
+
+def localmax(x, *, axis: int = 0):
+    """Local maxima along ``axis``; same contract as ``librosa.util.localmax``: ``x[i] > x[i-1]`` and ``x[i] >=
+    x[i+1]``, never at the first element, ``x[-1] > x[-2]`` at the last.  Computed on the GPU for integer, float32,
+    float64 and bool data (other dtypes are refused with UnsupportedOnGPU).  ``x`` may be a host array or a
+    DeviceArray (layout "c" or "ft"); returns a bool array of the same shape, a DeviceArray of the same layout for
+    device input."""
+    return _localext(x, axis, True)
+
+
+def localmin(x, *, axis: int = 0):
+    """Local minima along ``axis``; same contract as ``librosa.util.localmin`` (``localmax`` mirrored)."""
+    return _localext(x, axis, False)

@@ -8,7 +8,8 @@ tests/golden/onset_v1.npz (tests/onset_cases.py), ``--sequence`` only tests/gold
 ``--cqt`` only tests/golden/cqt_v1.npz (tests/cqt_cases.py), ``--chroma`` only tests/golden/chroma_v1.npz
 (tests/chroma_cases.py), ``--iirt`` only tests/golden/iirt_v1.npz (tests/iirt_cases.py), ``--hybrid-cqt`` only
 tests/golden/hybrid_cqt_v1.npz (tests/hybrid_cqt_cases.py), and ``--feature-utils`` only
-tests/golden/feature_utils_v1.npz (tests/feature_utils_cases.py).
+tests/golden/feature_utils_v1.npz (tests/feature_utils_cases.py), and ``--piptrack`` only tests/golden/piptrack_v1.npz
+(tests/piptrack_cases.py).
 
 Needs a checkout of the reference (see tools/ref_shim.py); the tests only read the stored fixtures.  Also
 stores a handful of constant tables (mel bases, window sum-square, mel-scale known answers) produced by the
@@ -26,6 +27,7 @@ reference.
     python tools/make_golden.py --iirt
     python tools/make_golden.py --hybrid-cqt
     python tools/make_golden.py --feature-utils
+    python tools/make_golden.py --piptrack
 """
 from __future__ import annotations
 
@@ -600,6 +602,46 @@ def write_feature_utils():
     print("wrote", path, os.path.getsize(path), "bytes")
 
 
+def write_piptrack():
+    """tests/golden/piptrack_v1.npz: per case of tests/piptrack_cases.py that the GPU does not refuse, the reference's
+    piptrack result in sparse form (and, from y, its magnitude spectrogram), pitch_tuning value or localmax / localmin
+    mask, or its error (``<name>/error``)."""
+    import piptrack_cases as PC
+
+    ref = ref_shim.load_reference()
+    store = {}
+    for case in PC.CASES:
+        if case["refuse"]:
+            continue
+        name = case["name"]
+        with warnings.catch_warnings():
+            warnings.simplefilter("ignore")
+            try:
+                out = PC.call(ref, case)
+            except Exception as e:   # the reference's own error, stored as "Class: message"
+                store[f"{name}/error"] = np.array(f"{type(e).__name__}: {e}")
+                print(f"{name:40s} {store[f'{name}/error']}")
+                continue
+        if case["fn"] == "piptrack":
+            p, m = out
+            store[f"{name}/shape"] = np.array(p.shape, dtype=np.int64)
+            store[f"{name}/dtype"] = np.array(p.dtype.name)
+            store[f"{name}/idx"], store[f"{name}/p"], store[f"{name}/m"] = PC.sparse(p, m)
+            if case["y"] is not None:
+                kw = PC.piptrack_args(case)
+                store[f"{name}/S"] = ref.core.spectrum._spectrogram(
+                    y=kw["y"], n_fft=kw.get("n_fft", 2048), hop_length=kw.get("hop_length"), power=1,
+                    win_length=kw.get("win_length"), window=kw.get("window", "hann"), center=kw.get("center", True),
+                    pad_mode=kw.get("pad_mode", "constant"))[0]
+            print(f"{name:40s} {p.shape} {p.dtype} peaks={store[f'{name}/idx'].size}")
+        else:
+            store[f"{name}/out"] = np.asarray(out)
+            print(f"{name:40s} {store[f'{name}/out'].shape} {store[f'{name}/out'].dtype}")
+    path = os.path.join(ROOT, "tests", "golden", "piptrack_v1.npz")
+    np.savez_compressed(path, **store)
+    print("wrote", path, os.path.getsize(path), "bytes")
+
+
 if __name__ == "__main__":
     if "--pitch" in sys.argv[1:]:
         write_pitch()
@@ -623,5 +665,7 @@ if __name__ == "__main__":
         write_hybrid_cqt()
     elif "--feature-utils" in sys.argv[1:]:
         write_feature_utils()
+    elif "--piptrack" in sys.argv[1:]:
+        write_piptrack()
     else:
         main()
