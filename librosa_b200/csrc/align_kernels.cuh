@@ -16,7 +16,7 @@
 #include <float.h>
 #include <stdint.h>
 
-#include "argmax.cuh"
+#include "numerics.cuh"
 
 namespace b2l_align {
 using namespace b2l;
@@ -211,7 +211,7 @@ struct RqaRule {
     double bv = 0.0;
     int bi = kArgNone;
     if (s > (T)0) {
-      for (int k = 0; k < limit; ++k) argmax_merge(bv, bi, (double)score[at_c[k]], k);
+      for (int k = 0; k < limit; ++k) ArgmaxMerge()(bv, bi, (double)score[at_c[k]], k);
       score[at] = (T)__dadd_rn(bv, (double)s);
       ptr[at] = (signed char)bi;
     } else {
@@ -219,7 +219,7 @@ struct RqaRule {
         const double t = sim[at_c[k]] > (T)0 ? 1.0 : 0.0;
         const double v = __dsub_rn(__dsub_rn((double)score[at_c[k]], __dmul_rn(t, gap_onset)),
                                    __dmul_rn(1.0 - t, gap_extend));
-        argmax_merge(bv, bi, v, k);
+        ArgmaxMerge()(bv, bi, v, k);
       }
       const T out = (T)(bv > 0.0 ? bv : 0.0);
       score[at] = out;
@@ -271,9 +271,9 @@ __global__ void __launch_bounds__(32) dtw_walk_kernel(WalkArgs a) {
     bool all_inf = true;
     for (long long c = lane; c < a.m; c += 32) {
       all_inf &= isinf(row[c]);
-      argmax_merge(bv, bi, -row[c], c);
+      ArgmaxMerge()(bv, bi, -row[c], c);
     }
-    warp_argmax(bv, bi);
+    warp_select(bv, bi, ArgmaxMerge());
     all_inf = __all_sync(0xffffffffu, all_inf);
     if (a.check_end && all_inf) {
       if (lane == 0) *a.len = -kWalkAllInf;
@@ -321,8 +321,8 @@ __global__ void __launch_bounds__(kArgThreads) rqa_argmax_kernel(const T* score,
   const long long lo = (long long)blockIdx.x * per_block, hi = min(total, lo + per_block);
   double v = 0.0;
   long long idx = kArgNone64;
-  for (long long k = lo + threadIdx.x; k < hi; k += kArgThreads) argmax_merge(v, idx, (double)score[k], k);
-  block_argmax(v, idx, s_v, s_i);
+  for (long long k = lo + threadIdx.x; k < hi; k += kArgThreads) ArgmaxMerge()(v, idx, (double)score[k], k);
+  block_select(v, idx, s_v, s_i, ArgmaxMerge());
   if (threadIdx.x == 0) { part_v[blockIdx.x] = v; part_i[blockIdx.x] = idx; }
 }
 
@@ -337,8 +337,8 @@ __global__ void __launch_bounds__(kArgThreads) rqa_walk_kernel(const signed char
   __shared__ long long s_i[kArgThreads / 32];
   double v = 0.0;
   long long idx = kArgNone64;
-  for (int k = threadIdx.x; k < n_parts; k += kArgThreads) argmax_merge(v, idx, part_v[k], part_i[k]);
-  block_argmax(v, idx, s_v, s_i);
+  for (int k = threadIdx.x; k < n_parts; k += kArgThreads) ArgmaxMerge()(v, idx, part_v[k], part_i[k]);
+  block_select(v, idx, s_v, s_i, ArgmaxMerge());
   if (threadIdx.x != 0) return;
   const long long i0 = idx / m, j0 = idx % m;
   for (int pass = 0; pass < 2; ++pass) {

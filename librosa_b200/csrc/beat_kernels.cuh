@@ -17,8 +17,10 @@
 #include <stdint.h>
 
 #include "../../include/b2l.h"
+#include "numerics.cuh"
 
 namespace b2l_beat {
+using namespace b2l;
 
 struct BeatArgs {
   const void* env;          // [clips][n]
@@ -42,15 +44,6 @@ struct BeatArgs {
   int hop_length;
   double sr;
 };
-
-__device__ __forceinline__ float add_rn(float a, float b) { return __fadd_rn(a, b); }
-__device__ __forceinline__ double add_rn(double a, double b) { return __dadd_rn(a, b); }
-__device__ __forceinline__ float sub_rn(float a, float b) { return __fsub_rn(a, b); }
-__device__ __forceinline__ double sub_rn(double a, double b) { return __dsub_rn(a, b); }
-__device__ __forceinline__ float mul_rn(float a, float b) { return __fmul_rn(a, b); }
-__device__ __forceinline__ double mul_rn(double a, double b) { return __dmul_rn(a, b); }
-__device__ __forceinline__ float sqrt_rn(float a) { return __fsqrt_rn(a); }
-__device__ __forceinline__ double sqrt_rn(double a) { return __dsqrt_rn(a); }
 
 // NumPy's pairwise summation (numpy/_core/src/umath/loops_utils.h.src) of f(0) .. f(n-1) in T, one thread.  The
 // recursion splits at n/2 rounded down to a multiple of 8 until a block holds at most 128 elements; it is walked
@@ -109,6 +102,7 @@ __device__ __forceinline__ int half_even(int fpb) {
   return (fpb & 1) ? ((k & 1) ? k + 1 : k) : k;
 }
 
+// local_extremum (numerics.cuh) gives the same result, but its eagerly loaded neighbours change beat_track_kernel's code
 template <class T>
 __device__ __forceinline__ bool is_localmax(const T* x, int i, int n) {
   if (i == 0) return false;   // util.localmax pads with the edge value: x[0] > x[0] never holds
@@ -119,7 +113,8 @@ struct Cand {
   double s;
   int loc;
 };
-// the reference scans loc downward and keeps the first strictly larger score: ties go to the larger loc
+// the reference scans loc downward and keeps the first strictly larger score: ties go to the larger loc.  Kept with
+// its own butterfly below: warp_select (numerics.cuh), with this rule or a merge calling it, changes the kernel's code.
 __device__ __forceinline__ Cand better(Cand a, Cand b) {
   if (b.loc < 0) return a;
   if (a.loc < 0) return b;
@@ -158,8 +153,7 @@ __global__ void __launch_bounds__(256) beat_track_kernel(BeatArgs a) {
     });
     const int dof = n - 1 > 0 ? n - 1 : 0;
     const T var = (T)((double)ss / (double)dof);
-    const T tiny = sizeof(T) == 4 ? (T)1.17549435e-38f : (T)2.2250738585072014e-308;
-    s_denom = add_rn(sqrt_rn(var), tiny);
+    s_denom = add_rn(sqrt_rn(var), tiny_of<T>());
     s_count = 0;
     s_first = n;
     s_med[0] = s_med[1] = TC(0);
@@ -195,7 +189,7 @@ __global__ void __launch_bounds__(256) beat_track_kernel(BeatArgs a) {
       if (v != v) nan = true;
       else m = fmax(m, v);
     }
-    for (int o = 16; o; o >>= 1) m = fmax(m, __shfl_xor_sync(0xffffffffu, m, o));
+    m = warp_reduce(m, [](double u, double v) { return fmax(u, v); });
     nan = __any_sync(0xffffffffu, nan);
     if (lane == 0) s_red[warp] = nan ? NAN : m;
     __syncthreads();
@@ -279,7 +273,7 @@ __global__ void __launch_bounds__(256) beat_track_kernel(BeatArgs a) {
       for (int i = tid; i < n; i += nt)
         if (is_localmax(cum, i, n) && cum[i] >= thr) tail = i;
     }
-    for (int o = 16; o; o >>= 1) tail = max(tail, __shfl_xor_sync(0xffffffffu, tail, o));
+    tail = warp_reduce(tail, [](int u, int v) { return max(u, v); });
     if (lane == 0) s_ired[warp] = tail;
     __syncthreads();
     if (tid == 0) {
@@ -342,10 +336,7 @@ __global__ void any_nonzero_kernel(const T* __restrict__ x, long long n, int* __
 }
 
 // ---- librosa.beat.plp (beat.py:320-507) -------------------------------------------------------------------------
-__device__ __forceinline__ float cabs_(float2 z) { return hypotf(z.x, z.y); }
-__device__ __forceinline__ double cabs_(double2 z) { return hypot(z.x, z.y); }
-__device__ __forceinline__ float log1p_(float x) { return log1pf(x); }
-__device__ __forceinline__ double log1p_(double x) { return log1p(x); }
+// np.max with a NaN: a canonical NaN here, not MaxNan's NaN operand (numerics.cuh), which changes plp_select's code
 template <class R> __device__ __forceinline__ R rmax_nan(R a, R b) { return (a != a || b != b) ? (R)NAN : (a > b ? a : b); }
 
 // One warp per (row, frame) of a Fourier tempogram X [rows * frames][n_bins] (bins contiguous, C = float2 or
@@ -370,7 +361,7 @@ __global__ void plp_select_kernel(C* __restrict__ X, long long n_frames, int n_b
     if (logprior) m = (R)((double)m + logprior[b]);
     peak = rmax_nan(peak, m);
   }
-  for (int o = 16; o; o >>= 1) peak = rmax_nan(peak, (R)__shfl_xor_sync(0xffffffffu, peak, o));
+  peak = warp_reduce(peak, [](R u, R v) { return rmax_nan(u, v); });
   R mre = (R)-INFINITY, mim = (R)-INFINITY;
   bool first = true;
   for (int b = lane; b < n_bins; b += 32) {
@@ -383,6 +374,7 @@ __global__ void plp_select_kernel(C* __restrict__ X, long long n_frames, int n_b
     if (first || z.x > mre || (z.x == mre && z.y > mim)) { mre = z.x; mim = z.y; }
     first = false;
   }
+  // not warp_select (numerics.cuh): with this rule as its merge it changes the kernel's code
   for (int o = 16; o; o >>= 1) {
     const R ore = (R)__shfl_xor_sync(0xffffffffu, mre, o), oim = (R)__shfl_xor_sync(0xffffffffu, mim, o);
     if (ore > mre || (ore == mre && oim > mim)) { mre = ore; mim = oim; }
@@ -417,6 +409,7 @@ __global__ void plp_finish_kernel(T* __restrict__ x, int n, int* __restrict__ st
     if (!isfinite(v)) bad = true;
     else m = v > m ? v : m;
   }
+  // not warp_reduce (numerics.cuh): it changes the float instance's code
   for (int o = 16; o; o >>= 1) {
     const T other = __shfl_xor_sync(0xffffffffu, m, o);
     m = other > m ? other : m;
@@ -427,8 +420,7 @@ __global__ void plp_finish_kernel(T* __restrict__ x, int n, int* __restrict__ st
   if (threadIdx.x == 0) {
     T r = T(0);
     for (int w = 0; w < (int)(blockDim.x >> 5); ++w) r = s_max[w] > r ? s_max[w] : r;
-    const T tiny = sizeof(T) == 4 ? (T)1.17549435e-38f : (T)2.2250738585072014e-308;
-    s_max[0] = r < tiny ? T(1) : r;
+    s_max[0] = r < tiny_of<T>() ? T(1) : r;
     if (s_bad) atomicOr(status, B2L_STATUS_NOT_FINITE_VALUE);
   }
   __syncthreads();

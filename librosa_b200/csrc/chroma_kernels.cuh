@@ -15,7 +15,10 @@
 #pragma once
 #include <stdint.h>
 
+#include "numerics.cuh"
+
 namespace b2l_chroma {
+using namespace b2l;
 
 constexpr int kThreads = 256;
 
@@ -45,9 +48,6 @@ struct FoldArgs {
   void* out;               // [clip][n_chroma][T] chroma dtype, or [clip][6][T] double (tonnetz)
   int* status;
 };
-
-template <class T>
-__device__ __forceinline__ T tiny_of() { return sizeof(T) == 4 ? (T)1.17549435e-38f : (T)2.2250738585072014e-308; }
 
 // numpy's array ** scalar: the fast paths of its scalar power, else pow
 __device__ __forceinline__ double np_pow(double x, double e) {
@@ -80,8 +80,9 @@ __device__ double column_length(const T* v, int stride, int n, int kind, double 
 
 template <class In>
 struct Mag;
+// |x| of complex64, correctly rounded through double: not cqt's np_abs (NumPy's x86 loop) nor plp's cabs_ (hypotf)
 template <>
-struct Mag<float2> {   // |x| of complex64, correctly rounded through double
+struct Mag<float2> {
   typedef float R;
   static __device__ __forceinline__ float get(float2 v) {
     const double re = v.x, im = v.y;

@@ -196,14 +196,4 @@ __host__ __device__ inline float key_to_float(unsigned int k) {
 #endif
 }
 
-// librosa.util.localmax / localmin at position i of a line of n >= 2 values (librosa/util/utils.py:1029-1178): never
-// at i = 0; cur > prev and cur >= next inside the line (cur < prev and cur <= next for a minimum); cur > prev alone at
-// i = n - 1, where `next` is ignored.  A NaN compares false.  piptrack_kernel and localext_kernel share this test.
-template <class T>
-__device__ __forceinline__ bool local_extremum(bool is_max, long long i, long long n, T prev, T cur, T next) {
-  if (i == 0) return false;
-  if (is_max) return cur > prev && (i == n - 1 || cur >= next);
-  return cur < prev && (i == n - 1 || cur <= next);
-}
-
 }  // namespace b2l

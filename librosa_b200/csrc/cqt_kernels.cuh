@@ -32,7 +32,7 @@ constexpr int kDivide = 0x10;   // B2L_CQT_DIVIDE
 // np.abs of complex64 as NumPy's vectorised loop computes it on x86 (AVX2 / AVX-512 with FMA): the larger part
 // times sqrt(fma(r, r, 1)), r the smaller part over the larger, in float32.  It is not always the correctly rounded
 // |z| (about a third of random inputs differ from it by one ulp), so the projection does not use the chroma fold's
-// correctly rounded Mag.
+// correctly rounded Mag, nor plp's cabs_ (hypotf, numerics.cuh).
 __device__ __forceinline__ float np_abs(float2 v) {
   const float re = fabsf(v.x), im = fabsf(v.y);
   if (isinf(re) || isinf(im)) return INFINITY;

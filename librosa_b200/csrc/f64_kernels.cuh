@@ -12,6 +12,7 @@
 
 #include "common.cuh"
 #include "fft64.cuh"
+#include "numerics.cuh"
 
 namespace b2l {
 
@@ -219,8 +220,7 @@ __global__ void mel64_kernel(const double* __restrict__ S, const float* __restri
     const MelBand b = band[m];
     double acc = 0.0;
     for (int i = lane; i < b.len; i += 32) acc = fma((double)mel_w[b.off + i], row[b.lo + i], acc);
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+    acc = warp_reduce(acc, [](double u, double v) { return u + v; });
     if (lane == 0) out[(clip * n_mels + m) * T + t] = acc;
   }
 }
@@ -246,8 +246,7 @@ __global__ void db64_kernel(const double* __restrict__ in, long long per_clip, d
     dst[i] = v;
     m = fmax(m, v);
   }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) m = fmax(m, __shfl_xor_sync(0xffffffffu, m, o));
+  m = warp_reduce(m, [](double u, double v) { return fmax(u, v); });
   if ((threadIdx.x & 31) == 0 && m > -INFINITY) atomicMax(clip_max + clip, double_to_key(m));
 }
 // np.maximum(log_spec, log_spec.max(per clip) - top_db) (:1875-1881)

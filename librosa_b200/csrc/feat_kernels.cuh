@@ -6,6 +6,7 @@
 // and a batched transpose used as a layout adapter.  Included by feature_api.cu only.
 #pragma once
 #include "common.cuh"
+#include "numerics.cuh"
 #include "stats.cuh"
 
 namespace b2l {
@@ -603,8 +604,7 @@ __global__ void pip_pass_kernel(const float* __restrict__ S, long long n_rows, i
       s_row[i] = v;
       mx = fmaxf(mx, v);
     }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+    mx = warp_reduce(mx, [](float u, float v) { return fmaxf(u, v); });
     __syncwarp();
     const float ref = a.ref_abs >= 0.0f ? a.ref_abs : a.threshold * mx;
     for (int k = a.k_lo + lane; k < a.k_hi; k += 32) {
@@ -912,8 +912,7 @@ __global__ void db_kernel(const float* __restrict__ in, long long per_clip, floa
     oc[i] = v;
     mx = fmaxf(mx, v);
   }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+  mx = warp_reduce(mx, [](float u, float v) { return fmaxf(u, v); });
   if ((threadIdx.x & 31) == 0 && mx > -INFINITY) atomicMax(clip_max + clip, float_to_key(mx));
 }
 

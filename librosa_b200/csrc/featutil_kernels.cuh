@@ -20,8 +20,10 @@
 #include <stdint.h>
 
 #include "common.cuh"
+#include "numerics.cuh"
 
 namespace b2l_featutil {
+using namespace b2l;
 
 constexpr int kMaxWidth = B2L_DELTA_MAX_WIDTH;
 constexpr int kThreads = 256;
@@ -52,16 +54,6 @@ struct DeltaArgs {
   int* status;
 };
 
-template <class T>
-__device__ __forceinline__ double widen(T v) { return (double)v; }
-
-template <class T>
-__device__ __forceinline__ T narrow(double v);
-template <>
-__device__ __forceinline__ float narrow<float>(double v) { return __double2float_rn(v); }
-template <>
-__device__ __forceinline__ double narrow<double>(double v) { return v; }
-
 // Sample p (-h <= p < n + h) of the padded line starting at xr, samples `stride` apart.
 template <class T>
 __device__ __forceinline__ double load_line(const T* __restrict__ xr, long long stride, long long p, const DeltaArgs& a) {
@@ -70,7 +62,7 @@ __device__ __forceinline__ double load_line(const T* __restrict__ xr, long long 
     if (src < 0) return a.cval;
     p = src;
   }
-  return widen(__ldg(xr + p * stride));
+  return (double)__ldg(xr + p * stride);
 }
 
 // ndimage's correlation at one output; X(jj) is the sample jj positions from it, fw points at the centre tap.
@@ -101,7 +93,7 @@ __device__ double interp_edge(const T* __restrict__ xr, long long stride, long l
   bool bad = false;
   double acc = 0.0;
   for (int k = 0; k < w; ++k) {
-    const double v = widen(__ldg(xw + k * stride));
+    const double v = (double)__ldg(xw + k * stride);
     bad |= !isfinite(v);
     const double t = __dmul_rn(__ldg(e + k), v);
     acc = k == 0 ? t : __dadd_rn(acc, t);
@@ -229,7 +221,7 @@ __global__ void __launch_bounds__(kThreads) stack_memory_kernel(StackArgs a) {
 }
 
 // librosa.util.localmax / localmin along the middle axis of x [outer][n][inner] (n >= 2) into one byte per element:
-// local_extremum (common.cuh) of each element and its neighbours on the line.  One output per thread in memory order;
+// local_extremum (numerics.cuh) of each element and its neighbours on the line.  One output per thread in memory order;
 // CONTIG (inner == 1) spares the division by inner, as delta's row path does.
 template <class T, bool CONTIG>
 __global__ void __launch_bounds__(kThreads) localext_kernel(const T* __restrict__ x, long long total, long long n,
@@ -240,7 +232,7 @@ __global__ void __launch_bounds__(kThreads) localext_kernel(const T* __restrict_
     const T cur = x[e];
     const T prev = j > 0 ? x[e - s] : cur;
     const T next = j < n - 1 ? x[e + s] : cur;
-    out[e] = b2l::local_extremum(is_max, j, n, prev, cur, next);
+    out[e] = local_extremum(is_max, j, n, prev, cur, next);
   }
 }
 

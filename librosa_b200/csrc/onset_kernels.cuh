@@ -18,38 +18,16 @@
 #include <stdint.h>
 
 #include "../../include/b2l.h"
+#include "numerics.cuh"
 
 namespace b2l_onset {
+using namespace b2l;
 
 // verdict flags (word 0 of the flags pair; word 1 is the pick count)
 constexpr int kNonzero = 1, kNonfinite = 2;
 constexpr int kGreedy = 0, kDpCount = 1, kDpValue = 2;
 constexpr int kChunk = 8192;              // frames per candidate bitmask in shared memory
 constexpr int kWords = kChunk / 32;
-
-__device__ __forceinline__ float sub_rn(float a, float b) { return __fsub_rn(a, b); }
-__device__ __forceinline__ double sub_rn(double a, double b) { return __dsub_rn(a, b); }
-__device__ __forceinline__ float add_rn(float a, float b) { return __fadd_rn(a, b); }
-__device__ __forceinline__ double add_rn(double a, double b) { return __dadd_rn(a, b); }
-__device__ __forceinline__ float div_rn(float a, float b) { return __fdiv_rn(a, b); }
-__device__ __forceinline__ double div_rn(double a, double b) { return __ddiv_rn(a, b); }
-template <class T> __device__ __forceinline__ bool finite_(T v) { return isfinite(v); }
-
-// np.min / np.max: NaN wins
-struct MinNan { template <class T> __device__ T operator()(T a, T b) const { return a != a ? a : (b != b ? b : (b < a ? b : a)); } };
-struct MaxNan { template <class T> __device__ T operator()(T a, T b) const { return a != a ? a : (b != b ? b : (b > a ? b : a)); } };
-
-template <class T, class Op>
-__device__ T block_reduce(T v, Op op, T* s_red) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
-  for (int o = 16; o; o >>= 1) v = op(v, __shfl_xor_sync(0xffffffffu, v, o));
-  __syncthreads();
-  if (lane == 0) s_red[warp] = v;
-  __syncthreads();
-  v = s_red[0];
-  for (int w = 1; w < nw; ++w) v = op(v, s_red[w]);
-  return v;
-}
 
 // One CTA per row of x [rows][n].  With out != NULL the row is normalised like onset_detect(normalize=True):
 // x - min(x) (NaN wins), divided by max of that difference (NaN wins) + tiny, every step in T.  flags[0] gets

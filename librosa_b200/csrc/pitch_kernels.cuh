@@ -13,9 +13,9 @@
 #pragma once
 #include <float.h>
 
-#include "argmax.cuh"
 #include "common.cuh"
 #include "fft_engine.cuh"
+#include "numerics.cuh"
 
 namespace b2l {
 
@@ -170,25 +170,17 @@ __device__ __forceinline__ double pitch_shift(const float* x, int i, int n) {
   return fabs(b) >= fabs(a) ? 0.0 : -b / a;
 }
 // np.argmin order: the first NaN wins, else the first minimum.
-__device__ __forceinline__ bool argmin_before(float va, int ia, float vb, int ib) {
-  const bool na = isnan(va), nb = isnan(vb);
-  if (na != nb) return na;
-  if (na) return ia < ib;
-  return va < vb || (va == vb && ia < ib);
-}
-__device__ __forceinline__ void warp_argmin(float& v, int& i) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    const float ov = __shfl_xor_sync(0xffffffffu, v, o);
-    const int oi = __shfl_xor_sync(0xffffffffu, i, o);
-    if (argmin_before(ov, oi, v, i)) { v = ov; i = oi; }
+struct ArgminMerge {
+  __device__ __forceinline__ void operator()(float& v, int& i, float ov, int oi) const {
+    if (before(ov, oi, v, i)) { v = ov; i = oi; }
   }
-}
-__device__ __forceinline__ double warp_sum_f64(double v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
+  static __device__ __forceinline__ bool before(float va, int ia, float vb, int ib) {
+    const bool na = isnan(va), nb = isnan(vb);
+    if (na != nb) return na;
+    if (na) return ia < ib;
+    return va < vb || (va == vb && ia < ib);
+  }
+};
 
 // Copies one CMND row into the warp's shared slice.
 __device__ __forceinline__ void load_row(float* dst, const float* src, int n, int lane) {
@@ -218,8 +210,8 @@ __global__ void __launch_bounds__(256) yin_pick_kernel(const float* __restrict__
       float bv = x[0];
       int bi = 0;
       for (int i = lane; i < n_lags; i += 32)
-        if (argmin_before(x[i], i, bv, bi)) { bv = x[i]; bi = i; }
-      warp_argmin(bv, bi);
+        if (ArgminMerge::before(x[i], i, bv, bi)) { bv = x[i]; bi = i; }   // the merge functor changes the code
+      warp_select(bv, bi, ArgminMerge());
       pick = bi;
     }
     if (lane == 0) f0[row] = sr / ((double)(min_period + pick) + pitch_shift(x, pick, n_lags));
@@ -299,10 +291,10 @@ __global__ void __launch_bounds__(128) pyin_obs_kernel(const PyinObsArgs a) {
         else lo = mid + 1;
       }
       s_cls[q] = lo - 1;
-      if (gi == 0x7fffffff || argmin_before(h, q, gv, gi)) { gv = h; gi = q; }
+      if (gi == 0x7fffffff || ArgminMerge::before(h, q, gv, gi)) { gv = h; gi = q; }
     }
     if (gi == 0x7fffffff) gv = __int_as_float(0x7f800000);   // lanes without a trough: +inf, index past the end
-    warp_argmin(gv, gi);
+    warp_select(gv, gi, ArgminMerge());
     for (int j = lane; j < T; j += 32) {
       int c = 0;
       for (int q = 0; q < n_tr; ++q) c += s_cls[q] <= j;
@@ -323,7 +315,7 @@ __global__ void __launch_bounds__(128) pyin_obs_kernel(const PyinObsArgs a) {
           }
         }
       }
-      acc = warp_sum_f64(acc);
+      acc = warp_reduce(acc, [](double u, double v) { return u + v; });
       if (lane == 0) s_p[q] = acc;
     }
     __syncwarp();
@@ -466,8 +458,8 @@ __global__ void __launch_bounds__(256) viterbi_kernel(const ViterbiArgs a) {
   // ---- first argmax of the last row (np.argmax: the first NaN, else the first maximum)
   double bv = -INFINITY;
   int bi = kArgNone;
-  for (int j = tid; j < S; j += nt) argmax_merge(bv, bi, prev[j], j);
-  block_argmax(bv, bi, s_red_v, s_red_i);
+  for (int j = tid; j < S; j += nt) ArgmaxMerge()(bv, bi, prev[j], j);
+  block_select(bv, bi, s_red_v, s_red_i, ArgmaxMerge());
   if (tid == 0) {
     // ---- backtrace and the state -> (f0, voiced) map (:844-850)
     int s = bi;
@@ -488,17 +480,6 @@ __global__ void __launch_bounds__(256) viterbi_kernel(const ViterbiArgs a) {
 // librosa.piptrack (core/pitch.py:182-366) and librosa.pitch_tuning (:112-179) in the reference's roundings: every
 // operation the reference does in the spectrogram's type T is one separately rounded operation here (no contracted
 // FMA), and what it promotes to float64 is computed in float64 and rounded once.
-__device__ __forceinline__ float add_rn(float a, float b) { return __fadd_rn(a, b); }
-__device__ __forceinline__ double add_rn(double a, double b) { return __dadd_rn(a, b); }
-__device__ __forceinline__ float sub_rn(float a, float b) { return __fsub_rn(a, b); }
-__device__ __forceinline__ double sub_rn(double a, double b) { return __dsub_rn(a, b); }
-__device__ __forceinline__ float mul_rn(float a, float b) { return __fmul_rn(a, b); }
-__device__ __forceinline__ double mul_rn(double a, double b) { return __dmul_rn(a, b); }
-__device__ __forceinline__ float div_rn(float a, float b) { return __fdiv_rn(a, b); }
-__device__ __forceinline__ double div_rn(double a, double b) { return __ddiv_rn(a, b); }
-template <class T> __device__ __forceinline__ T from_double(double v);
-template <> __device__ __forceinline__ float from_double<float>(double v) { return __double2float_rn(v); }
-template <> __device__ __forceinline__ double from_double<double>(double v) { return v; }
 
 // Bits of b2l_piptrack's sign word: what S.min() < 0 needs (a NaN makes the minimum NaN, which is not < 0).
 constexpr unsigned kSignNegative = 1u, kSignNaN = 2u;
@@ -522,7 +503,7 @@ template <class T>
 __device__ __forceinline__ T parabolic_shift(T l, T c, T r) {
   const double a = __dsub_rn((double)add_rn(r, l), __dmul_rn(2.0, (double)c));
   const double b = __dmul_rn((double)sub_rn(r, l), 0.5);
-  return fabs(b) >= fabs(a) ? T(0) : from_double<T>(__ddiv_rn(-b, a));
+  return fabs(b) >= fabs(a) ? T(0) : narrow<T>(__ddiv_rn(-b, a));
 }
 
 template <class T>
@@ -553,7 +534,7 @@ __global__ void __launch_bounds__(256) piptrack_kernel(const PiptrackArgs<T> a) 
   const int F = a.F;
   T* s_row = reinterpret_cast<T*>(pip_smem) + (size_t)warp * ((F + 3) & ~3);
   const bool use_abs = a.abs_mode == 1 || (a.abs_mode == 2 && (*a.sign & (kSignNegative | kSignNaN)) == kSignNegative);
-  const T thr_t = from_double<T>(a.threshold);   // NumPy's threshold * max in T (a Python float is cast to T)
+  const T thr_t = narrow<T>(a.threshold);   // NumPy's threshold * max in T (a Python float is cast to T)
   for (long long r = (long long)blockIdx.x * nw + warp; r < a.n_rows; r += (long long)gridDim.x * nw) {
     const long long clip = r / a.n_frames, t = r - clip * a.n_frames;
     const T* src = a.S + clip * F * a.n_frames + t * a.frame_stride;
@@ -566,8 +547,7 @@ __global__ void __launch_bounds__(256) piptrack_kernel(const PiptrackArgs<T> a) 
       nan |= v != v;
       mx = fmax(mx, v);
     }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) mx = fmax(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+    mx = warp_reduce(mx, [](T u, T v) { return fmax(u, v); });
     if (__any_sync(0xffffffffu, nan)) mx = T(NAN);
     __syncwarp();
     double ref = a.ref_abs;
@@ -589,7 +569,7 @@ __global__ void __launch_bounds__(256) piptrack_kernel(const PiptrackArgs<T> a) 
             shift = parabolic_shift(l, c, rr);
           }
           mag = add_rn(c, mul_rn(mul_rn(T(0.5), avg), shift));    // S + 0.5 * avg * shift
-          pitch = from_double<T>(__ddiv_rn(__dmul_rn(__dadd_rn((double)k, (double)shift), a.sr), a.n_fft));
+          pitch = narrow<T>(__ddiv_rn(__dmul_rn(__dadd_rn((double)k, (double)shift), a.sr), a.n_fft));
         }
       }
       po[k] = pitch;
@@ -616,7 +596,7 @@ __global__ void __launch_bounds__(256) tuning_hist_kernel(const T* __restrict__ 
     const T v = __ldg(f + e);
     if (!(v > T(0))) continue;
     ++positive;
-    const T x = mul_rn(bins_per_octave, from_double<T>(log2((double)div_rn(v, T(27.5)))));
+    const T x = mul_rn(bins_per_octave, narrow<T>(log2((double)div_rn(v, T(27.5)))));
     T res = fmod(x, T(1));
     if (res < T(0)) res = add_rn(res, T(1));
     else if (res == T(0)) res = T(0);

@@ -12,6 +12,7 @@
 
 #include "../../include/b2l.h"
 #include "fft64.cuh"
+#include "numerics.cuh"
 
 namespace b2l {
 
@@ -31,20 +32,6 @@ struct TempogramArgs {
 __host__ __device__ inline size_t tempogram_smem_doubles(int log2m, int win) {
   const size_t M = (size_t)1 << log2m;
   return 2 * M + (M + 1) + (size_t)win + 32;
-}
-
-// Block-wide reduction of one double per thread in a fixed order (the same result on every run); red holds 32.
-template <class Op>
-__device__ double block_reduce64(double v, double* red, Op op) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = (blockDim.x + 31) >> 5;
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v = op(v, __shfl_xor_sync(0xffffffffu, v, o));
-  if (lane == 0) red[warp] = v;
-  __syncthreads();
-  double r = red[0];
-  for (int i = 1; i < nw; ++i) r = op(r, red[i]);
-  __syncthreads();
-  return r;
 }
 
 // One CTA per (row, frame):
@@ -117,12 +104,24 @@ __global__ void tempogram_kernel(const TempogramArgs a) {
       default: break;
     }
   }
+  // Block-wide reduction in a fixed order (the same result on every run).  Not block_reduce (numerics.cuh): this one
+  // has its barrier after the read rather than before the write, and moving it changes the kernel's code.
+  auto reduce = [&](double v, auto op) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = (blockDim.x + 31) >> 5;
+    v = warp_reduce(v, op);
+    if (lane == 0) red[warp] = v;
+    __syncthreads();
+    double r = red[0];
+    for (int i = 1; i < nw; ++i) r = op(r, red[i]);
+    __syncthreads();
+    return r;
+  };
   double length = 1.0;
-  if (a.norm == B2L_TG_NORM_MAX) length = block_reduce64(part, red, [](double u, double v) { return fmax(u, v); });
-  else if (a.norm == B2L_TG_NORM_MIN) length = block_reduce64(part, red, [](double u, double v) { return fmin(u, v); });
-  else if (a.norm == B2L_TG_NORM_COUNT) length = block_reduce64(part, red, [](double u, double v) { return u + v; });
+  if (a.norm == B2L_TG_NORM_MAX) length = reduce(part, [](double u, double v) { return fmax(u, v); });
+  else if (a.norm == B2L_TG_NORM_MIN) length = reduce(part, [](double u, double v) { return fmin(u, v); });
+  else if (a.norm == B2L_TG_NORM_COUNT) length = reduce(part, [](double u, double v) { return u + v; });
   else if (a.norm == B2L_TG_NORM_P)
-    length = pow(block_reduce64(part, red, [](double u, double v) { return u + v; }), 1.0 / a.norm_p);
+    length = pow(reduce(part, [](double u, double v) { return u + v; }), 1.0 / a.norm_p);
   if (length < DBL_MIN) length = 1.0;      // below tiny(float64): left as it is
   double* o = a.out + item * W;
   for (int k = threadIdx.x; k < W; k += blockDim.x) o[k] = p[k] / length;
@@ -144,21 +143,17 @@ __device__ __forceinline__ double tempo_score(double v, double lp) { return log1
 __device__ __forceinline__ double tempo_score(float v, double lp) { return (double)log1pf(1e6f * v) + lp; }
 
 // np.argmax order: NaN first, then the larger score, then the smaller lag
-__device__ __forceinline__ bool tempo_before(double v, int k, double bv, int bk) {
-  const bool vn = isnan(v), bn = isnan(bv);
-  if (vn != bn) return vn;
-  if (!vn && v != bv) return v > bv;
-  return k < bk;
-}
-
-__device__ __forceinline__ void tempo_warp_best(double& v, int& k) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    const double ov = __shfl_xor_sync(0xffffffffu, v, o);
-    const int ok = __shfl_xor_sync(0xffffffffu, k, o);
-    if (tempo_before(ov, ok, v, k)) { v = ov; k = ok; }
+struct TempoMerge {
+  __device__ __forceinline__ void operator()(double& bv, int& bk, double v, int k) const {
+    if (before(v, k, bv, bk)) { bv = v; bk = k; }
   }
-}
+  static __device__ __forceinline__ bool before(double v, int k, double bv, int bk) {
+    const bool vn = isnan(v), bn = isnan(bv);
+    if (vn != bn) return vn;
+    if (!vn && v != bv) return v > bv;
+    return k < bk;
+  }
+};
 
 // aggregate=np.mean: one CTA per row.  Each thread owns lags and sums their frames in increasing order, so the
 // result does not depend on scheduling; the mean of a float32 tempogram is rounded to float32.
@@ -174,16 +169,17 @@ __global__ void tempo_mean_kernel(const TempoArgs a) {
     const T* gk = g + k * a.lag_stride;
     double s = 0.0;
     for (int f = 0; f < a.n_frames; ++f) s += (double)gk[f * a.frame_stride];
-    const double sc = tempo_score((T)(s / (double)a.n_frames), a.logprior[k]);
-    if (tempo_before(sc, k, best, bk)) { best = sc; bk = k; }
+    TempoMerge()(best, bk, tempo_score((T)(s / (double)a.n_frames), a.logprior[k]), k);
   }
-  tempo_warp_best(best, bk);
+  warp_select(best, bk, TempoMerge());
+  // not block_select (numerics.cuh): its warp count rounds blockDim up, which changes this kernel's code; the merge
+  // functor in the loop below changes it too, so the loop applies TempoMerge::before itself
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   if (lane == 0) { s_v[warp] = best; s_k[warp] = bk; }
   __syncthreads();
   if (threadIdx.x == 0) {
     for (int i = 1; i < (int)(blockDim.x >> 5); ++i)
-      if (tempo_before(s_v[i], s_k[i], best, bk)) { best = s_v[i]; bk = s_k[i]; }
+      if (TempoMerge::before(s_v[i], s_k[i], best, bk)) { best = s_v[i]; bk = s_k[i]; }
     a.out[row] = a.bpms[bk];
   }
 }
@@ -200,10 +196,9 @@ __global__ void tempo_frames_kernel(const TempoArgs a) {
   double best = -INFINITY;
   int bk = 0x7fffffff;
   for (int k = lane; k < a.n_lags; k += 32) {
-    const double sc = tempo_score(g[k * a.lag_stride], a.logprior[k]);
-    if (tempo_before(sc, k, best, bk)) { best = sc; bk = k; }
+    TempoMerge()(best, bk, tempo_score(g[k * a.lag_stride], a.logprior[k]), k);
   }
-  tempo_warp_best(best, bk);
+  warp_select(best, bk, TempoMerge());
   if (lane == 0) a.out[warp] = a.bpms[bk];
 }
 

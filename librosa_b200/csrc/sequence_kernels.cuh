@@ -11,7 +11,7 @@
 #pragma once
 #include <float.h>
 
-#include "argmax.cuh"
+#include "numerics.cuh"
 
 namespace b2l_seq {
 using namespace b2l;
@@ -179,7 +179,7 @@ __global__ void __launch_bounds__(128) viterbi_small_kernel(const DecodeArgs a) 
   }
   double bv = v;
   int bi = j < S ? j : kArgNone;
-  warp_argmax<W>(bv, bi);
+  warp_select<W>(bv, bi, ArgmaxMerge());
   __syncwarp();   // the group's back-pointer stores are visible to its lane 0
   if (live && j == 0) {
     a.logp[p] = bv;
@@ -248,8 +248,8 @@ __global__ void __launch_bounds__(256) viterbi_cta_kernel(const DecodeArgs a) {
   for (int g = 0; g < G; ++g) {
     double bv = -INFINITY;
     int bi = kArgNone;
-    for (int j = tid; j < S; j += nt) argmax_merge(bv, bi, last[g * S + j], j);
-    block_argmax(bv, bi, s_rv, s_ri);
+    for (int j = tid; j < S; j += nt) ArgmaxMerge()(bv, bi, last[g * S + j], j);
+    block_select(bv, bi, s_rv, s_ri, ArgmaxMerge());
     if (tid == 0) { s_last[g] = bi; s_logp[g] = bv; }
     __syncthreads();
   }
