@@ -830,6 +830,59 @@ int b2l_f64_dct(b2l_ctx* ctx, const double* d_L, int64_t n_clips, int32_t n_mels
 int b2l_nnls_mel(b2l_ctx* ctx, const float* d_mel, int64_t n_clips, int64_t n_frames, int32_t n_mels, int32_t n_bins,
                  const float* h_basis, const float* h_pinv, float step, int32_t n_iter, float inv_power, float* d_out);
 
+/* ---- nearest neighbours (segment.recurrence_matrix, decompose.nn_filter) ------------------------ */
+#define B2L_NN_MAX_FRAMES 65536       /* frames of one recurrence matrix */
+#define B2L_NN_MAX_CANDIDATES 4096    /* sklearn's n_neighbors = min(t - 1, k + 2 width) */
+#define B2L_NN_MAX_STATS 256          /* links per frame of the affinity bandwidth statistics (k + 1) */
+enum b2l_nn_metric { B2L_NN_EUCLIDEAN = 0, B2L_NN_COSINE = 1 };
+enum b2l_nn_bandwidth {
+  B2L_NN_BW_SCALAR = 0, B2L_NN_BW_MEAN_K = 1, B2L_NN_BW_GMEAN_K = 2, B2L_NN_BW_MEAN_K_AVG = 3,
+  B2L_NN_BW_GMEAN_K_AVG = 4, B2L_NN_BW_MEAN_K_AVG_AND_PAIR = 5, B2L_NN_BW_MED_K_SCALAR = 6
+};
+enum b2l_nn_aggregate { B2L_NN_MEAN = 0, B2L_NN_MEDIAN = 1, B2L_NN_AVERAGE = 2 };
+typedef struct b2l_nn_desc {
+  int32_t metric;        /* enum b2l_nn_metric */
+  int32_t mode;          /* 0 connectivity, 1 distance, 2 affinity */
+  int32_t k, width;
+  int32_t n_cand;        /* min(t - 1, k + 2 width) */
+  int32_t sym, self_link;
+  int32_t f64;           /* distances are rounded to float64 (else float32) before any statistic or output */
+  int32_t bw_mode;       /* enum b2l_nn_bandwidth (affinity mode) */
+  int32_t src_f64;       /* the source data is float64 (else float32) */
+  double bandwidth;      /* B2L_NN_BW_SCALAR */
+  /* feature f = lead * n_feat + g of frame i is src[lead * lead_stride + g * feat_stride + i * frame_stride] */
+  int64_t n_lead, n_feat, lead_stride, feat_stride, frame_stride;
+} b2l_nn_desc;
+/* librosa.segment.recurrence_matrix (segment.py:391-706) of t frames as a neighbour table: row i of d_idx / d_val
+ * [t][k_out] (k_out >= min(k, n_cand) + 1) holds the links of frame i (column i of the reference's csc_array),
+ * ascending frame index, d_count[i] of them; d_val is 1 (connectivity), the distance rounded to the output dtype
+ * (distance) or exp(-distance / bandwidth) in that dtype (affinity).  Float64 distances (FP64 tensor cores), d(i, j)
+ * == d(j, i) bit for bit; candidates in (distance, index) order.  Synchronises (finite check, bandwidth errors).
+ * Data with a NaN or an infinity sets *h_not_finite = 1 and computes nothing. */
+int b2l_nn_graph(b2l_ctx* ctx, const b2l_nn_desc* desc, const void* d_src, int64_t t, int32_t k_out, int32_t* d_idx,
+                 double* d_val, int32_t* d_count, int32_t* h_not_finite);
+typedef struct b2l_nn_filter_desc {
+  int32_t agg;           /* enum b2l_nn_aggregate */
+  int32_t s_f64;         /* S is float64 (else float32) */
+  int32_t r_f64;         /* np.average computes in float64 (np.result_type(S, weights)) */
+  int32_t max_count;     /* the largest neighbour count (median) */
+  int64_t stride;        /* entries of frame i start at i * stride when d_start is NULL */
+} b2l_nn_filter_desc;
+/* decompose.nn_filter's aggregation (decompose.py:550-592): d_S [n_lead][t][n_bins] ("ft"), frame i's neighbours
+ * d_idx[start_i .. start_i + d_count[i]) with weights d_w (values of the compute dtype; average only), out like S.
+ * *h_zero_weight = 1 when some frame's weights sum to zero (np.average raises; synchronises for average). */
+int b2l_nn_filter(b2l_ctx* ctx, const b2l_nn_filter_desc* desc, const void* d_S, int64_t n_lead, int64_t t,
+                  int64_t n_bins, const int64_t* d_start, const int32_t* d_count, const int32_t* d_idx,
+                  const double* d_w, void* d_out, int32_t* h_zero_weight);
+/* The dense C-ordered t x t matrix (B2L_ELEM_F32 / F64 / BOOL) of a b2l_nn_graph table: rec[j, i] = d_val of link
+ * (i, j), zero elsewhere. */
+int b2l_nn_dense(b2l_ctx* ctx, const int32_t* d_idx, const double* d_val, const int32_t* d_count, int64_t t,
+                 int32_t k_out, int32_t elem, void* d_rec);
+/* scipy.sparse.csc_array of a dense C-ordered t x t matrix (B2L_ELEM_F32 / F64 / BOOL): pass 0 writes the non-zero
+ * count of every column, pass 1 the rows (ascending) and values of column i at d_start[i]. */
+int b2l_nn_compact(b2l_ctx* ctx, const void* d_rec, int32_t elem, int64_t t, int32_t pass, int32_t* d_count,
+                   const int64_t* d_start, int32_t* d_idx, double* d_w);
+
 /* ---- multi-GPU split / join (one process per GPU; NCCL over NVLink) --------------------------- */
 /* 128-byte NCCL unique id, created on rank 0 and handed to the other ranks by the launcher. */
 int b2l_comm_unique_id(void* id128);

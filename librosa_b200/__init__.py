@@ -6,7 +6,7 @@ window_sumsquare``, ``util.frame`` (and the small helpers around them) with libr
 shapes, dtypes, warnings and exceptions.  The arithmetic runs in hand-written CUDA kernels reached
 through a C ABI (``include/b2l.h``) with ctypes — no PyTorch, no Triton, no CPU fallback.
 """
-from . import beat, core, decompose, effects, feature, filters, onset, sequence, util
+from . import beat, core, decompose, effects, feature, filters, onset, segment, sequence, util
 from ._native import (
     Context,
     DeviceArray,
@@ -48,7 +48,7 @@ def to_device(arr, device=None):
 
 
 __all__ = [
-    "stream", "resample", "stft", "istft", "griffinlim", "power_to_db", "amplitude_to_db", "pcen", "phase_vocoder", "reassigned_spectrogram", "db_to_power", "db_to_amplitude", "_spectrogram", "feature", "filters", "util", "core", "onset", "beat", "decompose", "effects", "sequence",
+    "stream", "resample", "stft", "istft", "griffinlim", "power_to_db", "amplitude_to_db", "pcen", "phase_vocoder", "reassigned_spectrogram", "db_to_power", "db_to_amplitude", "_spectrogram", "feature", "filters", "util", "core", "onset", "beat", "decompose", "effects", "segment", "sequence",
     "hz_to_mel", "mel_to_hz", "hz_to_octs", "estimate_tuning", "pitch_tuning", "piptrack", "yin", "pyin", "cqt", "vqt", "pseudo_cqt", "hybrid_cqt", "cqt_frequencies", "iirt", "mel_frequencies", "fft_frequencies", "tempo_frequencies", "fourier_tempo_frequencies", "frames_to_samples", "frames_to_time", "samples_to_time", "ParameterError", "LibrosaError",
     "Context", "DeviceArray", "default_context", "device_count", "pinned_empty", "to_device", "device_copy",
     "NativeLibraryError", "UnsupportedOnGPU", "bind_host_to_device",

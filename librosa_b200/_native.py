@@ -251,6 +251,32 @@ CHROMA_NORM_NONE, CHROMA_NORM_INF, CHROMA_NORM_NEG_INF, CHROMA_NORM_ZERO, CHROMA
 CHROMA_PLAIN, CHROMA_CENS, CHROMA_TONNETZ = range(3)   # enum b2l_chroma_epilogue
 
 
+class NnDesc(C.Structure):
+    """struct b2l_nn_desc (include/b2l.h)."""
+    _fields_ = [("metric", C.c_int32), ("mode", C.c_int32), ("k", C.c_int32), ("width", C.c_int32),
+                ("n_cand", C.c_int32), ("sym", C.c_int32), ("self_link", C.c_int32), ("f64", C.c_int32),
+                ("bw_mode", C.c_int32), ("src_f64", C.c_int32), ("bandwidth", C.c_double), ("n_lead", C.c_int64),
+                ("n_feat", C.c_int64), ("lead_stride", C.c_int64), ("feat_stride", C.c_int64),
+                ("frame_stride", C.c_int64)]
+
+
+class NnFilterDesc(C.Structure):
+    """struct b2l_nn_filter_desc (include/b2l.h)."""
+    _fields_ = [("agg", C.c_int32), ("s_f64", C.c_int32), ("r_f64", C.c_int32), ("max_count", C.c_int32),
+                ("stride", C.c_int64)]
+
+
+NN_MAX_FRAMES, NN_MAX_CANDIDATES, NN_MAX_STATS = 65536, 4096, 256   # B2L_NN_MAX_FRAMES / _CANDIDATES / _STATS
+NN_EUCLIDEAN, NN_COSINE = 0, 1                                         # enum b2l_nn_metric
+NN_METRICS = {"euclidean": NN_EUCLIDEAN, "cosine": NN_COSINE}
+(NN_BW_SCALAR, NN_BW_MEAN_K, NN_BW_GMEAN_K, NN_BW_MEAN_K_AVG, NN_BW_GMEAN_K_AVG, NN_BW_MEAN_K_AVG_AND_PAIR,
+ NN_BW_MED_K_SCALAR) = range(7)                                        # enum b2l_nn_bandwidth
+NN_BANDWIDTHS = {"mean_k": NN_BW_MEAN_K, "gmean_k": NN_BW_GMEAN_K, "mean_k_avg": NN_BW_MEAN_K_AVG,
+                 "gmean_k_avg": NN_BW_GMEAN_K_AVG, "mean_k_avg_and_pair": NN_BW_MEAN_K_AVG_AND_PAIR,
+                 "med_k_scalar": NN_BW_MED_K_SCALAR}
+NN_MEAN, NN_MEDIAN, NN_AVERAGE = range(3)                              # enum b2l_nn_aggregate
+
+
 DTW_METRICS = {"euclidean": 0, "sqeuclidean": 1, "cityblock": 2, "chebyshev": 3, "cosine": 4}   # enum b2l_dtw_metric
 BEAT_FRAMES, BEAT_SAMPLES, BEAT_TIME = range(3)   # enum b2l_beat_units
 SEQ_PLAIN, SEQ_DISC, SEQ_BINARY = range(3)        # enum b2l_seq_mode
@@ -365,6 +391,11 @@ def _declare(lib):
         "b2l_delta": (C.c_int, [_vp, P(DeltaDesc), _vp, _i64, _i64, _i64, _vp]),
         "b2l_stack_memory": (C.c_int, [_vp, P(StackDesc), _vp, _i64, _i64, _i64, _vp, _vp]),
         "b2l_localext": (C.c_int, [_vp, _vp, C.c_int32, C.c_int32, _i64, _i64, _i64, _vp]),
+        "b2l_nn_graph": (C.c_int, [_vp, P(NnDesc), _vp, _i64, C.c_int32, _vp, _vp, _vp, P(C.c_int32)]),
+        "b2l_nn_filter": (C.c_int, [_vp, P(NnFilterDesc), _vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp, _vp,
+                                    P(C.c_int32)]),
+        "b2l_nn_dense": (C.c_int, [_vp, _vp, _vp, _vp, _i64, C.c_int32, C.c_int32, _vp]),
+        "b2l_nn_compact": (C.c_int, [_vp, _vp, C.c_int32, _i64, C.c_int32, _vp, _vp, _vp, _vp]),
         "b2l_chroma_fold": (C.c_int, [_vp, P(ChromaDesc), _vp, _i64, _i64, _vp]),
         "b2l_chroma_smooth": (C.c_int, [_vp, _vp, _i64, C.c_int32, _i64, C.c_int32, _vp, _vp, C.c_int32, C.c_int32,
                                         C.c_int32, C.c_double, _vp]),

@@ -9,7 +9,7 @@ tests/golden/onset_v1.npz (tests/onset_cases.py), ``--sequence`` only tests/gold
 (tests/chroma_cases.py), ``--iirt`` only tests/golden/iirt_v1.npz (tests/iirt_cases.py), ``--hybrid-cqt`` only
 tests/golden/hybrid_cqt_v1.npz (tests/hybrid_cqt_cases.py), and ``--feature-utils`` only
 tests/golden/feature_utils_v1.npz (tests/feature_utils_cases.py), and ``--piptrack`` only tests/golden/piptrack_v1.npz
-(tests/piptrack_cases.py).
+(tests/piptrack_cases.py), ``--nn-filter`` only tests/golden/nn_filter_v1.npz (tests/nn_filter_cases.py).
 
 Needs a checkout of the reference (see tools/ref_shim.py); the tests only read the stored fixtures.  Also
 stores a handful of constant tables (mel bases, window sum-square, mel-scale known answers) produced by the
@@ -642,6 +642,39 @@ def write_piptrack():
     print("wrote", path, os.path.getsize(path), "bytes")
 
 
+def write_nn_filter():
+    """tests/golden/nn_filter_v1.npz: per case of tests/nn_filter_cases.py, the reference's recurrence matrix (csc
+    indptr / indices / data) and, for nn_filter cases, its output, or its error (``<name>/error``)."""
+    import nn_filter_cases as NC
+
+    ref = ref_shim.load_reference()
+    store = {}
+    for case in NC.CASES:
+        name = case["name"]
+        with warnings.catch_warnings():
+            warnings.simplefilter("ignore")
+            try:
+                out = NC.call(ref, case)
+            except Exception as e:   # the reference's own error, stored as "Class: message"
+                store[f"{name}/error"] = np.array(f"{type(e).__name__}: {e}")
+                print(f"{name:40s} {store[f'{name}/error']}")
+                if case["fn"] == "nn":   # the rec of a failing nn_filter case is still stored
+                    S, clean = NC.filter_input(case)
+                    out = (ref.segment.recurrence_matrix(clean, sparse=True, **case["rec_kw"]), None)
+                else:
+                    continue
+        rec, res = (out, None) if case["fn"] == "rec" else out
+        store[f"{name}/indptr"] = rec.indptr.astype(np.int64)
+        store[f"{name}/indices"] = rec.indices.astype(np.int32)
+        store[f"{name}/data"] = rec.data
+        if res is not None:
+            store[f"{name}/out"] = res
+        print(f"{name:40s} nnz={rec.nnz} {rec.dtype}")
+    path = os.path.join(ROOT, "tests", "golden", "nn_filter_v1.npz")
+    np.savez_compressed(path, **store)
+    print("wrote", path, os.path.getsize(path), "bytes")
+
+
 if __name__ == "__main__":
     if "--pitch" in sys.argv[1:]:
         write_pitch()
@@ -667,5 +700,7 @@ if __name__ == "__main__":
         write_feature_utils()
     elif "--piptrack" in sys.argv[1:]:
         write_piptrack()
+    elif "--nn-filter" in sys.argv[1:]:
+        write_nn_filter()
     else:
         main()
