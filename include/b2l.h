@@ -405,9 +405,10 @@ int b2l_sub(b2l_ctx* ctx, const float* d_x, const float* d_y, int64_t n, float* 
  *                   mag >= mag_threshold. */
 typedef struct b2l_pip_desc {
   int32_t k_lo, k_hi;      /* bins with fmin <= f < fmax */
-  float threshold;         /* peaks must exceed threshold * max over the frame ... */
-  float ref_abs;           /* ... or this absolute value when >= 0 (piptrack(ref=number)) */
-  double hz_per_bin;       /* sr / n_fft */
+  double threshold;        /* peaks must exceed threshold * max over the frame ... */
+  int32_t thr_wide;        /* ... formed in float64 (a float64 threshold) rather than in float32 ... */
+  double ref_abs;          /* ... or this absolute value when >= 0 (piptrack(ref=number)) */
+  double sr, n_fft;        /* pitch = (k + shift) * sr / n_fft */
   int32_t mode;
   uint32_t prefix;
   float mag_threshold;
@@ -419,7 +420,7 @@ int b2l_pip_pass(b2l_ctx* ctx, const b2l_pip_desc* desc, const float* d_S, int64
 /* util.normalize(x, norm, axis=-2) of [n_clips][n_rows][n_frames] (util/utils.py:797-1026, default threshold and
  * fill): norm_kind 0 = inf, 1 = -inf, 2 = number of non-zeros, 3 = p-norm (norm_p > 0). */
 int b2l_normalize_rows(b2l_ctx* ctx, const float* d_in, int64_t n_clips, int64_t n_rows, int64_t n_frames,
-                       int32_t norm_kind, float norm_p, float* d_out);
+                       int32_t norm_kind, double norm_p, float* d_out);
 /* ---- SURVEY 8f rank 3: harmonic / percussive separation, librosa.decompose.hpss (decompose.py:241-389) --------
  * d_mag [n_clips][n_frames][n_bins] magnitudes.  harm / perc = running medians over win_harm frames / win_perc
  * bins (scipy.ndimage.median_filter, reflect boundary), turned into soft masks (util.softmask, `power`, margins).

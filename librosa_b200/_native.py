@@ -94,8 +94,8 @@ class ContrastDesc(C.Structure):
 
 class PipDesc(C.Structure):
     """struct b2l_pip_desc (include/b2l.h)."""
-    _fields_ = [("k_lo", C.c_int32), ("k_hi", C.c_int32), ("threshold", C.c_float), ("ref_abs", C.c_float),
-                ("hz_per_bin", C.c_double), ("mode", C.c_int32), ("prefix", C.c_uint32), ("mag_threshold", C.c_float),
+    _fields_ = [("k_lo", C.c_int32), ("k_hi", C.c_int32), ("threshold", C.c_double), ("thr_wide", C.c_int32),
+                ("ref_abs", C.c_double), ("sr", C.c_double), ("n_fft", C.c_double), ("mode", C.c_int32), ("prefix", C.c_uint32), ("mag_threshold", C.c_float),
                 ("bins_per_octave", C.c_float), ("n_res_bins", C.c_int32)]
 
 
@@ -344,7 +344,7 @@ def _declare(lib):
         "b2l_spectral_contrast": (C.c_int, [_vp, P(ContrastDesc), _vp, _i64, _i64, C.c_int32, _vp, _vp]),
         "b2l_sub": (C.c_int, [_vp, _vp, _vp, _i64, _vp]),
         "b2l_pip_pass": (C.c_int, [_vp, P(PipDesc), _vp, _i64, C.c_int32, _vp, _vp]),
-        "b2l_normalize_rows": (C.c_int, [_vp, _vp, _i64, _i64, _i64, C.c_int32, C.c_float, _vp]),
+        "b2l_normalize_rows": (C.c_int, [_vp, _vp, _i64, _i64, _i64, C.c_int32, C.c_double, _vp]),
         "b2l_hpss": (C.c_int, [_vp, P(HpssDesc), _vp, _vp, _i64, _i64, _i64, _vp, _vp]),
         "b2l_cabs": (C.c_int, [_vp, _vp, _i64, _vp]),
         "b2l_reassign": (C.c_int, [_vp, P(ReassignDesc), _vp, _vp, _vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp, _vp]),

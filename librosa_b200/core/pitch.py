@@ -41,13 +41,10 @@ def _tuning_from_device_spec(Sd, sr, n_fft, *, resolution, bins_per_octave, fmin
         fmin = np.maximum(fmin, 0)
         fmax = np.minimum(fmax, float(sr) / 2)
         mask = np.flatnonzero((fmin <= freqs) & (freqs < fmax))
+        ref_frame, thr, thr_wide, ref_abs = _pip_reference(threshold, ref, np.dtype(np.float32))
         desc = nat.PipDesc(k_lo=int(mask[0]) if mask.size else 0, k_hi=int(mask[-1]) + 1 if mask.size else 0,
-                           threshold=float(threshold), ref_abs=-1.0, hz_per_bin=float(sr) / n_fft,
-                           bins_per_octave=float(bins_per_octave))
-        if ref is not None and ref is not np.max:
-            if callable(ref):
-                raise nat.UnsupportedOnGPU("piptrack(ref=callable) other than np.max is not supported on the GPU")
-            desc.ref_abs = float(np.abs(ref))
+                           threshold=thr, thr_wide=thr_wide, ref_abs=-1.0 if ref_frame else ref_abs, sr=float(sr),
+                           n_fft=float(n_fft), bins_per_octave=float(bins_per_octave))
         rows = pl.clip_count(Sd.shape[:-2]) * T
         hist = (C.c_uint64 * 2048)()
 
@@ -132,6 +129,18 @@ _GRADIENT_TOO_SMALL = ("Shape of array too small to calculate a numerical gradie
                        "are required.")
 
 
+def _pip_reference(threshold, ref, dtype):
+    """piptrack's reference level as (ref_frame, threshold, thr_wide, ref_abs); refuses a callable ``ref`` other
+    than np.max."""
+    if ref is None or ref is np.max:
+        # threshold * np.max(S, axis=-2) in NumPy's promotion: a Python float stays in S's dtype, a float64 scalar
+        # widens the product of a float32 spectrogram
+        return 1, float(threshold), int(dtype == np.float32 and np.result_type(threshold, np.float32) == np.float64), 0.0
+    if callable(ref):
+        raise nat.UnsupportedOnGPU("piptrack(ref=callable) other than np.max is not supported on the GPU")
+    return 0, 0.0, 0, float(np.abs(ref))   # S > |ref| compares in float64 (|ref| is a float64 or int64 scalar)
+
+
 def _piptrack_desc(F, n_fft, dtype, *, sr, fmin, fmax, threshold, ref):
     """The b2l_piptrack_desc of one call, after the reference's checks in its order (fft_frequencies, np.gradient's
     length check, then the reference value); refuses a callable ``ref`` other than np.max and rows too long for
@@ -144,15 +153,7 @@ def _piptrack_desc(F, n_fft, dtype, *, sr, fmin, fmax, threshold, ref):
     mask = np.flatnonzero((fmin <= freqs) & (freqs < fmax))
     desc = nat.PiptrackDesc(f64=int(dtype == np.float64), k_lo=int(mask[0]) if mask.size else 0,
                             k_hi=int(mask[-1]) + 1 if mask.size else 0, sr=float(sr), n_fft=float(n_fft))
-    if ref is None or ref is np.max:
-        # threshold * np.max(S, axis=-2) in NumPy's promotion: a Python float stays in S's dtype, a float64 scalar
-        # widens the product of a float32 spectrogram
-        desc.ref_frame, desc.threshold = 1, float(threshold)
-        desc.thr_wide = int(dtype == np.float32 and np.result_type(threshold, np.float32) == np.float64)
-    elif callable(ref):
-        raise nat.UnsupportedOnGPU("piptrack(ref=callable) other than np.max is not supported on the GPU")
-    else:
-        desc.ref_abs = float(np.abs(ref))   # S > |ref| compares in float64 (|ref| is a float64 or int64 scalar)
+    desc.ref_frame, desc.threshold, desc.thr_wide, desc.ref_abs = _pip_reference(threshold, ref, dtype)
     if ((F + 3) & ~3) * dtype.itemsize > nat.PIPTRACK_MAX_ROW_BYTES:
         raise nat.UnsupportedOnGPU(f"piptrack: a row of {F} {dtype} bins does not fit in shared memory on the GPU")
     return desc

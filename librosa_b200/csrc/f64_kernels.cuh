@@ -242,12 +242,13 @@ __global__ void db64_kernel(const double* __restrict__ in, long long per_clip, d
   double* dst = out + (long long)clip * per_clip;
   double m = -INFINITY;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < per_clip; i += (long long)gridDim.x * blockDim.x) {
-    const double v = 10.0 * log10(fmax(amin, src[i])) - db_sub;
+    const double v = 10.0 * log10(MaxNan()(amin, src[i])) - db_sub;
     dst[i] = v;
-    m = fmax(m, v);
+    m = MaxNan()(m, v);
   }
-  m = warp_reduce(m, [](double u, double v) { return fmax(u, v); });
-  if ((threadIdx.x & 31) == 0 && m > -INFINITY) atomicMax(clip_max + clip, double_to_key(m));
+  m = warp_reduce(m, MaxNan());
+  // a NaN maximum (np.maximum keeps a NaN cell) is the all-ones key: no finite key exceeds it, key_to_double reads NaN
+  if ((threadIdx.x & 31) == 0 && !(m == -INFINITY)) atomicMax(clip_max + clip, m != m ? ~0ull : double_to_key(m));
 }
 // np.maximum(log_spec, log_spec.max(per clip) - top_db) (:1875-1881)
 __global__ void db64_clamp_kernel(double* __restrict__ x, long long per_clip, double top_db,
@@ -256,7 +257,7 @@ __global__ void db64_clamp_kernel(double* __restrict__ x, long long per_clip, do
   double* dst = x + (long long)clip * per_clip;
   const double floor_v = key_to_double(clip_max[clip]) - top_db;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < per_clip; i += (long long)gridDim.x * blockDim.x)
-    dst[i] = fmax(dst[i], floor_v);
+    dst[i] = MaxNan()(dst[i], floor_v);
 }
 
 // C[c][k][t] = sum_m dct[k][m] L[c][m][t]   (scipy.fft.dct along the mel axis as an explicit matrix, lifter folded in)

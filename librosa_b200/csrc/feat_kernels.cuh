@@ -202,40 +202,44 @@ struct OnsetArgs {
   int bounds[33];
   int n_ch, lag, max_size, pad_width, n_rows, T;
 };
+// The flux of row m at lag frame tp: np.maximum(0, S[m][tp + lag] - ref[m][tp]), a NaN difference kept (as
+// np.maximum keeps it).  The max filter lets a NaN in the window through as NaN (np.maximum's rule; scipy's
+// running-max filter returns a NaN or skips it depending on where it sits in the window).
+__device__ __forceinline__ float onset_flux(const float* __restrict__ Sc, const OnsetArgs& a, int m, int tp) {
+  float ref;
+  if (a.max_size == 1) {
+    ref = Sc[(long long)m * a.T + tp];
+  } else {
+    ref = -INFINITY;
+    const int lo = m - a.max_size / 2;
+    for (int j = 0; j < a.max_size; ++j) {
+      int mm = lo + j;
+      while (mm < 0 || mm >= a.n_rows) mm = mm < 0 ? -mm - 1 : 2 * a.n_rows - mm - 1;
+      ref = MaxNan()(ref, Sc[(long long)mm * a.T + tp]);
+    }
+  }
+  const float d = sub_rn(Sc[(long long)m * a.T + tp + a.lag], ref);
+  return d != d ? d : fmaxf(0.0f, d);
+}
 __global__ void onset_kernel(const float* __restrict__ S, OnsetArgs a, float* __restrict__ out) {
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
   if (t >= a.T) return;
-  const long long clip = blockIdx.y;
+  const long long clip = blockIdx.y;   // the entry offsets S and out per slice of at most 65 535 clips
   const float* Sc = S + clip * (long long)a.n_rows * a.T;
   const int tp = t - a.pad_width;
   const bool live = tp >= 0 && tp + a.lag < a.T;
   const int n_out = a.n_ch > 0 ? a.n_ch : a.n_rows;
   float* oc = out + clip * (long long)n_out * a.T + t;
-  auto flux = [&](int m) -> float {
-    float ref;
-    if (a.max_size == 1) {
-      ref = Sc[(long long)m * a.T + tp];
-    } else {
-      ref = -INFINITY;
-      const int lo = m - a.max_size / 2;
-      for (int j = 0; j < a.max_size; ++j) {
-        int mm = lo + j;
-        while (mm < 0 || mm >= a.n_rows) mm = mm < 0 ? -mm - 1 : 2 * a.n_rows - mm - 1;
-        ref = fmaxf(ref, Sc[(long long)mm * a.T + tp]);
-      }
-    }
-    return fmaxf(0.0f, Sc[(long long)m * a.T + tp + a.lag] - ref);
-  };
   if (a.n_ch == 0) {
-    for (int m = 0; m < a.n_rows; ++m) oc[(long long)m * a.T] = live ? flux(m) : 0.0f;
+    for (int m = 0; m < a.n_rows; ++m) oc[(long long)m * a.T] = live ? onset_flux(Sc, a, m, tp) : 0.0f;
     return;
   }
   for (int c = 0; c < a.n_ch; ++c) {
     float acc = 0.0f;
     const int m0 = a.bounds[c], m1 = a.bounds[c + 1];
     if (live)
-      for (int m = m0; m < m1; ++m) acc += flux(m);
-    oc[(long long)c * a.T] = live && m1 > m0 ? acc / (float)(m1 - m0) : (live ? __int_as_float(0x7fc00000) : 0.0f);
+      for (int m = m0; m < m1; ++m) acc = add_rn(acc, onset_flux(Sc, a, m, tp));
+    oc[(long long)c * a.T] = live && m1 > m0 ? div_rn(acc, (float)(m1 - m0)) : (live ? __int_as_float(0x7fc00000) : 0.0f);
   }
 }
 // The same flux aggregated with np.median over each channel's rows (util.sync(..., aggregate=np.median)): for an
@@ -262,23 +266,7 @@ __global__ void onset_median_kernel(const float* __restrict__ S, OnsetArgs a, in
       const bool live = t < a.T && tp >= 0 && tp + a.lag < a.T;
       for (int r = r_ld; r < P; r += r_step) {
         float v = INFINITY;
-        if (r < R && live) {
-          const int m = m0 + r;
-          float ref;
-          if (a.max_size == 1) {
-            ref = Sc[(long long)m * a.T + tp];
-          } else {
-            ref = -INFINITY;
-            const int lo = m - a.max_size / 2;
-            for (int j = 0; j < a.max_size; ++j) {
-              int mm = lo + j;
-              while (mm < 0 || mm >= a.n_rows) mm = mm < 0 ? -mm - 1 : 2 * a.n_rows - mm - 1;
-              ref = fmaxf(ref, Sc[(long long)mm * a.T + tp]);
-            }
-          }
-          const float d = __fsub_rn(Sc[(long long)m * a.T + tp + a.lag], ref);
-          v = d != d ? d : fmaxf(0.0f, d);
-        }
+        if (r < R && live) v = onset_flux(Sc, a, m0 + r, tp);
         s_col[f_ld * (P + 1) + r] = v;
       }
     }
@@ -316,7 +304,8 @@ __global__ void onset_median_kernel(const float* __restrict__ S, OnsetArgs a, in
   }
 }
 
-// detrend: scipy.signal.lfilter([1, -1], [1, -0.99]) along time (direct form II transposed), one thread per row
+// detrend: scipy.signal.lfilter([1, -1], [1, -0.99]) along time (direct form II transposed), one thread per row,
+// in float32 with one rounding per operation (the error bound is derived in tests/test_gpu_feature_kernels_tail.py)
 __global__ void detrend_kernel(float* __restrict__ x, long long n_rows, int T) {
   const long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (r >= n_rows) return;
@@ -324,8 +313,8 @@ __global__ void detrend_kernel(float* __restrict__ x, long long n_rows, int T) {
   float z = 0.0f;
   for (int t = 0; t < T; ++t) {
     const float in = xr[t];
-    const float y = in + z;
-    z = -in + 0.99f * y;
+    const float y = add_rn(in, z);
+    z = sub_rn(mul_rn(0.99f, y), in);
     xr[t] = y;
   }
 }
@@ -576,11 +565,14 @@ __global__ void sub_kernel(const float* __restrict__ x, const float* __restrict_
 // the spectrogram (one warp per frame row) and accumulates one histogram —
 //   mode 0/1/2: radix-select digits (11 + 11 + 10 bits) of the order-preserving key of mag -> exact median
 //   mode 3:     residual histogram of the peaks with mag >= mag_threshold.
+// The peaks, their pitch and mag and the residual follow piptrack_kernel / tuning_hist_kernel's rules
+// (numerics.cuh), so a pass counts exactly what pitch_tuning would over the public piptrack's output.
 struct PipArgs {
   int k_lo, k_hi;
-  float threshold;          // relative to the frame maximum when ref_abs < 0, else unused
-  float ref_abs;            // >= 0: absolute reference value (piptrack(ref=number))
-  double hz_per_bin;        // sr / n_fft
+  double threshold;         // relative to the frame maximum when ref_abs < 0, else unused
+  double ref_abs;           // >= 0: absolute reference value (piptrack(ref=number)), compared in float64
+  int thr_wide;             // threshold * max in float64 rather than float32
+  double sr, n_fft;
   int mode;
   unsigned int prefix;      // digits selected so far (mode 1: top 11 bits, mode 2: top 22 bits)
   float mag_threshold;
@@ -594,6 +586,7 @@ __global__ void pip_pass_kernel(const float* __restrict__ S, long long n_rows, i
   const int nw = blockDim.x >> 5, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   float* s_row = s_dyn + (size_t)warp * ((F + 3) & ~3);
   const int n_hist = a.mode == 3 ? a.n_res_bins : (a.mode == 2 ? 1024 : 2048);
+  const float thr_t = narrow<float>(a.threshold);   // a Python float threshold is cast to float32
   for (int i = threadIdx.x; i < n_hist; i += blockDim.x) s_hist[i] = 0;
   __syncthreads();
   for (long long r = (long long)blockIdx.x * nw + warp; r < n_rows; r += (long long)gridDim.x * nw) {
@@ -602,32 +595,27 @@ __global__ void pip_pass_kernel(const float* __restrict__ S, long long n_rows, i
     for (int i = lane; i < F; i += 32) {
       const float v = __ldg(src + i);
       s_row[i] = v;
-      mx = fmaxf(mx, v);
+      mx = MaxNan()(mx, v);
     }
-    mx = warp_reduce(mx, [](float u, float v) { return fmaxf(u, v); });
+    mx = warp_reduce(mx, MaxNan());                     // np.max: a NaN in the frame makes ref NaN (no peaks)
     __syncwarp();
-    const float ref = a.ref_abs >= 0.0f ? a.ref_abs : a.threshold * mx;
-    for (int k = a.k_lo + lane; k < a.k_hi; k += 32) {
-      if (k < 1) continue;
-      const float c = s_row[k], l = s_row[k - 1];
-      const float cm = c > ref ? c : 0.0f, lm = l > ref ? l : 0.0f;
-      bool is_peak;
+    double ref = a.ref_abs;
+    if (ref < 0.0) ref = a.thr_wide ? __dmul_rn(a.threshold, (double)mx) : (double)mul_rn(thr_t, mx);
+    auto thr = [&](float v) { return (double)v > ref ? v : mul_rn(v, 0.0f); };   // S * (S > ref)
+    for (int k = max(a.k_lo, 1) + lane; k < a.k_hi; k += 32) {
+      const bool last = k == F - 1;
+      const float c = s_row[k], l = s_row[k - 1], rr = last ? c : s_row[k + 1];
+      if (!local_extremum(true, k, F, thr(l), thr(c), thr(rr))) continue;
       float shift = 0.0f, avg;
-      if (k == F - 1) {
-        is_peak = cm > lm;
-        avg = c - l;                                   // np.gradient, one-sided at the edge
+      if (last) {
+        avg = sub_rn(c, l);                              // np.gradient, one-sided at the edge
       } else {
-        const float rr = s_row[k + 1];
-        const float rm = rr > ref ? rr : 0.0f;
-        is_peak = cm > lm && cm >= rm;
-        const float pa = rr + l - 2.0f * c, pb = (rr - l) * 0.5f;
-        if (fabsf(pb) < fabsf(pa)) shift = -pb / pa;
-        avg = (rr - l) * 0.5f;
+        avg = mul_rn(sub_rn(rr, l), 0.5f);
+        shift = parabolic_shift(l, c, rr);
       }
-      if (!is_peak) continue;
-      const float pitch = (float)(((double)k + (double)shift) * a.hz_per_bin);
+      const float pitch = narrow<float>(__ddiv_rn(__dmul_rn(__dadd_rn((double)k, (double)shift), a.sr), a.n_fft));
       if (!(pitch > 0.0f)) continue;
-      const float mag = c + 0.5f * avg * shift;
+      const float mag = parabolic_mag(c, avg, shift);
       const unsigned int key = float_to_key(mag);
       if (a.mode == 0) {
         atomicAdd(&s_hist[key >> 21], 1u);
@@ -636,15 +624,8 @@ __global__ void pip_pass_kernel(const float* __restrict__ S, long long n_rows, i
       } else if (a.mode == 2) {
         if ((key >> 10) == a.prefix) atomicAdd(&s_hist[key & 0x3ffu], 1u);
       } else if (mag >= a.mag_threshold) {
-        // residual of the pitch modulo one bin of the chroma scale (pitch_tuning, core/pitch.py:161-170)
-        const float x = a.bins_per_octave * log2f(pitch / 27.5f);
-        float res = x - floorf(x);
-        if (res >= 0.5f) res -= 1.0f;
-        int b = (int)floor(((double)res + 0.5) * a.n_res_bins);
-        b = max(0, min(a.n_res_bins - 1, b));
-        while (b > 0 && (double)res < edges[b]) --b;
-        while (b < a.n_res_bins - 1 && (double)res >= edges[b + 1]) ++b;
-        atomicAdd(&s_hist[b], 1u);
+        const float res = tuning_residual(pitch, a.bins_per_octave);
+        if (res == res) atomicAdd(&s_hist[residual_bin(res, a.n_res_bins, edges)], 1u);
       }
     }
     __syncwarp();
@@ -655,25 +636,29 @@ __global__ void pip_pass_kernel(const float* __restrict__ S, long long n_rows, i
 }
 
 // util.normalize(S, norm, axis=-2) of [clip][rows][T] blocks with the default threshold / fill
-// (librosa/util/utils.py:797-1026): columns whose norm is below tiny(float32) are left unscaled.
+// (librosa/util/utils.py:797-1026): mag = |S| in float64, the column length summed over rows in order as NumPy sums
+// a non-last axis, columns whose length is below tiny(float32) left unscaled, and S / length formed in float64 and
+// rounded once to float32.  NumPy's mag**p and length**(1/p) take exact shortcuts for p = 1, 2 and 1/2 (copy,
+// square, square root); other p go through pow.
 // norm_kind: 0 = inf (max |x|), 1 = -inf (min |x|), 2 = count of non-zeros, 3 = p-norm with p = norm_p.
-__global__ void normalize_rows_kernel(const float* __restrict__ x, int rows, int T, int norm_kind, float norm_p,
+__global__ void normalize_rows_kernel(const float* __restrict__ x, int rows, int T, int norm_kind, double norm_p,
                                       float* __restrict__ out) {
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
   if (t >= T) return;
   const float* xc = x + (long long)blockIdx.y * rows * T + t;
   float* oc = out + (long long)blockIdx.y * rows * T + t;
-  float len = norm_kind == 1 ? INFINITY : 0.0f;
+  double len = norm_kind == 1 ? INFINITY : 0.0;
   for (int r = 0; r < rows; ++r) {
-    const float v = fabsf(xc[(long long)r * T]);
-    if (norm_kind == 0) len = fmaxf(len, v);
-    else if (norm_kind == 1) len = fminf(len, v);
-    else if (norm_kind == 2) len += v > 0.0f ? 1.0f : 0.0f;
-    else len += norm_p == 1.0f ? v : (norm_p == 2.0f ? v * v : powf(v, norm_p));
+    const double v = fabs((double)xc[(long long)r * T]);
+    if (norm_kind == 0) len = MaxNan()(len, v);
+    else if (norm_kind == 1) len = MinNan()(len, v);
+    else if (norm_kind == 2) len += v > 0.0 ? 1.0 : 0.0;
+    else len = add_rn(len, norm_p == 1.0 ? v : norm_p == 2.0 ? mul_rn(v, v) : norm_p == 0.5 ? sqrt_rn(v) : pow(v, norm_p));
   }
-  if (norm_kind == 3 && norm_p != 1.0f) len = norm_p == 2.0f ? sqrtf(len) : powf(len, 1.0f / norm_p);
-  if (len < 1.17549435e-38f) len = 1.0f;
-  for (int r = 0; r < rows; ++r) oc[(long long)r * T] = xc[(long long)r * T] / len;
+  if (norm_kind == 3 && norm_p != 1.0)
+    len = norm_p == 2.0 ? sqrt_rn(len) : norm_p == 0.5 ? mul_rn(len, len) : pow(len, div_rn(1.0, norm_p));
+  if (len < (double)tiny_of<float>()) len = 1.0;
+  for (int r = 0; r < rows; ++r) oc[(long long)r * T] = narrow<float>(div_rn((double)xc[(long long)r * T], len));
 }
 
 // Median-filtering harmonic / percussive separation (librosa/decompose.py:241-389, hpss) on a magnitude
@@ -900,6 +885,9 @@ __global__ void resample_poly_kernel(const float* __restrict__ x, long long x_st
 }
 
 // ------------------------------------------------------------------ power_to_db
+// 10 log10(np.maximum(amin, S)) - db_sub, then np.maximum(log_spec, log_spec.max(per clip) - top_db)
+// (librosa/core/spectrum.py:1866-1881).  np.maximum keeps a NaN cell, and a NaN clip maximum makes the whole clip NaN
+// under top_db: a NaN maximum is stored as the all-ones key, which no finite key exceeds and key_to_float reads as NaN.
 __global__ void db_kernel(const float* __restrict__ in, long long per_clip, float amin, float db_sub,
                           unsigned int* __restrict__ clip_max, float* __restrict__ out) {
   const int clip = blockIdx.y;
@@ -908,12 +896,12 @@ __global__ void db_kernel(const float* __restrict__ in, long long per_clip, floa
   float mx = -INFINITY;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < per_clip;
        i += (long long)gridDim.x * blockDim.x) {
-    float v = 10.0f * log10f(fmaxf(amin, ic[i])) - db_sub;
+    const float v = 10.0f * log10f(MaxNan()(amin, ic[i])) - db_sub;
     oc[i] = v;
-    mx = fmaxf(mx, v);
+    mx = MaxNan()(mx, v);
   }
-  mx = warp_reduce(mx, [](float u, float v) { return fmaxf(u, v); });
-  if ((threadIdx.x & 31) == 0 && mx > -INFINITY) atomicMax(clip_max + clip, float_to_key(mx));
+  mx = warp_reduce(mx, MaxNan());
+  if ((threadIdx.x & 31) == 0 && !(mx == -INFINITY)) atomicMax(clip_max + clip, mx != mx ? 0xffffffffu : float_to_key(mx));
 }
 
 __global__ void db_clamp_kernel(float* __restrict__ x, long long per_clip, const unsigned int* __restrict__ clip_max,
@@ -923,7 +911,7 @@ __global__ void db_clamp_kernel(float* __restrict__ x, long long per_clip, const
   const float floor_v = key_to_float(clip_max[clip]) - top_db;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < per_clip;
        i += (long long)gridDim.x * blockDim.x)
-    xc[i] = fmaxf(xc[i], floor_v);
+    xc[i] = MaxNan()(xc[i], floor_v);
 }
 
 // ------------------------------------------------------------------ Griffin-Lim phase update

@@ -136,8 +136,7 @@ static int onset_args(const b2l_onset_desc* d, int min_channels, const char* cha
   if (d->pad_width < 0) return fail(B2L_ERR_INVALID, "negative pad_width");
   if (d->n_channels < min_channels || d->n_channels > 32) return fail(B2L_ERR_UNSUPPORTED, "%s", channels_msg);
   if (n_clips <= 0 || n_rows <= 0 || n_frames <= 0) return B2L_OK;
-  if (n_clips > kMaxGridY || n_rows > 0x7fffffffLL || n_frames > 0x7fffffffLL)
-    return fail(B2L_ERR_UNSUPPORTED, "onset: batch too large");
+  if (n_rows > 0x7fffffffLL || n_frames > 0x7fffffffLL) return fail(B2L_ERR_UNSUPPORTED, "onset: batch too large");
   for (int i = 0; i <= d->n_channels; ++i) {
     a->bounds[i] = d->bounds[i];
     if (a->bounds[i] < 0 || a->bounds[i] > n_rows || (i > 0 && a->bounds[i] < a->bounds[i - 1]))
@@ -159,9 +158,13 @@ extern "C" int b2l_onset_from_spec(b2l_ctx* c, const b2l_onset_desc* d, const fl
   int rc = onset_args(d, 0, "at most 32 onset channels", n_clips, n_rows, n_frames, &a);
   if (rc || a.T == 0) return rc;
   DeviceGuard g(c->device);
-  rc = launch(c, onset_kernel, dim3((unsigned)((n_frames + 127) / 128), (unsigned)n_clips), 128, 0, d_S, a, d_out);
+  const long long n_out = a.n_ch > 0 ? a.n_ch : a.n_rows;
+  rc = for_clip_slices(n_clips, [&](int64_t c0, int64_t m) {
+    return launch(c, onset_kernel, dim3((unsigned)((n_frames + 127) / 128), (unsigned)m), 128, 0,
+                  d_S + c0 * n_rows * n_frames, a, d_out + c0 * n_out * n_frames);
+  });
   if (rc || !d->detrend) return rc;
-  const long long rows = (long long)n_clips * (a.n_ch > 0 ? a.n_ch : a.n_rows);
+  const long long rows = (long long)n_clips * n_out;
   return launch(c, detrend_kernel, (unsigned)((rows + 127) / 128), 128, 0, d_out, rows, a.T);
 }
 
@@ -180,8 +183,11 @@ extern "C" int b2l_onset_median_from_spec(b2l_ctx* c, const b2l_onset_desc* d, c
   while (P < widest) P <<= 1;
   const size_t smem = (size_t)kOnsetMedFrames * (P + 1) * sizeof(float);
   DeviceGuard g(c->device);
-  const dim3 grid((unsigned)((n_frames + kOnsetMedFrames - 1) / kOnsetMedFrames), (unsigned)n_clips);
-  rc = launch(c, onset_median_kernel, grid, 256, smem, d_S, a, P, d_out);
+  rc = for_clip_slices(n_clips, [&](int64_t c0, int64_t m) {
+    const dim3 grid((unsigned)((n_frames + kOnsetMedFrames - 1) / kOnsetMedFrames), (unsigned)m);
+    return launch(c, onset_median_kernel, grid, 256, smem, d_S + c0 * n_rows * n_frames, a, P,
+                  d_out + c0 * a.n_ch * n_frames);
+  });
   if (rc || !d->detrend) return rc;
   const long long rows = (long long)n_clips * a.n_ch;
   return launch(c, detrend_kernel, (unsigned)((rows + 127) / 128), 128, 0, d_out, rows, a.T);
@@ -292,7 +298,9 @@ extern "C" int b2l_pip_pass(b2l_ctx* c, const b2l_pip_desc* d, const float* d_S,
   a.k_hi = d->k_hi;
   a.threshold = d->threshold;
   a.ref_abs = d->ref_abs;
-  a.hz_per_bin = d->hz_per_bin;
+  a.thr_wide = d->thr_wide;
+  a.sr = d->sr;
+  a.n_fft = d->n_fft;
   a.mode = d->mode;
   a.prefix = d->prefix;
   a.mag_threshold = d->mag_threshold;
@@ -313,15 +321,18 @@ extern "C" int b2l_pip_pass(b2l_ctx* c, const b2l_pip_desc* d, const float* d_S,
 }
 
 extern "C" int b2l_normalize_rows(b2l_ctx* c, const float* d_in, int64_t n_clips, int64_t n_rows, int64_t n_frames,
-                                  int32_t norm_kind, float norm_p, float* d_out) {
+                                  int32_t norm_kind, double norm_p, float* d_out) {
   if (!c || !d_in || !d_out) return fail(B2L_ERR_INVALID, "NULL argument");
   if (norm_kind < 0 || norm_kind > 3) return fail(B2L_ERR_INVALID, "bad norm kind %d", norm_kind);
-  if (norm_kind == 3 && !(norm_p > 0.0f)) return fail(B2L_ERR_INVALID, "Unsupported norm: %g", norm_p);
+  if (norm_kind == 3 && !(norm_p > 0.0)) return fail(B2L_ERR_INVALID, "Unsupported norm: %g", norm_p);
   if (n_clips <= 0 || n_rows <= 0 || n_frames <= 0) return B2L_OK;
-  if (n_clips > kMaxGridY || n_rows > 0x7fffffffLL || n_frames > 0x7fffffffLL) return fail(B2L_ERR_UNSUPPORTED, "normalize: batch too large");
+  if (n_rows > 0x7fffffffLL || n_frames > 0x7fffffffLL) return fail(B2L_ERR_UNSUPPORTED, "normalize: batch too large");
   DeviceGuard g(c->device);
-  return launch(c, normalize_rows_kernel, dim3((unsigned)((n_frames + 127) / 128), (unsigned)n_clips), 128, 0, d_in,
-                (int)n_rows, (int)n_frames, norm_kind, norm_p, d_out);
+  return for_clip_slices(n_clips, [&](int64_t c0, int64_t m) {
+    const size_t off = (size_t)c0 * (size_t)n_rows * (size_t)n_frames;
+    return launch(c, normalize_rows_kernel, dim3((unsigned)((n_frames + 127) / 128), (unsigned)m), 128, 0, d_in + off,
+                  (int)n_rows, (int)n_frames, norm_kind, norm_p, d_out + off);
+  });
 }
 
 extern "C" int b2l_cabs(b2l_ctx* c, const void* d_complex, int64_t n, float* d_out) {

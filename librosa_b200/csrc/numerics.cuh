@@ -111,6 +111,50 @@ struct ArgmaxMerge {
   }
 };
 
+// ------------------------------------------------------------------ piptrack / pitch_tuning rules
+// librosa.piptrack (core/pitch.py:182-366) and pitch_tuning (:112-179) in the reference's roundings; the public
+// piptrack kernel and the tuning passes (pitch_kernels.cuh, feat_kernels.cuh) share them, so estimate_tuning sees
+// exactly the peaks piptrack returns.
+
+// The reference's _parabolic_interpolation stencil at an interior bin with neighbours l and r: numba evaluates
+// a = (r + l) - 2 * c and b = (r - l) / 2 with the sums in T and the rest promoted to float64, returns 0 when
+// |b| >= |a| (NaN fails the test), else -b / a, and rounds the shift to T once when it is stored.
+template <class T>
+__device__ __forceinline__ T parabolic_shift(T l, T c, T r) {
+  const double a = __dsub_rn((double)add_rn(r, l), __dmul_rn(2.0, (double)c));
+  const double b = __dmul_rn((double)sub_rn(r, l), 0.5);
+  return fabs(b) >= fabs(a) ? T(0) : narrow<T>(__ddiv_rn(-b, a));
+}
+
+// The interpolated magnitude S + 0.5 * avg * shift, each operation rounded in T (avg: np.gradient of S at the bin).
+template <class T>
+__device__ __forceinline__ T parabolic_mag(T c, T avg, T shift) {
+  return add_rn(c, mul_rn(mul_rn(T(0.5), avg), shift));
+}
+
+// pitch_tuning's residual of a frequency v > 0: mod(bins_per_octave * log2(v / 27.5), 1) folded to [-0.5, 0.5), in T
+// with np.mod's rounding (fmod, then + 1 when negative); log2 is the float64 log2 rounded to T.  NaN for v = inf.
+template <class T>
+__device__ __forceinline__ T tuning_residual(T v, T bins_per_octave) {
+  const T x = mul_rn(bins_per_octave, narrow<T>(log2((double)div_rn(v, T(27.5)))));
+  T res = fmod(x, T(1));
+  if (res < T(0)) res = add_rn(res, T(1));
+  else if (res == T(0)) res = T(0);
+  if (res >= T(0.5)) res = sub_rn(res, T(1));
+  return res;
+}
+
+// np.histogram's bin of a non-NaN residual over n_bins bins with float64 edges (edges[b] <= x < edges[b + 1], the
+// last bin closed).
+template <class T>
+__device__ __forceinline__ int residual_bin(T res, int n_bins, const double* __restrict__ edges) {
+  int b = (int)floor(((double)res + 0.5) * n_bins);
+  b = max(0, min(n_bins - 1, b));
+  while (b > 0 && (double)res < edges[b]) --b;
+  while (b < n_bins - 1 && (double)res >= edges[b + 1]) ++b;
+  return b;
+}
+
 // 1-D librosa.util.localmax / localmin at position i of a line of n >= 2 values (librosa/util/utils.py:1029-1178):
 // never at i = 0; cur > prev and cur >= next inside the line (cur < prev and cur <= next for a minimum); cur > prev
 // alone at i = n - 1, where `next` is ignored.  A NaN compares false.

@@ -496,16 +496,6 @@ __global__ void __launch_bounds__(256) sign_scan_kernel(const T* __restrict__ x,
   if ((threadIdx.x & 31) == 0 && bits) atomicOr(word, bits);
 }
 
-// The reference's _parabolic_interpolation stencil at an interior bin with neighbours l and r: numba evaluates
-// a = (r + l) - 2 * c and b = (r - l) / 2 with the sums in T and the rest promoted to float64, returns 0 when
-// |b| >= |a| (NaN fails the test), else -b / a, and rounds the shift to T once when it is stored.
-template <class T>
-__device__ __forceinline__ T parabolic_shift(T l, T c, T r) {
-  const double a = __dsub_rn((double)add_rn(r, l), __dmul_rn(2.0, (double)c));
-  const double b = __dmul_rn((double)sub_rn(r, l), 0.5);
-  return fabs(b) >= fabs(a) ? T(0) : narrow<T>(__ddiv_rn(-b, a));
-}
-
 template <class T>
 struct PiptrackArgs {
   const T* S;                // [clip] x (F bins, n_frames frames); bin k of frame t at t * frame_stride + k * bin_stride
@@ -568,7 +558,7 @@ __global__ void __launch_bounds__(256) piptrack_kernel(const PiptrackArgs<T> a) 
             avg = mul_rn(sub_rn(rr, l), T(0.5));                    // (S[k+1] - S[k-1]) / 2
             shift = parabolic_shift(l, c, rr);
           }
-          mag = add_rn(c, mul_rn(mul_rn(T(0.5), avg), shift));    // S + 0.5 * avg * shift
+          mag = parabolic_mag(c, avg, shift);
           pitch = narrow<T>(__ddiv_rn(__dmul_rn(__dadd_rn((double)k, (double)shift), a.sr), a.n_fft));
         }
       }
@@ -596,17 +586,9 @@ __global__ void __launch_bounds__(256) tuning_hist_kernel(const T* __restrict__ 
     const T v = __ldg(f + e);
     if (!(v > T(0))) continue;
     ++positive;
-    const T x = mul_rn(bins_per_octave, narrow<T>(log2((double)div_rn(v, T(27.5)))));
-    T res = fmod(x, T(1));
-    if (res < T(0)) res = add_rn(res, T(1));
-    else if (res == T(0)) res = T(0);
-    if (res >= T(0.5)) res = sub_rn(res, T(1));
+    const T res = tuning_residual(v, bins_per_octave);
     if (res != res) continue;
-    int b = (int)floor(((double)res + 0.5) * n_bins);
-    b = max(0, min(n_bins - 1, b));
-    while (b > 0 && (double)res < edges[b]) --b;
-    while (b < n_bins - 1 && (double)res >= edges[b + 1]) ++b;
-    atomicAdd(&s_cnt[b], 1u);
+    atomicAdd(&s_cnt[residual_bin(res, n_bins, edges)], 1u);
   }
   positive = __reduce_add_sync(0xffffffffu, positive);
   if ((threadIdx.x & 31) == 0 && positive) atomicAdd(&counts[n_bins], (unsigned long long)positive);
