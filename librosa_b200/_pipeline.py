@@ -174,13 +174,11 @@ def is_pow2(n: int) -> bool:
 
 
 def mr_covers(n_fft: int) -> bool:
-    """True when the mixed-radix kernel (csrc/mr_kernel.cuh) takes the forward transform: even n_fft that is not a
+    """True for the frame lengths of the mixed-radix kernels (csrc/mr_kernel.cuh): even n_fft up to 4096 that is not a
     power of two and whose half has no prime factor above 5 (400, 320, 480, 800, 960, 1200, ...).  Mirror of
-    ``mr_factor`` in csrc/plan.cu; ``B2L_MR=0`` sends these sizes back to the chirp-z kernels."""
+    ``mr_factor`` in csrc/plan.cu."""
     n_fft = int(n_fft)
     if is_pow2(n_fft) or n_fft < 12 or n_fft > MAX_MR_N_FFT or (n_fft & 1):
-        return False
-    if os.environ.get("B2L_MR", "") not in ("", "1"):
         return False
     m = n_fft // 2
     for q in (5, 3, 2):
@@ -189,38 +187,37 @@ def mr_covers(n_fft: int) -> bool:
     return m == 1
 
 
-def fused_front_end(n_fft: int) -> bool:
-    """Frame lengths whose melspectrogram / mfcc run as ONE fused kernel (+ the DCT kernel): powers of two
-    (fwd_kernel) and the mixed-radix sizes (mr_kernel).  Everything else composes the spectrogram kernel with the
-    ``S=`` kernels on the device."""
-    return is_pow2(n_fft) or mr_covers(n_fft)
+def transform_path(n_fft: int):
+    """Which float32 transform serves frame length ``n_fft`` (host mirror of ``plan_path`` in csrc/plan.cu):
 
-
-def require_supported_n_fft(n_fft: int, inverse: bool = False):
-    """Power-of-two n_fft in [8, 8192] runs on the packed real-FFT kernels; even n_fft up to 4096 whose half is
-    5-smooth (400, 480, 960, 1200, 3000, ...) on the mixed-radix kernels; any other n_fft in [3, 2047] (the
-    reference tests' 501 / 1023 / 1025, ...) on the chirp-z kernels (forward and inverse).  Everything else
-    librosa accepts is refused loudly by the float32 path — there is no CPU fallback (host float32 data of such
-    sizes takes the FP64 kernels, see ``wide_route``)."""
+    * "pow2": powers of two from 8 to 8192, on the packed real-FFT kernels (fwd_kernel / inv_kernel); their
+      melspectrogram / mfcc run as one fused kernel;
+    * "mr": even sizes up to 4096 whose half has no prime factor above 5 (400, 480, 960, 1200, 3000, ...), on the
+      mixed-radix kernels (mr_kernel / mr_inv_kernel), with a fused melspectrogram / mfcc too;
+    * "czt": every other size from 3 to 2047 (the reference tests' 501 / 1023 / 1025, ...), on the chirp-z kernels
+      (czt_kernel / czt_inv_kernel); melspectrogram, mfcc and the spectral statistics compose the spectrogram
+      kernel with the ``S=`` kernels on the device;
+    * None: no float32 kernels (host float32 data of such sizes takes the FP64 kernels, see ``wide_route``)."""
     n_fft = int(n_fft)
     if is_pow2(n_fft):
-        if MIN_N_FFT <= n_fft <= MAX_N_FFT:
-            return
+        return "pow2" if MIN_N_FFT <= n_fft <= MAX_N_FFT else None
+    if mr_covers(n_fft):
+        return "mr"
+    return "czt" if 3 <= n_fft <= MAX_CZT_N_FFT else None
+
+
+def require_supported_n_fft(n_fft: int):
+    """Refuses a frame length ``transform_path`` has no float32 kernels for, loudly: there is no CPU fallback."""
+    n_fft = int(n_fft)
+    if transform_path(n_fft) is not None:
+        return
+    if is_pow2(n_fft):
         raise nat.UnsupportedOnGPU(
             f"n_fft={n_fft}: the sm_90a kernels are built for powers of two from {MIN_N_FFT} to {MAX_N_FFT} "
             "(no CPU fallback)")
-    if not (3 <= n_fft <= MAX_CZT_N_FFT) and not mr_covers(n_fft):
-        raise nat.UnsupportedOnGPU(f"n_fft={n_fft}: non-power-of-two sizes are supported from 3 to {MAX_CZT_N_FFT}, and "
-                                   f"even sizes up to {MAX_MR_N_FFT} whose half has no prime factor above 5 "
-                                   "(no CPU fallback)")
-
-
-def f32_kernels_cover(n_fft: int) -> bool:
-    """True when the float32 hot-path kernels are built for this frame length."""
-    n_fft = int(n_fft)
-    if is_pow2(n_fft):
-        return MIN_N_FFT <= n_fft <= MAX_N_FFT
-    return 3 <= n_fft <= MAX_CZT_N_FFT or mr_covers(n_fft)
+    raise nat.UnsupportedOnGPU(f"n_fft={n_fft}: non-power-of-two sizes are supported from 3 to {MAX_CZT_N_FFT}, and "
+                               f"even sizes up to {MAX_MR_N_FFT} whose half has no prime factor above 5 "
+                               "(no CPU fallback)")
 
 
 def wide_route(y, req_dtype, n_fft: int) -> bool:
@@ -232,7 +229,7 @@ def wide_route(y, req_dtype, n_fft: int) -> bool:
 
     if np.dtype(req_dtype) == np.float64 and native_float64(req_dtype):
         return True
-    return (not isinstance(y, nat.DeviceArray)) and not f32_kernels_cover(n_fft) and _f64.supported(n_fft)
+    return (not isinstance(y, nat.DeviceArray)) and transform_path(n_fft) is None and _f64.supported(n_fft)
 
 
 def context_for(x):

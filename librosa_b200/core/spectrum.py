@@ -179,7 +179,7 @@ def istft(stft_matrix, *, hop_length: Optional[int] = None, win_length: Optional
         n_frames = T_stored
     in_dtype = np.dtype(stft_matrix.dtype)
     if (in_dtype == np.complex128 and pl.native_float64(in_dtype)) or \
-            (in_dtype == np.complex64 and not on_device and not pl.f32_kernels_cover(n_fft) and f64.supported(n_fft)):
+            (in_dtype == np.complex64 and not on_device and pl.transform_path(n_fft) is None and f64.supported(n_fft)):
         wide = stft_matrix if in_dtype == np.complex128 else stft_matrix.astype(np.complex128)
         return _istft_f64(wide, n_frames, T_stored, F, n_fft, hop_length, win_length, window, win, center,
                           dtype if dtype is not None else dtype_c2r(in_dtype), length, out)
@@ -197,7 +197,7 @@ def istft(stft_matrix, *, hop_length: Optional[int] = None, win_length: Optional
     out_len = _istft_out_len(n_fft, hop_length, n_frames, center, length)
     lead = tuple(stft_matrix.shape[:-2])
     _check_istft_out(out, lead + (out_len,))
-    pl.require_supported_n_fft(n_fft, inverse=True)
+    pl.require_supported_n_fft(n_fft)
     with pl.Scope(stft_matrix) as sc:
         ctx = sc.ctx
         key = ("stft", n_fft, hop_length, bool(center), "constant", wkey)
@@ -628,7 +628,7 @@ def griffinlim(S, *, n_iter: int = 32, hop_length: Optional[int] = None, win_len
     eps = float(tiny(np.zeros(1, dtype=cdtype)))
     F, T = S.shape[-2], S.shape[-1]
     n_clips = pl.clip_count(S.shape[:-2])
-    pl.require_supported_n_fft(n_fft, inverse=True)
+    pl.require_supported_n_fft(n_fft)
     with pl.Scope(S) as sc:
         ctx = sc.ctx
         L = nat.lib()

@@ -22,6 +22,11 @@ namespace b2l {
 #define B2L_CZT_SIZES(X) X(5) X(6) X(7) X(8) X(9) X(10) X(11) X(12)
 constexpr int kMinLog2M = 2, kMaxLog2M = 12;
 
+// The transform that serves a plan's n_fft, decided once by plan_path (plan.cu): fwd_kernel / inv_kernel for the
+// powers of two, mr_kernel / mr_inv_kernel for the even sizes with a 5-smooth half, czt_kernel / czt_inv_kernel for
+// the rest of 3 .. 2047.
+enum Path { PATH_POW2, PATH_MR, PATH_CZT };
+
 struct CztArgs;
 struct CztInvArgs;
 typedef void (*FwdKernel)(FwdArgs);
@@ -112,6 +117,7 @@ struct b2l_ctx {
 struct b2l_plan {
   b2l_ctx* ctx = nullptr;
   int n_fft = 0, hop = 0, center = 0, pad_mode = 0, log2m = 0;
+  b2l::Path path = b2l::PATH_POW2;   // only this path's tables below are built
   // every device allocation of the plan (b2l_plan_destroy frees them); the row tables below add theirs lazily
   mutable std::vector<void*> allocs;
   float* d_win_fwd = nullptr;   // window * 1/2
@@ -132,15 +138,15 @@ struct b2l_plan {
   mutable std::map<int, RowTable> row_tables;
   int power_mode = 2;
   float power = 2.0f;
-  // chirp-z path for n_fft that is not a power of two (czt_kernel.cuh): transform size P = 2^log2p
-  int czt = 0, log2p = 0;
+  // chirp-z path (czt_kernel.cuh): transform size P = 2^log2p
+  int log2p = 0;
   float2* d_czt_wb = nullptr;   // [n_fft] window * b
   float2* d_czt_bk = nullptr;   // [1 + n_fft/2] b
   float2* d_czt_hf = nullptr;   // [P] FFT_P(h)/P followed by the engine's inter-pass twiddles
   float2* d_czt_bfull = nullptr;   // [n_fft] b (inverse)
   float2* d_czt_wbi = nullptr;     // [n_fft] conj(b) * window / n_fft (inverse)
-  // mixed-radix path for even n_fft whose half is 5-smooth (mr_kernel.cuh)
-  int mr = 0, mr_n_pass = 0, mr_tw_count = 0;
+  // mixed-radix path (mr_kernel.cuh)
+  int mr_n_pass = 0, mr_tw_count = 0;
   int mr_radix[b2l::kMrMaxPass] = {0}, mr_tw_off[b2l::kMrMaxPass] = {0};
   float* d_mr_win = nullptr;       // [n_fft] window * 1/2
   float* d_mr_win_inv = nullptr;   // [n_fft] window / n_fft (inverse)

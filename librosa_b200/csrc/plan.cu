@@ -88,6 +88,33 @@ static bool mr_factor(int n_fft, std::vector<int>& radices) {
   return m == 1 && (int)radices.size() <= kMrMaxPass && !radices.empty();
 }
 
+// Which transform serves n_fft >= 1 (host mirror: _pipeline.transform_path), with what that path needs: *log2m for a
+// power of two, the radix schedule for the mixed-radix kernels, *log2p (chirp-z size P = 2^log2p >= 2 n_fft - 1, at
+// least one warp of the engine) for the chirp-z kernels, which are built up to P = 4096.
+static int plan_path(int n_fft, Path* path, int* log2m, int* log2p, std::vector<int>& radices) {
+  const int l2n = ilog2_exact(n_fft);
+  if (l2n >= 0) {
+    if (l2n - 1 < kMinLog2M || l2n - 1 > kMaxLog2M)
+      return fail(B2L_ERR_UNSUPPORTED,
+                  "n_fft=%d: the sm_90a kernels are built for powers of two from %d to %d (no CPU fallback)", n_fft,
+                  2 << kMinLog2M, 2 << kMaxLog2M);
+    *path = PATH_POW2;
+    *log2m = l2n - 1;
+    return B2L_OK;
+  }
+  if (mr_factor(n_fft, radices)) {
+    *path = PATH_MR;
+    return B2L_OK;
+  }
+  if (n_fft > 2047)
+    return fail(B2L_ERR_UNSUPPORTED,
+                "n_fft=%d: non-power-of-two sizes are supported from 3 to 2047, and even sizes up to 4096 whose half "
+                "has no prime factor above 5 (no CPU fallback)", n_fft);
+  *path = PATH_CZT;
+  for (*log2p = 5; (1 << *log2p) < 2 * n_fft - 1;) ++*log2p;
+  return B2L_OK;
+}
+
 // ------------------------------------------------------------------ table builders
 // windows and twiddles of fwd_kernel / inv_kernel (n_fft a power of two)
 static int build_pow2(b2l_plan* p, const double* window) {
@@ -146,7 +173,6 @@ static int build_czt(b2l_plan* p, const double* window) {
 // mixed-radix tables (odd radices first, see mr_kernel.cuh) for the radix schedule of mr_factor
 static int build_mr(b2l_plan* p, const std::vector<int>& radices, const double* window) {
   const int N = p->n_fft;
-  p->mr = 1;
   p->mr_n_pass = (int)radices.size();
   std::vector<float2> tw;
   int sub = 1;
@@ -245,23 +271,10 @@ extern "C" int b2l_plan_create(b2l_ctx* c, const b2l_plan_desc* d, b2l_plan** ou
   if (!c || !d || !out) return fail(B2L_ERR_INVALID, "NULL argument");
   if (d->n_fft < 1) return fail(B2L_ERR_INVALID, "n_fft=%d must be positive", d->n_fft);
   if (d->hop_length < 1) return fail(B2L_ERR_INVALID, "hop_length=%d must be a positive integer", d->hop_length);
-  const int l2n = ilog2_exact(d->n_fft);
-  int czt_log2p = 0;
+  Path path = PATH_POW2;
+  int log2m = -1, log2p = 0;
   std::vector<int> radices;
-  const bool mr = l2n < 0 && mr_factor(d->n_fft, radices);
-  if (l2n < 0) {
-    // not a power of two: Bluestein with P = next power of two >= 2*n_fft - 1 (czt_kernel.cuh)
-    while ((1 << czt_log2p) < 2 * d->n_fft - 1) ++czt_log2p;
-    if (czt_log2p < 5) czt_log2p = 5;
-    if (d->n_fft < 3 || (czt_log2p > 12 && !mr))
-      return fail(B2L_ERR_UNSUPPORTED,
-                  "n_fft=%d: non-power-of-two sizes are supported from 3 to 2047, and even sizes up to 4096 whose half "
-                  "has no prime factor above 5 (no CPU fallback)", d->n_fft);
-  } else if (l2n - 1 < kMinLog2M || l2n - 1 > kMaxLog2M) {
-    return fail(B2L_ERR_UNSUPPORTED,
-                "n_fft=%d: the sm_90a kernels are built for powers of two from %d to %d (no CPU fallback)",
-                d->n_fft, 2 << kMinLog2M, 2 << kMaxLog2M);
-  }
+  if (int rc = plan_path(d->n_fft, &path, &log2m, &log2p, radices)) return rc;
   if (!d->h_window) return fail(B2L_ERR_INVALID, "window is NULL");
   if (d->pad_mode < 0 || d->pad_mode > B2L_PAD_EMPTY) return fail(B2L_ERR_INVALID, "bad pad_mode %d", d->pad_mode);
   if (d->n_mels < 0 || d->n_mfcc < 0) return fail(B2L_ERR_INVALID, "negative n_mels / n_mfcc");
@@ -277,22 +290,17 @@ extern "C" int b2l_plan_create(b2l_ctx* c, const b2l_plan_desc* d, b2l_plan** ou
   p->hop = d->hop_length;
   p->center = d->center ? 1 : 0;
   p->pad_mode = d->pad_mode;
-  p->log2m = l2n - 1;
+  p->path = path;
+  p->log2m = log2m;
+  p->log2p = log2p;
   p->power = d->power;
   p->power_mode = d->power == 2.0f ? 2 : (d->power == 1.0f ? 1 : 0);
   p->amin = d->amin;
   p->ref_value = d->ref_value;
   p->top_db = d->top_db;
-  int rc = B2L_OK;
-  if (l2n >= 0) {
-    rc = build_pow2(p, d->h_window);
-  } else {
-    p->czt = 1;
-    p->log2m = -1;
-    p->log2p = czt_log2p > 12 ? 0 : czt_log2p;   // 0: beyond the chirp-z range, the mixed-radix kernels alone serve this size
-    if (p->log2p) rc = build_czt(p, d->h_window);
-    if (rc == B2L_OK && mr) rc = build_mr(p, radices, d->h_window);
-  }
+  int rc = path == PATH_POW2 ? build_pow2(p, d->h_window)
+           : path == PATH_MR ? build_mr(p, radices, d->h_window)
+                             : build_czt(p, d->h_window);
   if (rc == B2L_OK && d->n_mels > 0) rc = build_mel(p, d->h_mel_basis, d->n_mels);
   if (rc == B2L_OK && d->n_mels > 0 && d->n_mels <= 16) rc = build_dense_mel(p, d->h_mel_basis);
   if (rc == B2L_OK && d->n_mfcc > 0) rc = build_dct(p, d->h_dct_basis, d->n_mfcc);

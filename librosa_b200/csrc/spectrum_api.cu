@@ -4,7 +4,6 @@
 // mr_kernel.cuh: they define non-template kernels, whose host stubs a second including unit would define again.
 #include <cuda_runtime.h>
 #include <math.h>
-#include <stdlib.h>
 #include <string.h>
 
 #include <algorithm>
@@ -53,29 +52,6 @@ static int cta_variants(const HostFftCfg& cfg, int out[3]) {
   return n;
 }
 static int variant_threads(int variant) { return variant == 116 ? 512 : variant * 32; }
-
-// ------------------------------------------------------------------ which kernels serve a plan
-enum Path { PATH_POW2, PATH_MR, PATH_CZT, PATH_NONE };
-enum Entry {
-  ENTRY_SPECTRUM,   // stft, spectrogram, istft
-  ENTRY_MEL,        // melspectrogram, mfcc
-  ENTRY_STATS,      // spectral_stats
-};
-// B2L_MR=0 sends the spectrum entry points of the mixed-radix sizes back to the chirp-z kernels where those exist
-// (n_fft <= 2047).  Read on every call: a plan outlives changes of the environment.
-static bool mr_enabled(const b2l_plan* p) {
-  if (p->log2p == 0) return true;   // no chirp-z tables for this size
-  const char* e = getenv("B2L_MR");
-  return !(e && *e) || atoi(e) != 0;
-}
-static Path route(const b2l_plan* p, Entry entry) {
-  if (!p->czt) return PATH_POW2;
-  switch (entry) {
-    case ENTRY_SPECTRUM: return p->mr && mr_enabled(p) ? PATH_MR : PATH_CZT;
-    case ENTRY_MEL: return p->mr ? PATH_MR : PATH_NONE;   // B2L_MR does not apply here
-    default: return PATH_NONE;
-  }
-}
 
 // ------------------------------------------------------------------ forward launches
 // The checks the forward paths share, in order: plan ownership, clip geometry, signal length, then the device
@@ -345,7 +321,7 @@ static int run_mr(b2l_ctx* c, const b2l_plan* p, int mode, int log_mode, const f
 extern "C" int b2l_stft(b2l_ctx* c, const b2l_plan* p, const float* d_y, int64_t n_clips, int64_t n, int64_t y_stride,
                         void* d_D) {
   if (!c || !p) return fail(B2L_ERR_INVALID, "NULL ctx / plan");
-  switch (route(p, ENTRY_SPECTRUM)) {
+  switch (p->path) {
     case PATH_MR: return run_mr(c, p, 0, 0, d_y, n_clips, n, y_stride, (float2*)d_D, nullptr);
     case PATH_CZT: return run_czt(c, p, 0, d_y, n_clips, n, y_stride, (float2*)d_D, nullptr);
     default: return run_forward(c, p, MODE_STFT, 0, d_y, n_clips, n, y_stride, (float2*)d_D, nullptr);
@@ -354,7 +330,7 @@ extern "C" int b2l_stft(b2l_ctx* c, const b2l_plan* p, const float* d_y, int64_t
 extern "C" int b2l_spectrogram(b2l_ctx* c, const b2l_plan* p, const float* d_y, int64_t n_clips, int64_t n,
                                int64_t y_stride, float* d_S) {
   if (!c || !p) return fail(B2L_ERR_INVALID, "NULL ctx / plan");
-  switch (route(p, ENTRY_SPECTRUM)) {
+  switch (p->path) {
     case PATH_MR: return run_mr(c, p, 1, 0, d_y, n_clips, n, y_stride, nullptr, d_S);
     case PATH_CZT: return run_czt(c, p, 1, d_y, n_clips, n, y_stride, nullptr, d_S);
     default: return run_forward(c, p, MODE_SPEC, 0, d_y, n_clips, n, y_stride, nullptr, d_S);
@@ -386,7 +362,7 @@ extern "C" int b2l_scan_finite_f64(b2l_ctx* c, const double* d_y, int64_t n_clip
 extern "C" int b2l_spectral_stats(b2l_ctx* c, const b2l_plan* p, const b2l_stats_desc* d, const float* d_y,
                                   int64_t n_clips, int64_t n, int64_t y_stride, const float* d_freq, float* d_out) {
   if (!c || !p) return fail(B2L_ERR_INVALID, "NULL ctx / plan");
-  if (route(p, ENTRY_STATS) == PATH_NONE)
+  if (p->path != PATH_POW2)
     return fail(B2L_ERR_UNSUPPORTED,
                 "n_fft=%d: compose b2l_spectrogram + b2l_spectral_stats_from_spec for non-power-of-two sizes", p->n_fft);
   StatsCall sc;
@@ -399,9 +375,9 @@ extern "C" int b2l_spectral_stats(b2l_ctx* c, const b2l_plan* p, const b2l_stats
 extern "C" int b2l_melspectrogram(b2l_ctx* c, const b2l_plan* p, const float* d_y, int64_t n_clips, int64_t n,
                                   int64_t y_stride, float* d_mel) {
   if (!c || !p) return fail(B2L_ERR_INVALID, "NULL ctx / plan");
-  switch (route(p, ENTRY_MEL)) {
+  switch (p->path) {
     case PATH_MR: return run_mr(c, p, 2, 0, d_y, n_clips, n, y_stride, nullptr, d_mel);
-    case PATH_NONE:
+    case PATH_CZT:
       return fail(B2L_ERR_UNSUPPORTED, "n_fft=%d: compose b2l_spectrogram + b2l_mel_project for non-power-of-two sizes",
                   p->n_fft);
     default: return run_forward(c, p, MODE_MEL, 0, d_y, n_clips, n, y_stride, nullptr, d_mel);
@@ -438,8 +414,7 @@ extern "C" int b2l_mfcc(b2l_ctx* c, const b2l_plan* p, const float* d_y, int64_t
                         float* d_mfcc, float* d_logmel) {
   if (!c || !p) return fail(B2L_ERR_INVALID, "NULL ctx / plan");
   if (p->n_mfcc == 0) return fail(B2L_ERR_INVALID, "plan has no mfcc stage");
-  const Path path = route(p, ENTRY_MEL);
-  if (path == PATH_NONE)
+  if (p->path == PATH_CZT)
     return fail(B2L_ERR_UNSUPPORTED, "n_fft=%d: compose spectrogram, mel_project, power_to_db and dct_project for "
                 "non-power-of-two sizes", p->n_fft);
   if (n_clips <= 0) return n_clips == 0 ? B2L_OK : fail(B2L_ERR_INVALID, "negative n_clips");
@@ -457,8 +432,8 @@ extern "C" int b2l_mfcc(b2l_ctx* c, const b2l_plan* p, const float* d_y, int64_t
     scratch = (float*)own.p;
   }
   // mixed-radix frames (mr_kernel): the dB rows go to the scratch in the plain [clip][mel][frame] layout
-  const int tiled = path == PATH_POW2 ? 1 : 0;
-  rc = path == PATH_MR ? run_mr(c, p, 2, 1, d_y, n_clips, n, y_stride, nullptr, scratch)
+  const int tiled = p->path == PATH_POW2 ? 1 : 0;
+  rc = p->path == PATH_MR ? run_mr(c, p, 2, 1, d_y, n_clips, n, y_stride, nullptr, scratch)
                        : run_forward(c, p, MODE_MEL, 2, d_y, n_clips, n, y_stride, nullptr, scratch);
   return rc ? rc : launch_dct(c, p, scratch, n_clips, T, 1, d_mfcc, tiled);
 }
@@ -611,8 +586,7 @@ extern "C" int b2l_istft(b2l_ctx* c, const b2l_plan* p, const void* d_D, int64_t
     return fail(B2L_ERR_INVALID, "bad istft geometry");
   if (n_clips == 0 || out_len == 0) return B2L_OK;
   if (!d_D || !d_inv_wss || !d_y) return fail(B2L_ERR_INVALID, "NULL device pointer");
-  const Path path = route(p, ENTRY_SPECTRUM);
-  if (path == PATH_POW2)
+  if (p->path == PATH_POW2)
     return run_inverse(c, p, d_D, n_clips, n_frames_stored, n_frames_used, d_inv_wss, out_len, d_y, y_stride);
   // mixed-radix or chirp-z frames into the scratch array, then a gather overlap-add
   if (out_len > 0x7fffffffLL || n_clips > kMaxGridY) return fail(B2L_ERR_UNSUPPORTED, "istft batch too large");
@@ -620,7 +594,7 @@ extern "C" int b2l_istft(b2l_ctx* c, const b2l_plan* p, const void* d_D, int64_t
   const int L = p->n_fft;
   int rc = ensure_scratch(c, (size_t)n_clips * (size_t)n_frames_used * L * sizeof(float));
   if (rc == B2L_OK)
-    rc = path == PATH_MR ? run_mr_inverse(c, p, d_D, n_clips, n_frames_stored, n_frames_used)
+    rc = p->path == PATH_MR ? run_mr_inverse(c, p, d_D, n_clips, n_frames_stored, n_frames_used)
                          : run_czt_inverse(c, p, d_D, n_clips, n_frames_stored, n_frames_used);
   if (rc) return rc;
   const dim3 og((unsigned)row_blocks(out_len, 256, 8LL * c->sm_count, n_clips), (unsigned)n_clips);

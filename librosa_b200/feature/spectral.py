@@ -55,7 +55,7 @@ def melspectrogram(*, y=None, sr: float = 22050, S=None, n_fft: int = 2048, hop_
         with pl.Scope(y) as sc:
             return sc.result(_mel_f64(sc, y, n_fft, fr, center, power, basis), res_dtype, validate=True)
     pl.require_supported_n_fft(n_fft)
-    if not pl.fused_front_end(n_fft):
+    if pl.transform_path(n_fft) == "czt":
         # chirp-z frames: |STFT|**power on the device, then the band-sparse projection (two kernels)
         return _compose_nonpow2(y, lambda Sd: melspectrogram(S=Sd, sr=sr, n_fft=n_fft, **kwargs), res_dtype,
                                 n_fft=n_fft, hop_length=fr.hop, power=power, win_length=win_length,
@@ -219,7 +219,7 @@ def mfcc(*, y=None, sr: float = 22050, S=None, n_mfcc: int = 20, dct_type: int =
             return sc.result(out, res_dtype, validate=True)
     dct = _dct_basis(n_mels, n_mfcc, dct_type, norm, lifter)
     pl.require_supported_n_fft(n_fft)
-    if not pl.fused_front_end(n_fft):
+    if pl.transform_path(n_fft) == "czt":
         def tail(Sd):
             mel_d = melspectrogram(S=Sd, sr=sr, n_fft=n_fft, norm=mel_norm, **kwargs)
             return mfcc(S=power_to_db(mel_d), n_mfcc=n_mfcc, dct_type=dct_type, norm=norm, lifter=lifter)

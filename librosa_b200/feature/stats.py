@@ -95,7 +95,7 @@ def _stats_from_y(sc, y, desc, freq, sr, *, n_fft, hop_length, win_length, windo
     fr = pl.forward_front(y, n_fft, hop_length, win_length, window, center, pad_mode, native_ok=False)
     pl.require_supported_n_fft(n_fft)
     table, fkey, fdtype = _freq_table(freq, sr, n_fft, 1 + n_fft // 2)
-    if not pl.is_pow2(n_fft):
+    if pl.transform_path(n_fft) != "pow2":
         from .spectral import _compose_nonpow2
 
         def tail(Sd):

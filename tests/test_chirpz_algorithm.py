@@ -11,7 +11,7 @@ def czt_sizes():
     """Frame lengths 3 ... 2047 served by the chirp-z kernels: neither a power of two nor mixed-radix."""
     from librosa_b200 import _pipeline as pl
 
-    return [n for n in range(3, pl.MAX_CZT_N_FFT + 1) if not pl.is_pow2(n) and not pl.mr_covers(n)]
+    return [n for n in range(3, pl.MAX_CZT_N_FFT + 1) if pl.transform_path(n) == "czt"]
 
 
 def czt_p(L):
@@ -72,16 +72,14 @@ def inv_pair(XA, XB, w, L):
     return u.real, u.imag
 
 
-def test_chirpz_sizes_and_transform_sizes(monkeypatch):
-    monkeypatch.delenv("B2L_MR", raising=False)
+def test_chirpz_sizes_and_transform_sizes():
     sizes = czt_sizes()
     assert len(sizes) == 1962
     P = {czt_p(L) for L in sizes}
     assert sorted(P) == [1 << q for q in range(5, 13)]            # the eight instances of czt_inst.cu
 
 
-def test_paired_forward_and_inverse_for_every_size(monkeypatch):
-    monkeypatch.delenv("B2L_MR", raising=False)
+def test_paired_forward_and_inverse_for_every_size():
     rng = np.random.default_rng(0)
     for L in czt_sizes():
         b = tables(L)[1]
@@ -105,10 +103,9 @@ def test_paired_forward_and_inverse_for_every_size(monkeypatch):
         assert np.abs(yb - wb).max() <= 1e-13 * scale, L
 
 
-def test_gpu_sweep_covers_every_instance(monkeypatch):
+def test_gpu_sweep_covers_every_instance():
     """The size sweep of tests/test_gpu_chirpz.py reaches every chirp-z instance P at its smallest and largest
     frame length, and at an odd and an even one."""
-    monkeypatch.delenv("B2L_MR", raising=False)
     import test_gpu_chirpz as G
 
     sizes = czt_sizes()

@@ -436,18 +436,3 @@ def test_every_swept_size_takes_the_chirpz_route(lb):
     got = {L: counts(L) for L in sweep_sizes()}
     assert {L: c for L, c in got.items() if c != want} == {}
 
-
-# ------------------------------------------------------------------ mixed-radix sizes on the chirp-z kernels
-def test_mixed_radix_sizes_on_the_chirpz_kernels(lb, monkeypatch):
-    """B2L_MR=0 sends the 74 even 5-smooth frame lengths <= 2047 to the chirp-z kernels: forward and inverse against
-    the same reference, at the same bounds."""
-    from librosa_b200 import _pipeline as pl
-
-    smooth = [L for L in range(12, pl.MAX_CZT_N_FFT + 1, 2) if pl.mr_covers(L)]
-    assert len(smooth) == 74
-    monkeypatch.setenv("B2L_MR", "0")
-    assert not any(pl.mr_covers(L) for L in smooth)
-    for i, L in enumerate(smooth):
-        fwd, inv = sweep_case(lb, L, i)
-        check_norm(fwd, czt_p(L), f"B2L_MR=0 stft n_fft={L}")
-        check_norm(inv, czt_p(L), f"B2L_MR=0 istft n_fft={L}", inverse=True)

@@ -482,6 +482,38 @@ def test_first_refused_hop(lb, n_fft):
                     lb.feature.spectral_centroid(y=y, sr=22050, n_fft=n_fft, hop_length=stop)
 
 
+def test_plans_exist_exactly_where_a_transform_path_does(lb):
+    """The size rule is written twice, once per side of the C ABI: for every n_fft from 1 to 8200, b2l_plan_create
+    (plan_path in csrc/plan.cu) makes a plan exactly when _pipeline.transform_path names a path, and refuses every
+    other size with require_supported_n_fft's error type and text."""
+    from librosa_b200 import _native as nat
+    from librosa_b200 import _pipeline as pl
+
+    L = nat.lib()
+    win = np.ones(8200)
+    desc = nat.PlanDesc(hop_length=1, h_window=win.ctypes.data_as(ctypes.POINTER(ctypes.c_double)), power=2.0,
+                        amin=1e-10, ref_value=1.0, top_db=80.0)
+    wrong = []
+    for n_fft in range(1, 8201):
+        desc.n_fft = n_fft
+        h = ctypes.c_void_p()
+        rc = L.b2l_plan_create(lb.default_context().handle, ctypes.byref(desc), ctypes.byref(h))
+        if rc == nat.B2L_OK:
+            L.b2l_plan_destroy(h)
+            if pl.transform_path(n_fft) is None:
+                wrong.append((n_fft, "plan made"))
+            continue
+        msg = L.b2l_last_error().decode()
+        try:
+            pl.require_supported_n_fft(n_fft)
+            want = None
+        except nat.UnsupportedOnGPU as exc:
+            want = str(exc)
+        if rc != nat.B2L_ERR_UNSUPPORTED or msg != want:
+            wrong.append((n_fft, rc, msg, want))
+    assert not wrong, wrong[:10]
+
+
 # ------------------------------------------------------------------ every size, norm-wise; the spectrogram powers
 @pytest.mark.parametrize("n_fft", SIZES)
 def test_stft_every_size(lb, n_fft):

@@ -16,7 +16,7 @@ import warnings
 import numpy as np
 import pytest
 
-from cases import BY_NAME, CASES
+from cases import CASES
 from conftest import case_input
 
 pytestmark = pytest.mark.gpu
@@ -110,29 +110,6 @@ def test_case_against_oracle_and_reference_fixture(case, lb, oracle, golden):
     else:
         close(got, want, **TOL[case["op"]])
         close(got, fixture, **TOL[case["op"]])
-
-
-@pytest.mark.parametrize("name", ["stft_400_160_stereo_A", "stft_2000_500_nocenter_A", "stft_12_5_edge_A",
-                                  "stft_600_winlen400_hamming_A", "stft_486_oddhop_A", "mel_16000_400_80_B",
-                                  "mfcc_16000_400_C", "mfcc_16000_400_lifter_A", "istft_400_160_stereo",
-                                  "istft_2000_nocenter", "istft_486_oddhop"])
-def test_even_smooth_sizes_still_pass_on_the_chirpz_kernels(name, lb, oracle, golden, monkeypatch):
-    """Even frame lengths with a 5-smooth half take the mixed-radix kernel by default (mr_kernel.cuh); with
-    B2L_MR=0 they run on the chirp-z kernels (and the composed S= kernels) as before — both stay pinned."""
-    monkeypatch.setenv("B2L_MR", "0")
-    case = BY_NAME[name]
-    got = run_gpu(lb, case, golden)
-    if case["op"] == "istft":
-        D = golden[case["src"]]
-        n_fft = case["kw"].get("n_fft") or 2 * (D.shape[-2] - 1)
-        T, length = D.shape[-1], case["kw"].get("length")
-        if length:
-            hop = case["kw"].get("hop_length") or n_fft // 4
-            T = min(T, int(np.ceil((length + (2 * (n_fft // 2) if case["kw"].get("center", True) else 0)) / hop)))
-        _istft_close(oracle, got, run_oracle(oracle, case, golden), case["kw"], n_fft, T)
-        return
-    close(got, run_oracle(oracle, case, golden), **TOL[case["op"]])
-    close(got, golden[name], **TOL[case["op"]])
 
 
 def test_mixed_radix_device_resident_and_batch_identity(lb, oracle):
@@ -615,28 +592,26 @@ def test_two_rank_split_join_on_gpu(lb, oracle):
     close(results["mel"], oracle.melspectrogram(y=Y, sr=22050), **TOL["mel"])
 
 
-@pytest.mark.parametrize("mr", ["0", "1"], ids=["chirpz", "mixed_radix"])
-def test_chirpz_frames_are_paired_inside_a_clip(lb, oracle, monkeypatch, mr):
+@pytest.mark.parametrize("n_fft", [402, 400], ids=["chirpz", "mixed_radix"])
+def test_chirpz_frames_are_paired_inside_a_clip(lb, oracle, n_fft):
     """Two frames share one complex chirp-z transform; the pairs must not straddle clips: a clip 80 dB louder
     (or a non-finite one) next to a quiet clip may not touch the quiet clip's spectrum.  Per-clip tolerance.
-    n_fft = 400 runs on the mixed-radix kernel by default (one warp per frame: nothing is shared between frames);
-    B2L_MR=0 sends it to the chirp-z kernels this test was written for.  The inverse is chirp-z either way."""
+    n_fft = 402 (half 201 = 3 * 67) runs on the chirp-z kernels this test was written for, forward and inverse;
+    n_fft = 400 on the mixed-radix kernels (one warp per frame: nothing is shared between frames)."""
     import signals
+    from librosa_b200 import _pipeline as pl
 
-    monkeypatch.setenv("B2L_MR", mr)
-
+    assert pl.transform_path(n_fft) == {402: "czt", 400: "mr"}[n_fft]
     quiet = signals.make("A", (1, 4000), seed=3)[0] * 1e-4
     loud = signals.make("A", (1, 4000), seed=4)[0]
     Y = np.stack([loud, quiet, loud]).astype(np.float32)
-    kw = dict(n_fft=400, hop_length=160)                     # 26 frames per clip would pair evenly; 4001 -> odd count
-    Yo = np.concatenate([Y, Y[:, :1]], axis=1)               # 4001 samples: 26 frames -> use hop 150 for an odd count
-    kw = dict(n_fft=400, hop_length=150)
+    Yo = np.concatenate([Y, Y[:, :1]], axis=1)               # 4001 samples at hop 150: 27 frames, an odd count
+    kw = dict(n_fft=n_fft, hop_length=150)
     D, Do = lb.stft(Yo, **kw), oracle.stft(Yo, **kw)
     assert D.shape[-1] % 2 == 1                              # odd frame count: the last frame of a clip rides alone
     for c in range(3):
         close(D[c], Do[c], rtol=1e-4, atol_rel=1e-5)      # relative to THIS clip's peak
-    yr, yo = lb.istft(Do, hop_length=150, n_fft=400, length=Yo.shape[-1]), oracle.istft(Do, hop_length=150, n_fft=400,
-                                                                                      length=Yo.shape[-1])
+    yr, yo = lb.istft(Do, length=Yo.shape[-1], **kw), oracle.istft(Do, length=Yo.shape[-1], **kw)
     for c in range(3):
         close(yr[c], yo[c], rtol=1e-4, atol_rel=2e-5)
     # a clip with a NaN poisons only itself (device-resident input: no valid_audio check in front)

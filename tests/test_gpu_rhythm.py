@@ -125,11 +125,9 @@ def test_tempo_kernel_on_oracle_tg(name):
     _check_bpm(got, want, _margins(_oracle_scores(case, tg)), tol, name)
 
 
-@pytest.mark.parametrize("W,mr", [(256, "1"), (512, "1"), (384, "1"), (384, "0"), (343, "1")])
-def test_fourier_tempogram_vs_golden(rhythm_golden, monkeypatch, W, mr):
-    """stft at hop 1 on each forward path: fwd_kernel (256, 512), mr_kernel (384) and chirp-z (384 with B2L_MR=0,
-    343)."""
-    monkeypatch.setenv("B2L_MR", mr)
+@pytest.mark.parametrize("W", [256, 512, 384, 343], ids=lambda W: f"{W}-1")   # window length - stft hop
+def test_fourier_tempogram_vs_golden(rhythm_golden, W):
+    """stft at hop 1 on each forward path: fwd_kernel (256, 512), mr_kernel (384) and chirp-z (343)."""
     case = RC.BY_NAME[f"fourier/win{W}"]
     ref = rhythm_golden[case["name"]]
     got = _quiet(RC.run, lb, case)

@@ -310,32 +310,39 @@ def test_resample_argument_handling_without_a_gpu():
         lb.effects.pitch_shift(y, sr=22050, n_steps=1, bins_per_octave=0, res_type="polyphase")
 
 
-def test_frame_length_routing_table():
-    """Which kernels a frame length goes to (host mirror of csrc/plan.cu: b2l_plan_create / mr_factor): powers of two
-    8 .. 8192 -> fwd_kernel, the 96 even sizes 12 .. 4096 with a 5-smooth half -> the mixed-radix kernels (unless
-    B2L_MR=0), any other size up to 2047 -> chirp-z; the rest is refused by the float32 path."""
+def test_transform_path_table():
+    """Which kernels a frame length goes to (``transform_path``, host mirror of ``plan_path`` in csrc/plan.cu): powers
+    of two 8 .. 8192 -> fwd_kernel, the 96 even sizes 12 .. 4050 with a 5-smooth half -> the mixed-radix kernels, any
+    other size from 3 to 2047 -> chirp-z; the rest is refused by the float32 path.  The C side is held to the same
+    table at every size by tests/test_gpu_forward_spectrum.py."""
     from librosa_b200 import _pipeline as pl
 
-    smooth = [n for n in range(2, 5000) if pl.mr_covers(n)]
+    smooth = [n for n in range(2, 5000) if pl.transform_path(n) == "mr"]
     assert len(smooth) == 96 and smooth[0] == 12 and smooth[-1] == 4050
+    assert smooth == [n for n in range(2, 5000) if pl.mr_covers(n)]
     assert all(n % 2 == 0 and not pl.is_pow2(n) for n in smooth)
     for n in (400, 320, 480, 800, 960, 1200, 3000, 4000):
-        assert pl.mr_covers(n) and pl.fused_front_end(n) and pl.f32_kernels_cover(n)
-    for n in (401, 1025, 14, 2 * 7 * 25, 4098, 2048):
-        assert not pl.mr_covers(n)
+        assert pl.transform_path(n) == "mr"
+    for n in (401, 1025, 14, 2 * 7 * 25):
+        assert pl.transform_path(n) == "czt"
     for n in (8, 2048, 8192):
-        assert pl.fused_front_end(n)
+        assert pl.transform_path(n) == "pow2"
         pl.require_supported_n_fft(n)
+    for n in (501, 1023, 2047):
+        assert pl.transform_path(n) == "czt"
     for n in (501, 1023, 2047, 3000):
         pl.require_supported_n_fft(n)
-    for n in (3001, 2049, 16384, 4102):
+    for n in (3001, 2049, 16384, 4102, 4098, 4, 1):
+        assert pl.transform_path(n) is None
         with pytest.raises(UnsupportedOnGPU):
             pl.require_supported_n_fft(n)
-    os.environ["B2L_MR"] = "0"
-    try:
-        assert not pl.mr_covers(400) and pl.f32_kernels_cover(400) and not pl.f32_kernels_cover(3000)
-    finally:
-        del os.environ["B2L_MR"]
+    with pytest.raises(UnsupportedOnGPU, match=r"^n_fft=16384: the sm_90a kernels are built for powers of two from "
+                                               r"8 to 8192 \(no CPU fallback\)$"):
+        pl.require_supported_n_fft(16384)
+    with pytest.raises(UnsupportedOnGPU, match=r"^n_fft=3001: non-power-of-two sizes are supported from 3 to 2047, "
+                                               r"and even sizes up to 4096 whose half has no prime factor above 5 "
+                                               r"\(no CPU fallback\)$"):
+        pl.require_supported_n_fft(3001)
 
 
 def test_kernels_launch_only_through_launch():

@@ -73,7 +73,7 @@ def mr_irfft(X, n_fft):
 def smooth_sizes():
     from librosa_b200 import _pipeline as pl
 
-    return [n for n in range(12, 4097, 2) if pl.mr_covers(n)]
+    return [n for n in range(12, 4097, 2) if pl.transform_path(n) == "mr"]
 
 
 def test_schedule_and_transforms_for_every_size():
